@@ -1,13 +1,14 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the DSPi hot path on B200 (contract: see DESIGN.md §Measurement).
+"""bench.py — headline benchmark of the DSPi hot path on H100 (contract: see DESIGN.md §Measurement).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 One *step* = one pass of the 10-band EQ cascade over one batch: 65 536 channels x 6144 samples
 (= 64 firmware packets of 96 frames @96 kHz) per GPU, channel-major float32, in place.
 N>1 is launched by torchrun, one rank per GPU; channels shard with no data-path collective
 (weak scaling: 65 536 channels per GPU, 524 288 at N=8 = BASELINE config 5).
-Rank 0 prints ONE JSON line.
+Rank 0 prints ONE JSON line.  --dump-outputs DIR writes what the last timed step computed (a fixed sample
+of its channels) as DIR/*.npy, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -34,7 +35,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -258,6 +259,23 @@ def extra_configs(api, W, L, torch):
     return out
 
 
+DUMP_BYTES = 48 << 20
+
+
+def dump_outputs(out_dir, samples, q):
+    """Writes the samples one timed step left in place: a fixed, seeded sample of channels (all frames of each),
+    float32 (float64 for Q28, which holds every int32 exactly), with the channel indices beside it."""
+    Cn, T = samples.shape
+    itemsize = 8 if q else 4
+    n = max(1, min(Cn, DUMP_BYTES // (T * itemsize)))
+    rows = np.sort(np.random.default_rng(0).choice(Cn, size=n, replace=False))
+    import torch
+    y = samples.index_select(0, torch.from_numpy(rows).to(samples.device)).cpu().numpy()
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "samples.npy"), y.astype(np.float64 if q else np.float32))
+    np.save(os.path.join(out_dir, "channels.npy"), rows.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -271,6 +289,7 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's output (a fixed channel sample) as DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -315,7 +334,7 @@ def main():
     eng.upload(bq)
     kernel_info = eng.kernel_info()       # float engines compile K1 for their topology vector here, outside the timed region
 
-    # rotating input buffers, each larger than L2 (126 MB): 65536 x 6144 x 4 B = 1.5 GiB
+    # rotating input buffers, each larger than L2 (50 MB): 65536 x 6144 x 4 B = 1.5 GiB
     # inputs: the per-channel xorshift32 streams of SURVEY 8(d) (seed 123456789 ^ absolute channel), generated on the GPU
     nbuf = max(2, min(4, args.steps))
     bufs = W.inputs_device(Cn, T, nbuf, q, torch.device("cuda", local_rank), ch0=ch0)
@@ -344,6 +363,8 @@ def main():
     clocks = sampler.stop()
     ms = ev0.elapsed_time(ev1)
     launches = eng.launch_count - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, bufs[(args.steps - 1) % nbuf], q)
     if world > 1:
         t = torch.tensor([ms], dtype=torch.float64, device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -360,14 +381,8 @@ def main():
                 "peak_source": peak_src, "kernel": "eq_q28_kernel" if q else ("eq_f32_jit" if kernel_info.startswith("jit") else "eq_f32_kernel"),
                 "kernel_variant": kernel_info,
                 "algorithmic_bytes_per_launch": Cn * T * ALG_BYTES_PER_SAMPLE,
-                "note": ("integer-multiply bound, not HBM bound: 15 IMAD per band-sample on the half-rate IMAD pipe (DESIGN.md K2)" if q else
-                         "FP32-issue bound, not HBM bound: see DESIGN.md (60 FMA-pipe lane-ops per sample)")}
-    tr = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tr):
-        try:
-            roofline["traffic"] = json.load(open(tr)).get(f"{roofline['kernel']}:{args.arith}:{args.variant}")
-        except Exception:
-            pass
+                "note": ("15 IMAD per band-sample on the half-rate IMAD pipe (DESIGN.md K2); the binding resource is not profiled" if q else
+                         "60 FMA-pipe lane-ops per sample (DESIGN.md K1); whether FP32 issue or HBM binds is not profiled")}
 
     # end to end through the C ABI with HOST buffers (pinned): H2D + kernel(s) + D2H inside the timed region
     e2e = None

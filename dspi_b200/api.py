@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI (``include/dspi_b200.h``) — the call a Python host makes.
 
 There is no CPU path in this package: if ``libdspi_b200.so`` is missing or no
-sm_100 device is visible, construction fails loudly.
+sm_90 device is visible, construction fails loudly.
 """
 import ctypes as C
 import os
@@ -202,7 +202,7 @@ class PinnedBuffer:
 
 
 class EqEngine:
-    """Many independent 10-band cascades on one B200 (``dspi_eq_*``)."""
+    """Many independent 10-band cascades on one GPU (``dspi_eq_*``)."""
 
     def __init__(self, arith, n_channels, n_bands=L.NUM_BANDS, device=0):
         self.arith = ARITH[arith] if isinstance(arith, str) else int(arith)

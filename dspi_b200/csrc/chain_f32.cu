@@ -1,5 +1,5 @@
 // chain_f32.cu — the whole per-packet float signal chain of one DSPi device, for thousands of
-// independent device instances, sm_100a.
+// independent device instances, sm_90a.
 //
 // Reference: process_audio_packet(), firmware/DSPi/usb_audio.c:500-1317 — float pipeline :560-967,
 // single-core branch :874-960; crossfeed.c:132-156; leveller.c:148-262; pdm_generator.c:351-397.
@@ -12,7 +12,7 @@
 //
 //   chain_pre_kernel      warp = 16 instances x {L, R}: PCM unpack, preamp, the two loudness shelves; results leave
 //                         through a shared-memory transpose as ROWS [2 N][frames] (row = side * N + inst)
-//   K1 (eq_f32_kernel.cuh) the 10-band master EQ over those rows — the same TMA-fed packed-FFMA2 kernel
+//   K1 (eq_f32_kernel.cuh) the 10-band master EQ over those rows — the same TMA-fed two-channels-per-lane kernel
 //                         (and run-time specialisation) as the EQ engine, not a second implementation
 //   chain_post_kernel     warp = 16 instances x {L, R}: per-packet leveller (stereo-linked, 480-sample
 //                         look-ahead ring), input peaks, crossfeed; L <-> R exchange by __shfl_xor(.., 16)
@@ -810,7 +810,7 @@ int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t 
         c->launches++;
     }
     const ChainDev d = c->d;
-    const uint32_t n_sms = st.rest_sms ? st.rest_sms : 148;     // SMs the streaming stages run on (chain_streams.cuh)
+    const uint32_t n_sms = st.stream_sms();
     static const uint32_t kStreamCtas = [] { const char *e = getenv("DSPI_CHAIN_CTAS"); const int v = e ? atoi(e) : 0; return (uint32_t)(v >= 1 && v <= 8 ? v : 8); }();   // streaming CTAs (256 threads) per SM
     CU_OK(cudaEventRecord(st.ev_begin, c->stream));
     CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
@@ -901,7 +901,7 @@ int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc)
     if (desc->device < 0 || desc->device >= ndev) return fail(DSPI_ENODEV, "device %d out of range", desc->device);
     int major = 0;
     CU_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, desc->device));
-    if (major != 10) return fail(DSPI_ENODEV, "device %d is not sm_100", desc->device);
+    if (major != 9) return fail(DSPI_ENODEV, "device %d is not sm_90", desc->device);
     CU_OK(cudaSetDevice(desc->device));
     dspi_chain *c = new (std::nothrow) dspi_chain();
     if (!c) return fail(DSPI_ENOMEM, "host allocation failed");

@@ -42,10 +42,8 @@ __device__ __forceinline__ void pdm_modulate_frames(int32_t *__restrict__ pdm, c
             // reference).  With m = s >> 31 (0 when the bit is 1, -1 when it is 0), t2 = s + g - 2K and g2 = g + target - K:
             //   s' = m * -2K + t2      t2' = s' + g' - 2K = m * -3K + (t2 + g2 - 2K)      g2' = g' + target - K = m * -K + (g2 + target - K)
             // Every addend on the right depends on the PREVIOUS step only, so a decision is one shift (ALU pipe) feeding
-            // three independent IMADs (FMA pipe).  Cycles per decision, one warp per SM sub-partition on B200
-            // (scripts/pdm_ubench.cu, profiles/r2_ubench_pdm.txt): 11.9 for this form, 13.5 for two sums (s' and g' feed an
-            // add before the next IMAD), 15.2 for an fp32 formulation (saturating add as comparator), 18.0 for the mask
-            // form, 20.4 with predicated corrections, 23.4 for the reference's own statement order.
+            // three independent IMADs (FMA pipe): the shortest dependence per decision of the forms scripts/pdm_ubench.cu
+            // compares (two sums, an fp32 formulation, the mask form, predicated corrections, the reference's own order).
             uint32_t inv = 0;                                                // complement of the output word
             int32_t s = err2 + dither;
             const int32_t tg = target - 65535;

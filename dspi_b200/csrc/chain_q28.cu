@@ -1,5 +1,5 @@
 // chain_q28.cu — the whole per-packet signal chain in the RP2040's Q28 fixed-point arithmetic, for
-// thousands of independent device instances (2 inputs -> 5 outputs each), bit-exact, sm_100a.
+// thousands of independent device instances (2 inputs -> 5 outputs each), bit-exact, sm_90a.
 //
 // Reference: process_audio_packet(), firmware/DSPi/usb_audio.c:968-1283 (single-core branch
 // :1191-1276); fast_mul_q28 dsp_pipeline.c:47-58; fast_mul_q15 config.h:556-567; cascade
@@ -781,7 +781,7 @@ int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
     if (desc->device < 0 || desc->device >= ndev) return fail(DSPI_ENODEV, "device %d out of range", desc->device);
     int major = 0;
     CU_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, desc->device));
-    if (major != 10) return fail(DSPI_ENODEV, "device %d is not sm_100", desc->device);
+    if (major != 9) return fail(DSPI_ENODEV, "device %d is not sm_90", desc->device);
     CU_OK(cudaSetDevice(desc->device));
     dspi_chainq *c = new (std::nothrow) dspi_chainq();
     if (!c) return fail(DSPI_ENOMEM, "host allocation failed");
@@ -1145,7 +1145,7 @@ int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_d
         c->launches++;
     }
     const ChainQ d = c->d;
-    const uint32_t n_sms = st.rest_sms ? st.rest_sms : 148;     // SMs the streaming stages run on (chain_streams.cuh)
+    const uint32_t n_sms = st.stream_sms();
     static const uint32_t kStreamCtas = [] { const char *e = getenv("DSPI_CHAIN_CTAS"); const int v = e ? atoi(e) : 0; return (uint32_t)(v >= 1 && v <= 8 ? v : 8); }();   // streaming CTAs (256 threads) per SM
     CU_OK(cudaEventRecord(st.ev_begin, c->stream));
     CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));

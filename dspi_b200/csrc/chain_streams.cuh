@@ -13,7 +13,7 @@
 // Sharing SMs with the streaming stages slows exactly that chain down (their CTAs land on its SMs), and its resident
 // CTAs keep K1 - which needs a whole SM's register file per CTA - off those SMs.  So the engine splits the GPU with CUDA
 // green contexts: `pdm_sms` SMs run nothing but the modulator, every other kernel of the call runs on the rest
-// (profiles/r2_greenctx_probe.txt: a 64 / 84 split is honoured, no SM shared).  The driver entry points are looked up at
+// (scripts/greenctx_probe.cu checks that a split is honoured, no SM shared).  The driver entry points are looked up at
 // run time; without them (or with DSPI_PDM_SMS=0) the three priority streams of round 1 are used and results are the same.
 #pragma once
 #include <cstdlib>
@@ -97,13 +97,19 @@ struct ChainStreams {
     cudaEvent_t ev_begin = nullptr, ev_done = nullptr, ev_aux = nullptr, ev_front[kMaxSlices] = {}, ev_out[kMaxSlices] = {};
     CUgreenCtx g_pdm = nullptr, g_rest = nullptr;
     unsigned pdm_sms = 0, rest_sms = 0;                       // 0: no partition (priority streams on the whole GPU)
+    unsigned all_sms = 0;                                     // SM count of the device
 
-    // modulator CTAs are 128 threads (one warp per sub-partition): ceil(instances / 128) SMs, in the partition granularity of 8
+    // SMs the streaming stages run on
+    unsigned stream_sms() const { return rest_sms ? rest_sms : all_sms; }
+
+    // modulator CTAs are 128 threads (one warp per sub-partition): ceil(instances / 128) SMs, in the partition granularity of 8,
+    // at most 48.  On a 132-SM H100 SXM at 8192 instances, 48 modulator SMs beat 56 and 64 by 1-3 % per call (both chains)
+    // and 72 or 80 lose 10-25 %: the other stages need the SMs more.
     static unsigned wanted_pdm_sms(unsigned n_instances)
     {
         if (const char *e = getenv("DSPI_PDM_SMS")) return (unsigned)atoi(e);
         unsigned want = ((n_instances + 127u) / 128u + 7u) / 8u * 8u;
-        return want > 64u ? 64u : want;
+        return want > 48u ? 48u : want;
     }
 
     bool create_partition(int device, unsigned want, int prio_hi, int prio_mid, int prio_lo)
@@ -143,6 +149,9 @@ struct ChainStreams {
     {
         int lo = 0, hi = 0;                                   // numerically lower = higher priority
         cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+        int n_sms = 0;
+        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device);
+        all_sms = (unsigned)n_sms;
         // the modulator is the longest serial chain: its few CTAs are placed first whenever an SM frees a
         // slot; then the front; the many output CTAs fill what is left
         const int mid = hi < lo ? hi + 1 : lo;

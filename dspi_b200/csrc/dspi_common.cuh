@@ -1,4 +1,4 @@
-// dspi_common.cuh — sm_100a device helpers: mbarrier, TMA (cp.async.bulk.tensor), proxies.
+// dspi_common.cuh — sm_90a device helpers: mbarrier, TMA (cp.async.bulk.tensor), proxies.
 #pragma once
 #ifdef __CUDACC_RTC__
 // runtime compilation (eq_jit.cu): no host headers; the tensor map is an opaque 128-byte parameter
@@ -17,8 +17,6 @@ struct alignas(64) CUtensorMap { unsigned long long opaque[16]; };
 #endif
 
 namespace dspi {
-
-constexpr int kSmCount = 148;            // B200: 2 dies x 74 SMs
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p)
 {

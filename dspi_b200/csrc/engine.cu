@@ -1,6 +1,6 @@
 // engine.cu — the C-ABI of include/dspi_b200.h: EQ engine (K1 float / K2 Q28).
 //
-// No CPU fallback lives here: without an sm_100 device every create call fails with
+// No CPU fallback lives here: without an sm_90 device every create call fails with
 // DSPI_ENODEV and nothing else can be reached.
 #include <cstdarg>
 #include <cstdio>
@@ -107,7 +107,7 @@ int dspi_device_count(void)
     int ok = 0;
     for (int i = 0; i < n; i++) {
         int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) ok++;
+        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 9) ok++;
     }
     return ok;
 }
@@ -181,7 +181,7 @@ int dspi_eq_create(dspi_eq **out, const dspi_eq_desc *desc)
     if (desc->device < 0 || desc->device >= ndev) return fail(DSPI_ENODEV, "device %d out of range (%d visible)", desc->device, ndev);
     int major = 0;
     CU_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, desc->device));
-    if (major != 10) return fail(DSPI_ENODEV, "device %d has compute capability %d.x; the kernels are built for sm_100a only", desc->device, major);
+    if (major != 9) return fail(DSPI_ENODEV, "device %d has compute capability %d.x; the kernels are built for sm_90a only", desc->device, major);
     if (!encode_fn()) return fail(DSPI_ENODEV, "driver does not export cuTensorMapEncodeTiled");
     CU_OK(cudaSetDevice(desc->device));
 
@@ -595,9 +595,8 @@ int dspi_eq_process_device_range(dspi_eq *e, void *d_rows, uint32_t T, uint32_t 
 // consecutive chunks overlap, which also keeps BOTH directions of the link busy.  `remote` may be pinned host memory (PCIe)
 // or memory of a peer GPU with peer access enabled (NVLink): cudaMemcpyDefault resolves either.
 // A cascade kernel takes as long as its rows are long however few rows it gets (parallel over channels, serial over time:
-// 0.9 ms for 6144 frames) while a chunk fills only a few SMs, so every staging buffer has a kernel stream of its own and the
-// kernels of consecutive chunks run side by side; one kernel stream would cap the pipeline at one chunk per kernel time
-// (profiles/r2_e2e_chunk_sweep.txt: 32 MiB chunks 8.0, 16 MiB 3.9 G samples/s that way, 11.2 and 11.4 with the streams), and
+// about a millisecond for 6144 frames) while a chunk fills only a few SMs, so every staging buffer has a kernel stream of its own and the
+// kernels of consecutive chunks run side by side; one kernel stream would cap the pipeline at one chunk per kernel time, and
 // the ring is deep enough to cover copy + kernel + copy (kHostBufs).  Channels are independent, so chunk order and size change
 // no bit.  enqueue returns without waiting.
 namespace dspi {
@@ -607,8 +606,8 @@ int eq_process_remote_enqueue(dspi_eq *e, void *remote, uint32_t T, uint32_t ch0
     CU_OK(cudaSetDevice(e->desc.device));
     const uint32_t ld = (T + 3) & ~3u;                                      // device rows padded for TMA
     // chunk bytes: from a peer GPU over NVLink a chunk should take about (kernel time) / (kHostBufs - 3) to copy: 128 MiB.  Over PCIe
-    // 48 MiB measures best (profiles/r2_e2e_chunk_sweep.txt: 11.6 G samples/s; 16 MiB 11.4, 8 MiB 9.9 - smaller copies cost link
-    // efficiency faster than they shorten the ends of the pipeline).  DSPI_HOST_CHUNK_MB overrides both.
+    // 48 MiB chunks are used (smaller copies cost link efficiency faster than they shorten the ends of the pipeline).
+    // DSPI_HOST_CHUNK_MB overrides both.
     static const size_t chunk_mb_env = [] { const char *v = getenv("DSPI_HOST_CHUNK_MB"); const long n = v ? atol(v) : 0; return (size_t)(n >= 1 && n <= 1024 ? n : 0); }();
     cudaPointerAttributes pa;
     const bool on_device = cudaPointerGetAttributes(&pa, remote) == cudaSuccess && pa.type == cudaMemoryTypeDevice;

@@ -1,5 +1,5 @@
 // eq_core.cuh — arithmetic core of the float EQ cascade, shared by the EQ kernel (eq_f32.cu) and
-// the full-chain kernels (chain_f32.cu): value types (scalar / packed f32x2), the per-band
+// the full-chain kernels (chain_f32.cu): value types (scalar / register-pair f32x2), the per-band
 // register-tile loops (TDF2 biquad, Cytomic SVF with its four output mixes) and EqBank, which
 // holds all bands of one channel (or channel pair) in registers and runs a register tile of
 // kSub samples through them.  Reference: dsp_process_channel_block(), dsp_pipeline.c:281-365.
@@ -12,12 +12,12 @@ namespace core {
 constexpr int kSub = 8;             // samples per register tile
 
 // ---------------------------------------------------------------------------------------
-// value types: float (1 channel / lane) or P2 (2 channels / lane, packed f32x2)
+// value types: float (1 channel / lane) or P2 (2 channels / lane, a register pair)
 //
-// P2 is an opaque 64-bit register pair driven with inline PTX: keeping the pair as ONE .b64
-// virtual register forces ptxas to hold every sample/state/coefficient packed for the whole
-// kernel.  (With P2 + the __ffma2_rn intrinsics the halves are separate 32-bit values and
-// ptxas re-packs them with two MOVs around every packed instruction.)
+// P2 is an opaque 64-bit register pair driven with inline PTX.  sm_90 has no packed f32x2
+// arithmetic, so each P2 operation is two scalar .rn.ftz instructions on the halves of the
+// pair (the same roundings a packed instruction would apply); the pair gives every lane two
+// independent recurrences to interleave.
 // ---------------------------------------------------------------------------------------
 struct P2 { unsigned long long v; };
 
@@ -27,19 +27,28 @@ __device__ __forceinline__ float v_fma(float a, float b, float c) { return __fma
 __device__ __forceinline__ P2 v_mul(P2 a, P2 b)
 {
     P2 r;
-    asm("mul.rn.ftz.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
+    asm("{\n\t.reg .f32 a0, a1, b0, b1;\n\t"
+        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\t"
+        "mul.rn.ftz.f32 a0, a0, b0;\n\tmul.rn.ftz.f32 a1, a1, b1;\n\t"
+        "mov.b64 %0, {a0, a1};\n\t}" : "=l"(r.v) : "l"(a.v), "l"(b.v));
     return r;
 }
 __device__ __forceinline__ P2 v_add(P2 a, P2 b)
 {
     P2 r;
-    asm("add.rn.ftz.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
+    asm("{\n\t.reg .f32 a0, a1, b0, b1;\n\t"
+        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\t"
+        "add.rn.ftz.f32 a0, a0, b0;\n\tadd.rn.ftz.f32 a1, a1, b1;\n\t"
+        "mov.b64 %0, {a0, a1};\n\t}" : "=l"(r.v) : "l"(a.v), "l"(b.v));
     return r;
 }
 __device__ __forceinline__ P2 v_fma(P2 a, P2 b, P2 c)
 {
     P2 r;
-    asm("fma.rn.ftz.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
+    asm("{\n\t.reg .f32 a0, a1, b0, b1, c0, c1;\n\t"
+        "mov.b64 {a0, a1}, %1;\n\tmov.b64 {b0, b1}, %2;\n\tmov.b64 {c0, c1}, %3;\n\t"
+        "fma.rn.ftz.f32 a0, a0, b0, c0;\n\tfma.rn.ftz.f32 a1, a1, b1, c1;\n\t"
+        "mov.b64 %0, {a0, a1};\n\t}" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
     return r;
 }
 __device__ __forceinline__ P2 p2_pack(float lo, float hi)
@@ -64,12 +73,12 @@ template <> __device__ __forceinline__ P2 v_set<P2>(float x) { return p2_pack(x,
 __device__ __forceinline__ float v_neg(float a) { return __int_as_float(__float_as_int(a) ^ 0x80000000); }
 __device__ __forceinline__ P2 v_neg(P2 a) { P2 r; r.v = a.v ^ 0x8000000080000000ull; return r; }
 
-// ptxas (12.9) contracts `mul.rn.f32x2` + `add.rn.f32x2` into FFMA2 even with --fmad=false and
-// even when the product is written as fma(a, b, -0.0) with a literal -0.0 (it folds that back to
-// a multiply first).  The strict flavour therefore forms packed products as fma(a, b, nz) where
-// nz = (-0.0, -0.0) arrives as a KERNEL PARAMETER: an exact product rounding (x + -0 == x for
-// every x, including both zeros) that the assembler cannot prove foldable.  Scalar FMUL/FADD
-// and every fused-flavour sequence are left alone by ptxas (checked in the SASS).
+// The strict flavour forms pair products as fma(a, b, nz) where nz = (-0.0, -0.0) arrives as a
+// KERNEL PARAMETER: an exact product rounding (x + -0 == x for every x, including both zeros)
+// that the assembler cannot prove foldable.  The scalar mul.rn / add.rn that the pair operations
+// issue on sm_90 are not contracted either, so this is not needed for correctness there; it stays
+// because it guarantees the strict roundings whatever the assembler does with explicit-rounding
+// arithmetic, and FFMA issues at the same rate as FMUL on the FMA pipe.
 template <bool FUSED> __device__ __forceinline__ float mulx(float a, float b, float) { return __fmul_rn(a, b); }
 template <bool FUSED> __device__ __forceinline__ P2 mulx(P2 a, P2 b, P2 nz)
 {

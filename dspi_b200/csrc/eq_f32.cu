@@ -1,20 +1,19 @@
 // eq_f32.cu — K1: float32 10-band EQ cascade (Cytomic SVF / TDF2 biquad hybrid) for
-// thousands of independent channels, sm_100a.
+// thousands of independent channels, sm_90a.
 //
 // Reference semantics: dsp_process_channel_block(), firmware/DSPi/dsp_pipeline.c:281-365
 // (band outer / sample inner, in place; the per-sample twin :256-279 yields the same values).
 //
 // Mapping
 //   * one warp owns a GROUP of 32*CPL channels for the whole launch; lane L carries channel
-//     L (and L+32 when CPL==2, packed in the two halves of an f32x2 register pair) — the
+//     L (and L+32 when CPL==2, held in the two halves of a 64-bit register pair) — the
 //     serial sample recurrence and all coefficients/state of the 10 bands live in registers;
 //   * samples are channel-major [C][T] in HBM; each warp streams its [32*CPL][32] tiles
 //     through a private 3-stage shared-memory ring with TMA (cp.async.bulk.tensor, 128-byte
 //     swizzle, mbarrier completion) and writes results back with TMA stores from the same
 //     buffers — no block-wide synchronisation anywhere;
-//   * CPL==2 uses Blackwell's packed FFMA2/FMUL2/FADD2 (fma/mul/add.rn.ftz.f32x2): the FMA
-//     pipe sees the same number of lane-operations but only half the issue slots, which
-//     leaves room for LDS/STS/branches next to a saturated FMA pipe.
+//   * CPL==2 gives every lane two independent recurrences (two scalar FFMAs per operation
+//     on sm_90), so the scheduler always has a second dependence chain to issue from.
 //
 // Arithmetic is written with explicit-rounding intrinsics only, so nvcc can neither contract
 // nor reassociate: FUSED follows GCC's -ffp-contract=fast pattern (what arm-none-eabi-gcc
@@ -62,9 +61,8 @@ cudaError_t launch_one(const EqLaunch &a, cudaStream_t stream)
     uint32_t slice_tiles = 0;
     uint32_t *sched = nullptr;
     const uint32_t ntiles = (a.T + kTileT - 1) / kTileT;
-    // The dynamic schedule is opt-in (DSPI_DBG=8): measured on B200 it loses ~6 % to the static one at
-    // 65536 channels - a scheduler left with ONE resident warp runs it well below half the two-warp rate,
-    // which eats the balance it buys (DESIGN.md, K1).
+    // The dynamic schedule is opt-in (DSPI_DBG=8): a scheduler left with ONE resident warp runs it well
+    // below half the two-warp rate, which eats the balance it buys (DESIGN.md, K1).
     if (a.sched && a.use_tma && ntiles >= 32 && (a.dbg & 8u)) {
         slice_tiles = 16;
         sched = a.sched;

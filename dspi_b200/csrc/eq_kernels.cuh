@@ -42,7 +42,7 @@ struct PerDeviceOnce {
 // per-thread message buffer behind dspi_last_error() (engine.cu)
 char *error_buffer(size_t *cap);
 
-// K1 — float cascade.  cpl: channels per lane (1 scalar FFMA, 2 packed FFMA2)
+// K1 — float cascade.  cpl: channels per lane (1, or 2 held in a register pair)
 cudaError_t launch_eq_f32(const EqLaunch &a, bool fused, int cpl, cudaStream_t stream);
 cudaError_t launch_pack_f32(const dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, float *coef, uint64_t *modes, int cpl, cudaStream_t stream);
 cudaError_t launch_unpack_f32(dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, const float *coef, int cpl, cudaStream_t stream);

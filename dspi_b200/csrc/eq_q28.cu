@@ -1,4 +1,4 @@
-// eq_q28.cu — K2: Q28 fixed-point 10-band TDF2 cascade (RP2040 arithmetic), bit-exact, sm_100a.
+// eq_q28.cu — K2: Q28 fixed-point 10-band TDF2 cascade (RP2040 arithmetic), bit-exact, sm_90a.
 //
 // Reference semantics: dsp_process_channel_block() in firmware/DSPi/dsp_process_rp2040.S:225-394;
 // every multiply is fast_mul_q28() (dsp_pipeline.c:47-58):
@@ -156,9 +156,8 @@ eq_q28_kernel(const __grid_constant__ CUtensorMap tmap, int32_t *__restrict__ sa
                 x[4 * h] = q.x; x[4 * h + 1] = q.y; x[4 * h + 2] = q.z; x[4 * h + 3] = q.w;
             }
             // Warps in which no band can be skipped outright get ONE straight-line block over all bands, so that ptxas overlaps
-            // band b+1's first samples with band b's last ones (the per-band branches below fence the scheduler: 32768 ch x 6144 on
-            // B200 ran at 62 G samples/s through them and run at 90 G through this block).  Lanes with a bypassed band keep their
-            // input and state through selects instead of a branch.
+            // band b+1's first samples with band b's last ones (the per-band branches below fence the scheduler).  Lanes with a
+            // bypassed band keep their input and state through selects instead of a branch.
             if (straight && nvalid == kSub) {
                 if (any_byp == 0) {
 #pragma unroll
@@ -269,8 +268,7 @@ cudaError_t launch_one(const EqLaunch &a, cudaStream_t stream)
 cudaError_t launch_eq_q28(const EqLaunch &a, cudaStream_t stream)
 {
     // register tile of 8 or 4 samples (DSPI_K2_SUB): the straight-line body is 10 bands x tile x ~27 instructions, 35 KB at 8.
-    // Halving it to cure the instruction-fetch stalls ncu shows costs more than it saves: 32768 ch x 6144 on B200 run at
-    // 63.9 G samples/s with 8-sample tiles and 56.2 G with 4 (less independent work between dependent IMADs), so 8 stays.
+    // Halving it shortens the body but leaves less independent work between dependent IMADs; 8 is the default.
     static const int sub = [] { const char *e = getenv("DSPI_K2_SUB"); return (e && atoi(e) == 8) ? 8 : ((e && atoi(e) == 4) ? 4 : 8); }();
     if (a.n_bands <= 10) return sub == 4 ? launch_one<10, 4>(a, stream) : launch_one<10, 8>(a, stream);
     return sub == 4 ? launch_one<12, 4>(a, stream) : launch_one<12, 8>(a, stream);

@@ -166,8 +166,9 @@ int dspi_sg_process(dspi_sg *g, void *d_full, uint32_t total_channels, uint32_t 
     const int W = g->world;
     std::vector<uint32_t> lo(W), hi(W);
     for (int r = 0; r < W; r++) dspi_eqx_shard_range(total_channels, (uint32_t)W, (uint32_t)r, &lo[r], &hi[r]);
-    // Transfer time of one direction: the root moves every peer's shard over its own links (measured 575 - 710 GB/s with
-    // grouped ncclSend / ncclRecv, profiles/r2_nccl_sg_*.txt); kernel time: ~0.17 us per frame (float; the Q28 cascade ~6x).
+    // Transfer time of one direction: the root moves every peer's shard over its own links (estimated at 650 GB/s for
+    // grouped ncclSend / ncclRecv); kernel time: ~0.17 us per frame (float; the Q28 cascade ~6x).  Both are estimates that
+    // only set the chunk count, which changes no bit.
     const double t_dir = (double)(total_channels - (hi[g->root] - lo[g->root])) * T * 4.0 / 650e9;
     const double t_kernel = (double)T * 0.17e-6 * 1.1;
     if (n_chunks == 0) {                                                     // automatic: steps of about half a millisecond

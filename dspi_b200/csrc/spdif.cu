@@ -1,4 +1,4 @@
-// spdif.cu — S/PDIF (IEC 60958) subframe encoder for the chain's 24-bit word streams, sm_100a.
+// spdif.cu — S/PDIF (IEC 60958) subframe encoder for the chain's 24-bit word streams, sm_90a.
 // The step right after the hot path (SURVEY.md §8 f-3): what the firmware does with every S/PDIF
 // producer buffer before the PIO serialiser sees it.
 //
@@ -106,7 +106,7 @@ static int spdif_check(int device, const void *a, const void *b, const uint8_t *
     if (device < 0 || device >= ndev) return fail(DSPI_ENODEV, "device %d out of range (%d visible)", device, ndev);
     int major = 0;
     CU_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) return fail(DSPI_ENODEV, "device %d is not sm_100", device);
+    if (major != 9) return fail(DSPI_ENODEV, "device %d is not sm_90", device);
     return DSPI_OK;
 }
 
@@ -120,8 +120,8 @@ int dspi_spdif_encode_device(int device, const int32_t *d_words, uint64_t n_stre
     CU_OK(cudaSetDevice(device));
     uint64_t cs40 = 0;
     for (int i = 0; i < 5; i++) cs40 |= (uint64_t)channel_status[i] << (8 * i);
-    int n_sms = 148;
-    cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device);
+    int n_sms = 0;
+    CU_OK(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device));
     const uint32_t bx = (frames + 255) / 256;
     // enough CTAs for ~4 waves of 8 resident CTAs per SM; every CTA then loops over streams
     uint64_t by = ((uint64_t)n_sms * 8 * 4 + bx - 1) / bx;

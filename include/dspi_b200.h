@@ -1,5 +1,5 @@
 /*
- * dspi_b200.h — C ABI of the B200-native DSPi signal-chain engine.
+ * dspi_b200.h — C ABI of the CUDA-native (H100, sm_90a) DSPi signal-chain engine.
  *
  * Drop-in boundary for the per-sample DSP hot path of WeebLabs/DSPi
  * (SURVEY.md §8b).  The reference has no FFI layer: the path is reached through
@@ -15,7 +15,7 @@
  *   - an engine belongs to one CUDA device and one stream; calls on one engine
  *     must be serialised by the caller (the firmware's single processing
  *     thread, main.c:743), different engines are independent;
- *   - there is NO CPU fallback: if no sm_100 device is present, create fails
+ *   - there is NO CPU fallback: if no sm_90 device is present, create fails
  *     with DSPI_ENODEV.
  */
 #ifndef DSPI_B200_H
@@ -37,7 +37,7 @@ enum {
     DSPI_OK       = 0,
     DSPI_EINVAL   = -22,   /* bad argument                                   */
     DSPI_ENOMEM   = -12,   /* host or device allocation failed               */
-    DSPI_ENODEV   = -19,   /* no sm_100 CUDA device / CUDA runtime unusable  */
+    DSPI_ENODEV   = -19,   /* no sm_90 CUDA device / CUDA runtime unusable   */
     DSPI_ECUDA    = -5,    /* a CUDA call failed (message in dspi_last_error) */
     DSPI_ERANGE   = -34    /* index / size outside the engine's shape        */
 };

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """BASELINE config 3 alone: N instances through the whole chain, device-resident, CUDA events.
-    python scripts/chain_bench.py [--instances 8192] [--packets 16] [--fpp 96] [--reps 3]
-Used under ncu for the per-kernel breakdown (profiles/*chain*)."""
+    python scripts/chain_bench.py [--instances 8192] [--packets 16] [--fpp 96] [--reps 3]"""
 import argparse
 import json
 import os

@@ -1,6 +1,6 @@
-// greenctx_probe.cu — can this driver carve the B200 into two SM partitions (CUDA green contexts) and do kernels launched
+// greenctx_probe.cu — can this driver carve the GPU into two SM partitions (CUDA green contexts) and do kernels launched
 // through a partition's stream stay on its SMs?  Diagnostics for the chain's modulator placement.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O2 -o scripts/_bin/greenctx_probe scripts/greenctx_probe.cu -lcuda
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O2 -o scripts/_bin/greenctx_probe scripts/greenctx_probe.cu -lcuda
 #include <cstdio>
 #include <cstring>
 #include <cuda.h>
