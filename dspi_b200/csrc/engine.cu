@@ -66,7 +66,7 @@ char *error_buffer(size_t *cap)
 
 struct dspi_eq {
     dspi_eq_desc desc;
-    int cpl;                 // channels per lane (float: 1 or 2; Q28: 1)
+    int cpl;                 // channels per lane (float: 1 or 2, which also fixes K1's stage geometry; Q28: 1)
     uint32_t rows;           // channels per group = 32 * cpl
     uint32_t n_groups;
     uint32_t c_pad;          // n_groups * rows
@@ -191,8 +191,11 @@ int dspi_eq_create(dspi_eq **out, const dspi_eq_desc *desc)
     e->desc = *desc;
     e->sig_dirty = true;
     const bool q28 = desc->arith == DSPI_ARITH_Q28;
-    e->cpl = 2;
-    if (const char *v = getenv("DSPI_F32_CPL")) e->cpl = atoi(v) == 1 ? 1 : 2;   // 1 = scalar FFMA variant, for A/B measurement
+    // K1 geometry: one channel per lane, 32 rows x 64 samples per stage (default), or a register pair per lane,
+    // 64 rows x 32 samples per stage (DSPI_F32_CPL=2, for A/B measurement).  Fixed at create time: the packed
+    // coefficient store is laid out by channels per lane.
+    e->cpl = 1;
+    if (const char *v = getenv("DSPI_F32_CPL")) e->cpl = atoi(v) == 2 ? 2 : 1;
     if (q28) e->cpl = 1;
     e->rows = 32u * e->cpl;
     e->n_groups = (desc->n_channels + e->rows - 1) / e->rows;
@@ -363,7 +366,8 @@ static int refresh_kernel_choice(dspi_eq *e)
     e->sig_dirty = false;
     e->jit = nullptr;
     if (e->desc.arith == DSPI_ARITH_Q28) { snprintf(e->kinfo, sizeof(e->kinfo), "aot q28 cascade (K2)"); return DSPI_OK; }
-    if (e->cpl != 2) { snprintf(e->kinfo, sizeof(e->kinfo), "aot scalar generic (DSPI_F32_CPL=1)"); return DSPI_OK; }
+    // the stage geometry closes every report, so that it shows which one ran
+    const char *geo = e->cpl == 1 ? "tile 32 rows x 64 samples, 1 ch/lane" : "tile 64 rows x 32 samples, 2 ch/lane";
     const uint32_t C = e->desc.n_channels, nb = e->desc.n_bands;
     const int nbt = nb <= 10 ? 10 : 12;
     const uint32_t step = C > 2048 ? C / 2048 : 1;
@@ -387,7 +391,7 @@ static int refresh_kernel_choice(dspi_eq *e)
     for (int b = 0; b < nbt; b++) tdf2 |= (uint64_t)dspi::kModeTdf2 << (4 * b);
     const unsigned pct = (unsigned)(100ull * best_n / cnt);
     if (best == tdf2 && (int)nb == nbt) {
-        snprintf(e->kinfo, sizeof(e->kinfo), "aot straight-line biquad (%u%% of sampled channels are all-TDF2)", pct);
+        snprintf(e->kinfo, sizeof(e->kinfo), "aot straight-line biquad (%u%% of sampled channels are all-TDF2); %s", pct, geo);
         return DSPI_OK;
     }
     bool force = false;
@@ -398,13 +402,13 @@ static int refresh_kernel_choice(dspi_eq *e)
     else if (2 * best_n < cnt) why = "no dominant topology vector";
     else if (!force && C < 1024) why = "engine below 1024 channels (DSPI_JIT=force overrides)";
     if (why) {
-        snprintf(e->kinfo, sizeof(e->kinfo), "aot generic column path (%s)", why);
+        snprintf(e->kinfo, sizeof(e->kinfo), "aot generic column path (%s); %s", why, geo);
         return DSPI_OK;
     }
     char msg[256] = "";
-    e->jit = dspi::jit::acquire(best, e->desc.arith == DSPI_ARITH_F32_FUSED, nbt, e->desc.device, msg, sizeof(msg));
-    if (e->jit) snprintf(e->kinfo, sizeof(e->kinfo), "jit sig=0x%llx nb=%d (%u%% of sampled channels)", (unsigned long long)best, nbt, pct);
-    else snprintf(e->kinfo, sizeof(e->kinfo), "aot generic column path (jit unavailable: %.200s)", msg);
+    e->jit = dspi::jit::acquire(best, e->desc.arith == DSPI_ARITH_F32_FUSED, nbt, e->cpl, e->desc.device, msg, sizeof(msg));
+    if (e->jit) snprintf(e->kinfo, sizeof(e->kinfo), "jit sig=0x%llx nb=%d (%u%% of sampled channels); %s", (unsigned long long)best, nbt, pct, geo);
+    else snprintf(e->kinfo, sizeof(e->kinfo), "aot generic column path (jit unavailable: %.200s); %s", msg, geo);
     return DSPI_OK;
 }
 
@@ -458,6 +462,10 @@ static int launch_eq(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, uint3
 
 // ---- engine-internal interface (eq_kernels.cuh) ------------------------------------------------
 namespace dspi {
+
+// Range calls start on multiples of 64 channels for float engines whatever their group size (32 or 64 rows), so that
+// callers' chunk boundaries do not depend on the geometry; Q28 engines keep their 32-channel groups.
+static uint32_t range_unit(const dspi_eq *e) { return e->desc.arith == DSPI_ARITH_Q28 ? e->rows : 64u; }
 
 void *eq_aos_mirror(dspi_eq *e) { return e->d_aos; }
 
@@ -547,7 +555,7 @@ int eq_process_on(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, cudaStre
 int eq_process_range_on(dspi_eq *e, void *d_rows, uint32_t T, uint32_t ld, uint32_t ch0, uint32_t n, cudaStream_t s)
 {
     if (T == 0 || n == 0) return DSPI_OK;
-    if (ch0 % e->rows) return fail(DSPI_EINVAL, "first channel %u is not a multiple of the engine's group size %u", ch0, e->rows);
+    if (ch0 % range_unit(e)) return fail(DSPI_EINVAL, "first channel %u is not a multiple of %u", ch0, range_unit(e));
     CU_OK(cudaSetDevice(e->desc.device));
     return launch_eq(e, d_rows, T, ld, ch0 / e->rows, (n + e->rows - 1) / e->rows, n, s);
 }
@@ -583,7 +591,7 @@ int dspi_eq_process_device_range(dspi_eq *e, void *d_rows, uint32_t T, uint32_t 
     if (T == 0 || n == 0) return DSPI_OK;
     if (ld < T) return fail(DSPI_EINVAL, "row stride %u < T %u", ld, T);
     if ((uint64_t)ch0 + n > e->desc.n_channels) return fail(DSPI_ERANGE, "channels [%u, %u) outside engine of %u", ch0, ch0 + n, e->desc.n_channels);
-    if (ch0 % e->rows) return fail(DSPI_EINVAL, "first channel %u is not a multiple of the engine's group size %u", ch0, e->rows);
+    if (ch0 % dspi::range_unit(e)) return fail(DSPI_EINVAL, "first channel %u is not a multiple of %u", ch0, dspi::range_unit(e));
     CU_OK(cudaSetDevice(e->desc.device));
     return launch_eq(e, d_rows, T, ld, ch0 / e->rows, (n + e->rows - 1) / e->rows, n, e->stream);
 }

@@ -2,14 +2,12 @@
 // the full-chain kernels (chain_f32.cu): value types (scalar / register-pair f32x2), the per-band
 // register-tile loops (TDF2 biquad, Cytomic SVF with its four output mixes) and EqBank, which
 // holds all bands of one channel (or channel pair) in registers and runs a register tile of
-// kSub samples through them.  Reference: dsp_process_channel_block(), dsp_pipeline.c:281-365.
+// N samples through them.  Reference: dsp_process_channel_block(), dsp_pipeline.c:281-365.
 #pragma once
 #include "eq_modes.cuh"
 
 namespace dspi {
 namespace core {
-
-constexpr int kSub = 8;             // samples per register tile
 
 // ---------------------------------------------------------------------------------------
 // value types: float (1 channel / lane) or P2 (2 channels / lane, a register pair)
@@ -327,12 +325,13 @@ struct EqBank {
     }
 
     // run x[0..nvalid) through all active bands, in place (x[nvalid..] is left unspecified)
-    __device__ __forceinline__ void run(V (&x)[kSub], int nvalid, const V nz)
+    template <int N>
+    __device__ __forceinline__ void run(V (&x)[N], int nvalid, const V nz)
     {
-        if (all_tdf2 && nvalid == kSub) {
+        if (all_tdf2 && nvalid == N) {
             // every band of every channel of this warp is a TDF2 biquad: one straight-line block,
             // no dispatch, the scheduler overlaps the bands (wavefront over band x sample)
-            V y[kSub];
+            V y[N];
 #pragma unroll
             for (int b = 0; b < NB; b += 2) {
                 tdf2_tile<FUSED>(x, y, c[b], st[b][0], st[b][1], nz);
@@ -340,14 +339,14 @@ struct EqBank {
             }
             return;
         }
-        V y[kSub];
+        V y[N];
 #pragma unroll
         for (int b = 0; b < NB; b++) {
             // ping-pong between x and y so no case has to move its results back
-            V(&in)[kSub] = (b & 1) ? y : x;
-            V(&out)[kSub] = (b & 1) ? x : y;
+            V(&in)[N] = (b & 1) ? y : x;
+            V(&out)[N] = (b & 1) ? x : y;
             const uint32_t m = (b < (int)nb_active) ? ((uint32_t)(mode_w >> (4 * b)) & 15u) : kModeBypass;
-            const bool fast = (((uni >> b) & 1u) || b >= (int)nb_active) && nvalid == kSub;
+            const bool fast = (((uni >> b) & 1u) || b >= (int)nb_active) && nvalid == N;
             if (fast) {
                 if (m == kModeTdf2) tdf2_tile<FUSED>(in, out, c[b], st[b][0], st[b][1], nz);
                 else if (m == kModeSvfPK) svf_tile<FUSED, kMixPK>(in, out, c[b], st[b][0], st[b][1], nz);
@@ -356,14 +355,14 @@ struct EqBank {
                 else if (m == kModeSvfHP) svf_tile<FUSED, kMixHP>(in, out, c[b], st[b][0], st[b][1], nz);
                 else {                                      // bypassed band: dsp_pipeline.c:288
 #pragma unroll
-                    for (int i = 0; i < kSub; i++) out[i] = in[i];
+                    for (int i = 0; i < N; i++) out[i] = in[i];
                 }
             } else {
-                float xs[CPL][kSub], ns0[CPL], ns1[CPL];
+                float xs[CPL][N], ns0[CPL], ns1[CPL];
 #pragma unroll
                 for (int h = 0; h < CPL; h++) {
 #pragma unroll
-                    for (int i = 0; i < kSub; i++) xs[h][i] = Lanes<V>::get(in[i], h);
+                    for (int i = 0; i < N; i++) xs[h][i] = Lanes<V>::get(in[i], h);
                     const uint32_t mh = (uint32_t)(mode_h[h] >> (4 * b)) & 15u;
                     const float2 ns = slow_band<FUSED>(xs[h], nvalid, mh, Lanes<V>::get(c[b][0], h), Lanes<V>::get(c[b][1], h),
                                                        Lanes<V>::get(c[b][2], h), Lanes<V>::get(c[b][3], h), Lanes<V>::get(c[b][4], h),
@@ -374,7 +373,7 @@ struct EqBank {
                 v_make(st[b][0], ns0);
                 v_make(st[b][1], ns1);
 #pragma unroll
-                for (int i = 0; i < kSub; i++) {
+                for (int i = 0; i < N; i++) {
                     float part[CPL];
 #pragma unroll
                     for (int h = 0; h < CPL; h++) part[h] = xs[h][i];
@@ -388,13 +387,13 @@ struct EqBank {
     // ---- compile-time signature: every band's topology is a template constant ------------------
     // (runtime-compiled kernels for engines whose channels all share one topology vector: the whole
     // cascade becomes one straight-line block like the all-biquad case, for any mix of SVF / TDF2)
-    template <unsigned long long W, int B, bool IN_X>
-    __device__ __forceinline__ void sig_from(V (&x)[kSub], V (&y)[kSub], const V nz)
+    template <unsigned long long W, int B, bool IN_X, int N>
+    __device__ __forceinline__ void sig_from(V (&x)[N], V (&y)[N], const V nz)
     {
         if constexpr (B < NB) {
             constexpr uint32_t m = (uint32_t)((W >> (4 * B)) & 15ull);
-            V(&in)[kSub] = IN_X ? x : y;
-            V(&out)[kSub] = IN_X ? y : x;
+            V(&in)[N] = IN_X ? x : y;
+            V(&out)[N] = IN_X ? y : x;
             if constexpr (m == kModeBypass) {
                 sig_from<W, B + 1, IN_X>(x, y, nz);
             } else {
@@ -404,7 +403,7 @@ struct EqBank {
             }
         } else if constexpr (!IN_X) {
 #pragma unroll
-            for (int i = 0; i < kSub; i++) x[i] = y[i];
+            for (int i = 0; i < N; i++) x[i] = y[i];
         }
     }
     // does every channel of this warp carry exactly the topology vector W (bands >= nb masked off)?
@@ -416,10 +415,10 @@ struct EqBank {
         for (int h = 0; h < CPL; h++) mine = mine && mode_h[h] == W;
         return __all_sync(0xffffffffu, mine);
     }
-    template <unsigned long long W>
-    __device__ __forceinline__ void run_sig(V (&x)[kSub], const V nz)
+    template <unsigned long long W, int N>
+    __device__ __forceinline__ void run_sig(V (&x)[N], const V nz)
     {
-        V y[kSub];
+        V y[N];
         sig_from<W, 0, true>(x, y, nz);
     }
 

@@ -8,12 +8,13 @@
 //   * one warp owns a GROUP of 32*CPL channels for the whole launch; lane L carries channel
 //     L (and L+32 when CPL==2, held in the two halves of a 64-bit register pair) — the
 //     serial sample recurrence and all coefficients/state of the 10 bands live in registers;
-//   * samples are channel-major [C][T] in HBM; each warp streams its [32*CPL][32] tiles
+//   * samples are channel-major [C][T] in HBM; each warp streams its [32*CPL][64/CPL] tiles
 //     through a private 3-stage shared-memory ring with TMA (cp.async.bulk.tensor, 128-byte
 //     swizzle, mbarrier completion) and writes results back with TMA stores from the same
 //     buffers — no block-wide synchronisation anywhere;
-//   * CPL==2 gives every lane two independent recurrences (two scalar FFMAs per operation
-//     on sm_90), so the scheduler always has a second dependence chain to issue from.
+//   * CPL==1 (the default) moves 256 B of each row per transfer; CPL==2 (DSPI_F32_CPL=2)
+//     moves 128 B but gives every lane two independent recurrences (two scalar FFMAs per
+//     operation on sm_90).  Both fill 8 warps x 3 stages x 8 KB of shared memory per SM.
 //
 // Arithmetic is written with explicit-rounding intrinsics only, so nvcc can neither contract
 // nor reassociate: FUSED follows GCC's -ffp-contract=fast pattern (what arm-none-eabi-gcc
@@ -28,11 +29,12 @@ namespace dspi {
 namespace {
 
 using namespace core;
+using k1::kStageBytes;
 using k1::kStages;
-using k1::kTileT;
+using k1::kWarps;
 
 template <typename V, bool FUSED, int NB, bool DYN>
-__global__ void __launch_bounds__(256 * 2 / Lanes<V>::CPL, 1)
+__global__ void __launch_bounds__(kWarps * 32, 1)
 eq_f32_kernel(const __grid_constant__ CUtensorMap tmap, float *__restrict__ samples, uint32_t ld, V *__restrict__ coef,
               const uint64_t *__restrict__ modes, uint32_t n_groups, uint32_t n_rows, uint32_t T, uint32_t nb_active, uint32_t use_tma, uint32_t dbg,
               unsigned long long nz_bits, uint32_t slice_tiles, uint32_t *__restrict__ sched)
@@ -43,9 +45,8 @@ eq_f32_kernel(const __grid_constant__ CUtensorMap tmap, float *__restrict__ samp
 template <typename V, bool FUSED, int NB>
 cudaError_t launch_one(const EqLaunch &a, cudaStream_t stream)
 {
-    constexpr int CPL = Lanes<V>::CPL;
-    constexpr int kWarps = 16 / CPL;
-    constexpr size_t smem = (size_t)kWarps * kStages * (32 * CPL) * kTileT * 4;
+    constexpr int kTileT = k1::tile_t<V>();
+    constexpr size_t smem = (size_t)kWarps * kStages * kStageBytes;
     auto kern = eq_f32_kernel<V, FUSED, NB, false>;
     auto kern_dyn = eq_f32_kernel<V, FUSED, NB, true>;
     static PerDeviceOnce once;                                  // per instantiation
@@ -63,8 +64,8 @@ cudaError_t launch_one(const EqLaunch &a, cudaStream_t stream)
     const uint32_t ntiles = (a.T + kTileT - 1) / kTileT;
     // The dynamic schedule is opt-in (DSPI_DBG=8): a scheduler left with ONE resident warp runs it well
     // below half the two-warp rate, which eats the balance it buys (DESIGN.md, K1).
-    if (a.sched && a.use_tma && ntiles >= 32 && (a.dbg & 8u)) {
-        slice_tiles = 16;
+    if (a.sched && a.use_tma && a.T >= 1024 && (a.dbg & 8u)) {
+        slice_tiles = 512 / kTileT;                             // time slices of 512 samples in either geometry
         sched = a.sched;
         if (grid > (uint32_t)a.n_sms) grid = a.n_sms;
         else if (grid < (uint32_t)a.n_sms && (uint32_t)a.n_sms * kWarps <= n_groups * ((ntiles + slice_tiles - 1) / slice_tiles)) grid = a.n_sms;

@@ -9,8 +9,24 @@ namespace k1 {
 
 using namespace core;
 
-constexpr int kTileT = 32;          // samples per shared-memory tile row: 128 B == swizzle span
+// Geometry.  A warp streams its 32*CPL channels (rows) through a private ring of kStages stages of
+// 8 KB; a CTA is kWarps such warps (192 KB of shared memory, one CTA per SM).  The stage of a
+// one-channel-per-lane warp is 32 rows x 64 samples, that of a channel-pair warp 64 rows x 32
+// samples.  A stage is loaded and stored as 32-sample boxes of 128 B per row (the 128-byte swizzle
+// span), placed one after the other: chunk k (16 B, 4 samples) of row r lives at
+//   (k / 8) * (rows * 128) + r * 128 + ((k % 8) ^ (r % 8)) * 16.
+// The wide stage moves 256 B of every row per transfer, both ways, so each DRAM page opened for a
+// row serves twice the data it does for 128 B.
 constexpr int kStages = 3;
+constexpr int kWarps = 8;
+constexpr uint32_t kStageBytes = 8192;
+template <typename V> __host__ __device__ constexpr int tile_t() { return 64 / Lanes<V>::CPL; }     // samples per stage
+template <typename V> __host__ __device__ constexpr int sub_t() { return tile_t<V>() / 4; }          // samples per register tile
+
+__device__ __forceinline__ uint32_t chunk_off(int r, int k, uint32_t half_bytes)
+{
+    return (uint32_t)(k >> 3) * half_bytes + r * 128 + ((((k & 7) ^ (r & 7))) << 4);
+}
 
 // SIG::enabled: the launch is known to have ONE topology vector SIG::word for every channel
 struct NoSig { static constexpr bool enabled = false; static constexpr unsigned long long word = 0; };
@@ -22,11 +38,14 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
 {
     constexpr int CPL = Lanes<V>::CPL;
     constexpr int kRows = 32 * CPL;
-    constexpr int kWarps = 16 / CPL;
-    constexpr uint32_t kStageBytes = kRows * kTileT * 4;
+    constexpr int kTileT = tile_t<V>();
+    constexpr int kSub = sub_t<V>();
+    constexpr int kHalves = kTileT / 32;                        // 32-sample boxes per stage
+    constexpr uint32_t kHalfBytes = kRows * 128;
+    static_assert(kRows * kTileT * 4 == (int)kStageBytes, "every geometry fills the same 8 KB stage");
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bars[16 / Lanes<V>::CPL][kStages];
+    __shared__ uint64_t bars[kWarps][kStages];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -42,7 +61,6 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
     const V nz = v_bits<V>(nz_bits);                            // (-0.0, -0.0): see mulx()
     const uint32_t ntiles = (T + kTileT - 1) / kTileT;
     const bool mem_on = !(dbg & 2u);                            // diagnostics: DSPI_DBG=2 runs the arithmetic without HBM traffic
-    const uint32_t sw = (lane & 7) << 4;                        // 128B-swizzle XOR for this lane's rows
 
     // ---- work distribution -------------------------------------------------------------------
     // A work item is (group g, time slice k): `slice_tiles` consecutive tiles of the 32*CPL channels
@@ -82,10 +100,14 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
         }
         const int c0 = g * kRows;                               // first channel (row) of this group
 
+        // boxes of a tile that start inside the row (a box wholly past T is neither loaded nor stored)
+        auto n_boxes = [&](uint32_t tile) { return kHalves == 1 || tile * kTileT + 32 < T ? kHalves : 1; };
         auto issue_load = [&](uint32_t tile, uint32_t seq) {    // lane 0 only; seq = position in this warp's ring sequence
             const uint32_t s = seq % kStages;
-            mbar_arrive_expect_tx(&full[s], kStageBytes);
-            tma_load_2d(my_smem + s * kStageBytes, &tmap, &full[s], tile * kTileT, c0);
+            const int nb = n_boxes(tile);
+            mbar_arrive_expect_tx(&full[s], nb * kHalfBytes);
+            for (int h = 0; h < nb; h++)                        // back to back: every row's boxes arrive together
+                tma_load_2d(my_smem + s * kStageBytes + h * kHalfBytes, &tmap, &full[s], tile * kTileT + h * 32, c0);
         };
         if (use_tma && mem_on && lane == 0) {
             if constexpr (DYN) tma_store_wait_read<0>();        // ring buffers of the previous item are drained
@@ -113,30 +135,34 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
             if (use_tma) {
                 if (mem_on) mbar_wait(&full[s], (tcount / kStages) & 1);
             } else {                                                // plain-load fallback (odd strides / unaligned bases)
-                const uint32_t t = tile * kTileT + lane;
                 for (int r = 0; r < kRows; r++) {
                     const uint32_t ch = c0 + r;
-                    float v = 0.0f;
-                    if (t < T && ch < n_rows) v = samples[(size_t)ch * ld + t];
-                    *reinterpret_cast<float *>(buf + r * 128 + ((((lane >> 2) << 4) ^ ((r & 7) << 4)) | ((lane & 3) << 2))) = v;
+                    for (int h = 0; h < kHalves; h++) {
+                        const uint32_t t = tile * kTileT + h * 32 + lane;
+                        float v = 0.0f;
+                        if (t < T && ch < n_rows) v = samples[(size_t)ch * ld + t];
+                        *reinterpret_cast<float *>(buf + chunk_off(r, h * 8 + (lane >> 2), kHalfBytes) + ((lane & 3) << 2)) = v;
+                    }
                 }
                 __syncwarp();
             }
 
             const int tile_valid = min((int)kTileT, (int)(T - tile * kTileT));
-            if (straight && tile_valid == kTileT && !(dbg & 4u)) {
+            // a partial tile whose length is a whole number of register tiles (the 32-sample tail of a 96-frame
+            // packet in a 64-sample stage) stays on the straight-line path
+            if (straight && tile_valid % kSub == 0 && !(dbg & 4u)) {
                 // ---- all-biquad warps: register tiles of kSub samples, straight-line over the 10 bands ----
     #pragma unroll 1
-                for (int sub = 0; sub < kTileT / kSub; sub++) {
-                    // two 16-byte chunks per row per sub-tile; chunk index XOR (row & 7)
+                for (int sub = 0; sub < tile_valid / kSub; sub++) {
+                    // kSub / 4 16-byte chunks per row per sub-tile (LDS.128, conflict-free: chunk index XOR (row & 7))
+                    constexpr int kQ = kSub / 4;
                     V x[kSub];
-                    float4 q[CPL][2];
+                    float4 q[CPL][kQ];
     #pragma unroll
-                    for (int h = 0; h < CPL; h++) {
-                        const uint8_t *row = buf + (lane + 32 * h) * 128;
-                        q[h][0] = *reinterpret_cast<const float4 *>(row + (((2 * sub) << 4) ^ sw));
-                        q[h][1] = *reinterpret_cast<const float4 *>(row + (((2 * sub + 1) << 4) ^ sw));
-                    }
+                    for (int h = 0; h < CPL; h++)
+    #pragma unroll
+                        for (int j = 0; j < kQ; j++)
+                            q[h][j] = *reinterpret_cast<const float4 *>(buf + chunk_off(lane + 32 * h, kQ * sub + j, kHalfBytes));
     #pragma unroll
                     for (int i = 0; i < kSub; i++) {
                         float part[CPL];
@@ -152,24 +178,21 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
                         else bank.run(x, kSub, nz);
                     }
     #pragma unroll
-                    for (int h = 0; h < CPL; h++) {
-                        uint8_t *row = buf + (lane + 32 * h) * 128;
-                        *reinterpret_cast<float4 *>(row + (((2 * sub) << 4) ^ sw)) =
-                            make_float4(Lanes<V>::get(x[0], h), Lanes<V>::get(x[1], h), Lanes<V>::get(x[2], h), Lanes<V>::get(x[3], h));
-                        *reinterpret_cast<float4 *>(row + (((2 * sub + 1) << 4) ^ sw)) =
-                            make_float4(Lanes<V>::get(x[4], h), Lanes<V>::get(x[5], h), Lanes<V>::get(x[6], h), Lanes<V>::get(x[7], h));
-                    }
+                    for (int h = 0; h < CPL; h++)
+    #pragma unroll
+                        for (int j = 0; j < kQ; j++)
+                            *reinterpret_cast<float4 *>(buf + chunk_off(lane + 32 * h, kQ * sub + j, kHalfBytes)) =
+                                make_float4(Lanes<V>::get(x[4 * j], h), Lanes<V>::get(x[4 * j + 1], h), Lanes<V>::get(x[4 * j + 2], h),
+                                            Lanes<V>::get(x[4 * j + 3], h));
                 }
             } else {
                 // ---- any other topology: band-outer over the tile, re-laid out in place as lane-private
                 //      columns of CPL-vectors (sample n of this lane at col[n * 32]) ----
-                float4 q[CPL][8];
+                float4 q[CPL][kTileT / 4];
     #pragma unroll
-                for (int h = 0; h < CPL; h++) {
-                    const uint8_t *row = buf + (lane + 32 * h) * 128;
+                for (int h = 0; h < CPL; h++)
     #pragma unroll
-                    for (int k = 0; k < 8; k++) q[h][k] = *reinterpret_cast<const float4 *>(row + ((k << 4) ^ sw));
-                }
+                    for (int k = 0; k < kTileT / 4; k++) q[h][k] = *reinterpret_cast<const float4 *>(buf + chunk_off(lane + 32 * h, k, kHalfBytes));
                 __syncwarp();                                       // every row is in registers before columns overwrite them
                 V *col = reinterpret_cast<V *>(buf) + lane;
     #pragma unroll
@@ -194,20 +217,20 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
                 }
                 __syncwarp();
     #pragma unroll
-                for (int h = 0; h < CPL; h++) {
-                    uint8_t *row = buf + (lane + 32 * h) * 128;
+                for (int h = 0; h < CPL; h++)
     #pragma unroll
-                    for (int k = 0; k < 8; k++)
-                        *reinterpret_cast<float4 *>(row + ((k << 4) ^ sw)) = make_float4(back[h][4 * k], back[h][4 * k + 1], back[h][4 * k + 2], back[h][4 * k + 3]);
-                }
+                    for (int k = 0; k < kTileT / 4; k++)
+                        *reinterpret_cast<float4 *>(buf + chunk_off(lane + 32 * h, k, kHalfBytes)) =
+                            make_float4(back[h][4 * k], back[h][4 * k + 1], back[h][4 * k + 2], back[h][4 * k + 3]);
             }
 
             if (use_tma) {
                 fence_proxy_async_smem();                           // my smem writes -> async proxy
                 __syncwarp();
                 if (lane == 0 && mem_on) {
-                    tma_store_2d(&tmap, buf, tile * kTileT, c0);
-                    tma_store_commit();
+                    const int nb = n_boxes(tile);
+                    for (int h = 0; h < nb; h++) tma_store_2d(&tmap, buf + h * kHalfBytes, tile * kTileT + h * 32, c0);
+                    tma_store_commit();                             // the stage leaves as one bulk group
                     const uint32_t nxt = tile + kStages - 1;        // refill the buffer stored one iteration ago
                     if (nxt < tile_end) {
                         tma_store_wait_read<1>();
@@ -216,11 +239,13 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
                 }
             } else {
                 __syncwarp();
-                const uint32_t t = tile * kTileT + lane;
                 for (int r = 0; r < kRows; r++) {
                     const uint32_t ch = c0 + r;
-                    const float v = *reinterpret_cast<const float *>(buf + r * 128 + ((((lane >> 2) << 4) ^ ((r & 7) << 4)) | ((lane & 3) << 2)));
-                    if (t < T && ch < n_rows) samples[(size_t)ch * ld + t] = v;
+                    for (int h = 0; h < kHalves; h++) {
+                        const uint32_t t = tile * kTileT + h * 32 + lane;
+                        const float v = *reinterpret_cast<const float *>(buf + chunk_off(r, h * 8 + (lane >> 2), kHalfBytes) + ((lane & 3) << 2));
+                        if (t < T && ch < n_rows) samples[(size_t)ch * ld + t] = v;
+                    }
                 }
                 __syncwarp();
             }
