@@ -40,6 +40,7 @@ SYMBOLS = [
     "dspi_eqx_upload_biquads", "dspi_eqx_download_biquads", "dspi_eqx_process_host", "dspi_eqx_process_root", "dspi_eqx_launch_count",
     "dspi_chain_set_dynamics_device", "dspi_chainq_set_dynamics_device", "dspi_chain_sm_partition", "dspi_chainq_sm_partition",
     "dspi_chain_set_preset_mute", "dspi_chain_get_preset_mute", "dspi_chainq_set_preset_mute", "dspi_chainq_get_preset_mute",
+    "dspi_chain_process_packets_host", "dspi_chain_process_packets_device", "dspi_chainq_process_packets_host", "dspi_chainq_process_packets_device",
 ]
 
 
@@ -136,6 +137,8 @@ def lib():
             getattr(h, pre + "_get_preset_mute").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_set_dynamics_device").argtypes = [vp, u32, u32, vp, C.c_float]
             getattr(h, pre + "_sm_partition").argtypes = [vp, vp, vp]
+            getattr(h, pre + "_process_packets_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
+            getattr(h, pre + "_process_packets_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
         h.dspi_eq_process_device_range.argtypes = [vp, vp, u32, u32, u32, u32]
         h.dspi_bind_host_to_device.argtypes = [C.c_int]
         h.dspi_nccl_unique_id.argtypes = [vp]
@@ -352,6 +355,16 @@ class ScatterGather:
             self._h = C.c_void_p()
 
 
+def _packet_table(packet_frames):
+    """Any integer sequence of packet lengths -> (uint16 array, total frames).  The library rejects lengths outside
+    1..192; values that would wrap in uint16 are rejected here."""
+    t = np.asarray(packet_frames, np.int64).reshape(-1)
+    if t.size and (t.min() < 0 or t.max() > 0xFFFF):
+        raise DspiError("packet lengths must be 1..192 frames")
+    t = np.ascontiguousarray(t, np.uint16)
+    return t, int(t.sum(dtype=np.int64))
+
+
 def bind_host_to_device(device):
     """NUMA-bind this thread and its future allocations to the device's PCIe node; returns the node or -1."""
     return int(lib().dspi_bind_host_to_device(int(device)))
@@ -462,6 +475,28 @@ class ChainEngine:
                                                C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
                                                C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
                                                C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def process_packets_host(self, pcm, bit_depth, packet_frames, want_spdif=True, want_pdm=True, want_status=True):
+        """One USB packet per entry of ``packet_frames`` (its length in frames, shared by every instance).
+        ``pcm``: uint8 [n_instances, F * bytes_per_frame] with F = sum(packet_frames).  Returns (spdif, pdm, status)."""
+        t, F = _packet_table(packet_frames)
+        pcm = np.ascontiguousarray(pcm)
+        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
+        spdif = np.zeros((self.n_instances, 4, F, 2), np.int32) if want_spdif else None
+        pdm = np.zeros((self.n_instances, F, 8), np.uint32) if want_pdm else None
+        status = np.zeros(self.n_instances, L.STATUS) if want_status else None
+        _check(lib().dspi_chain_process_packets_host(self._h, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
+                                                     spdif.ctypes.data if want_spdif else None, pdm.ctypes.data if want_pdm else None,
+                                                     status.ctypes.data if want_status else None))
+        return spdif, pdm, status
+
+    def process_packets_device(self, pcm_ptr, bit_depth, packet_frames, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
+        """``process_packets_host`` with device pointers, asynchronous on the engine stream (outputs for F = sum(packet_frames))."""
+        t, _ = _packet_table(packet_frames)
+        _check(lib().dspi_chain_process_packets_device(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
+                                                       C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
+                                                       C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                       C.c_void_p(int(status_ptr)) if status_ptr else None))
 
     def sync(self):
         _check(lib().dspi_chain_sync(self._h))
@@ -720,6 +755,25 @@ class ChainEngineQ28:
                                                 C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
                                                 C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
                                                 C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def process_packets_host(self, pcm, bit_depth, packet_frames):
+        """As ``ChainEngine.process_packets_host``; spdif [n_instances, 2, F, 2]."""
+        t, F = _packet_table(packet_frames)
+        pcm = np.ascontiguousarray(pcm)
+        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
+        spdif = np.zeros((self.n_instances, 2, F, 2), np.int32)
+        pdm = np.zeros((self.n_instances, F, 8), np.uint32)
+        status = np.zeros(self.n_instances, L.STATUS_Q28)
+        _check(lib().dspi_chainq_process_packets_host(self._h, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
+                                                      spdif.ctypes.data, pdm.ctypes.data, status.ctypes.data))
+        return spdif, pdm, status
+
+    def process_packets_device(self, pcm_ptr, bit_depth, packet_frames, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
+        t, _ = _packet_table(packet_frames)
+        _check(lib().dspi_chainq_process_packets_device(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
+                                                        C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
+                                                        C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                        C.c_void_p(int(status_ptr)) if status_ptr else None))
 
     def sync(self):
         _check(lib().dspi_chainq_sync(self._h))

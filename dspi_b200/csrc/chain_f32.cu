@@ -38,6 +38,7 @@
 
 #include "eq_kernels.cuh"
 #include "chain_pdm.cuh"
+#include "chain_schedule.cuh"
 #include "chain_streams.cuh"
 #include "dynamics.cuh"
 
@@ -74,6 +75,7 @@ struct ChainDev {
     float *vol_base, *vol_master, *o_glin;        // [N_pad] host volume (:569), [N_pad] master volume, [9][N_pad] outputs[o].gain_linear
     float *pmg;                                   // [N_pad] the constant preset_mute_gain of dspi_chain_set_params
     float *vmm;                                   // [packets of the call][N_pad] vol_mul_master (:571) of envelope-mode instances
+    const uint32_t *off;                          // [packets of the call + 1] first frame of each packet (chain_schedule.cuh)
 };
 
 // a*b + c, c - a*b in the flavour's rounding (scalar: negation is free)
@@ -225,18 +227,18 @@ chain_pre_kernel(ChainDev d, const uint8_t *__restrict__ pcm, uint32_t bit_depth
 // ---------------------------------------------------------------------------------------------
 template <bool FUSED>
 __global__ void __launch_bounds__(128)
-chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
+chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t longest)
 {
-    extern __shared__ float smem[];                       // per warp: packet columns [fpp][33] + look-ahead reads [fpp][33]
+    extern __shared__ float smem[];                       // per warp: packet columns [longest][33] + look-ahead reads [longest][33]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t side = lane >> 4;
     const uint32_t inst16 = (blockIdx.x * (blockDim.x >> 5) + warp) * 16;
     if (inst16 >= d.N_pad) return;
     const uint32_t inst = inst16 + (lane & 15);
     const uint32_t Np = d.N_pad;
-    float *xw = smem + (size_t)warp * 2 * fpp * kXs;      // xw[t * 33 + r]: column r of this warp
+    float *xw = smem + (size_t)warp * 2 * longest * kXs;  // xw[t * 33 + r]: column r of this warp
     float *xs = xw + lane;                                // own column
-    float *hs = xw + (size_t)fpp * kXs + lane;            // held look-ahead samples, own column
+    float *hs = xw + (size_t)longest * kXs + lane;        // held look-ahead samples, own column
 
     const uint8_t flags = d.flags[inst];
     const bool lev_on = flags & F_LEV, xf_on = flags & F_XFEED, lookahead = flags & F_LOOKAHEAD;
@@ -254,22 +256,22 @@ chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
     float peak_in = 0.0f;
     uint16_t clip = 0;
     for (uint32_t p = p0; p < p0 + n_packets; p++) {
-        const uint32_t f0 = p * fpp;
+        const uint32_t f0 = d.off[p], count = d.off[p + 1] - f0;          // the leveller's block is this packet
         // The look-ahead ring is read one slot per sample, each read just before that slot is overwritten
         // (leveller.c:231-237), and a packet (<= 192 frames) never laps the 480-slot ring: all of this
         // packet's reads are issued now as asynchronous copies, together with the packet itself.
         if (lev_on && lookahead) {
             uint32_t idx = la_idx;
-            for (uint32_t i = 0; i < fpp; i++) {
+            for (uint32_t i = 0; i < count; i++) {
                 cp_async_4(hs + i * kXs, la_buf + (size_t)idx * Np);
                 if (++idx >= (uint32_t)kLa) idx = 0;
             }
         }
         // packet in: lane = frame, coalesced row reads, transposed into lane-private columns (asynchronous
-        // copies again: 32 rows x fpp/32 independent requests in flight instead of one load-store pair at a time)
+        // copies again: 32 rows x count/32 independent requests in flight instead of one load-store pair at a time)
         for (int r = 0; r < 32; r++) {
             const float *row = d.mrow + ((size_t)(r >> 4) * Np + inst16 + (r & 15)) * d.ldF + f0;
-            for (uint32_t t = lane; t < fpp; t += 32) cp_async_4(xw + t * kXs + r, row + t);
+            for (uint32_t t = lane; t < count; t += 32) cp_async_4(xw + t * kXs + r, row + t);
         }
         cp_async_commit();
         cp_async_wait_all();
@@ -296,7 +298,7 @@ chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
         if (__any_sync(0xffffffffu, lev_on)) {
             const float a_rms = lvc[0], one_minus = __fadd_rn(1.0f, -a_rms);
             float e = env;
-            for (uint32_t i = 0; i < fpp; i++) {                             // leveller.c:161-166
+            for (uint32_t i = 0; i < count; i++) {                             // leveller.c:161-166
                 const float s = xs[i * kXs];
                 e = fm<FUSED>(a_rms, e, __fmul_rn(one_minus, __fmul_rn(s, s)));
             }
@@ -314,17 +316,17 @@ chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
                 if (gc_db > lvc[8]) gc_db = lvc[8];
             }
             const float alpha_s = (gc_db < smooth_db) ? lvc[1] : lvc[2];     // :198
-            const float alpha = (float)pow((double)alpha_s, (double)(float)fpp);
+            const float alpha = (float)pow((double)alpha_s, (double)(float)count);
             const float new_smooth = fm<FUSED>(alpha, smooth_db, __fmul_rn(__fadd_rn(1.0f, -alpha), gc_db));
             const float new_gain = (float)pow(10.0, (double)__fdiv_rn(new_smooth, 20.0f));
             // every lane walks the same shuffles; only instances with the leveller on commit results
             const float prev_for_ramp = gain_lin;
             float gain, gain_step;
-            if (fpp == 1) { gain = new_gain; gain_step = 0.0f; }
-            else { gain_step = __fdiv_rn(__fadd_rn(new_gain, -prev_for_ramp), (float)(fpp - 1)); gain = prev_for_ramp; }
+            if (count == 1) { gain = new_gain; gain_step = 0.0f; }
+            else { gain_step = __fdiv_rn(__fadd_rn(new_gain, -prev_for_ramp), (float)(count - 1)); gain = prev_for_ramp; }
             // the leveller's per-sample part and PASS 3 share one loop: ramp, look-ahead exchange and peak limit of sample
             // i+1 do not depend on the crossfeed recurrence of sample i, so the serial chains overlap
-            for (uint32_t i = 0; i < fpp; i++) {                             // :228-259, then usb_audio.c:741-749
+            for (uint32_t i = 0; i < count; i++) {                             // :228-259, then usb_audio.c:741-749
                 const float x0 = xs[i * kXs];
                 float o = x0;
                 if (lev_on && lookahead) {
@@ -354,13 +356,13 @@ chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
                 gain_lin = new_gain;
             }
         } else {
-            for (uint32_t i = 0; i < fpp; i++) peak_and_crossfeed(i, xs[i * kXs]);
+            for (uint32_t i = 0; i < count; i++) peak_and_crossfeed(i, xs[i * kXs]);
         }
         peak_in = pk;                                                        // peaks describe the last packet
         if (pk > 1.001f) clip |= (uint16_t)(1u << side);                     // config.h:53
         __syncwarp();
         // packet out: back into the same rows, coalesced
-        for (uint32_t t = lane; t < fpp; t += 32) {
+        for (uint32_t t = lane; t < count; t += 32) {
 #pragma unroll 8
             for (int r = 0; r < 32; r++)
                 d.mrow[((size_t)(r >> 4) * Np + inst16 + (r & 15)) * d.ldF + f0 + t] = xw[t * kXs + r];
@@ -431,7 +433,7 @@ chain_mix_kernel(ChainDev d, uint32_t f_begin, uint32_t f_end)
 // update_preset_mute_envelope() (usb_audio.c:466-498) for every packet of the call, one instance per thread, and the
 // volume chain of :569-571 that depends on it: vmm[p] = (vol_base * g_p) * master_volume_linear.  Same operations, same
 // order as dspi_preset_mute_step() on the host.
-__global__ void chain_env_kernel(ChainDev d, uint32_t n_packets, uint32_t fpp)
+__global__ void chain_env_kernel(ChainDev d, uint32_t n_packets)
 {
     const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t Np = d.N_pad;
@@ -442,13 +444,14 @@ __global__ void chain_env_kernel(ChainDev d, uint32_t n_packets, uint32_t fpp)
     unsigned long long ts = ((unsigned long long)fs * 8ull + 999ull) / 1000ull;          // :459-464
     if (ts < 1ull) ts = 1ull;
     if (ts > 0xFFFFFFFFull) ts = 0xFFFFFFFFull;
-    float step = __fdiv_rn((float)fpp, (float)(uint32_t)ts);                             // :486
-    if (step > 1.0f) step = 1.0f;
     const float vol_base = d.vol_base[inst], master = d.vol_master[inst];
     for (uint32_t p = 0; p < n_packets; p++) {
+        const uint32_t count = d.off[p + 1] - d.off[p];                                  // sample_count of this packet
+        float step = __fdiv_rn((float)count, (float)(uint32_t)ts);                       // :486
+        if (step > 1.0f) step = 1.0f;
         const bool active = loading != 0;                                                // :469
         if (active) {
-            if (counter > fpp) counter -= fpp;
+            if (counter > count) counter -= count;
             else { counter = 0; loading = 0; }
         }
         const float target = active ? 0.0f : 1.0f;
@@ -527,13 +530,14 @@ struct OutCfg {
     float gain;                        // constant gain of the call (no envelope)
     float glin;                        // outputs[o].gain_linear
     const float *vmm;                  // envelope mode: vol_mul_master per packet, stride N_pad; else nullptr
-    uint32_t fpp, Np;
+    const uint32_t *off;               // packet offsets of the call
+    uint32_t Np;
     uint32_t dl;                       // delay & (MAX - 1): MAX aliases to 0 (SURVEY a-10)
     const float *row;                  // orow row of this (output, instance)
     const float *ring;
 };
 
-__device__ __forceinline__ OutCfg out_cfg(const ChainDev &d, uint32_t o, uint32_t inst, bool any_delay, uint32_t fpp)
+__device__ __forceinline__ OutCfg out_cfg(const ChainDev &d, uint32_t o, uint32_t inst, bool any_delay)
 {
     OutCfg c;
     const uint32_t Np = d.N_pad;
@@ -545,7 +549,7 @@ __device__ __forceinline__ OutCfg out_cfg(const ChainDev &d, uint32_t o, uint32_
     c.gain = d.o_gain[o * Np + inst];
     c.glin = d.o_glin[o * Np + inst];
     c.vmm = d.env[4 * Np + inst] ? d.vmm + inst : nullptr;
-    c.fpp = fpp;
+    c.off = d.off;
     c.Np = Np;
     c.delay_on = any_delay && dly > 0;                                       // usb_audio.c:898-901
     c.dl = (uint32_t)dly & (kMaxDelay - 1);
@@ -554,20 +558,21 @@ __device__ __forceinline__ OutCfg out_cfg(const ChainDev &d, uint32_t o, uint32_
     return c;
 }
 
-// output gain in force at frame T of the call (usb_audio.c:886-887): constant, or following the envelope packet by packet
-__device__ __forceinline__ float gain_at(const OutCfg &c, uint32_t T)
+// output gain in force at frame T of the call (usb_audio.c:886-887): constant, or following the envelope packet by packet;
+// p is the packet of T or a later one
+__device__ __forceinline__ float gain_at(const OutCfg &c, uint32_t T, uint32_t p)
 {
     if (!c.vmm) return c.gain;
-    return c.mute ? 0.0f : __fmul_rn(c.glin, c.vmm[(size_t)(T / c.fpp) * c.Np]);
+    return c.mute ? 0.0f : __fmul_rn(c.glin, c.vmm[(size_t)packet_of(c.off, T, p) * c.Np]);
 }
 
-// the sample output `c` emits at frame T of this call (T counted from the start of the call):
+// the sample output `c` emits at frame T (in packet p) of this call (T counted from the start of the call):
 // write-then-read per sample (:902-909) means frame T emits the post-gain sample of frame T - dl;
 // inside the call that sample is still in the output rows, before it only the ring has it
-__device__ __forceinline__ float out_sample(const OutCfg &c, uint32_t T, uint32_t widx0)
+__device__ __forceinline__ float out_sample(const OutCfg &c, uint32_t T, uint32_t p, uint32_t widx0)
 {
-    if (!c.delay_on) return out_gain(c.row[T], c.enabled, gain_at(c, T));
-    if (T >= c.dl) return out_gain(c.row[T - c.dl], c.enabled, gain_at(c, T - c.dl));
+    if (!c.delay_on) return out_gain(c.row[T], c.enabled, gain_at(c, T, p));
+    if (T >= c.dl) return out_gain(c.row[T - c.dl], c.enabled, gain_at(c, T - c.dl, p));
     return c.ring[(widx0 + T - c.dl) & (kMaxDelay - 1)];
 }
 
@@ -582,14 +587,14 @@ __device__ __forceinline__ float warp_max(float v)
 }
 
 __global__ void __launch_bounds__(256)
-chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp, uint32_t F, int32_t *__restrict__ spdif_out)
+chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * n_packets;
     const uint32_t Np = d.N_pad;
     for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
         const uint32_t inst = (uint32_t)(u / n_packets), p = p0 + (uint32_t)(u % n_packets);
-        const uint32_t f0 = p * fpp;
+        const uint32_t f0 = d.off[p], count = d.off[p + 1] - f0;
         const bool last = p == p0 + n_packets - 1;
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
@@ -597,21 +602,21 @@ chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp, 
         for (int k = 0; k <= 4; k++) {                                        // four S/PDIF pairs, then the sub alone
             const bool is_sub = k == 4;
             const uint32_t oa = 2 * k, ob = is_sub ? oa : oa + 1;
-            const OutCfg ca = out_cfg(d, oa, inst, any_delay, fpp), cb = out_cfg(d, ob, inst, any_delay, fpp);
+            const OutCfg ca = out_cfg(d, oa, inst, any_delay), cb = out_cfg(d, ob, inst, any_delay);
             float pka = 0.0f, pkb = 0.0f;
             constexpr int kB = 4;                                            // independent loads in flight per lane
-            for (uint32_t tb = lane; tb < fpp; tb += 32 * kB) {
+            for (uint32_t tb = lane; tb < count; tb += 32 * kB) {
                 float xa[kB], xb[kB];
 #pragma unroll
                 for (int j = 0; j < kB; j++) {
                     const uint32_t t = tb + 32 * j;
-                    xa[j] = t < fpp ? out_sample(ca, f0 + t, widx0) : 0.0f;
-                    xb[j] = (!is_sub && t < fpp) ? out_sample(cb, f0 + t, widx0) : 0.0f;
+                    xa[j] = t < count ? out_sample(ca, f0 + t, p, widx0) : 0.0f;
+                    xb[j] = (!is_sub && t < count) ? out_sample(cb, f0 + t, p, widx0) : 0.0f;
                 }
 #pragma unroll
                 for (int j = 0; j < kB; j++) {
                     const uint32_t t = tb + 32 * j, T = f0 + t;
-                    if (t >= fpp) break;
+                    if (t >= count) break;
                     const float aa = fabsf(xa[j]), ab = fabsf(xb[j]);
                     if (aa > pka) pka = aa;
                     if (ab > pkb) pkb = ab;
@@ -647,7 +652,7 @@ chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t fpp, 
 // once per call, after every outpost launch of the call: the delay rings take the last <= 4096 post-gain
 // samples (older writes of this call would have been overwritten anyway), the shared write index advances
 __global__ void __launch_bounds__(256)
-chain_ring_kernel(ChainDev d, uint32_t F, uint32_t fpp)
+chain_ring_kernel(ChainDev d, uint32_t F, uint32_t n_packets)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * kOuts;
@@ -656,11 +661,11 @@ chain_ring_kernel(ChainDev d, uint32_t F, uint32_t fpp)
         const uint32_t inst = (uint32_t)(u / kOuts), o = (uint32_t)(u % kOuts);
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
-        const OutCfg c = out_cfg(d, o, inst, any_delay, fpp);
+        const OutCfg c = out_cfg(d, o, inst, any_delay);
         if (c.delay_on) {                                                    // outputs without delay never touch their ring
             float *ring = d.dline + ((size_t)o * Np + inst) * kMaxDelay;
             for (uint32_t T = (F > (uint32_t)kMaxDelay ? F - kMaxDelay : 0u) + lane; T < F; T += 32)
-                ring[(widx0 + T) & (kMaxDelay - 1)] = out_gain(c.row[T], c.enabled, gain_at(c, T));
+                ring[(widx0 + T) & (kMaxDelay - 1)] = out_gain(c.row[T], c.enabled, gain_at(c, T, n_packets - 1));
         }
         if (o == 0 && lane == 0) d.widx_out[inst] = any_delay ? (widx0 + F) & (kMaxDelay - 1) : widx0;   // :911, once per packet
     }
@@ -741,6 +746,7 @@ struct dspi_chain {
     dspi_status *d_status;
     uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
     uint32_t vmm_packets;            // capacity of d.vmm in packets
+    dspi::PacketSchedule sched;      // packet lengths of the current call
 };
 
 namespace {
@@ -779,13 +785,16 @@ cudaError_t init_states(dspi_chain *c)
     return cudaStreamSynchronize(c->stream);
 }
 
+// one call over the schedule c->sched has checked: its offsets go to the device first, on the engine stream
 template <bool FUSED>
-int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *d_spdif, uint32_t *d_pdm,
+int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, int32_t *d_spdif, uint32_t *d_pdm,
                  dspi_status *d_status)
 {
-    const uint32_t F = n_packets * fpp;
+    dspi::PacketSchedule &ps = c->sched;
+    const uint32_t n_packets = ps.n_packets, F = ps.frames;
+    CU_OK(ps.upload(packet_frames, c->stream, &c->launches));
     auto post = dspi::chain_post_kernel<FUSED>;
-    const size_t post_smem = (size_t)4 * 2 * fpp * dspi::kXs * 4;           // 4 warps x (packet + look-ahead columns)
+    const size_t post_smem = (size_t)4 * 2 * ps.longest * dspi::kXs * 4;    // 4 warps x (longest packet + look-ahead columns)
     static dspi::PerDeviceOnce once;                                // per instantiation (flavour)
     int dev = 0;
     if (once.needs(&dev)) {
@@ -805,7 +814,7 @@ int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t 
             CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(float)));
             c->vmm_packets = n_packets;
         }
-        dspi::chain_env_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets, fpp);
+        dspi::chain_env_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets);
         CU_OK(cudaGetLastError());
         c->launches++;
     }
@@ -816,13 +825,13 @@ int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t 
     CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
     for (uint32_t sl = 0; sl < n_slices; sl++) {
         const uint32_t p0 = slice_bounds[sl], p1 = slice_bounds[sl + 1];
-        const uint32_t fb = p0 * fpp, fe = p1 * fpp;
+        const uint32_t fb = ps.off[p0], fe = ps.off[p1];
         int rc;
         // ---- front: unpack + loudness -> master EQ (K1) -> leveller + crossfeed
         dspi::chain_pre_kernel<FUSED><<<(d.N_pad / 16 + 1) / 2, 64, 0, st.s_front>>>(d, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
         CU_OK(cudaGetLastError());
         if ((rc = dspi::eq_process_on(c->eq_m, d.mrow + fb, fe - fb, d.ldF, st.s_front)) != DSPI_OK) return rc;
-        post<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, fpp);
+        post<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, ps.longest);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_front[sl], st.s_front));
         // ---- outputs: matrix -> per-output EQ (K1) -> gain / delay / metering / conversion
@@ -830,7 +839,7 @@ int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t 
         dspi::chain_mix_kernel<FUSED><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
         CU_OK(cudaGetLastError());
         if ((rc = dspi::eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
-        dspi::chain_outpost_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, fpp, F, d_spdif);
+        dspi::chain_outpost_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, d_spdif);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
         // ---- modulator
@@ -839,7 +848,7 @@ int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t 
         CU_OK(cudaGetLastError());
         c->launches += 5;
     }
-    dspi::chain_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, fpp);     // after the last outpost launch (stream order)
+    dspi::chain_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets);   // after the last outpost launch (stream order)
     CU_OK(cudaGetLastError());
     c->launches++;
     std::swap(c->d.widx_in, c->d.widx_out);
@@ -876,6 +885,7 @@ int dspi_chain_destroy(dspi_chain *c)
     cudaSetDevice(c->desc.device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     c->st.destroy();
+    c->sched.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -907,6 +917,7 @@ int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc)
     if (!c) return fail(DSPI_ENOMEM, "host allocation failed");
     c->stream = nullptr;
     c->st = dspi::ChainStreams();
+    c->sched = dspi::PacketSchedule();
     c->eq_m = c->eq_o = nullptr;
     c->d_aos = nullptr; c->launches = 0; c->d_pcm = nullptr; c->pcm_bytes = 0; c->d_spdif = nullptr; c->spdif_bytes = 0;
     c->d_pdmout = nullptr; c->pdmout_bytes = 0; c->d_status = nullptr;
@@ -933,6 +944,8 @@ int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc)
     cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = c->st.create(desc->device, desc->n_instances);
 #define TRY(x) if (e == cudaSuccess) e = (x)
+    TRY(c->sched.create(d.max_frames));
+    d.off = c->sched.d_off;
     TRY(dev_alloc(c, &c->d_aos, Np * dspi::kRoles * DSPI_MAX_BANDS));
     TRY(dev_alloc(c, &d.preamp, 2 * Np));
     TRY(dev_alloc(c, &d.flags, Np));
@@ -1229,14 +1242,56 @@ static int check_process(dspi_chain *c, const void *pcm, uint32_t bit_depth, uin
     return DSPI_OK;
 }
 
+static int check_packets(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames)
+{
+    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
+    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
+    const char *why = "";
+    const int rc = c->sched.check(n_packets, packet_frames, &why);
+    if (rc == DSPI_ERANGE) return fail(rc, "%s %u", why, c->desc.max_frames);
+    return rc ? fail(rc, "%s", why) : DSPI_OK;
+}
+
+int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                      int32_t *d_spdif, uint32_t *d_pdm, dspi_status *d_status)
+{
+    int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    if (c->desc.arith == DSPI_ARITH_F32_FUSED) return launch_chain<true>(c, d_pcm, bit_depth, packet_frames, d_spdif, d_pdm, d_status);
+    return launch_chain<false>(c, d_pcm, bit_depth, packet_frames, d_spdif, d_pdm, d_status);
+}
+
+int dspi_chain_process_packets_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                    int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status)
+{
+    int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    const size_t N = c->desc.n_instances, F = c->sched.frames;
+    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 4 * F * 2 * 4, pd_bytes = N * F * 8 * 4;
+    if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
+    if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
+    if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream)); }
+    CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    rc = dspi_chain_process_packets_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr,
+                                           pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
+    if (rc) return rc;
+    if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
+    if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
+    if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(dspi_status), cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+// the uniform schedule: n_packets packets of fpp frames
 int dspi_chain_process_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *d_spdif,
                               uint32_t *d_pdm, dspi_status *d_status)
 {
     int rc = check_process(c, d_pcm, bit_depth, n_packets, fpp);
     if (rc) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    if (c->desc.arith == DSPI_ARITH_F32_FUSED) return launch_chain<true>(c, d_pcm, bit_depth, n_packets, fpp, d_spdif, d_pdm, d_status);
-    return launch_chain<false>(c, d_pcm, bit_depth, n_packets, fpp, d_spdif, d_pdm, d_status);
+    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
+    return dspi_chain_process_packets_device(c, d_pcm, bit_depth, n_packets, table.data(), d_spdif, d_pdm, d_status);
 }
 
 int dspi_chain_process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif_out,
@@ -1244,21 +1299,8 @@ int dspi_chain_process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, 
 {
     int rc = check_process(c, pcm, bit_depth, n_packets, fpp);
     if (rc) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t N = c->desc.n_instances, F = (size_t)n_packets * fpp;
-    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 4 * F * 2 * 4, pd_bytes = N * F * 8 * 4;
-    if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
-    if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
-    if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream)); }
-    CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = dspi_chain_process_device(c, c->d_pcm, bit_depth, n_packets, fpp, spdif_out ? c->d_spdif : nullptr, pdm_out ? c->d_pdmout : nullptr,
-                                   status ? c->d_status : nullptr);
-    if (rc) return rc;
-    if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(dspi_status), cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
+    return dspi_chain_process_packets_host(c, pcm, bit_depth, n_packets, table.data(), spdif_out, pdm_out, status);
 }
 
 

@@ -19,6 +19,7 @@
 
 #include "eq_kernels.cuh"
 #include "chain_pdm.cuh"
+#include "chain_schedule.cuh"
 #include "chain_streams.cuh"
 #include "dynamics.cuh"
 
@@ -58,6 +59,7 @@ struct ChainQ {
     float *o_glin;                                 // [5][N_pad] outputs[o].gain_linear
     int32_t *pmg;                                  // [N_pad] the constant preset_mute_gain of dspi_chainq_set_params, as Q15 (:976-978)
     int32_t *vmm;                                  // [packets of the call][N_pad] vol_mul_master (:980) of envelope-mode instances
+    const uint32_t *off;                           // [packets of the call + 1] first frame of each packet (chain_schedule.cuh)
 };
 
 // fast_mul_q28(), dsp_pipeline.c:47-58: 32-bit wrapping, lo*lo partial product dropped
@@ -192,18 +194,18 @@ chainq_pre_kernel(ChainQ d, const uint8_t *__restrict__ pcm, uint32_t bit_depth,
 // post: Q28 leveller (leveller.c:275-389), input peaks, crossfeed (crossfeed.c:161-180), per packet
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
-chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
+chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t longest)
 {
-    extern __shared__ int32_t smem_q[];                    // per warp: packet columns [fpp][33] + look-ahead reads [fpp][33]
+    extern __shared__ int32_t smem_q[];                    // per warp: packet columns [longest][33] + look-ahead reads [longest][33]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t side = lane >> 4;
     const uint32_t inst16 = (blockIdx.x * (blockDim.x >> 5) + warp) * 16;
     if (inst16 >= d.N_pad) return;
     const uint32_t inst = inst16 + (lane & 15);
     const size_t Np = d.N_pad;
-    int32_t *xw = smem_q + (size_t)warp * 2 * fpp * kXs;
+    int32_t *xw = smem_q + (size_t)warp * 2 * longest * kXs;
     int32_t *xs = xw + lane;
-    int32_t *hs = xw + (size_t)fpp * kXs + lane;
+    int32_t *hs = xw + (size_t)longest * kXs + lane;
 
     const uint8_t flags = d.flags[inst];
     const bool lev_on = flags & F_LEV, xf_on = flags & F_XFEED, lookahead = flags & F_LOOKAHEAD;
@@ -221,17 +223,17 @@ chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
     int32_t peak_last = 0;
     uint16_t clip = 0;
     for (uint32_t p = p0; p < p0 + n_packets; p++) {
-        const uint32_t f0 = p * fpp;
+        const uint32_t f0 = d.off[p], count = d.off[p + 1] - f0;          // the leveller's block is this packet
         if (lev_on && lookahead) {                                            // see chain_post_kernel (chain_f32.cu)
             uint32_t idx = la_idx;
-            for (uint32_t i = 0; i < fpp; i++) {
+            for (uint32_t i = 0; i < count; i++) {
                 cp_async_4(hs + i * kXs, la_buf + (size_t)idx * Np);
                 if (++idx >= (uint32_t)kLa) idx = 0;
             }
         }
         for (int r = 0; r < 32; r++) {
             const int32_t *row = d.mrow + ((size_t)(r >> 4) * Np + inst16 + (r & 15)) * d.ldF + f0;
-            for (uint32_t t = lane; t < fpp; t += 32) cp_async_4(xw + t * kXs + r, row + t);
+            for (uint32_t t = lane; t < count; t += 32) cp_async_4(xw + t * kXs + r, row + t);
         }
         cp_async_commit();
         cp_async_wait_all();
@@ -259,7 +261,7 @@ chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
             const int32_t a_rms = __float2int_rz(__fmul_rn(lvc[0], 268435456.0f));                       // :286
             const int32_t one_minus = kUnity - a_rms;
             int32_t e = env;
-            for (uint32_t i = 0; i < fpp; i++) {                                                         // :292-299
+            for (uint32_t i = 0; i < count; i++) {                                                         // :292-299
                 const int32_t s = xs[i * kXs];
                 const int32_t sq = mul_q28(s, s);
                 e = mul_q28(a_rms, e) + mul_q28(one_minus, sq);
@@ -277,24 +279,24 @@ chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
                 if (gc_db > lvc[8]) gc_db = lvc[8];
             }
             const float alpha_s = (gc_db < smooth_db) ? lvc[1] : lvc[2];
-            const float alpha = (float)pow((double)alpha_s, (double)(float)fpp);                          // :327
+            const float alpha = (float)pow((double)alpha_s, (double)(float)count);                          // :327
             const float new_smooth = __fadd_rn(__fmul_rn(alpha, smooth_db), __fmul_rn(__fadd_rn(1.0f, -alpha), gc_db));   // :328-329
             const float gl = (float)pow(10.0, (double)__fdiv_rn(new_smooth, 20.0f));                      // :332
             const int32_t g_cur = __float2int_rz(__fmul_rn(gl, 268435456.0f));                            // :334 (saturating)
             const int32_t g_prev = gain_q;
-            // :352 is gain = prev + (int32)((int64)(cur - prev) * i / (fpp - 1)) per sample (C division: towards zero).  With
-            // diff = Q * D + R (D = fpp - 1, R with the sign of diff, |R| < D) the quotient is Q * i + trunc(R * i / D), both terms
+            // :352 is gain = prev + (int32)((int64)(cur - prev) * i / (count - 1)) per sample (C division: towards zero).  With
+            // diff = Q * D + R (D = count - 1, R with the sign of diff, |R| < D) the quotient is Q * i + trunc(R * i / D), both terms
             // of one sign, so it is carried incrementally: off += Q, acc += R, one correction when |acc| reaches D.  All in
             // 32-bit wrapping arithmetic, which is the int32 cast of :352; no 64-bit division in the per-sample loop.
             const int32_t g_diff = (int32_t)((uint32_t)g_cur - (uint32_t)g_prev);
-            const int32_t den = fpp > 1 ? (int32_t)(fpp - 1) : 1;
+            const int32_t den = count > 1 ? (int32_t)(count - 1) : 1;
             const int32_t ramp_q = g_diff / den, ramp_r = g_diff - ramp_q * den;
             uint32_t off = 0;
             int32_t acc = 0;
             // The leveller's per-sample part and PASS 3 share one loop: the ramp, the look-ahead exchange and the peak limit of
             // sample i+1 do not depend on the crossfeed recurrence of sample i, so the two serial chains overlap.
-            for (uint32_t i = 0; i < fpp; i++) {                                                          // :347-386, :1065-1073
-                int32_t gain = fpp == 1 ? g_cur : (int32_t)((uint32_t)g_prev + off);                      // :352
+            for (uint32_t i = 0; i < count; i++) {                                                          // :347-386, :1065-1073
+                int32_t gain = count == 1 ? g_cur : (int32_t)((uint32_t)g_prev + off);                      // :352
                 off += (uint32_t)ramp_q;
                 acc += ramp_r;
                 if (acc >= den) { acc -= den; off++; }
@@ -329,12 +331,12 @@ chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp)
                 gain_q = g_cur;
             }
         } else {
-            for (uint32_t i = 0; i < fpp; i++) peak_and_crossfeed(i, xs[i * kXs]);
+            for (uint32_t i = 0; i < count; i++) peak_and_crossfeed(i, xs[i * kXs]);
         }
         peak_last = pk;
         if (pk > kClipThresh) clip |= (uint16_t)(1u << side);
         __syncwarp();
-        for (uint32_t t = lane; t < fpp; t += 32) {
+        for (uint32_t t = lane; t < count; t += 32) {
 #pragma unroll 8
             for (int r = 0; r < 32; r++)
                 d.mrow[((size_t)(r >> 4) * Np + inst16 + (r & 15)) * d.ldF + f0 + t] = xw[t * kXs + r];
@@ -401,7 +403,7 @@ chainq_mix_kernel(ChainQ d, uint32_t f_begin, uint32_t f_end)
 // ---------------------------------------------------------------------------------------------
 // update_preset_mute_envelope() (usb_audio.c:466-498) for every packet of the call, one instance per thread, then the Q15
 // volume chain of :976-980: pmg = (int32)(g * 32768 + 0.5) clamped, vmm[p] = mul_q15(mul_q15(vol_base, pmg), master_q15)
-__global__ void chainq_env_kernel(ChainQ d, uint32_t n_packets, uint32_t fpp)
+__global__ void chainq_env_kernel(ChainQ d, uint32_t n_packets)
 {
     const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
     const size_t Np = d.N_pad;
@@ -412,13 +414,14 @@ __global__ void chainq_env_kernel(ChainQ d, uint32_t n_packets, uint32_t fpp)
     unsigned long long ts = ((unsigned long long)fs * 8ull + 999ull) / 1000ull;
     if (ts < 1ull) ts = 1ull;
     if (ts > 0xFFFFFFFFull) ts = 0xFFFFFFFFull;
-    float step = __fdiv_rn((float)fpp, (float)(uint32_t)ts);
-    if (step > 1.0f) step = 1.0f;
     const int32_t vol_base = d.vol_base[inst], master = d.vol_master[inst];
     for (uint32_t p = 0; p < n_packets; p++) {
+        const uint32_t count = d.off[p + 1] - d.off[p];                                  // sample_count of this packet
+        float step = __fdiv_rn((float)count, (float)(uint32_t)ts);
+        if (step > 1.0f) step = 1.0f;
         const bool active = loading != 0;
         if (active) {
-            if (counter > fpp) counter -= fpp;
+            if (counter > count) counter -= count;
             else { counter = 0; loading = 0; }
         }
         const float target = active ? 0.0f : 1.0f;
@@ -494,13 +497,14 @@ struct OutCfgQ {
     int32_t gain;                      // constant gain of the call (no envelope)
     float glin;                        // outputs[o].gain_linear
     const int32_t *vmm;                // envelope mode: vol_mul_master per packet, stride N_pad; else nullptr
-    uint32_t fpp; size_t Np;
+    const uint32_t *off;               // packet offsets of the call
+    size_t Np;
     uint32_t dl;                       // delay & (MAX - 1): MAX aliases to 0 (SURVEY a-10)
     const int32_t *row;
     const int32_t *ring;
 };
 
-__device__ __forceinline__ OutCfgQ outq_cfg(const ChainQ &d, uint32_t o, uint32_t inst, bool any_delay, uint32_t fpp)
+__device__ __forceinline__ OutCfgQ outq_cfg(const ChainQ &d, uint32_t o, uint32_t inst, bool any_delay)
 {
     OutCfgQ c;
     const size_t Np = d.N_pad;
@@ -512,7 +516,7 @@ __device__ __forceinline__ OutCfgQ outq_cfg(const ChainQ &d, uint32_t o, uint32_
     c.gain = d.o_gain[o * Np + inst];
     c.glin = d.o_glin[o * Np + inst];
     c.vmm = d.env[4 * Np + inst] ? d.vmm + inst : nullptr;
-    c.fpp = fpp;
+    c.off = d.off;
     c.Np = Np;
     c.delay_on = any_delay && dly > 0;
     c.dl = (uint32_t)dly & (kMaxDelay - 1);
@@ -521,26 +525,27 @@ __device__ __forceinline__ OutCfgQ outq_cfg(const ChainQ &d, uint32_t o, uint32_
     return c;
 }
 
-// output gain in force at frame T of the call (usb_audio.c:1204-1205): constant, or following the envelope packet by packet
-__device__ __forceinline__ int32_t gainq_at(const OutCfgQ &c, uint32_t T)
+// output gain in force at frame T of the call (usb_audio.c:1204-1205): constant, or following the envelope packet by packet;
+// p is the packet of T or a later one
+__device__ __forceinline__ int32_t gainq_at(const OutCfgQ &c, uint32_t T, uint32_t p)
 {
     if (!c.vmm) return c.gain;
-    return c.mute ? 0 : __float2int_rz(__fmul_rn(c.glin, (float)c.vmm[(size_t)(T / c.fpp) * c.Np]));
+    return c.mute ? 0 : __float2int_rz(__fmul_rn(c.glin, (float)c.vmm[(size_t)packet_of(c.off, T, p) * c.Np]));
 }
 
-// frame T of the call emits the post-gain sample of frame T - dl: inside the call from the output rows,
+// frame T (in packet p) of the call emits the post-gain sample of frame T - dl: inside the call from the output rows,
 // before it from the ring (see chain_f32.cu)
-__device__ __forceinline__ int32_t outq_sample(const OutCfgQ &c, uint32_t T, uint32_t widx0)
+__device__ __forceinline__ int32_t outq_sample(const OutCfgQ &c, uint32_t T, uint32_t p, uint32_t widx0)
 {
-    if (!c.delay_on) return outq_gain(c.row[T], c.enabled, gainq_at(c, T));
-    if (T >= c.dl) return outq_gain(c.row[T - c.dl], c.enabled, gainq_at(c, T - c.dl));
+    if (!c.delay_on) return outq_gain(c.row[T], c.enabled, gainq_at(c, T, p));
+    if (T >= c.dl) return outq_gain(c.row[T - c.dl], c.enabled, gainq_at(c, T - c.dl, p));
     return c.ring[(widx0 + T - c.dl) & (kMaxDelay - 1)];
 }
 
 __device__ __forceinline__ int32_t clip_s24(int32_t w) { return w > 0x7FFFFF ? 0x7FFFFF : (w < -0x800000 ? -0x800000 : w); }   // config.h:547-551
 
 __global__ void __launch_bounds__(256)
-chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp, uint32_t F, int32_t *__restrict__ spdif_out)
+chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * n_packets;
@@ -548,7 +553,7 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp, u
     constexpr int kPairs = (kOuts - 1) / 2;
     for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
         const uint32_t inst = (uint32_t)(u / n_packets), p = p0 + (uint32_t)(u % n_packets);
-        const uint32_t f0 = p * fpp;
+        const uint32_t f0 = d.off[p], count = d.off[p + 1] - f0;
         const bool last = p == p0 + n_packets - 1;
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
@@ -556,21 +561,21 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp, u
         for (int k = 0; k <= kPairs; k++) {                                   // the S/PDIF pairs, then the sub alone
             const bool is_sub = k == kPairs;
             const uint32_t oa = 2 * k, ob = is_sub ? oa : oa + 1;
-            const OutCfgQ ca = outq_cfg(d, oa, inst, any_delay, fpp), cb = outq_cfg(d, ob, inst, any_delay, fpp);
+            const OutCfgQ ca = outq_cfg(d, oa, inst, any_delay), cb = outq_cfg(d, ob, inst, any_delay);
             int32_t pka = 0, pkb = 0;
             constexpr int kB = 4;
-            for (uint32_t tb = lane; tb < fpp; tb += 32 * kB) {
+            for (uint32_t tb = lane; tb < count; tb += 32 * kB) {
                 int32_t xa[kB], xb[kB];
 #pragma unroll
                 for (int j = 0; j < kB; j++) {
                     const uint32_t t = tb + 32 * j;
-                    xa[j] = t < fpp ? outq_sample(ca, f0 + t, widx0) : 0;
-                    xb[j] = (!is_sub && t < fpp) ? outq_sample(cb, f0 + t, widx0) : 0;
+                    xa[j] = t < count ? outq_sample(ca, f0 + t, p, widx0) : 0;
+                    xb[j] = (!is_sub && t < count) ? outq_sample(cb, f0 + t, p, widx0) : 0;
                 }
 #pragma unroll
                 for (int j = 0; j < kB; j++) {
                     const uint32_t t = tb + 32 * j, T = f0 + t;
-                    if (t >= fpp) break;
+                    if (t >= count) break;
                     const int32_t aa = abs(xa[j]), ab = abs(xb[j]);
                     if (aa > pka) pka = aa;
                     if (ab > pkb) pkb = ab;
@@ -602,7 +607,7 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t fpp, u
 }
 
 __global__ void __launch_bounds__(256)
-chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t fpp)
+chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t n_packets)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * kOuts;
@@ -611,11 +616,11 @@ chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t fpp)
         const uint32_t inst = (uint32_t)(u / kOuts), o = (uint32_t)(u % kOuts);
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
-        const OutCfgQ c = outq_cfg(d, o, inst, any_delay, fpp);
+        const OutCfgQ c = outq_cfg(d, o, inst, any_delay);
         if (c.delay_on) {
             int32_t *ring = d.dline + ((size_t)o * Np + inst) * kMaxDelay;
             for (uint32_t T = (F > (uint32_t)kMaxDelay ? F - kMaxDelay : 0u) + lane; T < F; T += 32)
-                ring[(widx0 + T) & (kMaxDelay - 1)] = outq_gain(c.row[T], c.enabled, gainq_at(c, T));
+                ring[(widx0 + T) & (kMaxDelay - 1)] = outq_gain(c.row[T], c.enabled, gainq_at(c, T, n_packets - 1));
         }
         if (o == 0 && lane == 0) d.widx_out[inst] = any_delay ? (widx0 + F) & (kMaxDelay - 1) : widx0;
     }
@@ -709,6 +714,7 @@ struct dspi_chainq {
     dspi_status_q28 *d_status;
     uint32_t env_instances;          // instances in envelope mode
     uint32_t vmm_packets;            // capacity of d.vmm in packets
+    dspi::PacketSchedule sched;      // packet lengths of the current call
 };
 
 namespace {
@@ -756,6 +762,7 @@ int dspi_chainq_destroy(dspi_chainq *c)
     cudaSetDevice(c->desc.device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     c->st.destroy();
+    c->sched.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -787,6 +794,7 @@ int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
     if (!c) return fail(DSPI_ENOMEM, "host allocation failed");
     c->stream = nullptr;
     c->st = dspi::ChainStreams();
+    c->sched = dspi::PacketSchedule();
     c->eq_m = c->eq_o = nullptr;
     c->d_aos = nullptr; c->launches = 0; c->d_pcm = nullptr; c->pcm_bytes = 0; c->d_spdif = nullptr; c->spdif_bytes = 0;
     c->d_pdmout = nullptr; c->pdmout_bytes = 0; c->d_status = nullptr;
@@ -813,6 +821,8 @@ int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
     cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = c->st.create(desc->device, desc->n_instances);
 #define TRY(x) if (e == cudaSuccess) e = (x)
+    TRY(c->sched.create(d.max_frames));
+    d.off = c->sched.d_off;
     TRY(dev_alloc(c, &c->d_aos, Np * dspi::kRoles * DSPI_MAX_BANDS));
     TRY(dev_alloc(c, &d.preamp, 2 * Np));
     TRY(dev_alloc(c, &d.flags, Np));
@@ -1111,17 +1121,37 @@ int dspi_chainq_download_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, dsp
     return DSPI_OK;
 }
 
-int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *d_spdif,
-                               uint32_t *d_pdm, dspi_status_q28 *d_status)
+static int check_process(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp)
 {
-    if (!c || !d_pcm) return fail(DSPI_EINVAL, "null argument");
+    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
     if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
     if (fpp == 0 || fpp > DSPI_PACKET_MAX) return fail(DSPI_EINVAL, "frames_per_packet must be 1..%d", DSPI_PACKET_MAX);
     if (n_packets == 0) return fail(DSPI_EINVAL, "n_packets must be > 0");
     if ((uint64_t)n_packets * fpp > c->desc.max_frames) return fail(DSPI_ERANGE, "%u frames exceed max_frames %u", n_packets * fpp, c->desc.max_frames);
+    return DSPI_OK;
+}
+
+static int check_packets(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames)
+{
+    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
+    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
+    const char *why = "";
+    const int rc = c->sched.check(n_packets, packet_frames, &why);
+    if (rc == DSPI_ERANGE) return fail(rc, "%s %u", why, c->desc.max_frames);
+    return rc ? fail(rc, "%s", why) : DSPI_OK;
+}
+
+int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                       int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
+{
+    int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    const uint32_t F = n_packets * fpp;
-    const size_t post_smem = (size_t)4 * 2 * fpp * dspi::kXs * 4;           // 4 warps x (packet + look-ahead columns)
+    // the schedule's offsets go to the device first, on the engine stream
+    dspi::PacketSchedule &ps = c->sched;
+    const uint32_t F = ps.frames;
+    CU_OK(ps.upload(packet_frames, c->stream, &c->launches));
+    const size_t post_smem = (size_t)4 * 2 * ps.longest * dspi::kXs * 4;    // 4 warps x (longest packet + look-ahead columns)
     static dspi::PerDeviceOnce once;
     int dev = 0;
     if (once.needs(&dev)) {
@@ -1140,7 +1170,7 @@ int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_d
             CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(int32_t)));
             c->vmm_packets = n_packets;
         }
-        dspi::chainq_env_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets, fpp);
+        dspi::chainq_env_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets);
         CU_OK(cudaGetLastError());
         c->launches++;
     }
@@ -1151,19 +1181,19 @@ int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_d
     CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
     for (uint32_t sl = 0; sl < n_slices; sl++) {
         const uint32_t p0 = slice_bounds[sl], p1 = slice_bounds[sl + 1];
-        const uint32_t fb = p0 * fpp, fe = p1 * fpp;
+        const uint32_t fb = ps.off[p0], fe = ps.off[p1];
         int rc;
         dspi::chainq_pre_kernel<<<(d.N_pad / 16 + 1) / 2, 64, 0, st.s_front>>>(d, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
         CU_OK(cudaGetLastError());
         if ((rc = dspi::eq_process_on(c->eq_m, d.mrow + fb, fe - fb, d.ldF, st.s_front)) != DSPI_OK) return rc;
-        dspi::chainq_post_kernel<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, fpp);
+        dspi::chainq_post_kernel<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, ps.longest);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_front[sl], st.s_front));
         CU_OK(cudaStreamWaitEvent(st.s_out, st.ev_front[sl], 0));
         dspi::chainq_mix_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
         CU_OK(cudaGetLastError());
         if ((rc = dspi::eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
-        dspi::chainq_outpost_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, fpp, F, d_spdif);
+        dspi::chainq_outpost_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, d_spdif);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
         CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_out[sl], 0));
@@ -1171,7 +1201,7 @@ int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_d
         CU_OK(cudaGetLastError());
         c->launches += 5;
     }
-    dspi::chainq_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, fpp);            // after the last outpost launch (stream order)
+    dspi::chainq_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets);      // after the last outpost launch (stream order)
     CU_OK(cudaGetLastError());
     c->launches++;
     std::swap(c->d.widx_in, c->d.widx_out);
@@ -1187,26 +1217,45 @@ int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_d
     return DSPI_OK;
 }
 
-int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif_out,
-                             uint32_t *pdm_out, dspi_status_q28 *status)
+int dspi_chainq_process_packets_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                     int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
 {
-    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
-    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
+    int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    const size_t N = c->desc.n_instances, F = (size_t)n_packets * fpp;
+    const size_t N = c->desc.n_instances, F = c->sched.frames;
     const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 2 * F * 2 * 4, pd_bytes = N * F * 8 * 4;
     if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
     if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
     if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream)); }
     CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    int rc = dspi_chainq_process_device(c, c->d_pcm, bit_depth, n_packets, fpp, spdif_out ? c->d_spdif : nullptr, pdm_out ? c->d_pdmout : nullptr,
-                                        status ? c->d_status : nullptr);
+    rc = dspi_chainq_process_packets_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr,
+                                            pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
     if (rc) return rc;
     if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(dspi_status_q28), cudaMemcpyDeviceToHost, c->stream));
     CU_OK(cudaStreamSynchronize(c->stream));
     return DSPI_OK;
+}
+
+// the uniform schedule: n_packets packets of fpp frames
+int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *d_spdif,
+                               uint32_t *d_pdm, dspi_status_q28 *d_status)
+{
+    int rc = check_process(c, d_pcm, bit_depth, n_packets, fpp);
+    if (rc) return rc;
+    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
+    return dspi_chainq_process_packets_device(c, d_pcm, bit_depth, n_packets, table.data(), d_spdif, d_pdm, d_status);
+}
+
+int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif_out,
+                             uint32_t *pdm_out, dspi_status_q28 *status)
+{
+    int rc = check_process(c, pcm, bit_depth, n_packets, fpp);
+    if (rc) return rc;
+    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
+    return dspi_chainq_process_packets_host(c, pcm, bit_depth, n_packets, table.data(), spdif_out, pdm_out, status);
 }
 
 

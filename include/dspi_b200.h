@@ -298,7 +298,7 @@ typedef struct {
     uint32_t n_instances;
     uint32_t n_bands;        /* channel_band_counts[] value (10)                                    */
     int32_t  device;
-    uint32_t max_frames;     /* largest n_packets * frames_per_packet of one process call           */
+    uint32_t max_frames;     /* most frames of one process call (sum of its packet lengths)         */
 } dspi_chain_desc;
 
 int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc);
@@ -363,6 +363,22 @@ int dspi_chain_process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, 
 /* same with DEVICE pointers; asynchronous on the engine stream */
 int dspi_chain_process_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t frames_per_packet,
                               int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status *d_status);
+/* n_packets USB packets whose lengths are packet_frames[0 .. n_packets) (each 1..DSPI_PACKET_MAX; HOST memory, read
+ * during the call, reusable by the caller as soon as the call returns).  The schedule is shared by every instance of the
+ * call.  F = sum of packet_frames <= max_frames; pcm, spdif_out, pdm_out and status are laid out as for
+ * dspi_chain_process_host with n_frames = F.  usb_audio.c:500 with data_len = packet_frames[p] * bytes per frame: the
+ * leveller's block gain, the preset-mute envelope step and the last-packet peaks follow each packet's own length, so a
+ * 44.1 kHz stream (nine 44-frame packets, then one of 45) or a feedback-paced one (n-1, n or n+1 frames) runs bit-exact
+ * in one call.  dspi_chain_process_* with frames_per_packet is this call with n_packets equal lengths.
+ * Per-instance schedules (different lengths for different instances of one call) are not supported: every row of the
+ * call's EQ stages would need its own length.
+ * Errors: DSPI_EINVAL for a NULL table, n_packets == 0, a length of 0 or above DSPI_PACKET_MAX, or a bit depth other than
+ * 16 or 24; DSPI_ERANGE when the lengths add up to more than max_frames.  The _device form stays asynchronous on the
+ * engine stream and never waits for the device (the packet offsets travel as kernel parameters). */
+int dspi_chain_process_packets_host  (dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                      int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status);
+int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                      int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status *d_status);
 int dspi_chain_sync(dspi_chain *c);
 void *dspi_chain_stream(dspi_chain *c);
 uint64_t dspi_chain_launch_count(dspi_chain *c);
@@ -434,6 +450,11 @@ int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth
                              int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status);
 int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t frames_per_packet,
                                int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
+/* a packet_frames[n_packets] schedule, as dspi_chain_process_packets_* (usb_audio.c:968 with data_len per packet) */
+int dspi_chainq_process_packets_host  (dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                       int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status);
+int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                       int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
 int dspi_chainq_sync(dspi_chainq *c);
 void *dspi_chainq_stream(dspi_chainq *c);
 uint64_t dspi_chainq_launch_count(dspi_chainq *c);

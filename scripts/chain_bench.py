@@ -1,12 +1,18 @@
 #!/usr/bin/env python
 """BASELINE config 3 alone: N instances through the whole chain, device-resident, CUDA events.
-    python scripts/chain_bench.py [--instances 8192] [--packets 16] [--fpp 96] [--reps 3]"""
+    python scripts/chain_bench.py [--instances 8192] [--packets 16] [--fpp 96] [--reps 3] [--schedule uniform|44k1|feedback]
+
+--schedule picks the packet lengths of a call: `uniform` is --packets packets of --fpp frames at 96 kHz through
+dspi_chain(q)_process_device; `44k1` is the 44.1 kHz cadence (nine 44-frame packets, then one of 45) at fs = 44100, and
+`feedback` seeded lengths in {95, 96, 97} at 96 kHz (an asynchronous device's feedback pacing), both through
+dspi_chain(q)_process_packets_device.  The real-time factor uses the schedule's own sample rate."""
 import argparse
 import json
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np                                        # noqa: E402
 import torch                                              # noqa: E402
 from dspi_b200 import api, workloads as W                  # noqa: E402
 
@@ -17,8 +23,16 @@ ap.add_argument("--fpp", type=int, default=96)
 ap.add_argument("--reps", type=int, default=3)
 ap.add_argument("--arith", default="f32f")
 ap.add_argument("--no-sub", action="store_true", help="disable the sub output: no modulator work (isolates the other stages)")
+ap.add_argument("--schedule", choices=["uniform", "44k1", "feedback"], default="uniform")
 a = ap.parse_args()
-N, F, fs = a.instances, a.packets * a.fpp, 96000.0
+if a.schedule == "uniform":
+    frames, fs = None, 96000.0
+elif a.schedule == "44k1":
+    frames, fs = np.resize(np.array([44] * 9 + [45], np.uint16), a.packets), 44100.0
+else:
+    frames, fs = np.random.default_rng(1).integers(95, 98, a.packets).astype(np.uint16), 96000.0
+N = a.instances
+F = a.packets * a.fpp if frames is None else int(frames.sum())
 q28 = a.arith == "q28"
 if q28:
     P, bq = W.chain_config3_q28(N, fs=fs)
@@ -35,13 +49,22 @@ pcm = torch.randint(0, 256, (N, F * 6), dtype=torch.uint8, device="cuda")
 spdif = torch.empty((N, 2 if q28 else 4, F, 2), dtype=torch.int32, device="cuda")
 pdm = torch.empty((N, F, 8), dtype=torch.int32, device="cuda")
 torch.cuda.synchronize()
-eng.process_device(pcm.data_ptr(), 24, a.packets, a.fpp, spdif.data_ptr(), pdm.data_ptr())
+
+
+def step():
+    if frames is None:
+        eng.process_device(pcm.data_ptr(), 24, a.packets, a.fpp, spdif.data_ptr(), pdm.data_ptr())
+    else:
+        eng.process_packets_device(pcm.data_ptr(), 24, frames, spdif.data_ptr(), pdm.data_ptr())
+
+
+step()
 eng.sync()
 if q28:                                                   # no stream accessor on the Q28 chain: host clock around synchronised calls
     import time
     t0 = time.perf_counter()
     for _ in range(a.reps):
-        eng.process_device(pcm.data_ptr(), 24, a.packets, a.fpp, spdif.data_ptr(), pdm.data_ptr())
+        step()
     eng.sync()
     ms = (time.perf_counter() - t0) * 1e3 / a.reps
 else:
@@ -49,9 +72,10 @@ else:
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(st)
     for _ in range(a.reps):
-        eng.process_device(pcm.data_ptr(), 24, a.packets, a.fpp, spdif.data_ptr(), pdm.data_ptr())
+        step()
     e1.record(st)
     eng.sync()
     ms = e0.elapsed_time(e1) / a.reps
-print(json.dumps({"instances": N, "frames": F, "sm_partition": eng.sm_partition(), "ms_per_step": ms, "instance_frames_per_s": N * F / (ms * 1e-3),
+print(json.dumps({"schedule": a.schedule, "packets": a.packets, "fs": fs, "instances": N, "frames": F, "sm_partition": eng.sm_partition(),
+                  "ms_per_step": ms, "instance_frames_per_s": N * F / (ms * 1e-3),
                   "arith": a.arith, "output_channel_samples_per_s": N * n_out * F / (ms * 1e-3), "realtime_factor": (F / fs) / (ms * 1e-3)}))
