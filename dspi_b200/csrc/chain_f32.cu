@@ -30,6 +30,7 @@
 // tuned against the roofline.  All per-instance parameters and states are SoA arrays with the instance
 // index innermost.
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1305,7 +1306,7 @@ int dspi_chain_process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, 
 
 
 // ---- checkpoint / resume: everything a later process call depends on besides the parameters ----------------
-static void state_sections(dspi_chain *c, std::vector<std::pair<void *, size_t>> &v)
+static void state_sections(dspi_chain *c, std::vector<std::pair<void *, size_t>> &v, bool with_eq = true)
 {
     const size_t Np = c->d.N_pad;
     v.push_back({ c->d.loud_st, 8 * Np * 4 });
@@ -1319,21 +1320,32 @@ static void state_sections(dspi_chain *c, std::vector<std::pair<void *, size_t>>
     v.push_back({ c->d.peaks, (size_t)dspi::kRoles * Np * 2 });
     v.push_back({ c->d.clip, Np * 2 });
     v.push_back({ c->d.env, 5 * Np * 4 });                                 // preset-mute envelope state and mode
+    if (!with_eq) return;
     dspi::eq_state_sections(c->eq_m, v);
     dspi::eq_state_sections(c->eq_o, v);
 }
 
-struct StateHeader { uint32_t magic, version, arith, n_instances, n_bands, n_sections; uint64_t bytes; };
+// Version 2 records the K1 geometry (channels per lane, DSPI_F32_CPL) that the two EQ engines' packed stores were laid out
+// for, so that a blob resumes in an engine created under either geometry.  Version 1 blobs have no such fields and are read
+// as one channel per lane.
+struct StateHeader { uint32_t magic, version, arith, n_instances, n_bands, n_sections; uint64_t bytes; uint32_t cpl_m, cpl_o; };
 static const uint32_t kStateMagic = 0x53505344u;          // "DSPS"
+static const size_t kHeaderV1 = offsetof(StateHeader, cpl_m);
+
+// blob size for this engine's shape with header `hdr` bytes and EQ stores laid out for cpl_m / cpl_o channels per lane
+static size_t state_bytes(dspi_chain *c, size_t hdr, int cpl_m, int cpl_o)
+{
+    std::vector<std::pair<void *, size_t>> v;
+    state_sections(c, v, false);
+    size_t n = hdr + dspi::eq_state_bytes(c->eq_m, cpl_m) + dspi::eq_state_bytes(c->eq_o, cpl_o);
+    for (auto &s : v) n += s.second;
+    return n;
+}
 
 size_t dspi_chain_state_size(dspi_chain *c)
 {
     if (!c) return 0;
-    std::vector<std::pair<void *, size_t>> v;
-    state_sections(c, v);
-    size_t n = sizeof(StateHeader);
-    for (auto &s : v) n += s.second;
-    return n;
+    return state_bytes(c, sizeof(StateHeader), dspi::eq_geometry(c->eq_m), dspi::eq_geometry(c->eq_o));
 }
 
 int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap)
@@ -1344,7 +1356,8 @@ int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap)
     CU_OK(cudaSetDevice(c->desc.device));
     std::vector<std::pair<void *, size_t>> v;
     state_sections(c, v);
-    StateHeader h = { kStateMagic, 1u, c->desc.arith, c->desc.n_instances, c->desc.n_bands, (uint32_t)v.size(), (uint64_t)need };
+    StateHeader h = { kStateMagic, 2u, c->desc.arith, c->desc.n_instances, c->desc.n_bands, (uint32_t)v.size(), (uint64_t)need,
+                      (uint32_t)dspi::eq_geometry(c->eq_m), (uint32_t)dspi::eq_geometry(c->eq_o) };
     memcpy(blob, &h, sizeof(h));
     char *p = (char *)blob + sizeof(h);
     for (auto &s : v) {
@@ -1358,24 +1371,36 @@ int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap)
 int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len)
 {
     if (!c || !blob) return fail(DSPI_EINVAL, "null argument");
-    std::vector<std::pair<void *, size_t>> v;
-    state_sections(c, v);
+    std::vector<std::pair<void *, size_t>> v, all;
+    state_sections(c, v, false);
+    state_sections(c, all);
     StateHeader h;
-    if (len < sizeof(h)) return fail(DSPI_EINVAL, "state blob too short");
-    memcpy(&h, blob, sizeof(h));
-    if (h.magic != kStateMagic || h.version != 1u) return fail(DSPI_EINVAL, "not a dspi_b200 state blob (magic %08x version %u)", h.magic, h.version);
-    if (h.arith != c->desc.arith || h.n_instances != c->desc.n_instances || h.n_bands != c->desc.n_bands || h.n_sections != v.size() ||
-        h.bytes != dspi_chain_state_size(c) || len < h.bytes)
+    if (len < kHeaderV1) return fail(DSPI_EINVAL, "state blob too short");
+    memcpy(&h, blob, kHeaderV1);
+    h.cpl_m = h.cpl_o = 1;
+    if (h.magic != kStateMagic || (h.version != 1u && h.version != 2u))
+        return fail(DSPI_EINVAL, "not a dspi_b200 state blob (magic %08x version %u)", h.magic, h.version);
+    const size_t hdr = h.version == 1u ? kHeaderV1 : sizeof(h);
+    if (len < hdr) return fail(DSPI_EINVAL, "state blob too short");
+    memcpy(&h, blob, hdr);
+    if ((h.cpl_m != 1 && h.cpl_m != 2) || (h.cpl_o != 1 && h.cpl_o != 2))
+        return fail(DSPI_EINVAL, "state blob names an unknown K1 geometry (%u, %u channels per lane)", h.cpl_m, h.cpl_o);
+    if (h.arith != c->desc.arith || h.n_instances != c->desc.n_instances || h.n_bands != c->desc.n_bands || h.n_sections != all.size() ||
+        h.bytes != state_bytes(c, hdr, (int)h.cpl_m, (int)h.cpl_o) || len < h.bytes)
         return fail(DSPI_EINVAL, "state blob belongs to a different engine shape (%u instances, arith %u, %llu bytes)", h.n_instances, h.arith,
                     (unsigned long long)h.bytes);
     CU_OK(cudaSetDevice(c->desc.device));
-    const char *p = (const char *)blob + sizeof(h);
+    const char *p = (const char *)blob + hdr;
     for (auto &s : v) {
         CU_OK(cudaMemcpyAsync(s.first, p, s.second, cudaMemcpyHostToDevice, c->stream));
         p += s.second;
     }
     CU_OK(cudaStreamSynchronize(c->stream));
-    int rc = dspi::eq_state_imported(c->eq_m, c->stream);
+    int rc = dspi::eq_state_load(c->eq_m, p, (int)h.cpl_m, c->stream);
+    p += dspi::eq_state_bytes(c->eq_m, (int)h.cpl_m);
+    if (rc == DSPI_OK) rc = dspi::eq_state_load(c->eq_o, p, (int)h.cpl_o, c->stream);
+    if (rc) return rc;
+    rc = dspi::eq_state_imported(c->eq_m, c->stream);
     if (rc == DSPI_OK) rc = dspi::eq_state_imported(c->eq_o, c->stream);
     if (rc) return rc;
     std::vector<uint32_t> on(c->d.N);

@@ -544,6 +544,57 @@ int eq_state_imported(dspi_eq *e, cudaStream_t s)
     return remask(e, s);
 }
 
+int eq_geometry(const dspi_eq *e) { return e->cpl; }
+
+// channels of the packed store (and of the mirror) when laid out for `cpl` channels per lane
+static size_t padded_channels(const dspi_eq *e, int cpl)
+{
+    const size_t rows = 32u * (size_t)cpl;
+    return (e->desc.n_channels + rows - 1) / rows * rows;
+}
+
+size_t eq_state_bytes(const dspi_eq *e, int cpl)
+{
+    const size_t c_pad = padded_channels(e, cpl);
+    if (e->desc.arith == DSPI_ARITH_Q28) return c_pad / 32 * DSPI_MAX_BANDS * 20 * 32 * 4 + c_pad * DSPI_MAX_BANDS * e->aos_elem;
+    return c_pad * DSPI_MAX_BANDS * 8 * 4 + c_pad * 8 + c_pad * DSPI_MAX_BANDS * e->aos_elem;
+}
+
+int eq_state_load(dspi_eq *e, const void *src, int cpl, cudaStream_t s)
+{
+    CU_OK(cudaSetDevice(e->desc.device));
+    if (cpl == e->cpl) {
+        std::vector<std::pair<void *, size_t>> v;
+        eq_state_sections(e, v);
+        const char *p = (const char *)src;
+        for (auto &sec : v) {
+            CU_OK(cudaMemcpyAsync(sec.first, p, sec.second, cudaMemcpyHostToDevice, s));
+            p += sec.second;
+        }
+        CU_OK(cudaStreamSynchronize(s));
+        return DSPI_OK;
+    }
+    if (e->desc.arith == DSPI_ARITH_Q28 || (cpl != 1 && cpl != 2)) return fail(DSPI_EINVAL, "state saved for %d channels per lane", cpl);
+    // Another geometry: the mirror's bytes do not depend on it.  Take the saved mirror, bring its state fields up to
+    // date from the saved packed store (in the layout it was saved in), then rebuild this engine's packed store and
+    // topology words from it, exactly as an upload would.
+    const uint32_t n = e->desc.n_channels;
+    const size_t c_pad = padded_channels(e, cpl);
+    const size_t coef_bytes = c_pad * DSPI_MAX_BANDS * 8 * 4;
+    const char *mirror = (const char *)src + coef_bytes + c_pad * 8;
+    CU_OK(cudaMemcpyAsync(e->d_aos, mirror, (size_t)n * DSPI_MAX_BANDS * e->aos_elem, cudaMemcpyHostToDevice, s));
+    float *saved = nullptr;
+    CU_OK(cudaMalloc((void **)&saved, coef_bytes));
+    cudaError_t err = cudaMemcpyAsync(saved, src, coef_bytes, cudaMemcpyHostToDevice, s);
+    if (err == cudaSuccess) err = launch_unpack_f32((dspi_biquad_f32 *)e->d_aos, 0, n, saved, cpl, s);
+    if (err == cudaSuccess) err = launch_pack_f32((const dspi_biquad_f32 *)e->d_aos, 0, n, (float *)e->d_coef, e->d_modes, e->cpl, s);
+    if (err == cudaSuccess) err = cudaStreamSynchronize(s);
+    cudaFree(saved);
+    if (err != cudaSuccess) return fail(DSPI_ECUDA, "state conversion from %d to %d channels per lane: %s", cpl, e->cpl, cudaGetErrorString(err));
+    e->launches += 2;
+    return DSPI_OK;
+}
+
 int eq_process_on(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, cudaStream_t s)
 {
     if (T == 0) return DSPI_OK;

@@ -310,16 +310,36 @@ struct EqBank {
         all_tdf2 = __all_sync(0xffffffffu, mine);
     }
 
-    __device__ __forceinline__ void store(V *base, bool shared_state = false) const
+    // `halves`: how many of this lane's CPL channels belong to the launch (0..CPL; channel lane + 32 h
+    // for h < halves).  The others are rows past the end of a range call, i.e. channels outside it:
+    // their state words are left as they are.
+    __device__ __forceinline__ void store(V *base, int halves, bool shared_state = false) const
     {
+        if (halves >= CPL) {
 #pragma unroll
-        for (int b = 0; b < NB; b++) {
-            if (shared_state) {
-                st_cg(base + (b * 8 + 6) * 32, st[b][0]);
-                st_cg(base + (b * 8 + 7) * 32, st[b][1]);
-            } else {
-                base[(b * 8 + 6) * 32] = st[b][0];
-                base[(b * 8 + 7) * 32] = st[b][1];
+            for (int b = 0; b < NB; b++) {
+                if (shared_state) {
+                    st_cg(base + (b * 8 + 6) * 32, st[b][0]);
+                    st_cg(base + (b * 8 + 7) * 32, st[b][1]);
+                } else {
+                    base[(b * 8 + 6) * 32] = st[b][0];
+                    base[(b * 8 + 7) * 32] = st[b][1];
+                }
+            }
+        } else if constexpr (CPL == 2) {
+            if (halves == 1) {                                  // channel lane only: the low float of each pair
+#pragma unroll
+                for (int b = 0; b < NB; b++) {
+                    float *s0 = reinterpret_cast<float *>(base + (b * 8 + 6) * 32);
+                    float *s1 = reinterpret_cast<float *>(base + (b * 8 + 7) * 32);
+                    if (shared_state) {
+                        st_cg(s0, Lanes<V>::get(st[b][0], 0));
+                        st_cg(s1, Lanes<V>::get(st[b][1], 0));
+                    } else {
+                        *s0 = Lanes<V>::get(st[b][0], 0);
+                        *s1 = Lanes<V>::get(st[b][1], 0);
+                    }
+                }
             }
         }
     }

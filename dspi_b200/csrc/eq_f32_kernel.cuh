@@ -252,7 +252,10 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
         }
 
 
-        bank.store(my_coef, DYN);                                // filter state back to the coefficient store
+        int halves = 0;                                         // rows >= n_rows are channels outside a range call
+#pragma unroll
+        for (int h = 0; h < CPL; h++) halves += (uint32_t)(c0 + 32 * h + lane) < n_rows ? 1 : 0;
+        bank.store(my_coef, halves, DYN);                       // filter state back to the coefficient store
         if constexpr (!DYN) break;
         __threadfence();                                        // state visible before the slice counter moves
         __syncwarp();

@@ -73,6 +73,13 @@ int eq_process_remote_enqueue(dspi_eq *e, void *remote, uint32_t T, uint32_t ch0
 int eq_process_remote_wait(dspi_eq *e);
 void eq_state_sections(dspi_eq *e, std::vector<std::pair<void *, size_t>> &out);   // coefficient + state store (and topology words)
 int eq_state_imported(dspi_eq *e, cudaStream_t s);
+// checkpoints across K1 geometries: the packed store is laid out by channels per lane (1 or 2, DSPI_F32_CPL at create time;
+// always 1 for Q28).  eq_state_bytes: size of eq_state_sections() for this engine's shape laid out for `cpl`.  eq_state_load:
+// writes sections saved from an engine of the same shape laid out for `cpl` (host memory, in section order), converting them
+// to this engine's layout when `cpl` differs; synchronous.
+int eq_geometry(const dspi_eq *e);
+size_t eq_state_bytes(const dspi_eq *e, int cpl);
+int eq_state_load(dspi_eq *e, const void *src, int cpl, cudaStream_t s);
 // coeff.cu: dsp_compute_coefficients() for channels [ch0, ch0 + n) of a mirror, recipes [n][12] on the device (clamped in place)
 cudaError_t launch_coeffs(bool q28, dspi_eq_param *d_recipes, void *d_aos, uint32_t ch0, uint32_t n, float fs, cudaStream_t stream);
 cudaError_t launch_skip_q28(int32_t *coef, const uint8_t *skip, uint32_t n, cudaStream_t stream);

@@ -237,10 +237,12 @@ eq_q28_kernel(const __grid_constant__ CUtensorMap tmap, int32_t *__restrict__ sa
             __syncwarp();
         }
     }
+    if ((uint32_t)(c0 + lane) < n_rows) {                       // rows past the end of a range call are channels outside it
 #pragma unroll
-    for (int b = 0; b < NB; b++) {
-        cg[(b * kSlots + 15) * 32 + lane] = (int32_t)s1[b];
-        cg[(b * kSlots + 16) * 32 + lane] = (int32_t)s2[b];
+        for (int b = 0; b < NB; b++) {
+            cg[(b * kSlots + 15) * 32 + lane] = (int32_t)s1[b];
+            cg[(b * kSlots + 16) * 32 + lane] = (int32_t)s2[b];
+        }
     }
     if (use_tma && lane == 0) tma_store_wait_all<0>();
 }

@@ -147,7 +147,8 @@ int dspi_eq_set_params_device(dspi_eq *e, uint32_t ch0, uint32_t n, dspi_eq_para
  * filters[ch], samples[ch], T, ch) — packet size does not change the values. */
 int dspi_eq_process_device(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld);
 /* The same for channels [ch0, ch0 + n) only: d_rows points at the row of channel ch0 ([n][ld], device memory); ch0 must be a
- * multiple of 64.  For callers that stream a large block through in pieces (dspi_b200/sharding.py pipelines NCCL transfers
+ * multiple of 64, n may be any count.  Channels outside [ch0, ch0 + n) are left untouched: their samples and their filter
+ * state.  For callers that stream a large block through in pieces (dspi_b200/sharding.py pipelines NCCL transfers
  * against it).  Asynchronous on the engine's stream. */
 int dspi_eq_process_device_range(dspi_eq *e, void *d_rows, uint32_t T, uint32_t ld, uint32_t ch0, uint32_t n);
 /* Host block: staged through the device in 48 MiB channel chunks (DSPI_HOST_CHUNK_MB in the environment overrides). */
@@ -346,7 +347,8 @@ int dspi_chain_get_preset_mute(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_p
 /* Checkpoint / resume (the dspi_state_export/import of SURVEY 8 b): everything a later process call depends on besides
  * dspi_chain_set_params' records - filter coefficients and state, loudness / crossfeed / leveller state, look-ahead and
  * delay rings, write index, modulator state, meters.  The blob is private to this library (header + raw arrays) and only
- * loads into an engine of the same shape. */
+ * loads into an engine of the same shape.  It records the K1 stage geometry (DSPI_F32_CPL) it was written under and
+ * loads into an engine created under either one. */
 size_t dspi_chain_state_size(dspi_chain *c);
 int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap);
 int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len);
