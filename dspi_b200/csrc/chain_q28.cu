@@ -857,19 +857,6 @@ int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
     TRY(dev_alloc(c, &d.vol_master, Np));
     TRY(dev_alloc(c, &d.o_glin, dspi::kOuts * Np));
     TRY(dev_alloc(c, &d.pmg, Np));
-    // every band of every channel starts bypassed (dsp_init_default_filters, dsp_pipeline.c:177-199)
-    if (e == cudaSuccess) {
-        std::vector<dspi_biquad_q28> byp(Np * dspi::kRoles * DSPI_MAX_BANDS);
-        memset(byp.data(), 0, byp.size() * sizeof(dspi_biquad_q28));
-        for (auto &q : byp) q.bypass = 1;
-        e = cudaMemcpyAsync(dspi::eq_aos_mirror(c->eq_m), byp.data(), 2 * Np * DSPI_MAX_BANDS * sizeof(dspi_biquad_q28), cudaMemcpyHostToDevice, c->stream);
-        if (e == cudaSuccess)
-            e = cudaMemcpyAsync(dspi::eq_aos_mirror(c->eq_o), byp.data(), dspi::kOuts * Np * DSPI_MAX_BANDS * sizeof(dspi_biquad_q28), cudaMemcpyHostToDevice, c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(c->d_aos, byp.data(), byp.size() * sizeof(dspi_biquad_q28), cudaMemcpyHostToDevice, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e == cudaSuccess && (dspi::eq_pack_range(c->eq_m, 0, 2 * d.N_pad, c->stream) || dspi::eq_pack_range(c->eq_o, 0, dspi::kOuts * d.N_pad, c->stream)))
-            e = cudaErrorUnknown;
-    }
     TRY(init_states(c));
 #undef TRY
     if (e != cudaSuccess) {

@@ -169,6 +169,28 @@ int dspi_bind_host_to_device(int device)
     return node;
 }
 
+// Writes the record dsp_compute_coefficients() makes of a flat recipe (bypass set, b0 = 1, everything else zero) into every
+// band of channels [0, c_pad) of the mirror: one row from the host, then doubling device-to-device copies.
+static cudaError_t fill_default_records(dspi_eq *e)
+{
+    const bool q28 = e->desc.arith == DSPI_ARITH_Q28;
+    const size_t row = (size_t)DSPI_MAX_BANDS * e->aos_elem;
+    alignas(8) unsigned char rec[DSPI_MAX_BANDS * sizeof(dspi_biquad_f32)];
+    memset(rec, 0, sizeof(rec));
+    for (int b = 0; b < DSPI_MAX_BANDS; b++) {
+        dspi_eq_param p;
+        memset(&p, 0, sizeof(p));
+        p.band = (uint8_t)b; p.type = DSPI_FILTER_FLAT; p.freq = 1000.0f; p.Q = 0.707f;
+        if (q28) dspi_compute_coefficients_q28(&p, (dspi_biquad_q28 *)rec + b, 48000.0f);
+        else dspi_compute_coefficients_f32(&p, (dspi_biquad_f32 *)rec + b, 48000.0f);
+    }
+    char *dst = (char *)e->d_aos;
+    cudaError_t err = cudaMemcpyAsync(dst, rec, row, cudaMemcpyHostToDevice, e->stream);
+    for (size_t k = 1; err == cudaSuccess && k < e->c_pad; k *= 2)
+        err = cudaMemcpyAsync(dst + k * row, dst, std::min<size_t>(k, e->c_pad - k) * row, cudaMemcpyDeviceToDevice, e->stream);
+    return err;
+}
+
 int dspi_eq_create(dspi_eq **out, const dspi_eq_desc *desc)
 {
     if (!out || !desc) return fail(DSPI_EINVAL, "null argument");
@@ -226,6 +248,11 @@ int dspi_eq_create(dspi_eq **out, const dspi_eq_desc *desc)
         if ((err = cudaMemsetAsync(e->d_modes, 0, (size_t)e->c_pad * 8, e->stream)) != cudaSuccess) goto cuda_fail;
     }
     // every band of every (padding) channel starts bypassed, like dsp_init_default_filters() (dsp_pipeline.c:177-199)
+    if ((err = fill_default_records(e)) != cudaSuccess) goto cuda_fail;
+    err = q28 ? dspi::launch_pack_q28((const dspi_biquad_q28 *)e->d_aos, 0, e->c_pad, (int32_t *)e->d_coef, e->stream)
+              : dspi::launch_pack_f32((const dspi_biquad_f32 *)e->d_aos, 0, e->c_pad, (float *)e->d_coef, e->d_modes, e->cpl, e->stream);
+    if (err != cudaSuccess) goto cuda_fail;
+    e->launches++;
     if ((err = cudaStreamSynchronize(e->stream)) != cudaSuccess) goto cuda_fail;
     *out = e;
     return DSPI_OK;

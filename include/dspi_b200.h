@@ -112,6 +112,10 @@ typedef struct {
     uint32_t flags;          /* 0                                                     */
 } dspi_eq_desc;
 
+/* A new engine holds, in every band of every channel, the record dsp_compute_coefficients() makes of a flat recipe
+ * (dsp_init_default_filters(), dsp_pipeline.c:177-199): bypass set, b0 = 1, all other coefficients and the state zero.
+ * It passes audio through until coefficients are uploaded, and dspi_eq_set_param on it gives a one-band EQ.  Chain
+ * engines start the same way: instances whose biquads were never uploaded run with every filter row bypassed. */
 int dspi_eq_create(dspi_eq **out, const dspi_eq_desc *desc);
 int dspi_eq_destroy(dspi_eq *e);
 
@@ -316,8 +320,11 @@ int dspi_chain_download_biquads(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_
 /* dsp_recalculate_all_filters() for n instances on the GPU: recipes[n][11][DSPI_MAX_BANDS] = filter_recipes[][] of each
  * instance (host memory, clamped in place); see dspi_eq_set_params_device for the arithmetic and the libm policy */
 int dspi_chain_set_eq_params_device(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_eq_param *recipes, float sample_rate);
-/* pipeline reset: clears leveller, loudness, delay-line and PDM state (leveller_reset_state(),
- * pdm_processing_loop() restart path); filter state is part of the biquads */
+/* Pipeline reset of every instance: leveller state (leveller_reset_state(): envelopes and smoothed gain cleared, gains 1,
+ * look-ahead buffer and index cleared), the modulator's state (pdm_processing_loop() restart path: integrators and error
+ * cleared, dither seed 123456789), loudness shelf state, delay lines and their write index, and the meters (peaks and
+ * sticky clip flags).  Kept: the EQ filter state (part of the biquads), the crossfeed state and the preset-mute envelope.
+ * Ordered after earlier asynchronous process calls on the engine stream. */
 int dspi_chain_reset_state(dspi_chain *c);
 /* The preset-mute envelope inside the engine (update_preset_mute_envelope(), usb_audio.c:466-498, called once per packet
  * at :532): states[n] puts instances [inst0, inst0+n) into envelope mode - from then on every packet of every process
@@ -440,7 +447,7 @@ int dspi_chainq_set_params(dspi_chainq *c, uint32_t inst0, uint32_t n, const dsp
 int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_biquad_q28 *biquads);
 int dspi_chainq_download_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_biquad_q28 *biquads);
 int dspi_chainq_set_eq_params_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_eq_param *recipes, float sample_rate);   /* recipes[n][7][12] */
-int dspi_chainq_reset_state(dspi_chainq *c);
+int dspi_chainq_reset_state(dspi_chainq *c);                                  /* as dspi_chain_reset_state */
 int dspi_chainq_set_dynamics_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_dynamics_config *cfgs, float sample_rate);
 int dspi_chainq_set_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz);   /* Q15 use of the gain: usb_audio.c:976-980 */
 int dspi_chainq_get_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states);
