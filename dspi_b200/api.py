@@ -41,6 +41,8 @@ SYMBOLS = [
     "dspi_chain_set_dynamics_device", "dspi_chainq_set_dynamics_device", "dspi_chain_sm_partition", "dspi_chainq_sm_partition",
     "dspi_chain_set_preset_mute", "dspi_chain_get_preset_mute", "dspi_chainq_set_preset_mute", "dspi_chainq_get_preset_mute",
     "dspi_chain_process_packets_host", "dspi_chain_process_packets_device", "dspi_chainq_process_packets_host", "dspi_chainq_process_packets_device",
+    "dspi_chain_set_spdif_tx", "dspi_chain_get_spdif_tx", "dspi_chainq_set_spdif_tx", "dspi_chainq_get_spdif_tx",
+    "dspi_chain_process_subframes_host", "dspi_chain_process_subframes_device", "dspi_chainq_process_subframes_host", "dspi_chainq_process_subframes_device",
 ]
 
 
@@ -139,6 +141,10 @@ def lib():
             getattr(h, pre + "_sm_partition").argtypes = [vp, vp, vp]
             getattr(h, pre + "_process_packets_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_process_packets_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
+            getattr(h, pre + "_set_spdif_tx").argtypes = [vp, u32, u32, vp]
+            getattr(h, pre + "_get_spdif_tx").argtypes = [vp, u32, u32, vp]
+            getattr(h, pre + "_process_subframes_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
+            getattr(h, pre + "_process_subframes_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
         h.dspi_eq_process_device_range.argtypes = [vp, vp, u32, u32, u32, u32]
         h.dspi_bind_host_to_device.argtypes = [C.c_int]
         h.dspi_nccl_unique_id.argtypes = [vp]
@@ -370,9 +376,61 @@ def bind_host_to_device(device):
     return int(lib().dspi_bind_host_to_device(int(device)))
 
 
-class ChainEngine:
+class _ChainSpdif:
+    """What both chain engines share: each instance's S/PDIF transmitter (block position + channel status) and the
+    process form whose output stage writes S/PDIF subframes (``*_spdif_tx``, ``*_process_subframes_*``)."""
+
+    def set_spdif_tx(self, block_pos, channel_status, inst0=0):
+        """Transmitter state of instances [inst0, inst0+n): ``block_pos`` an int or [n] (0..191), ``channel_status`` 5 bytes
+        or uint8 [n, 5]; a single value on either side applies to all n.  Takes effect from the next process call."""
+        bp = np.asarray(block_pos, np.int64).reshape(-1)
+        cs = np.frombuffer(bytes(channel_status), np.uint8) if isinstance(channel_status, (bytes, bytearray)) else np.asarray(channel_status, np.uint8)
+        cs = cs.reshape(-1, 5)
+        n = max(bp.size, cs.shape[0])
+        if bp.size not in (1, n) or cs.shape[0] not in (1, n):
+            raise ValueError("block_pos and channel_status give different instance counts")
+        if bp.size and (bp.min() < 0 or bp.max() > 255):
+            raise DspiError("block_pos must be 0..191")
+        rec = np.zeros(n, L.SPDIF_TX)
+        rec["block_pos"] = bp
+        rec["channel_status"] = cs
+        _check(getattr(lib(), self._PRE + "_set_spdif_tx")(self._h, int(inst0), int(n), rec.ctypes.data_as(C.c_void_p)))
+
+    def get_spdif_tx(self, n=None, inst0=0):
+        """SPDIF_TX [n]: block position of the next frame and channel status, after the last call issued."""
+        n = self.n_instances - inst0 if n is None else n
+        out = np.zeros(n, L.SPDIF_TX)
+        _check(getattr(lib(), self._PRE + "_get_spdif_tx")(self._h, int(inst0), int(n), out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def process_subframes_host(self, pcm, bit_depth, packet_frames, want_subframes=True, want_pdm=True, want_status=True):
+        """As ``process_packets_host``, S/PDIF out as subframes: uint32 [n_instances, pairs, F, 2, 2] ({l, h} per subframe,
+        the array ``spdif_encode_host`` makes of the words, reshaped).  Returns (subframes, pdm, status)."""
+        t, F = _packet_table(packet_frames)
+        pcm = np.ascontiguousarray(pcm)
+        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
+        sub = np.zeros((self.n_instances, self._PAIRS, F, 2, 2), np.uint32) if want_subframes else None
+        pdm = np.zeros((self.n_instances, F, 8), np.uint32) if want_pdm else None
+        status = np.zeros(self.n_instances, self._STATUS) if want_status else None
+        _check(getattr(lib(), self._PRE + "_process_subframes_host")(self._h, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
+                                                                     sub.ctypes.data if want_subframes else None,
+                                                                     pdm.ctypes.data if want_pdm else None,
+                                                                     status.ctypes.data if want_status else None))
+        return sub, pdm, status
+
+    def process_subframes_device(self, pcm_ptr, bit_depth, packet_frames, subframes_ptr=0, pdm_ptr=0, status_ptr=0):
+        """``process_subframes_host`` with device pointers (subframes 16-byte aligned), asynchronous on the engine stream."""
+        t, _ = _packet_table(packet_frames)
+        _check(getattr(lib(), self._PRE + "_process_subframes_device")(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
+                                                                       C.c_void_p(int(subframes_ptr)) if subframes_ptr else None,
+                                                                       C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                                       C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+
+class ChainEngine(_ChainSpdif):
     """Many independent DSPi device instances, whole signal chain (``dspi_chain_*``)."""
     _PRE = "dspi_chain"
+    _PAIRS, _STATUS = 4, L.STATUS
 
     def __init__(self, arith, n_instances, max_frames, n_bands=L.NUM_BANDS, device=0):
         self.arith = ARITH[arith] if isinstance(arith, str) else int(arith)
@@ -654,9 +712,10 @@ def master_volume(db):
     return lin.value, q.value
 
 
-class ChainEngineQ28:
+class ChainEngineQ28(_ChainSpdif):
     """Many independent RP2040-shape instances (2 in -> 5 out), Q28 arithmetic (``dspi_chainq_*``)."""
     _PRE = "dspi_chainq"
+    _PAIRS, _STATUS = 2, L.STATUS_Q28
 
     def __init__(self, n_instances, max_frames, n_bands=L.NUM_BANDS, device=0):
         self.n_instances, self.max_frames, self.device = int(n_instances), int(max_frames), int(device)

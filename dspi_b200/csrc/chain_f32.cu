@@ -19,10 +19,13 @@
 //   chain_mix_kernel      lane = frame: the 2 x 9 matrix, writes output ROWS [9 N][frames]
 //   K1                    per-output EQ over the 9 N rows (muted / disabled rows are masked out)
 //   chain_outpost_kernel  lane = frame, warp = (instance, packet): gain, delay, peak/clip metering,
-//                         float -> 24-bit S/PDIF pairs (coalesced 8-byte stores), Q28 for the modulator.
-//                         A delayed sample that lies inside the current call is read from the output
-//                         rows; only older history comes from the delay ring in HBM.
-//   chain_ring_kernel     once per call: the last <= 4096 post-gain samples go into the rings
+//                         float -> 24-bit S/PDIF pairs (coalesced 8-byte stores) or, in its SUBFRAMES
+//                         instantiation, those pairs encoded straight into biphase-mark subframes at the
+//                         instance's S/PDIF block position and channel status (spdif_bmc.cuh, 16-byte stores),
+//                         Q28 for the modulator.  A delayed sample that lies inside the current call is read
+//                         from the output rows; only older history comes from the delay ring in HBM.
+//   chain_ring_kernel     once per call: the last <= 4096 post-gain samples go into the rings, every
+//                         instance's S/PDIF block position advances by the call's frame count
 //   chain_pdm_kernel      one instance per lane: 256x oversampled 2nd-order delta-sigma (chain_pdm.cuh)
 //
 // Everything with a serial recurrence but little arithmetic keeps lane = instance; everything without
@@ -42,6 +45,7 @@
 #include "chain_schedule.cuh"
 #include "chain_streams.cuh"
 #include "dynamics.cuh"
+#include "spdif_bmc.cuh"
 
 namespace dspi {
 namespace {
@@ -587,8 +591,12 @@ __device__ __forceinline__ float warp_max(float v)
     return v;
 }
 
+// SUBFRAMES = false: spdif_out is [N][4][F][2] int32 words.  SUBFRAMES = true: it is [N][4][F] uint4 subframe pairs
+// {l, h, l, h}, each instance's frames encoded at its own block position and channel status (spdif_bmc.cuh) - what
+// dspi_spdif_encode_* makes of the words, without the words buffer.
+template <bool SUBFRAMES>
 __global__ void __launch_bounds__(256)
-chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out)
+chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out, SpdifTx tx)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * n_packets;
@@ -599,6 +607,8 @@ chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, in
         const bool last = p == p0 + n_packets - 1;
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
+        const uint32_t bp = SUBFRAMES ? tx.bp[inst] : 0u;
+        const uint64_t cs40 = SUBFRAMES ? tx.cs40[inst] : 0ull;
         unsigned int clip = 0;
         for (int k = 0; k <= 4; k++) {                                        // four S/PDIF pairs, then the sub alone
             const bool is_sub = k == 4;
@@ -629,7 +639,12 @@ chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, in
                             w.x = __float2int_rz(__fmul_rn(fmaxf(-1.0f, fminf(1.0f, xa[j])), 8388607.0f));
                             w.y = __float2int_rz(__fmul_rn(fmaxf(-1.0f, fminf(1.0f, xb[j])), 8388607.0f));
                         }
-                        *reinterpret_cast<int2 *>(spdif_out + (((size_t)inst * 4 + k) * F + T) * 2) = w;
+                        if (SUBFRAMES) {                                      // 16 bytes per lane: 512 contiguous bytes per warp store
+                            const uint32_t pos = (bp + T) % 192u;
+                            reinterpret_cast<uint4 *>(spdif_out)[((size_t)inst * 4 + k) * F + T] = encode_frame(w, spdif_pre_left(pos), spdif_cs_bit(pos, cs40));
+                        } else {
+                            *reinterpret_cast<int2 *>(spdif_out + (((size_t)inst * 4 + k) * F + T) * 2) = w;
+                        }
                     }
                 }
             }
@@ -651,9 +666,10 @@ chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, in
 }
 
 // once per call, after every outpost launch of the call: the delay rings take the last <= 4096 post-gain
-// samples (older writes of this call would have been overwritten anyway), the shared write index advances
+// samples (older writes of this call would have been overwritten anyway), the shared write index advances, and so
+// does the S/PDIF block position - by all F frames whatever the call copied out (the transmitter sends every frame)
 __global__ void __launch_bounds__(256)
-chain_ring_kernel(ChainDev d, uint32_t F, uint32_t n_packets)
+chain_ring_kernel(ChainDev d, uint32_t F, uint32_t n_packets, uint32_t *__restrict__ spdif_bp)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * kOuts;
@@ -668,7 +684,10 @@ chain_ring_kernel(ChainDev d, uint32_t F, uint32_t n_packets)
             for (uint32_t T = (F > (uint32_t)kMaxDelay ? F - kMaxDelay : 0u) + lane; T < F; T += 32)
                 ring[(widx0 + T) & (kMaxDelay - 1)] = out_gain(c.row[T], c.enabled, gain_at(c, T, n_packets - 1));
         }
-        if (o == 0 && lane == 0) d.widx_out[inst] = any_delay ? (widx0 + F) & (kMaxDelay - 1) : widx0;   // :911, once per packet
+        if (o == 0 && lane == 0) {
+            d.widx_out[inst] = any_delay ? (widx0 + F) & (kMaxDelay - 1) : widx0;   // :911, once per packet
+            spdif_bp[inst] = (spdif_bp[inst] + F % 192u) % 192u;
+        }
     }
 }
 
@@ -742,9 +761,10 @@ struct dspi_chain {
     std::vector<void *> allocs;
     uint64_t launches;
     void *d_pcm; size_t pcm_bytes;   // host-path staging
-    int32_t *d_spdif; size_t spdif_bytes;
+    int32_t *d_spdif; size_t spdif_bytes;   // host-path staging of the S/PDIF output, words or subframes
     uint32_t *d_pdmout; size_t pdmout_bytes;
     dspi_status *d_status;
+    dspi::SpdifTx tx;                // S/PDIF transmitter state; not part of the state blob (dspi_chain_get/set_spdif_tx)
     uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     dspi::PacketSchedule sched;      // packet lengths of the current call
@@ -786,10 +806,20 @@ cudaError_t init_states(dspi_chain *c)
     return cudaStreamSynchronize(c->stream);
 }
 
+// a new engine's transmitters: block position 0, the channel status init_spdif_buffer() stamps (audio_spdif.c:82-88)
+cudaError_t init_spdif_tx(dspi_chain *c)
+{
+    const std::vector<uint64_t> cs(c->d.N_pad, dspi::kSpdifDefaultCs40);
+    cudaError_t e = cudaMemsetAsync(c->tx.bp, 0, (size_t)c->d.N_pad * 4, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(c->tx.cs40, cs.data(), (size_t)c->d.N_pad * 8, cudaMemcpyHostToDevice, c->stream);
+    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
+}
+
 // one call over the schedule c->sched has checked: its offsets go to the device first, on the engine stream
+// d_spdif: words, or subframes when `subframes` is set (either may be NULL)
 template <bool FUSED>
-int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, int32_t *d_spdif, uint32_t *d_pdm,
-                 dspi_status *d_status)
+int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, void *d_spdif, bool subframes,
+                 uint32_t *d_pdm, dspi_status *d_status)
 {
     dspi::PacketSchedule &ps = c->sched;
     const uint32_t n_packets = ps.n_packets, F = ps.frames;
@@ -840,7 +870,10 @@ int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, const uin
         dspi::chain_mix_kernel<FUSED><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
         CU_OK(cudaGetLastError());
         if ((rc = dspi::eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
-        dspi::chain_outpost_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, d_spdif);
+        if (subframes && d_spdif)
+            dspi::chain_outpost_kernel<true><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
+        else
+            dspi::chain_outpost_kernel<false><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
         // ---- modulator
@@ -849,7 +882,7 @@ int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, const uin
         CU_OK(cudaGetLastError());
         c->launches += 5;
     }
-    dspi::chain_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets);   // after the last outpost launch (stream order)
+    dspi::chain_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets, c->tx.bp);   // after the last outpost launch (stream order)
     CU_OK(cudaGetLastError());
     c->launches++;
     std::swap(c->d.widx_in, c->d.widx_out);
@@ -923,6 +956,7 @@ int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc)
     c->d_aos = nullptr; c->launches = 0; c->d_pcm = nullptr; c->pcm_bytes = 0; c->d_spdif = nullptr; c->spdif_bytes = 0;
     c->d_pdmout = nullptr; c->pdmout_bytes = 0; c->d_status = nullptr;
     c->env_instances = 0; c->vmm_packets = 0;
+    c->tx.bp = nullptr; c->tx.cs40 = nullptr;
     c->desc = *desc;
     ChainDev &d = c->d;
     memset(&d, 0, sizeof(d));
@@ -980,7 +1014,10 @@ int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc)
     TRY(dev_alloc(c, &d.vol_master, Np));
     TRY(dev_alloc(c, &d.o_glin, dspi::kOuts * Np));
     TRY(dev_alloc(c, &d.pmg, Np));
+    TRY(dev_alloc(c, &c->tx.bp, Np));
+    TRY(dev_alloc(c, &c->tx.cs40, Np));
     TRY(init_states(c));
+    TRY(init_spdif_tx(c));
 #undef TRY
     if (e != cudaSuccess) {
         fail(e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA, "chain setup: %s", cudaGetErrorString(e));
@@ -1253,35 +1290,91 @@ static int check_packets(dspi_chain *c, const void *pcm, uint32_t bit_depth, uin
     return rc ? fail(rc, "%s", why) : DSPI_OK;
 }
 
-int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                      int32_t *d_spdif, uint32_t *d_pdm, dspi_status *d_status)
+static int process_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                          void *d_spdif, bool subframes, uint32_t *d_pdm, dspi_status *d_status)
 {
     int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
+    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
     CU_OK(cudaSetDevice(c->desc.device));
-    if (c->desc.arith == DSPI_ARITH_F32_FUSED) return launch_chain<true>(c, d_pcm, bit_depth, packet_frames, d_spdif, d_pdm, d_status);
-    return launch_chain<false>(c, d_pcm, bit_depth, packet_frames, d_spdif, d_pdm, d_status);
+    if (c->desc.arith == DSPI_ARITH_F32_FUSED) return launch_chain<true>(c, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
+    return launch_chain<false>(c, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
 }
 
-int dspi_chain_process_packets_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                    int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status)
+// host memory in and out, staged through the engine's device buffers
+static int process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                        void *spdif_out, bool subframes, uint32_t *pdm_out, dspi_status *status)
 {
     int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     const size_t N = c->desc.n_instances, F = c->sched.frames;
-    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 4 * F * 2 * 4, pd_bytes = N * F * 8 * 4;
+    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 4 * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
     if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
     if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
     if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream)); }
     CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = dspi_chain_process_packets_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr,
-                                           pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
+    rc = process_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
+                        pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
     if (rc) return rc;
     if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(dspi_status), cudaMemcpyDeviceToHost, c->stream));
     CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                      int32_t *d_spdif, uint32_t *d_pdm, dspi_status *d_status)
+{
+    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
+}
+
+int dspi_chain_process_packets_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                    int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status)
+{
+    return process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
+}
+
+int dspi_chain_process_subframes_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                        dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status *d_status)
+{
+    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
+}
+
+int dspi_chain_process_subframes_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                      dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status *status)
+{
+    return process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
+}
+
+int dspi_chain_set_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
+{
+    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    std::vector<uint32_t> bp(n);
+    std::vector<uint64_t> cs(n);
+    if (!dspi::spdif_tx_unpack(tx, n, bp.data(), cs.data())) return fail(DSPI_EINVAL, "block_pos must be 0..191");
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));   // behind earlier calls
+    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+int dspi_chain_get_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
+{
+    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    std::vector<uint32_t> bp(n);
+    std::vector<uint64_t> cs(n);
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaMemcpyAsync(bp.data(), c->tx.bp + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaMemcpyAsync(cs.data(), c->tx.cs40 + inst0, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    dspi::spdif_tx_pack(bp.data(), cs.data(), n, tx);
     return DSPI_OK;
 }
 

@@ -7,7 +7,7 @@
 //
 // Same stage-wise decomposition as chain_f32.cu: pre (unpack, preamp, loudness) -> K2 over the master rows
 // -> post (leveller, peaks, crossfeed) -> mix -> K2 over the output rows -> outpost (gain, delay, metering,
-// 24-bit words) -> ring update -> modulator, on three streams over packet slices.  The EQ rows run through
+// 24-bit words or S/PDIF subframes) -> ring update -> modulator, on three streams over packet slices.  The EQ rows run through
 // the Q28 cascade kernel of the EQ engine (eq_q28.cu: TMA ring, coefficients pre-split in registers);
 // everything is integer-pipe bound (about 27 integer ops per band-sample).
 #include <cstdarg>
@@ -22,6 +22,7 @@
 #include "chain_schedule.cuh"
 #include "chain_streams.cuh"
 #include "dynamics.cuh"
+#include "spdif_bmc.cuh"
 
 namespace dspi {
 namespace {
@@ -544,8 +545,11 @@ __device__ __forceinline__ int32_t outq_sample(const OutCfgQ &c, uint32_t T, uin
 
 __device__ __forceinline__ int32_t clip_s24(int32_t w) { return w > 0x7FFFFF ? 0x7FFFFF : (w < -0x800000 ? -0x800000 : w); }   // config.h:547-551
 
+// SUBFRAMES = false: spdif_out is [N][2][F][2] int32 words; true: [N][2][F] uint4 subframe pairs at each instance's
+// block position and channel status (as chain_f32.cu)
+template <bool SUBFRAMES>
 __global__ void __launch_bounds__(256)
-chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out)
+chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out, SpdifTx tx)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * n_packets;
@@ -557,6 +561,8 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int
         const bool last = p == p0 + n_packets - 1;
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
+        const uint32_t bp = SUBFRAMES ? tx.bp[inst] : 0u;
+        const uint64_t cs40 = SUBFRAMES ? tx.cs40[inst] : 0ull;
         unsigned int clip = 0;
         for (int k = 0; k <= kPairs; k++) {                                   // the S/PDIF pairs, then the sub alone
             const bool is_sub = k == kPairs;
@@ -584,7 +590,12 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int
                     } else if (spdif_out) {
                         int2 w = make_int2(0, 0);
                         if (!ca.pair_off) { w.x = clip_s24((xa[j] + 32) >> 6); w.y = clip_s24((xb[j] + 32) >> 6); }   // :1254-1255
-                        *reinterpret_cast<int2 *>(spdif_out + (((size_t)inst * kPairs + k) * F + T) * 2) = w;
+                        if (SUBFRAMES) {                                      // 16 bytes per lane: 512 contiguous bytes per warp store
+                            const uint32_t pos = (bp + T) % 192u;
+                            reinterpret_cast<uint4 *>(spdif_out)[((size_t)inst * kPairs + k) * F + T] = encode_frame(w, spdif_pre_left(pos), spdif_cs_bit(pos, cs40));
+                        } else {
+                            *reinterpret_cast<int2 *>(spdif_out + (((size_t)inst * kPairs + k) * F + T) * 2) = w;
+                        }
                     }
                 }
             }
@@ -607,7 +618,7 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int
 }
 
 __global__ void __launch_bounds__(256)
-chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t n_packets)
+chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t n_packets, uint32_t *__restrict__ spdif_bp)
 {
     const int lane = threadIdx.x & 31;
     const uint64_t units = (uint64_t)d.N * kOuts;
@@ -622,7 +633,10 @@ chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t n_packets)
             for (uint32_t T = (F > (uint32_t)kMaxDelay ? F - kMaxDelay : 0u) + lane; T < F; T += 32)
                 ring[(widx0 + T) & (kMaxDelay - 1)] = outq_gain(c.row[T], c.enabled, gainq_at(c, T, n_packets - 1));
         }
-        if (o == 0 && lane == 0) d.widx_out[inst] = any_delay ? (widx0 + F) & (kMaxDelay - 1) : widx0;
+        if (o == 0 && lane == 0) {
+            d.widx_out[inst] = any_delay ? (widx0 + F) & (kMaxDelay - 1) : widx0;
+            spdif_bp[inst] = (spdif_bp[inst] + F % 192u) % 192u;          // every frame of the call was sent
+        }
     }
 }
 
@@ -709,9 +723,10 @@ struct dspi_chainq {
     std::vector<void *> allocs;
     uint64_t launches;
     void *d_pcm; size_t pcm_bytes;
-    int32_t *d_spdif; size_t spdif_bytes;
+    int32_t *d_spdif; size_t spdif_bytes;   // host-path staging of the S/PDIF output, words or subframes
     uint32_t *d_pdmout; size_t pdmout_bytes;
     dspi_status_q28 *d_status;
+    dspi::SpdifTx tx;                // S/PDIF transmitter state; not part of the state blob (dspi_chainq_get/set_spdif_tx)
     uint32_t env_instances;          // instances in envelope mode
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     dspi::PacketSchedule sched;      // packet lengths of the current call
@@ -750,6 +765,15 @@ cudaError_t init_states(dspi_chainq *c)
     if ((e = cudaMemsetAsync(c->d.peaks, 0, (size_t)dspi::kRoles * Np * 2, c->stream)) != cudaSuccess) return e;
     if ((e = cudaMemsetAsync(c->d.clip, 0, Np * 2, c->stream)) != cudaSuccess) return e;
     return cudaStreamSynchronize(c->stream);
+}
+
+// a new engine's transmitters: block position 0, the channel status init_spdif_buffer() stamps (audio_spdif.c:82-88)
+cudaError_t init_spdif_tx(dspi_chainq *c)
+{
+    const std::vector<uint64_t> cs(c->d.N_pad, dspi::kSpdifDefaultCs40);
+    cudaError_t e = cudaMemsetAsync(c->tx.bp, 0, (size_t)c->d.N_pad * 4, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(c->tx.cs40, cs.data(), (size_t)c->d.N_pad * 8, cudaMemcpyHostToDevice, c->stream);
+    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
 }
 
 }  // namespace
@@ -799,6 +823,7 @@ int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
     c->d_aos = nullptr; c->launches = 0; c->d_pcm = nullptr; c->pcm_bytes = 0; c->d_spdif = nullptr; c->spdif_bytes = 0;
     c->d_pdmout = nullptr; c->pdmout_bytes = 0; c->d_status = nullptr;
     c->env_instances = 0; c->vmm_packets = 0;
+    c->tx.bp = nullptr; c->tx.cs40 = nullptr;
     c->desc = *desc;
     ChainQ &d = c->d;
     memset(&d, 0, sizeof(d));
@@ -857,7 +882,10 @@ int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
     TRY(dev_alloc(c, &d.vol_master, Np));
     TRY(dev_alloc(c, &d.o_glin, dspi::kOuts * Np));
     TRY(dev_alloc(c, &d.pmg, Np));
+    TRY(dev_alloc(c, &c->tx.bp, Np));
+    TRY(dev_alloc(c, &c->tx.cs40, Np));
     TRY(init_states(c));
+    TRY(init_spdif_tx(c));
 #undef TRY
     if (e != cudaSuccess) {
         fail(e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA, "chainq setup: %s", cudaGetErrorString(e));
@@ -1128,11 +1156,13 @@ static int check_packets(dspi_chainq *c, const void *pcm, uint32_t bit_depth, ui
     return rc ? fail(rc, "%s", why) : DSPI_OK;
 }
 
-int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                       int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
+// d_spdif: words, or subframes when `subframes` is set (either may be NULL)
+static int process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                          void *d_spdif, bool subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
 {
     int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
+    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
     CU_OK(cudaSetDevice(c->desc.device));
     // the schedule's offsets go to the device first, on the engine stream
     dspi::PacketSchedule &ps = c->sched;
@@ -1180,7 +1210,10 @@ int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32
         dspi::chainq_mix_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
         CU_OK(cudaGetLastError());
         if ((rc = dspi::eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
-        dspi::chainq_outpost_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, d_spdif);
+        if (subframes && d_spdif)
+            dspi::chainq_outpost_kernel<true><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
+        else
+            dspi::chainq_outpost_kernel<false><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
         CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_out[sl], 0));
@@ -1188,7 +1221,7 @@ int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32
         CU_OK(cudaGetLastError());
         c->launches += 5;
     }
-    dspi::chainq_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets);      // after the last outpost launch (stream order)
+    dspi::chainq_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets, c->tx.bp);      // after the last outpost launch (stream order)
     CU_OK(cudaGetLastError());
     c->launches++;
     std::swap(c->d.widx_in, c->d.widx_out);
@@ -1204,25 +1237,80 @@ int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32
     return DSPI_OK;
 }
 
-int dspi_chainq_process_packets_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                     int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
+// host memory in and out, staged through the engine's device buffers
+static int process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                        void *spdif_out, bool subframes, uint32_t *pdm_out, dspi_status_q28 *status)
 {
     int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     const size_t N = c->desc.n_instances, F = c->sched.frames;
-    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 2 * F * 2 * 4, pd_bytes = N * F * 8 * 4;
+    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 2 * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
     if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
     if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
     if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream)); }
     CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = dspi_chainq_process_packets_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr,
-                                            pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
+    rc = process_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
+                        pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
     if (rc) return rc;
     if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(dspi_status_q28), cudaMemcpyDeviceToHost, c->stream));
     CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                       int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
+{
+    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
+}
+
+int dspi_chainq_process_packets_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                     int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
+{
+    return process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
+}
+
+int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                         dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
+{
+    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
+}
+
+int dspi_chainq_process_subframes_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                       dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status_q28 *status)
+{
+    return process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
+}
+
+int dspi_chainq_set_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
+{
+    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    std::vector<uint32_t> bp(n);
+    std::vector<uint64_t> cs(n);
+    if (!dspi::spdif_tx_unpack(tx, n, bp.data(), cs.data())) return fail(DSPI_EINVAL, "block_pos must be 0..191");
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));   // behind earlier calls
+    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+int dspi_chainq_get_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
+{
+    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    std::vector<uint32_t> bp(n);
+    std::vector<uint64_t> cs(n);
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaMemcpyAsync(bp.data(), c->tx.bp + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaMemcpyAsync(cs.data(), c->tx.cs40 + inst0, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    dspi::spdif_tx_pack(bp.data(), cs.data(), n, tx);
     return DSPI_OK;
 }
 

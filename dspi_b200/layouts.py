@@ -160,6 +160,10 @@ BULK_STATE = np.dtype({
 PRESET_MUTE = np.dtype([("loading", "u1"), ("reserved", "u1", (3,)), ("counter", "<u4"), ("smooth_gain", "<f4")])
 assert PRESET_MUTE.itemsize == 12
 
+# dspi_spdif_tx (include/dspi_b200.h): S/PDIF transmitter state of one chain instance, audio_spdif.c:82-88, :372-388
+SPDIF_TX = np.dtype([("channel_status", "u1", (5,)), ("block_pos", "u1"), ("reserved", "u1", (2,))])
+assert SPDIF_TX.itemsize == 8
+
 # dspi_dynamics_config (include/dspi_b200.h): crossfeed_config + leveller_config + loudness globals + host volume
 DYNAMICS_CONFIG = np.dtype([
     ("xf_enabled", "u1"), ("xf_itd_enabled", "u1"), ("xf_preset", "u1"), ("_p0", "u1"), ("xf_custom_fc", "<f4"), ("xf_custom_feed_db", "<f4"),

@@ -323,7 +323,8 @@ int dspi_chain_set_eq_params_device(dspi_chain *c, uint32_t inst0, uint32_t n, d
 /* Pipeline reset of every instance: leveller state (leveller_reset_state(): envelopes and smoothed gain cleared, gains 1,
  * look-ahead buffer and index cleared), the modulator's state (pdm_processing_loop() restart path: integrators and error
  * cleared, dither seed 123456789), loudness shelf state, delay lines and their write index, and the meters (peaks and
- * sticky clip flags).  Kept: the EQ filter state (part of the biquads), the crossfeed state and the preset-mute envelope.
+ * sticky clip flags).  Kept: the EQ filter state (part of the biquads), the crossfeed state, the preset-mute envelope and
+ * the S/PDIF transmitter state (block position and channel status, dspi_chain_set_spdif_tx).
  * Ordered after earlier asynchronous process calls on the engine stream. */
 int dspi_chain_reset_state(dspi_chain *c);
 /* The preset-mute envelope inside the engine (update_preset_mute_envelope(), usb_audio.c:466-498, called once per packet
@@ -355,7 +356,9 @@ int dspi_chain_get_preset_mute(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_p
  * dspi_chain_set_params' records - filter coefficients and state, loudness / crossfeed / leveller state, look-ahead and
  * delay rings, write index, modulator state, meters.  The blob is private to this library (header + raw arrays) and only
  * loads into an engine of the same shape.  It records the K1 stage geometry (DSPI_F32_CPL) it was written under and
- * loads into an engine created under either one. */
+ * loads into an engine created under either one.  The S/PDIF transmitter state is not in the blob (its format is
+ * unchanged): a resume that continues the S/PDIF stream needs dspi_chain_state_import followed by
+ * dspi_chain_set_spdif_tx with what dspi_chain_get_spdif_tx returned at the checkpoint. */
 size_t dspi_chain_state_size(dspi_chain *c);
 int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap);
 int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len);
@@ -453,7 +456,7 @@ int dspi_chainq_set_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, cons
 int dspi_chainq_get_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states);
 size_t dspi_chainq_state_size(dspi_chainq *c);
 int dspi_chainq_state_export(dspi_chainq *c, void *blob, size_t cap);
-int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len);
+int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len);   /* + dspi_chainq_set_spdif_tx, as dspi_chain_* */
 /* pcm as for dspi_chain_process_host; spdif_out [n_instances][2][n_frames][2]; pdm_out [n_instances][n_frames][8] */
 int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t frames_per_packet,
                              int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status);
@@ -579,6 +582,44 @@ int dspi_spdif_encode_device(int device, const int32_t *d_words, uint64_t n_stre
                              const uint8_t channel_status[5], dspi_spdif_subframe *d_subframes, void *cuda_stream);
 int dspi_spdif_encode_host(int device, const int32_t *words, uint64_t n_streams, uint32_t frames, uint32_t block_pos0,
                            const uint8_t channel_status[5], dspi_spdif_subframe *subframes);
+
+/* ---- S/PDIF subframes straight from the chain engines ------------------------------------------ */
+/* Every chain instance has one S/PDIF transmitter (audio_spdif.c:82-88, :372-388), shared by all its pairs - four on the
+ * RP2350 shape, two on the RP2040 shape (the firmware starts them together and feeds them the same frames): a block
+ * position block_pos (0..191) and the 5 consumer channel-status bytes.  Frame T of a call (0-based over the call's F
+ * frames) sits at block position (block_pos + T) % 192 on every pair of the instance.  EVERY process call - words form,
+ * subframe form, outputs NULL or not - advances block_pos to (block_pos + F) % 192: the transmitter sends every frame the
+ * chain produces.  A new engine starts each instance at block_pos 0 with the bytes init_spdif_buffer() stamps
+ * { 0x04, 0x00, 0x00, 0x00, 0x0B } (byte 3 is the sample-rate code: set it for the instance's rate).  The engine keeps it
+ * across calls; dspi_chain(q)_reset_state leaves it alone; it is not part of the state blob. */
+typedef struct { uint8_t channel_status[5]; uint8_t block_pos; uint8_t reserved[2]; } dspi_spdif_tx;   /* 8 bytes */
+#ifdef __cplusplus
+static_assert(sizeof(dspi_spdif_tx) == 8, "dspi_spdif_tx");
+#else
+_Static_assert(sizeof(dspi_spdif_tx) == 8, "dspi_spdif_tx");
+#endif
+/* tx[n] for instances [inst0, inst0+n).  _set_ runs on the engine stream behind earlier asynchronous process calls (it
+ * applies from the next call on) and has finished when it returns; _get_ waits for the engine stream, so it returns the
+ * state after the last call issued.  Errors: DSPI_ERANGE for a range past the end (also one whose end wraps in 32 bits),
+ * DSPI_EINVAL for NULL records or a block_pos >= 192 (nothing is written then); n = 0 does nothing. */
+int dspi_chain_set_spdif_tx (dspi_chain *c,  uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx);
+int dspi_chain_get_spdif_tx (dspi_chain *c,  uint32_t inst0, uint32_t n, dspi_spdif_tx *tx);
+int dspi_chainq_set_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx);
+int dspi_chainq_get_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx);
+/* As dspi_chain(q)_process_packets_*, with the S/PDIF output as subframes written by the output stage itself:
+ * subframes [n_instances][4 (Q28: 2)][F][2] dspi_spdif_subframe, i.e. exactly what dspi_spdif_encode_* makes of the
+ * [n_instances * pairs][F][2] words the words form writes, at each instance's own block position and channel status.
+ * Pairs whose two outputs are both disabled carry encoded zero words, as in the two-pass path.  No words buffer and no
+ * second pass.  Arguments are checked as for the _packets_ forms; d_subframes must be 16-byte aligned.  Any output may be
+ * NULL (the block position still advances). */
+int dspi_chain_process_subframes_host   (dspi_chain *c,  const void *pcm,   uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                         dspi_spdif_subframe *subframes,   uint32_t *pdm_out,   dspi_status *status);
+int dspi_chain_process_subframes_device (dspi_chain *c,  const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                         dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status *d_status);
+int dspi_chainq_process_subframes_host  (dspi_chainq *c, const void *pcm,   uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                         dspi_spdif_subframe *subframes,   uint32_t *pdm_out,   dspi_status_q28 *status);
+int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                         dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
 
 /* pinned host memory helpers */
 void *dspi_host_alloc(size_t bytes);
