@@ -43,6 +43,8 @@ SYMBOLS = [
     "dspi_chain_process_packets_host", "dspi_chain_process_packets_device", "dspi_chainq_process_packets_host", "dspi_chainq_process_packets_device",
     "dspi_chain_set_spdif_tx", "dspi_chain_get_spdif_tx", "dspi_chainq_set_spdif_tx", "dspi_chainq_get_spdif_tx",
     "dspi_chain_process_subframes_host", "dspi_chain_process_subframes_device", "dspi_chainq_process_subframes_host", "dspi_chainq_process_subframes_device",
+    "dspi_eq_response_host", "dspi_eq_response_device", "dspi_chain_response_host", "dspi_chain_response_device",
+    "dspi_chainq_response_host", "dspi_chainq_response_device",
 ]
 
 
@@ -145,6 +147,9 @@ def lib():
             getattr(h, pre + "_get_spdif_tx").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_process_subframes_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_process_subframes_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
+        for pre in ("dspi_eq", "dspi_chain", "dspi_chainq"):
+            getattr(h, pre + "_response_host").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
+            getattr(h, pre + "_response_device").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
         h.dspi_eq_process_device_range.argtypes = [vp, vp, u32, u32, u32, u32]
         h.dspi_bind_host_to_device.argtypes = [C.c_int]
         h.dspi_nccl_unique_id.argtypes = [vp]
@@ -280,6 +285,11 @@ class EqEngine:
         _check(lib().dspi_eq_set_params_device(self._h, int(ch0), int(r.shape[0]), r.ctypes.data_as(C.c_void_p), C.c_float(fs)))
         return r
 
+    def response(self, freqs, fs, ch0=0, n=None, out_ptr=0):
+        """Frequency response of channels [ch0, ch0+n) at ``freqs`` (Hz): complex64 [n, n_freqs] (``dspi_eq_response_host``).
+        With ``out_ptr`` (device memory for [n, n_freqs] complex64) it runs ``dspi_eq_response_device`` and returns None."""
+        return _response(self._h, "dspi_eq", (), self.n_channels, freqs, fs, ch0, n, out_ptr)
+
     def kernel_info(self):
         """Which kernel the next process call runs (triggers a pending run-time specialisation)."""
         buf = C.create_string_buffer(320)
@@ -369,6 +379,19 @@ def _packet_table(packet_frames):
         raise DspiError("packet lengths must be 1..192 frames")
     t = np.ascontiguousarray(t, np.uint16)
     return t, int(t.sum(dtype=np.int64))
+
+
+def _response(h, pre, shape, n_total, freqs, fs, first, n, out_ptr):
+    """Shared body of the ``response`` methods: complex64 [n, *shape, n_freqs] from ``*_response_host``, or None after
+    ``*_response_device`` into ``out_ptr`` (device memory, asynchronous on the engine stream)."""
+    f = np.ascontiguousarray(freqs, np.float32).reshape(-1)
+    n = n_total - first if n is None else int(n)
+    if out_ptr:
+        _check(getattr(lib(), pre + "_response_device")(h, int(first), n, f.ctypes.data, f.size, C.c_float(fs), C.c_void_p(int(out_ptr))))
+        return None
+    out = np.zeros((max(n, 0),) + tuple(shape) + (f.size,), np.complex64)
+    _check(getattr(lib(), pre + "_response_host")(h, int(first), n, f.ctypes.data, f.size, C.c_float(fs), out.ctypes.data))
+    return out
 
 
 def bind_host_to_device(device):
@@ -555,6 +578,11 @@ class ChainEngine(_ChainSpdif):
                                                        C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
                                                        C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
                                                        C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def response(self, freqs, fs, inst0=0, n=None, out_ptr=0):
+        """Frequency response of instances [inst0, inst0+n): complex64 [n, 9 outputs, 2 inputs, n_freqs]; with ``out_ptr``
+        (device memory) asynchronous on the engine stream, returning None."""
+        return _response(self._h, "dspi_chain", (L.CHAIN_OUTPUTS, 2), self.n_instances, freqs, fs, inst0, n, out_ptr)
 
     def sync(self):
         _check(lib().dspi_chain_sync(self._h))
@@ -833,6 +861,10 @@ class ChainEngineQ28(_ChainSpdif):
                                                         C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
                                                         C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
                                                         C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def response(self, freqs, fs, inst0=0, n=None, out_ptr=0):
+        """Frequency response of instances [inst0, inst0+n): complex64 [n, 5 outputs, 2 inputs, n_freqs] (see ChainEngine)."""
+        return _response(self._h, "dspi_chainq", (L.CHAINQ_OUTPUTS, 2), self.n_instances, freqs, fs, inst0, n, out_ptr)
 
     def sync(self):
         _check(lib().dspi_chainq_sync(self._h))

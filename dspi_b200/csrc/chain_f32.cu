@@ -45,6 +45,7 @@
 #include "chain_schedule.cuh"
 #include "chain_streams.cuh"
 #include "dynamics.cuh"
+#include "response.cuh"
 #include "spdif_bmc.cuh"
 
 namespace dspi {
@@ -728,6 +729,87 @@ __global__ void chain_status_kernel(ChainDev d, dspi_status *__restrict__ out)
     out[inst] = s;
 }
 
+// ---------------------------------------------------------------------------------------------
+// frequency response (dspi_chain_response_*): the linear, time-invariant part of the path the next call applies, from the
+// SoA parameters and the two EQ engines' mirrors (response.cuh).  CTA = one instance at a time, thread = one frequency:
+// the instance's 11 filter rows and loudness shelves become sections in shared memory once, then every thread composes
+// preamp -> loudness -> master EQ -> look-ahead delay -> crossfeed -> matrix -> output EQ -> gain -> delay for all 9 x 2
+// (output, input) pairs of its frequency.  Nothing here reads or writes the packed stores or any state.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128)
+chain_response_kernel(ChainDev d, const dspi_biquad_f32 *__restrict__ m_aos, const dspi_biquad_f32 *__restrict__ o_aos, uint32_t inst0,
+                      uint32_t n, const float *__restrict__ freqs, uint32_t nf, float fs, float2 *__restrict__ out)
+{
+    __shared__ Sect sec[kRoles][kMaxBands];
+    __shared__ Sect loud[2];
+    __shared__ int cnt[kRoles], n_loud;
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    const float fr = f < nf ? freqs[f] : 0.0f;
+    const Trig t = trig_at(fr, fs);
+    const uint32_t Np = d.N_pad;
+    for (uint32_t u = blockIdx.y; u < n; u += gridDim.y) {
+        const uint32_t inst = inst0 + u;
+        const uint8_t flags = d.flags[inst];
+        __syncthreads();
+        if (threadIdx.x < kRoles) {                                          // filters[role]: master L, R, Out1..9
+            const uint32_t role = threadIdx.x;
+            const dspi_biquad_f32 *row = role < 2 ? m_aos + ((size_t)role * Np + inst) * kMaxBands : o_aos + ((size_t)(role - 2) * Np + inst) * kMaxBands;
+            int k = 0;
+            for (uint32_t b = 0; b < d.nb; b++) {
+                Sect s;
+                if (sect_band(row[b], s)) sec[role][k++] = s;
+            }
+            cnt[role] = k;
+        } else if (threadIdx.x == 32) {                                      // loudness shelves, general SVF mix (usb_audio.c:689-718)
+            int k = 0;
+            for (int j = 0; j < 2 && (flags & F_LOUD); j++) {
+                if ((d.loud_byp[inst] >> j) & 1) continue;
+                const float *c = d.loud_c + (size_t)j * 6 * Np + inst;
+                loud[k++] = sect_svf(c[0], c[Np], c[2 * Np], c[3 * Np], c[4 * Np], c[5 * Np], 0u, true);
+            }
+            n_loud = k;
+        }
+        __syncthreads();
+        if (f >= nf) continue;
+        Cd pre = cascade_eval(loud, n_loud, t);
+        if ((flags & F_LEV) && (flags & F_LOOKAHEAD)) pre = cmul(pre, delay_phase(fr, kLa, fs));   // leveller at 0 dB: its look-ahead delay
+        Cd P[2];
+#pragma unroll
+        for (int s = 0; s < 2; s++) {
+            P[s] = cscale(pre, d.preamp[s * Np + inst]);
+            if (!(flags & F_BYPASS_MASTER)) P[s] = cmul(P[s], cascade_eval(sec[s], cnt[s], t));
+        }
+        // crossfeed.c:132-156: L' = (1 - LP) L + AP LP R, LP = a0 / (1 - b1 w), AP = (a + w) / (1 + a w)
+        Cd direct = { 1.0, 0.0 }, cross = { 0.0, 0.0 };
+        if (flags & F_XFEED) {
+            const double a0 = d.xf[0 * Np + inst], b1 = d.xf[1 * Np + inst], ap = d.xf[4 * Np + inst];
+            const Cd lp = cdiv({ a0, 0.0 }, { 1.0 - b1 * t.c1, -b1 * t.s1 });
+            const Cd apd = { 1.0 + ap * t.c1, ap * t.s1 };                 // 0 only for a = +-1 at DC / Nyquist: AP = a there
+            const Cd apv = (apd.re == 0.0 && apd.im == 0.0) ? Cd{ ap, 0.0 } : cdiv({ ap + t.c1, t.s1 }, apd);
+            direct = { 1.0 - lp.re, -lp.im };
+            cross = cmul(apv, lp);
+        }
+        const bool env = d.env[4 * Np + inst] != 0;                          // envelope mode: the gain reached so far
+        const float vmm_env = __fmul_rn(__fmul_rn(d.vol_base[inst], __uint_as_float(d.env[2 * Np + inst])), d.vol_master[inst]);
+        for (int o = 0; o < kOuts; o++) {
+            const uint8_t of = d.o_flags[o * Np + inst];
+            const float gain = !env ? d.o_gain[o * Np + inst] : ((of & O_MUTE) ? 0.0f : __fmul_rn(d.o_glin[o * Np + inst], vmm_env));
+            Cd h[2] = { { 0.0, 0.0 }, { 0.0, 0.0 } };
+            if ((of & O_ENABLED) && gain != 0.0f) {
+                Cd g = cascade_eval(sec[2 + o], (of & O_MUTE) ? 0 : cnt[2 + o], t);
+                g = cscale(g, gain);
+                const int32_t dly = d.o_dly[o * Np + inst];
+                if ((flags & F_ANY_DELAY) && dly > 0) g = cmul(g, delay_phase(fr, (uint32_t)dly & (kMaxDelay - 1), fs));   // MAX aliases to 0
+                const double gl = d.o_gl[o * Np + inst], gr = d.o_gr[o * Np + inst];
+                h[0] = cmul(g, cmul(cadd(cscale(direct, gl), cscale(cross, gr)), P[0]));
+                h[1] = cmul(g, cmul(cadd(cscale(cross, gl), cscale(direct, gr)), P[1]));
+            }
+            out[(((size_t)u * kOuts + o) * 2 + 0) * nf + f] = to_float2(h[0]);
+            out[(((size_t)u * kOuts + o) * 2 + 1) * nf + f] = to_float2(h[1]);
+        }
+    }
+}
+
 int fail(int code, const char *fmt, ...)
 {
     size_t cap = 0;
@@ -768,6 +850,7 @@ struct dspi_chain {
     uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     dspi::PacketSchedule sched;      // packet lengths of the current call
+    dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chain_response_*
 };
 
 namespace {
@@ -920,6 +1003,7 @@ int dspi_chain_destroy(dspi_chain *c)
     if (c->stream) cudaStreamSynchronize(c->stream);
     c->st.destroy();
     c->sched.destroy();
+    c->resp.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -1502,6 +1586,51 @@ int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len)
     c->env_instances = 0;
     for (uint32_t v : on) c->env_instances += v ? 1u : 0u;
     return DSPI_OK;
+}
+
+// Frequency response of instances [inst0, inst0 + n) on the engine stream; out: device [n][9][2][n_freqs] float2, or host
+// memory filled chunk by chunk through the staging buffer
+static int chain_response(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
+{
+    const char *why = "";
+    int rc = dspi::response_check_args(freqs, n_freqs, fs, out, &why);
+    if (rc) return fail(rc, "%s", why);
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(c->resp.upload(freqs, n_freqs, c->stream, &c->launches));
+    const dspi_biquad_f32 *m_aos = (const dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_m), *o_aos = (const dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_o);
+    auto launch = [&](uint32_t i0, uint32_t m, void *dst) -> cudaError_t {
+        const dim3 grid((n_freqs + 127) / 128, m < 65535u ? m : 65535u);
+        dspi::chain_response_kernel<<<grid, 128, 0, c->stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
+        c->launches++;
+        return cudaGetLastError();
+    };
+    if (!host) {
+        CU_OK(launch(inst0, n, out));
+        return DSPI_OK;
+    }
+    const size_t row_bytes = (size_t)dspi::kOuts * 2 * n_freqs * 2 * sizeof(float);
+    uint32_t rows = 0;
+    CU_OK(c->resp.stage(row_bytes, n, c->stream, &rows));
+    for (uint32_t i = 0; i < n; i += rows) {
+        const uint32_t m = n - i < rows ? n - i : rows;
+        CU_OK(launch(inst0 + i, m, c->resp.d_stage));
+        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->stream));
+        CU_OK(cudaStreamSynchronize(c->stream));
+    }
+    return DSPI_OK;
+}
+
+int dspi_chain_response_host(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
+{
+    return chain_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, out, true);
+}
+
+int dspi_chain_response_device(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out)
+{
+    return chain_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
 }
 
 int dspi_chain_sync(dspi_chain *c)

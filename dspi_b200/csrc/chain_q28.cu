@@ -22,6 +22,7 @@
 #include "chain_schedule.cuh"
 #include "chain_streams.cuh"
 #include "dynamics.cuh"
+#include "response.cuh"
 #include "spdif_bmc.cuh"
 
 namespace dspi {
@@ -674,6 +675,89 @@ __global__ void chainq_status_kernel(ChainQ d, dspi_status_q28 *__restrict__ out
     out[inst] = s;
 }
 
+// ---------------------------------------------------------------------------------------------
+// frequency response (dspi_chainq_response_*), as chain_f32.cu's chain_response_kernel in the RP2040's quantities: ratios of
+// Q28 values (coefficients / 2^28), the matrix and output gains as the Q15 integers the packet loop uses (/ 32768), output EQs
+// skipped while the master EQ is bypassed (quirk 3), MAX_DELAY 2048
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128)
+chainq_response_kernel(ChainQ d, const dspi_biquad_q28 *__restrict__ m_aos, const dspi_biquad_q28 *__restrict__ o_aos, uint32_t inst0,
+                       uint32_t n, const float *__restrict__ freqs, uint32_t nf, float fs, float2 *__restrict__ out)
+{
+    __shared__ Sect sec[kRoles][kMaxBands];
+    __shared__ Sect loud[2];
+    __shared__ int cnt[kRoles], n_loud;
+    const double kQ28 = 1.0 / 268435456.0, kQ15 = 1.0 / 32768.0;
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    const float fr = f < nf ? freqs[f] : 0.0f;
+    const Trig t = trig_at(fr, fs);
+    const size_t Np = d.N_pad;
+    for (uint32_t u = blockIdx.y; u < n; u += gridDim.y) {
+        const uint32_t inst = inst0 + u;
+        const uint8_t flags = d.flags[inst];
+        __syncthreads();
+        if (threadIdx.x < kRoles) {                                          // filters[role]: master L, R, Out1..4, sub
+            const uint32_t role = threadIdx.x;
+            const dspi_biquad_q28 *row = role < 2 ? m_aos + ((size_t)role * Np + inst) * kMaxBands : o_aos + ((size_t)(role - 2) * Np + inst) * kMaxBands;
+            int k = 0;
+            for (uint32_t b = 0; b < d.nb; b++) {
+                Sect s;
+                if (sect_band(row[b], s)) sec[role][k++] = s;
+            }
+            cnt[role] = k;
+        } else if (threadIdx.x == 32) {                                      // loudness shelves, Q28 TDF2 (usb_audio.c:1018-1047)
+            int k = 0;
+            for (int j = 0; j < 2 && (flags & F_LOUD); j++) {
+                if ((d.loud_byp[inst] >> j) & 1) continue;
+                const int32_t *c = d.loud_c + (size_t)j * 5 * Np + inst;
+                loud[k++] = sect_tdf2(c[0] * kQ28, c[Np] * kQ28, c[2 * Np] * kQ28, c[3 * Np] * kQ28, c[4 * Np] * kQ28);
+            }
+            n_loud = k;
+        }
+        __syncthreads();
+        if (f >= nf) continue;
+        Cd pre = cascade_eval(loud, n_loud, t);
+        if ((flags & F_LEV) && (flags & F_LOOKAHEAD)) pre = cmul(pre, delay_phase(fr, kLa, fs));
+        const bool master_on = !(flags & F_BYPASS_MASTER);
+        Cd P[2];
+#pragma unroll
+        for (int s = 0; s < 2; s++) {
+            P[s] = cscale(pre, d.preamp[s * Np + inst] * kQ28);
+            if (master_on) P[s] = cmul(P[s], cascade_eval(sec[s], cnt[s], t));
+        }
+        Cd direct = { 1.0, 0.0 }, cross = { 0.0, 0.0 };                      // crossfeed.c:161-180
+        if (flags & F_XFEED) {
+            const double a0 = d.xf[0 * Np + inst] * kQ28, b1 = d.xf[1 * Np + inst] * kQ28, ap = d.xf[4 * Np + inst] * kQ28;
+            const Cd lp = cdiv({ a0, 0.0 }, { 1.0 - b1 * t.c1, -b1 * t.s1 });
+            const Cd apd = { 1.0 + ap * t.c1, ap * t.s1 };                 // 0 only for a = +-1 at DC / Nyquist: AP = a there
+            const Cd apv = (apd.re == 0.0 && apd.im == 0.0) ? Cd{ ap, 0.0 } : cdiv({ ap + t.c1, t.s1 }, apd);
+            direct = { 1.0 - lp.re, -lp.im };
+            cross = cmul(apv, lp);
+        }
+        // envelope mode: the Q15 volume of the gain reached so far (usb_audio.c:976-980)
+        const bool env = d.env[4 * Np + inst] != 0;
+        int32_t pmg = __float2int_rz(__fadd_rn(__fmul_rn(__uint_as_float(d.env[2 * Np + inst]), 32768.0f), 0.5f));
+        pmg = pmg < 0 ? 0 : (pmg > 32768 ? 32768 : pmg);
+        const int32_t vmm_env = mul_q15(mul_q15(d.vol_base[inst], pmg), d.vol_master[inst]);
+        for (int o = 0; o < kOuts; o++) {
+            const uint8_t of = d.o_flags[o * Np + inst];
+            const int32_t gain = !env ? d.o_gain[o * Np + inst] : ((of & O_MUTE) ? 0 : __float2int_rz(__fmul_rn(d.o_glin[o * Np + inst], (float)vmm_env)));
+            Cd h[2] = { { 0.0, 0.0 }, { 0.0, 0.0 } };
+            if ((of & O_ENABLED) && gain != 0) {
+                Cd g = cascade_eval(sec[2 + o], ((of & O_MUTE) || !master_on) ? 0 : cnt[2 + o], t);
+                g = cscale(g, gain * kQ15);
+                const int32_t dly = d.o_dly[o * Np + inst];
+                if ((flags & F_ANY_DELAY) && dly > 0) g = cmul(g, delay_phase(fr, (uint32_t)dly & (kMaxDelay - 1), fs));
+                const double gl = d.o_gl[o * Np + inst] * kQ15, gr = d.o_gr[o * Np + inst] * kQ15;
+                h[0] = cmul(g, cmul(cadd(cscale(direct, gl), cscale(cross, gr)), P[0]));
+                h[1] = cmul(g, cmul(cadd(cscale(cross, gl), cscale(direct, gr)), P[1]));
+            }
+            out[(((size_t)u * kOuts + o) * 2 + 0) * nf + f] = to_float2(h[0]);
+            out[(((size_t)u * kOuts + o) * 2 + 1) * nf + f] = to_float2(h[1]);
+        }
+    }
+}
+
 int fail(int code, const char *fmt, ...)
 {
     size_t cap = 0;
@@ -730,6 +814,7 @@ struct dspi_chainq {
     uint32_t env_instances;          // instances in envelope mode
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     dspi::PacketSchedule sched;      // packet lengths of the current call
+    dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chainq_response_*
 };
 
 namespace {
@@ -787,6 +872,7 @@ int dspi_chainq_destroy(dspi_chainq *c)
     if (c->stream) cudaStreamSynchronize(c->stream);
     c->st.destroy();
     c->sched.destroy();
+    c->resp.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -1415,6 +1501,50 @@ int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len)
     c->env_instances = 0;
     for (uint32_t v : on) c->env_instances += v ? 1u : 0u;
     return DSPI_OK;
+}
+
+// Frequency response of instances [inst0, inst0 + n) on the engine stream (see chain_f32.cu); out [n][5][2][n_freqs] float2
+static int chainq_response(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
+{
+    const char *why = "";
+    int rc = dspi::response_check_args(freqs, n_freqs, fs, out, &why);
+    if (rc) return fail(rc, "%s", why);
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(c->resp.upload(freqs, n_freqs, c->stream, &c->launches));
+    const dspi_biquad_q28 *m_aos = (const dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_m), *o_aos = (const dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_o);
+    auto launch = [&](uint32_t i0, uint32_t m, void *dst) -> cudaError_t {
+        const dim3 grid((n_freqs + 127) / 128, m < 65535u ? m : 65535u);
+        dspi::chainq_response_kernel<<<grid, 128, 0, c->stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
+        c->launches++;
+        return cudaGetLastError();
+    };
+    if (!host) {
+        CU_OK(launch(inst0, n, out));
+        return DSPI_OK;
+    }
+    const size_t row_bytes = (size_t)dspi::kOuts * 2 * n_freqs * 2 * sizeof(float);
+    uint32_t rows = 0;
+    CU_OK(c->resp.stage(row_bytes, n, c->stream, &rows));
+    for (uint32_t i = 0; i < n; i += rows) {
+        const uint32_t m = n - i < rows ? n - i : rows;
+        CU_OK(launch(inst0 + i, m, c->resp.d_stage));
+        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->stream));
+        CU_OK(cudaStreamSynchronize(c->stream));
+    }
+    return DSPI_OK;
+}
+
+int dspi_chainq_response_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
+{
+    return chainq_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, out, true);
+}
+
+int dspi_chainq_response_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out)
+{
+    return chainq_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
 }
 
 int dspi_chainq_sync(dspi_chainq *c)

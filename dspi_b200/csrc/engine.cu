@@ -16,6 +16,7 @@
 
 #include "eq_kernels.cuh"
 #include "eq_jit.h"
+#include "response.cuh"
 
 namespace {
 
@@ -94,6 +95,7 @@ struct dspi_eq {
     bool sig_dirty;
     void *jit;               // run-time specialised K1 (eq_jit.cu) or nullptr = ahead-of-time kernels
     char kinfo[320];
+    dspi::ResponseBuffers resp;   // frequency table and host staging of dspi_eq_response_*
 };
 
 extern "C" {
@@ -282,6 +284,7 @@ int dspi_eq_destroy(dspi_eq *e)
     if (e->d_modes) cudaFree(e->d_modes);
     if (e->d_modes_eff) cudaFree(e->d_modes_eff);
     if (e->d_sched) cudaFree(e->d_sched);
+    e->resp.destroy();
     if (e->stream) cudaStreamDestroy(e->stream);
     if (e->s_h2d) cudaStreamDestroy(e->s_h2d);
     if (e->s_d2h) cudaStreamDestroy(e->s_d2h);
@@ -769,6 +772,47 @@ int dspi_eq_sync(dspi_eq *e)
 }
 
 void *dspi_eq_stream(dspi_eq *e) { return e ? (void *)e->stream : nullptr; }
+
+// Frequency response of channels [ch0, ch0 + n) from the mirror (response.cu), on the engine stream.  out: device memory
+// [n][n_freqs] float2 (host = false), or host memory filled chunk by chunk through the staging buffer (host = true).
+static int eq_response(dspi_eq *e, uint32_t ch0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
+{
+    const char *why = "";
+    int rc = dspi::response_check_args(freqs, n_freqs, fs, out, &why);
+    if (rc) return fail(rc, "%s", why);
+    if (!e) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)ch0 + n > e->desc.n_channels) return fail(DSPI_ERANGE, "channels [%u, %llu) outside engine of %u", ch0, (unsigned long long)ch0 + n, e->desc.n_channels);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(e->desc.device));
+    CU_OK(e->resp.upload(freqs, n_freqs, e->stream, &e->launches));
+    const bool q28 = e->desc.arith == DSPI_ARITH_Q28;
+    if (!host) {
+        CU_OK(dspi::launch_eq_response(q28, e->d_aos, ch0, n, e->desc.n_bands, e->resp.d_freq, n_freqs, fs, out, e->stream));
+        e->launches++;
+        return DSPI_OK;
+    }
+    const size_t row_bytes = (size_t)n_freqs * 2 * sizeof(float);
+    uint32_t rows = 0;
+    CU_OK(e->resp.stage(row_bytes, n, e->stream, &rows));
+    for (uint32_t c = 0; c < n; c += rows) {
+        const uint32_t m = n - c < rows ? n - c : rows;
+        CU_OK(dspi::launch_eq_response(q28, e->d_aos, ch0 + c, m, e->desc.n_bands, e->resp.d_freq, n_freqs, fs, e->resp.d_stage, e->stream));
+        e->launches++;
+        CU_OK(cudaMemcpyAsync((char *)out + (size_t)c * row_bytes, e->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, e->stream));
+        CU_OK(cudaStreamSynchronize(e->stream));
+    }
+    return DSPI_OK;
+}
+
+int dspi_eq_response_host(dspi_eq *e, uint32_t ch0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
+{
+    return eq_response(e, ch0, n, freqs_hz, n_freqs, sample_rate, out, true);
+}
+
+int dspi_eq_response_device(dspi_eq *e, uint32_t ch0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out)
+{
+    return eq_response(e, ch0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
+}
 uint64_t dspi_eq_launch_count(dspi_eq *e) { return e ? e->launches : 0; }
 
 }  // extern "C"

@@ -84,4 +84,7 @@ int eq_state_load(dspi_eq *e, const void *src, int cpl, cudaStream_t s);
 cudaError_t launch_coeffs(bool q28, dspi_eq_param *d_recipes, void *d_aos, uint32_t ch0, uint32_t n, float fs, cudaStream_t stream);
 cudaError_t launch_skip_q28(int32_t *coef, const uint8_t *skip, uint32_t n, cudaStream_t stream);
 cudaError_t launch_mask_modes(const uint64_t *raw, const uint8_t *skip, uint64_t *eff, uint32_t n, cudaStream_t stream);
+// response.cu: frequency response of channels [ch0, ch0 + n) of a mirror (bands b < nb) at d_freq[nf] -> d_out [n][nf] float2
+cudaError_t launch_eq_response(bool q28, const void *aos, uint32_t ch0, uint32_t n, uint32_t nb, const float *d_freq, uint32_t nf, float fs,
+                               void *d_out, cudaStream_t stream);
 }  // namespace dspi

@@ -621,6 +621,46 @@ int dspi_chainq_process_subframes_host  (dspi_chainq *c, const void *pcm,   uint
 int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                          dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
 
+/* ---- frequency response of EQ channels and chain instances ------------------------------------ */
+/* The complex transfer function H(e^{j omega}) of the linear, time-invariant part of the path the NEXT process call applies,
+ * read from the engine's device-resident coefficients and parameters at the point of the engine stream where the call is
+ * issued (so after every upload, set_params, device-side generation and process call issued before it) and evaluated at
+ * the caller's frequencies.  Read-only: it changes no coefficient, state, meter, envelope or S/PDIF transmitter field and
+ * never touches the packed K1 / K2 stores; a process call after it gives the same bytes as one without it.
+ * Every stage is taken from its recurrence as the processing runs it, as a 2-state model (DESIGN.md 4), formed and evaluated
+ * in double; each output value is rounded once to float.
+ *   EQ row: product over bands b < n_bands that are not bypassed - TDF2 (b0 + b1 z^-1 + b2 z^-2) / (1 + a1 z^-1 + a2 z^-2)
+ *     with the firmware's signs (s1 = b1 x - a1 y + s2), or the SVF of dsp_pipeline.c:290-345 with its svf_type's output mix;
+ *     Q28 coefficients enter as value / 2^28.  Bands >= n_bands are not processed and not included.
+ *   Float chain, input side s (unpacked sample, full scale 1.0) -> output o (float value before the 24-bit / Q28 conversion):
+ *     preamp; the loudness shelves if loudness is on (each shelf's bypass honoured); master EQ unless bypass_master_eq; the
+ *     leveller, when enabled with look-ahead, as its 480-sample delay at 0 dB gain - exact for signals under its gate once
+ *     the gain has settled, its level-dependent gain is not modelled; crossfeed if on, L' = (1 - LP) L + AP LP R with
+ *     LP = a0 / (1 - b1 z^-1), AP = (a + z^-1) / (1 + a z^-1); the matrix crosspoints (enabled, phase invert); the output EQ
+ *     (skipped for a muted or disabled output); the output gain gain_linear * vol_mul_master - host mute, the int16 volume
+ *     quirk (0 dB gives -1), master volume and the preset-mute gain: the constant preset_mute_gain outside envelope mode, the
+ *     envelope's current smooth gain inside it (during a fade: the gain reached so far, not the next packet's step); the
+ *     delay z^-(dly mod MAX) for dly > 0, so dly == MAX is no delay, as the ring does.  Disabled outputs are exactly 0; the
+ *     sub (output 9) is the value fed to the modulator.
+ *   Q28 chain: the same in the RP2040's quantities (ratios of Q28 values): preamp_q28, Q28 TDF2 loudness shelves, Q28
+ *     crossfeed, matrix gains as the Q15 integers the packet loop forms ((int32)(g * 32768)), the output gain as the Q15
+ *     integer of usb_audio.c:1204-1205, MAX = 2048, and output EQs skipped while the master EQ is bypassed (quirk 3).
+ *   Not modelled: float rounding, Q28 truncation, the leveller's level-dependent gain, the modulator's noise shaping.
+ * freqs_hz[n_freqs] (host memory, read during the call and reusable as soon as it returns; 0 <= f <= sample_rate / 2,
+ * finite), sample_rate > 0.  Output: interleaved float {re, im} pairs.
+ *   *_device: d_out is device memory; asynchronous on the engine stream.
+ *   *_host:   returns when the data is back; staged through a bounded device buffer in channel / instance chunks (32 MiB,
+ *             DSPI_HOST_CHUNK_MB in the environment overrides), never n x n_freqs at once.
+ * Errors: DSPI_EINVAL for NULL pointers, n_freqs == 0 or above 65536, a frequency that is NaN, negative or above Nyquist, a
+ * sample_rate that is not positive and finite; DSPI_ERANGE for a range past the end (also one whose end wraps in 32 bits);
+ * nothing is written then.  n == 0 does nothing.  All three EQ arithmetics are supported. */
+int dspi_eq_response_host       (dspi_eq *e,     uint32_t ch0,   uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out);    /* [n][n_freqs][2] */
+int dspi_eq_response_device     (dspi_eq *e,     uint32_t ch0,   uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out);
+int dspi_chain_response_host    (dspi_chain *c,  uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out);    /* [n][9][2 inputs][n_freqs][2] */
+int dspi_chain_response_device  (dspi_chain *c,  uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out);
+int dspi_chainq_response_host   (dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out);    /* [n][5][2][n_freqs][2] */
+int dspi_chainq_response_device (dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out);
+
 /* pinned host memory helpers */
 void *dspi_host_alloc(size_t bytes);
 void dspi_host_free(void *p);
