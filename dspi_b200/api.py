@@ -45,6 +45,7 @@ SYMBOLS = [
     "dspi_chain_process_subframes_host", "dspi_chain_process_subframes_device", "dspi_chainq_process_subframes_host", "dspi_chainq_process_subframes_device",
     "dspi_eq_response_host", "dspi_eq_response_device", "dspi_chain_response_host", "dspi_chain_response_device",
     "dspi_chainq_response_host", "dspi_chainq_response_device",
+    "dspi_chain_apply_bulk_device", "dspi_chainq_apply_bulk_device",
 ]
 
 
@@ -141,6 +142,7 @@ def lib():
             getattr(h, pre + "_get_preset_mute").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_set_dynamics_device").argtypes = [vp, u32, u32, vp, C.c_float]
             getattr(h, pre + "_sm_partition").argtypes = [vp, vp, vp]
+            getattr(h, pre + "_apply_bulk_device").argtypes = [vp, u32, u32, vp, vp, C.c_int, C.c_float, vp]
             getattr(h, pre + "_process_packets_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_process_packets_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_set_spdif_tx").argtypes = [vp, u32, u32, vp]
@@ -401,7 +403,22 @@ def bind_host_to_device(device):
 
 class _ChainSpdif:
     """What both chain engines share: each instance's S/PDIF transmitter (block position + channel status) and the
-    process form whose output stage writes S/PDIF subframes (``*_spdif_tx``, ``*_process_subframes_*``)."""
+    process form whose output stage writes S/PDIF subframes (``*_spdif_tx``, ``*_process_subframes_*``), and the ingest of
+    ``WireBulkParams`` packets on the GPU (``*_apply_bulk_device``)."""
+
+    def apply_bulk_device(self, packets, fs, inst0=0, host=None, exact_db=False):
+        """WIRE_BULK [n] -> instances [inst0, inst0+n) reconfigured on the GPU as ``bulk_params_apply`` and the firmware's main
+        loop would; ``host`` BULK_HOST [n] (default: volume 0 dB, not muted).  Returns the firmware's result codes, int32 [n]:
+        0 applied, -1 .. -4 rejected (that instance is left exactly as it was)."""
+        w = np.ascontiguousarray(packets, L.WIRE_BULK).reshape(-1)
+        hv = np.zeros(w.shape[0], L.BULK_HOST) if host is None else np.ascontiguousarray(host, L.BULK_HOST).reshape(-1)
+        if hv.shape[0] != w.shape[0]:
+            raise ValueError("packets and host give different instance counts")
+        res = np.zeros(w.shape[0], np.int32)
+        _check(getattr(lib(), self._PRE + "_apply_bulk_device")(self._h, int(inst0), int(w.shape[0]), w.ctypes.data_as(C.c_void_p),
+                                                                hv.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
+                                                                res.ctypes.data_as(C.c_void_p)))
+        return res
 
     def set_spdif_tx(self, block_pos, channel_status, inst0=0):
         """Transmitter state of instances [inst0, inst0+n): ``block_pos`` an int or [n] (0..191), ``channel_status`` 5 bytes

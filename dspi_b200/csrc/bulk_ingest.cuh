@@ -1,0 +1,267 @@
+// bulk_ingest.cuh — parameter ingest on the device, from the wire packet (SURVEY.md §8 f-1): bulk_params_apply() and the
+// main-loop work that follows it, for many instances of a chain engine at once, shared by chain_f32.cu and chain_q28.cu.
+//
+// Reference: bulk_params_apply() bulk_params.c:178-377 (validation :179-203, db_to_linear :49-56), dsp_update_delay_samples()
+// dsp_pipeline.c:216-239, the pending-flag handlers main.c:868-900, audio_set_volume() usb_audio.c:410-440.
+//
+// bulk_ingest_kernel: one warp per instance, kWarps instances per CTA.  Lane 0 brings the 2896-byte packet into shared memory
+// with one 1-D bulk copy on the warp's own mbarrier; every lane validates the header (the firmware returns before its first
+// write, so a rejected packet writes nothing but its result code); then the lanes share the work:
+//   lanes [0, 2 O)        crosspoint gains            lanes [2 O, 3 O)   output gains, flags, delay samples, skip rows
+//   lanes 3 O, 3 O + 1    preamp L / R                lane 3 O + 2       master volume
+//   lane 0 crossfeed, lane 1 leveller, lane 2 host volume + the loudness row it selects, then lane 0 the output gains
+//   all lanes             the 12 x roles recipes, 16 bytes each, into the role-major recipe buffer [role][n][12]
+// The recipes then go through the coefficient kernels of coeff.cu, one launch per sub-engine over all its roles (RoleRange).
+// The engine-specific stores (float or Q28 / Q15) are the engine's ParamStores, the same functions its dynamics kernel uses.
+//
+// Same arithmetic rules as coeff.cu / dynamics.cuh: every float operation is the reference's, rounded on its own
+// (-fmad=false, divisions spelled __fdiv_rn), libm in double rounded once, float -> int32 stores saturate.
+#pragma once
+#include <cstddef>
+#include <cstdio>
+
+#include "dspi_common.cuh"
+#include "dynamics.cuh"
+#include "eq_kernels.cuh"
+
+namespace dspi {
+
+// per-instance and per-output flag rows of the chain engines
+enum : uint8_t { F_BYPASS_MASTER = 1, F_LOUD = 2, F_XFEED = 4, F_LEV = 8, F_LOOKAHEAD = 16, F_ANY_DELAY = 32, F_SUB_ON = 64 };
+enum : uint8_t { O_ENABLED = 1, O_MUTE = 2, O_PAIR_OFF = 4 };
+
+// the derived flag words, one definition for dspi_chain(q)_set_params on the host and the ingest kernel on the device
+__host__ __device__ inline uint8_t chain_flags(bool bypass_master_eq, bool loudness, bool crossfeed, bool leveller, bool lookahead, bool any_delay,
+                                               bool sub_enabled)
+{
+    return (uint8_t)((bypass_master_eq ? F_BYPASS_MASTER : 0) | (loudness ? F_LOUD : 0) | (crossfeed ? F_XFEED : 0) | (leveller ? F_LEV : 0) |
+                     (lookahead ? F_LOOKAHEAD : 0) | (any_delay ? F_ANY_DELAY : 0) | (sub_enabled ? F_SUB_ON : 0));
+}
+// `pair_partner_enabled`: outputs[o ^ 1].enabled; the last output (the sub) has no S/PDIF pair (usb_audio.c:930-933)
+__host__ __device__ inline uint8_t output_flags(bool enabled, bool mute, bool has_pair, bool pair_partner_enabled)
+{
+    return (uint8_t)((enabled ? O_ENABLED : 0) | (mute ? O_MUTE : 0) | ((has_pair && !enabled && !pair_partner_enabled) ? O_PAIR_OFF : 0));
+}
+
+namespace bulk {
+
+constexpr int kWarps = 4;                                  // instances per CTA: 4 x 2896 B of packets = 11.3 KB shared memory
+constexpr uint32_t kChunk = 1024;                          // instances per staged chunk: 2.8 MB of packets, <= 2.1 MB of recipes
+constexpr uint32_t kPacketBytes = sizeof(dspi_wire_bulk_params);
+static_assert(kPacketBytes % 16 == 0, "the bulk copy moves multiples of 16 bytes");
+
+#define DSPI_WIRE_OFF(member) ((uint32_t)offsetof(dspi_wire_bulk_params, member))
+
+// bulk_params.c:49-56 — the firmware's own conversion: 4-term Taylor series of exp(), clamped
+__device__ inline float db_to_linear_fw(float db)
+{
+    if (db == 0.0f) return 1.0f;
+    if (db < -60.0f) db = -60.0f;
+    if (db > 20.0f) db = 20.0f;
+    const float x = db * 0.1151292546f;
+    const float linear = 1.0f + x + x * x * 0.5f + x * x * x * 0.1666667f + x * x * x * x * 0.0416667f;
+    return (linear < 0.0f) ? 0.0f : linear;
+}
+
+// bulk_params.c:179-203
+__device__ inline int32_t validate(const unsigned char *w, int platform_id, int n_channels, int n_outputs)
+{
+    const uint32_t version = w[DSPI_WIRE_OFF(header.format_version)];
+    if (version < 2 || version > DSPI_WIRE_FORMAT_VERSION) return -1;
+    if (w[DSPI_WIRE_OFF(header.platform_id)] != platform_id) return -2;
+    if (w[DSPI_WIRE_OFF(header.num_channels)] != n_channels) return -3;
+    if (w[DSPI_WIRE_OFF(header.num_output_channels)] != n_outputs) return -3;
+    const uint32_t len = *reinterpret_cast<const uint16_t *>(w + DSPI_WIRE_OFF(header.payload_length));
+    const uint32_t v2_size = kPacketBytes - 16 - 16 - 16 - 16;
+    if (len < v2_size || len > kPacketBytes) return -4;
+    return 0;
+}
+
+template <class S>
+__global__ void __launch_bounds__(kWarps * 32)
+bulk_ingest_kernel(typename S::Dev d, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *__restrict__ packets,
+                   const dspi_bulk_host *__restrict__ host, int exact_db, float fs, dspi_eq_param *__restrict__ recipes, int32_t *__restrict__ results)
+{
+    constexpr int O = S::kOuts, WO = DSPI_WIRE_MAX_OUTPUTS;
+    static_assert(3 * O + 3 <= 32, "one lane per gain");
+    __shared__ alignas(16) unsigned char pkt_s[kWarps][kPacketBytes];
+    __shared__ uint64_t bar_s[kWarps];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t i = blockIdx.x * kWarps + warp;
+    if (i >= n) return;
+    const unsigned char *w = pkt_s[warp];
+    uint64_t *bar = &bar_s[warp];
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        fence_mbar_init();
+        mbar_arrive_expect_tx(bar, kPacketBytes);
+        bulk_load_1d(pkt_s[warp], packets + i, kPacketBytes, bar);
+    }
+    __syncwarp();
+    mbar_wait(bar, 0);
+
+    const int32_t rc = validate(w, S::kPlatformId, S::kRoles, O);
+    if (lane == 0) results[i] = rc;
+    if (rc != 0) return;
+
+    auto f32 = [&](uint32_t off) { return *reinterpret_cast<const float *>(w + off); };
+    const uint32_t inst = inst0 + i, Np = d.N_pad;
+    const uint32_t version = w[DSPI_WIRE_OFF(header.format_version)];
+    const bool bypass_master = w[DSPI_WIRE_OFF(global.bypass)] != 0;                               // :217
+
+    // ---- one gain per lane (:206-215, :247-264, :351-375) ----
+    const bool is_xp = lane < 2 * O, is_out = !is_xp && lane < 3 * O, is_pre = lane == 3 * O || lane == 3 * O + 1, is_mv = lane == 3 * O + 2;
+    const uint32_t side = is_xp ? lane / O : (uint32_t)(lane - 3 * O), o = is_xp ? lane % O : (uint32_t)(lane - 2 * O);
+    const uint32_t xp_off = DSPI_WIRE_OFF(crosspoints) + (side * WO + o) * 8, out_off = DSPI_WIRE_OFF(outputs) + o * 12;
+    float db = 0.0f;
+    if (is_xp) db = f32(xp_off + 4);
+    else if (is_out) db = f32(out_off + 4);
+    else if (is_pre) db = version >= 6 ? f32(DSPI_WIRE_OFF(preamp.preamp_db) + side * 4) : f32(DSPI_WIRE_OFF(global.preamp_gain_db));
+    else if (is_mv) db = f32(DSPI_WIRE_OFF(master_volume.master_volume_db));
+    float lin = 0.0f;
+    if (is_mv) {                                                                                   // :361-374: always the exact conversion
+        if (isnan(db) || isinf(db)) db = 0.0f;
+        if (db < -128.0f) db = -128.0f;
+        if (db > 0.0f) db = 0.0f;
+        lin = db <= -128.0f ? 0.0f : dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f));
+    } else if (is_xp || is_out || is_pre) {
+        lin = exact_db ? dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f)) : db_to_linear_fw(db);
+    }
+    bool delayed = false;
+    if (is_xp) {
+        S::crosspoint(d, inst, side, o, w[xp_off] != 0, w[xp_off + 1] != 0, lin);
+    } else if (is_out) {
+        const bool enabled = w[out_off] != 0, mute = w[out_off + 1] != 0;
+        const bool partner = w[DSPI_WIRE_OFF(outputs) + (o ^ 1u) * 12] != 0;
+        d.o_glin[o * Np + inst] = lin;
+        d.o_flags[o * Np + inst] = output_flags(enabled, mute, o < (uint32_t)O - 1, partner);
+        d.skip_o[o * Np + inst] = S::output_eq_frozen(enabled, mute, bypass_master) ? 1 : 0;
+        float delay_ms = f32(out_off + 8);                                                         // dsp_update_delay_samples(), dsp_pipeline.c:216-239
+        if (o == (uint32_t)O - 1) delay_ms = delay_ms + dyn::fdiv(128.0f, fs) * 1000.0f;           // SUB_ALIGN_SAMPLES, config.h:93-95
+        int32_t ds = dyn::f2i_sat(dyn::fdiv(delay_ms * fs, 1000.0f));
+        if (ds > S::kMaxDelay) ds = S::kMaxDelay;
+        if (ds < 0) ds = 0;
+        d.o_dly[o * Np + inst] = ds;
+        delayed = ds > 0;
+    } else if (is_pre) {
+        S::preamp(d, inst, side, lin);
+    } else if (is_mv && version >= 6) {
+        S::master_volume(d, inst, lin);
+    }
+    const bool any_delay = __ballot_sync(0xffffffffu, delayed) != 0;                               // dsp_pipeline.c:237
+
+    // ---- the pending-flag handlers of the main loop (main.c:868-900), one generator per lane ----
+    dspi_leveller_config lev;                                                                      // :330-346: defaults below v4
+    lev.enabled = version >= 4 ? (w[DSPI_WIRE_OFF(leveller.enabled)] != 0) : 0;
+    lev.speed = version >= 4 ? w[DSPI_WIRE_OFF(leveller.speed)] : 0;
+    lev.lookahead = version >= 4 ? (w[DSPI_WIRE_OFF(leveller.lookahead)] != 0) : 1;
+    lev.amount = version >= 4 ? f32(DSPI_WIRE_OFF(leveller.amount)) : 50.0f;
+    lev.max_gain_db = version >= 4 ? f32(DSPI_WIRE_OFF(leveller.max_gain_db)) : 15.0f;
+    lev.gate_threshold_db = version >= 4 ? f32(DSPI_WIRE_OFF(leveller.gate_threshold_db)) : -96.0f;
+    const bool xf_enabled = w[DSPI_WIRE_OFF(crossfeed.enabled)] != 0, loud_enabled = w[DSPI_WIRE_OFF(global.loudness_enabled)] != 0;
+    const dspi_bulk_host hv = host[i];
+    uint32_t row;
+    const int16_t vol_mul = dyn::host_volume(hv.volume_8_8, row);
+    if (lane == 0) {
+        dspi_crossfeed_config xf;                                                                  // :225-230; the filter state is cleared (crossfeed.c:110-126)
+        xf.enabled = xf_enabled;
+        xf.itd_enabled = w[DSPI_WIRE_OFF(crossfeed.itd_enabled)] != 0;
+        xf.preset = w[DSPI_WIRE_OFF(crossfeed.preset)];
+        xf.custom_fc = f32(DSPI_WIRE_OFF(crossfeed.custom_fc));
+        xf.custom_feed_db = f32(DSPI_WIRE_OFF(crossfeed.custom_feed_db));
+        S::crossfeed(d, inst, xf, fs);
+        d.flags[inst] = chain_flags(bypass_master, loud_enabled, xf_enabled, lev.enabled, lev.lookahead, any_delay,
+                                    w[DSPI_WIRE_OFF(outputs) + (O - 1) * 12] != 0);
+        d.skip_m[inst] = d.skip_m[Np + inst] = bypass_master ? 1 : 0;                              // usb_audio.c:721-728
+    } else if (lane == 1) {
+        S::leveller(d, inst, lev, fs);
+    } else if (lane == 2) {
+        S::loudness(d, inst, row, f32(DSPI_WIRE_OFF(global.loudness_ref_spl)), f32(DSPI_WIRE_OFF(global.loudness_intensity_pct)), fs);
+    }
+    __syncwarp();                                          // the gain rows of this instance are written: audio_set_volume() reads them
+    if (lane == 0) S::host_volume(d, inst, vol_mul, hv.host_mute != 0);
+
+    // ---- filter_recipes[][] (:291-300), role-major for the coefficient kernels ----
+    for (uint32_t r = lane; r < (uint32_t)S::kRoles * kMaxBands; r += 32) {
+        const uint32_t role = r / kMaxBands, b = r % kMaxBands;
+        uint4 q = *reinterpret_cast<const uint4 *>(w + DSPI_WIRE_OFF(eq) + r * 16);                 // {type, reserved[3]}, freq, q, gain_db
+        q.x = role | b << 8 | (q.x & 0xFFu) << 16;                                                 // {channel, band, type, reserved}
+        reinterpret_cast<uint4 *>(recipes)[((size_t)role * n + i) * kMaxBands + b] = q;
+    }
+}
+
+// engine-owned staging of one chunk: packets, host volumes, recipes and result codes on the device
+struct Stage {
+    dspi_wire_bulk_params *packets = nullptr;
+    dspi_bulk_host *host = nullptr;
+    dspi_eq_param *recipes = nullptr;
+    int32_t *results = nullptr;
+    cudaError_t ensure(int roles)
+    {
+        if (results) return cudaSuccess;
+        cudaError_t e = cudaMalloc((void **)&packets, (size_t)kChunk * kPacketBytes);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&host, (size_t)kChunk * sizeof(dspi_bulk_host));
+        if (e == cudaSuccess) e = cudaMalloc((void **)&recipes, (size_t)kChunk * roles * kMaxBands * sizeof(dspi_eq_param));
+        if (e == cudaSuccess) e = cudaMalloc((void **)&results, (size_t)kChunk * sizeof(int32_t));
+        if (e != cudaSuccess) destroy();
+        return e;
+    }
+    void destroy()
+    {
+        cudaFree(packets); cudaFree(host); cudaFree(recipes); cudaFree(results);
+        packets = nullptr; host = nullptr; recipes = nullptr; results = nullptr;
+    }
+};
+
+inline int fail_cuda(cudaError_t e, const char *what)
+{
+    size_t cap = 0;
+    char *buf = error_buffer(&cap);
+    snprintf(buf, cap, "bulk ingest: %s -> %s", what, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA;
+}
+
+// The whole call for an engine (dspi_chain or dspi_chainq) whose arguments are checked.  Everything runs on the engine
+// stream, behind earlier process calls; the last step (eq_set_skip) synchronises it.
+template <class S, class Engine>
+int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host, int exact_db,
+          float fs, int32_t *results)
+{
+    cudaError_t e = stage.ensure(S::kRoles);
+    if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
+    cudaStream_t s = c->stream;
+    const uint32_t Np = c->d.N_pad;
+    for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
+        const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk, first = inst0 + i0;
+        e = cudaMemcpyAsync(stage.packets, packets + i0, (size_t)nc * kPacketBytes, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(stage.host, host + i0, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyHostToDevice, s);
+        if (e != cudaSuccess) return fail_cuda(e, "packet copy");
+        bulk_ingest_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, first, nc, stage.packets, stage.host, exact_db, fs,
+                                                                                 stage.recipes, stage.results);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "ingest kernel");
+        c->launches++;
+        // dsp_recalculate_all_filters(): state into the mirrors, coefficients from the recipes, mirrors back into the packed stores
+        RoleRange rm, ro;
+        rm.roles = 2; ro.roles = S::kRoles - 2;
+        rm.stride = ro.stride = Np;
+        rm.reject = ro.reject = stage.results;
+        int rc = eq_unpack_range(c->eq_m, first, nc, s, rm);
+        if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, first, nc, s, ro);
+        if (rc != DSPI_OK) return rc;
+        e = launch_coeffs(S::kQ28, stage.recipes, eq_aos_mirror(c->eq_m), first, nc, fs, s, rm);
+        if (e == cudaSuccess) e = launch_coeffs(S::kQ28, stage.recipes + (size_t)2 * nc * kMaxBands, eq_aos_mirror(c->eq_o), first, nc, fs, s, ro);
+        if (e != cudaSuccess) return fail_cuda(e, "coefficient kernels");
+        c->launches += 2;
+        rc = eq_pack_range(c->eq_m, first, nc, s, rm);
+        if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, first, nc, s, ro);
+        if (rc != DSPI_OK) return rc;
+        if ((e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
+            return fail_cuda(e, "result copy");
+    }
+    int rc = eq_set_skip(c->eq_m, c->d.skip_m, s);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, s);
+    return rc;
+}
+
+}  // namespace bulk
+}  // namespace dspi

@@ -41,6 +41,7 @@
 #include <vector>
 
 #include "eq_kernels.cuh"
+#include "bulk_ingest.cuh"
 #include "chain_pdm.cuh"
 #include "chain_schedule.cuh"
 #include "chain_streams.cuh"
@@ -57,9 +58,6 @@ constexpr int kMaxDelay = DSPI_CHAIN_MAX_DELAY;
 constexpr int kLa = DSPI_LA_SAMPLES;
 constexpr int kPkt = DSPI_PACKET_MAX;
 constexpr int kXs = 33;                           // shared-memory column stride: conflict-free for lane = instance AND lane = frame
-
-enum : uint8_t { F_BYPASS_MASTER = 1, F_LOUD = 2, F_XFEED = 4, F_LEV = 8, F_LOOKAHEAD = 16, F_ANY_DELAY = 32, F_SUB_ON = 64 };
-enum : uint8_t { O_ENABLED = 1, O_MUTE = 2, O_PAIR_OFF = 4 };
 
 struct ChainDev {
     uint32_t N, N_pad, nb, max_frames, ldF;       // ldF: row stride of mrow / orow / subq (frames, multiple of 4)
@@ -470,55 +468,90 @@ __global__ void chain_env_kernel(ChainDev d, uint32_t n_packets)
     d.env[2 * Np + inst] = __float_as_uint(g);
 }
 
+// The float stores of device-side parameter ingest, shared by chain_dynamics_kernel and the bulk ingest kernel
+// (bulk_ingest.cuh): one instance per call, written straight into the engine's arrays.
+struct ParamStores {
+    using Dev = ChainDev;
+    static constexpr int kRoles = dspi::kRoles, kOuts = dspi::kOuts, kMaxDelay = dspi::kMaxDelay, kPlatformId = 1;
+    static constexpr bool kQ28 = false;
+    // crossfeed_compute_coefficients(): coefficients and CLEARED filter state (crossfeed.c:110-126)
+    static __device__ void crossfeed(const ChainDev &d, uint32_t inst, const dspi_crossfeed_config &cfg, float fs)
+    {
+        const uint32_t Np = d.N_pad;
+        float a0, b1, ap;
+        dyn::crossfeed_coeffs(cfg, fs, a0, b1, ap);
+        d.xf[0 * Np + inst] = a0; d.xf[1 * Np + inst] = b1; d.xf[4 * Np + inst] = ap;
+        d.xf[2 * Np + inst] = 0.0f; d.xf[3 * Np + inst] = 0.0f; d.xf[5 * Np + inst] = 0.0f; d.xf[6 * Np + inst] = 0.0f;
+    }
+    // leveller_compute_coefficients()
+    static __device__ void leveller(const ChainDev &d, uint32_t inst, const dspi_leveller_config &cfg, float fs)
+    {
+        float lv[9];
+        dyn::leveller_coeffs(cfg, fs, lv);
+#pragma unroll
+        for (int k = 0; k < 9; k++) d.lev_c[k * d.N_pad + inst] = lv[k];
+    }
+    // loudness_recompute_table() for the table row audio_set_volume() selected
+    static __device__ void loudness(const ChainDev &d, uint32_t inst, uint32_t row, float ref_spl, float intensity_pct, float fs)
+    {
+        const uint32_t Np = d.N_pad;
+        float lo_db, hi_db;
+        dyn::loudness_row_gains((int)row, ref_spl, intensity_pct, lo_db, hi_db);
+        float c[6];
+        bool byp;
+        uint8_t lb = 0;
+        const float lfs = fs < 1.0f ? 48000.0f : fs;                         // loudness.c:171
+        dyn::shelf_svf(200.0f, 0.707f, lo_db, false, lfs, c, byp);
+        if (byp) lb |= 1;
+#pragma unroll
+        for (int k = 0; k < 6; k++) d.loud_c[(0 * 6 + k) * Np + inst] = c[k];
+        dyn::shelf_svf(6000.0f, 0.707f, hi_db, true, lfs, c, byp);
+        if (byp) lb |= 2;
+#pragma unroll
+        for (int k = 0; k < 6; k++) d.loud_c[(1 * 6 + k) * Np + inst] = c[k];
+        d.loud_byp[inst] = lb;
+    }
+    // host volume -> output gains (usb_audio.c:569-571, 886-887), from the gain rows in force
+    static __device__ void host_volume(const ChainDev &d, uint32_t inst, int16_t vol_mul, bool host_mute)
+    {
+        const uint32_t Np = d.N_pad;
+        const float vol_base = host_mute ? 0.0f : __fmul_rn((float)vol_mul, 1.0f / 32768.0f);
+        d.vol_base[inst] = vol_base;
+        const float vmm = __fmul_rn(__fmul_rn(vol_base, d.pmg[inst]), d.vol_master[inst]);
+        for (int o = 0; o < dspi::kOuts; o++)
+            d.o_gain[o * Np + inst] = (d.o_flags[o * Np + inst] & O_MUTE) ? 0.0f : __fmul_rn(d.o_glin[o * Np + inst], vmm);
+    }
+    // what dspi_chain_set_params stores for the preamp, the master volume and one crosspoint (usb_audio.c:760-764)
+    static __device__ void preamp(const ChainDev &d, uint32_t inst, uint32_t side, float linear) { d.preamp[side * d.N_pad + inst] = linear; }
+    static __device__ void master_volume(const ChainDev &d, uint32_t inst, float linear) { d.vol_master[inst] = linear; }
+    static __device__ void crosspoint(const ChainDev &d, uint32_t inst, uint32_t side, uint32_t o, bool enabled, bool invert, float linear)
+    {
+        (side ? d.o_gr : d.o_gl)[o * d.N_pad + inst] = enabled ? (invert ? -linear : linear) : 0.0f;
+    }
+    static __host__ __device__ bool output_eq_frozen(bool enabled, bool mute, bool) { return !enabled || mute; }   // :878-884
+};
+
 // Mass reconfiguration of the dynamics stages on the device (SURVEY f-1): what the main loop does for one instance when
 // crossfeed_update_pending / leveller_update_pending / loudness_recompute_pending are set (main.c:868-895) plus
-// audio_set_volume() (usb_audio.c:428-440), one instance per thread, written straight into the engine's arrays.
+// audio_set_volume() (usb_audio.c:428-440), one instance per thread.
 __global__ void chain_dynamics_kernel(ChainDev d, uint32_t inst0, uint32_t n, const dspi_dynamics_config *__restrict__ cfgs, float fs)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t inst = inst0 + i, Np = d.N_pad;
+    const uint32_t inst = inst0 + i;
     const dspi_dynamics_config cfg = cfgs[i];
     uint8_t flags = d.flags[inst] & (uint8_t)~(F_XFEED | F_LEV | F_LOOKAHEAD | F_LOUD);
-    // crossfeed_compute_coefficients(): coefficients and CLEARED filter state (crossfeed.c:110-126)
-    float a0, b1, ap;
-    dyn::crossfeed_coeffs(cfg.crossfeed, fs, a0, b1, ap);
-    d.xf[0 * Np + inst] = a0; d.xf[1 * Np + inst] = b1; d.xf[4 * Np + inst] = ap;
-    d.xf[2 * Np + inst] = 0.0f; d.xf[3 * Np + inst] = 0.0f; d.xf[5 * Np + inst] = 0.0f; d.xf[6 * Np + inst] = 0.0f;
+    ParamStores::crossfeed(d, inst, cfg.crossfeed, fs);
     if (cfg.crossfeed.enabled) flags |= F_XFEED;                             // crossfeed_bypassed = !enabled, main.c:882
-    // leveller_compute_coefficients(); leveller_bypassed = !enabled, main.c:886-894
-    float lv[9];
-    dyn::leveller_coeffs(cfg.leveller, fs, lv);
-#pragma unroll
-    for (int k = 0; k < 9; k++) d.lev_c[k * Np + inst] = lv[k];
+    ParamStores::leveller(d, inst, cfg.leveller, fs);                        // leveller_bypassed = !enabled, main.c:886-894
     if (cfg.leveller.enabled) flags |= F_LEV;
     if (cfg.leveller.lookahead) flags |= F_LOOKAHEAD;
-    // audio_set_volume(): vol_mul and the loudness row of that volume step; loudness_recompute_table() for that row
     uint32_t row;
     const int16_t vol_mul = dyn::host_volume(cfg.volume_8_8, row);
-    float lo_db, hi_db;
-    dyn::loudness_row_gains((int)row, cfg.loudness_ref_spl, cfg.loudness_intensity_pct, lo_db, hi_db);
-    float c[6];
-    bool byp;
-    uint8_t lb = 0;
-    const float lfs = fs < 1.0f ? 48000.0f : fs;                             // loudness.c:171
-    dyn::shelf_svf(200.0f, 0.707f, lo_db, false, lfs, c, byp);
-    if (byp) lb |= 1;
-#pragma unroll
-    for (int k = 0; k < 6; k++) d.loud_c[(0 * 6 + k) * Np + inst] = c[k];
-    dyn::shelf_svf(6000.0f, 0.707f, hi_db, true, lfs, c, byp);
-    if (byp) lb |= 2;
-#pragma unroll
-    for (int k = 0; k < 6; k++) d.loud_c[(1 * 6 + k) * Np + inst] = c[k];
-    d.loud_byp[inst] = lb;
+    ParamStores::loudness(d, inst, row, cfg.loudness_ref_spl, cfg.loudness_intensity_pct, fs);
     if (cfg.loudness_enabled) flags |= F_LOUD;
     d.flags[inst] = flags;
-    // host volume -> output gains (usb_audio.c:569-571, 886-887)
-    const float vol_base = cfg.host_mute ? 0.0f : __fmul_rn((float)vol_mul, 1.0f / 32768.0f);
-    d.vol_base[inst] = vol_base;
-    const float vmm = __fmul_rn(__fmul_rn(vol_base, d.pmg[inst]), d.vol_master[inst]);
-    for (int o = 0; o < kOuts; o++)
-        d.o_gain[o * Np + inst] = (d.o_flags[o * Np + inst] & O_MUTE) ? 0.0f : __fmul_rn(d.o_glin[o * Np + inst], vmm);
+    ParamStores::host_volume(d, inst, vol_mul, cfg.host_mute != 0);
 }
 
 // post-gain sample of output row `o` (what the delay line stores)
@@ -851,6 +884,7 @@ struct dspi_chain {
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     dspi::PacketSchedule sched;      // packet lengths of the current call
     dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chain_response_*
+    dspi::bulk::Stage bulk;          // device staging of dspi_chain_apply_bulk_device, allocated by its first call
 };
 
 namespace {
@@ -1004,6 +1038,7 @@ int dspi_chain_destroy(dspi_chain *c)
     c->st.destroy();
     c->sched.destroy();
     c->resp.destroy();
+    c->bulk.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -1156,23 +1191,17 @@ int dspi_chain_set_params(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_
             gr[o * n + i] = b;
             gain[o * n + i] = oc.mute ? 0.0f : oc.gain_linear * vol_mul_master;    // :886-887
             glin[o * n + i] = oc.gain_linear;
-            uint8_t f = (oc.enabled ? dspi::O_ENABLED : 0) | (oc.mute ? dspi::O_MUTE : 0);
-            if (o < dspi::kOuts - 1) {
-                const int partner = o ^ 1;
-                if (!oc.enabled && !p.matrix.outputs[partner].enabled) f |= dspi::O_PAIR_OFF;    // :930-933
-            }
-            oflags[o * n + i] = f;
-            skip_o[o * n + i] = (!oc.enabled || oc.mute) ? 1 : 0;            // :878-884: state frozen
+            const bool has_pair = o < dspi::kOuts - 1;                       // :930-933
+            oflags[o * n + i] = dspi::output_flags(oc.enabled, oc.mute, has_pair, has_pair && p.matrix.outputs[o ^ 1].enabled);
+            skip_o[o * n + i] = dspi::ParamStores::output_eq_frozen(oc.enabled, oc.mute, p.bypass_master_eq) ? 1 : 0;   // :878-884: state frozen
             int32_t ds = oc.delay_samples;
             if (ds > DSPI_CHAIN_MAX_DELAY) ds = DSPI_CHAIN_MAX_DELAY;
             if (ds < 0) ds = 0;
             dly[o * n + i] = ds;
             if (ds > 0) any_delay = true;                                    // dsp_pipeline.c:237
         }
-        flags[i] = (p.bypass_master_eq ? dspi::F_BYPASS_MASTER : 0) | (p.loudness_enabled ? dspi::F_LOUD : 0) |
-                   (p.crossfeed_enabled ? dspi::F_XFEED : 0) | (p.leveller_enabled ? dspi::F_LEV : 0) |
-                   (p.leveller_lookahead ? dspi::F_LOOKAHEAD : 0) | (any_delay ? dspi::F_ANY_DELAY : 0) |
-                   (p.matrix.outputs[dspi::kOuts - 1].enabled ? dspi::F_SUB_ON : 0);
+        flags[i] = dspi::chain_flags(p.bypass_master_eq, p.loudness_enabled, p.crossfeed_enabled, p.leveller_enabled, p.leveller_lookahead, any_delay,
+                                     p.matrix.outputs[dspi::kOuts - 1].enabled);
         skip_m[0 * n + i] = skip_m[1 * n + i] = p.bypass_master_eq ? 1 : 0;   // :721-728
         loud_byp[i] = (p.loudness[0].bypass ? 1 : 0) | (p.loudness[1].bypass ? 2 : 0);
         for (int j = 0; j < 2; j++) {
@@ -1285,6 +1314,17 @@ int dspi_chain_set_dynamics_device(dspi_chain *c, uint32_t inst0, uint32_t n, co
     if (e != cudaSuccess) return fail(DSPI_ECUDA, "dynamics coefficient generation: %s", cudaGetErrorString(e));
     c->launches++;
     return DSPI_OK;
+}
+
+int dspi_chain_apply_bulk_device(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
+                                 int exact_db, float sample_rate, int32_t *results)
+{
+    if (!c || !packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
+    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return dspi::bulk::apply<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, exact_db, sample_rate, results);
 }
 
 int dspi_chain_upload_biquads(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_biquad_f32 *biquads)

@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "eq_kernels.cuh"
+#include "bulk_ingest.cuh"
 #include "chain_pdm.cuh"
 #include "chain_schedule.cuh"
 #include "chain_streams.cuh"
@@ -36,9 +37,6 @@ constexpr int kPkt = DSPI_PACKET_MAX;
 constexpr int kXs = 33;                                       // shared-memory column stride: conflict-free for lane = instance AND lane = frame
 constexpr int32_t kUnity = 1 << 28;
 constexpr int32_t kClipThresh = (1 << 28) + 268;              // config.h:54
-
-enum : uint8_t { F_BYPASS_MASTER = 1, F_LOUD = 2, F_XFEED = 4, F_LEV = 8, F_LOOKAHEAD = 16, F_ANY_DELAY = 32, F_SUB_ON = 64 };
-enum : uint8_t { O_ENABLED = 1, O_MUTE = 2, O_PAIR_OFF = 4 };
 
 struct ChainQ {
     uint32_t N, N_pad, nb, max_frames, ldF;        // ldF: row stride of mrow / orow / subq (frames, multiple of 4)
@@ -439,53 +437,91 @@ __global__ void chainq_env_kernel(ChainQ d, uint32_t n_packets)
     d.env[2 * Np + inst] = __float_as_uint(g);
 }
 
+// The RP2040 stores (Q28 / Q15) of device-side parameter ingest, shared by chainq_dynamics_kernel and the bulk ingest kernel
+// (bulk_ingest.cuh): see chain_f32.cu
+struct ParamStores {
+    using Dev = ChainQ;
+    static constexpr int kRoles = dspi::kRoles, kOuts = dspi::kOuts, kMaxDelay = dspi::kMaxDelay, kPlatformId = 0;
+    static constexpr bool kQ28 = true;
+    static __device__ void crossfeed(const ChainQ &d, uint32_t inst, const dspi_crossfeed_config &cfg, float fs)
+    {
+        const size_t Np = d.N_pad;
+        float a0, b1, ap;
+        const bool xon = dyn::crossfeed_coeffs(cfg, fs, a0, b1, ap);
+        const float scale = 268435456.0f;                                    // crossfeed.c:115-118
+        d.xf[0 * Np + inst] = xon ? dyn::f2i_sat(__fmul_rn(a0, scale)) : 0;
+        d.xf[1 * Np + inst] = xon ? dyn::f2i_sat(__fmul_rn(b1, scale)) : 0;
+        d.xf[4 * Np + inst] = xon ? dyn::f2i_sat(__fmul_rn(ap, scale)) : 0;
+        d.xf[2 * Np + inst] = 0; d.xf[3 * Np + inst] = 0; d.xf[5 * Np + inst] = 0; d.xf[6 * Np + inst] = 0;
+    }
+    static __device__ void leveller(const ChainQ &d, uint32_t inst, const dspi_leveller_config &cfg, float fs)
+    {
+        float lv[9];
+        dyn::leveller_coeffs(cfg, fs, lv);
+#pragma unroll
+        for (int k = 0; k < 9; k++) d.lev_c[(size_t)k * d.N_pad + inst] = lv[k];
+    }
+    static __device__ void loudness(const ChainQ &d, uint32_t inst, uint32_t row, float ref_spl, float intensity_pct, float fs)
+    {
+        const size_t Np = d.N_pad;
+        float lo_db, hi_db;
+        dyn::loudness_row_gains((int)row, ref_spl, intensity_pct, lo_db, hi_db);
+        int32_t c[5];
+        bool byp;
+        uint8_t lb = 0;
+        const float lfs = fs < 1.0f ? 48000.0f : fs;
+        dyn::shelf_q28(200.0f, 0.707f, lo_db, false, lfs, c, byp);
+        if (byp) lb |= 1;
+#pragma unroll
+        for (int k = 0; k < 5; k++) d.loud_c[(0 * 5 + k) * Np + inst] = c[k];
+        dyn::shelf_q28(6000.0f, 0.707f, hi_db, true, lfs, c, byp);
+        if (byp) lb |= 2;
+#pragma unroll
+        for (int k = 0; k < 5; k++) d.loud_c[(1 * 5 + k) * Np + inst] = c[k];
+        d.loud_byp[inst] = lb;
+    }
+    static __device__ void host_volume(const ChainQ &d, uint32_t inst, int16_t vol_mul, bool host_mute)
+    {
+        const size_t Np = d.N_pad;
+        const int32_t vol_base = host_mute ? 0 : (int32_t)vol_mul;           // usb_audio.c:975
+        d.vol_base[inst] = vol_base;
+        const int32_t vmm = mul_q15(mul_q15(vol_base, d.pmg[inst]), d.vol_master[inst]);    // :979-980
+        for (int o = 0; o < dspi::kOuts; o++)
+            d.o_gain[o * Np + inst] = (d.o_flags[o * Np + inst] & O_MUTE) ? 0 : __float2int_rz(__fmul_rn(d.o_glin[o * Np + inst], (float)vmm));   // :1204-1205
+    }
+    // what dspi_chainq_set_params stores for the preamp (Q28), the master volume (Q15) and one crosspoint (Q15, :1084-1085)
+    static __device__ void preamp(const ChainQ &d, uint32_t inst, uint32_t side, float linear)
+    {
+        d.preamp[(size_t)side * d.N_pad + inst] = dyn::f2i_sat(__fmul_rn(linear, 268435456.0f));
+    }
+    static __device__ void master_volume(const ChainQ &d, uint32_t inst, float linear) { d.vol_master[inst] = dyn::f2i_sat(__fmul_rn(linear, 32768.0f)); }
+    static __device__ void crosspoint(const ChainQ &d, uint32_t inst, uint32_t side, uint32_t o, bool enabled, bool invert, float linear)
+    {
+        (side ? d.o_gr : d.o_gl)[(size_t)o * d.N_pad + inst] = enabled ? dyn::f2i_sat(__fmul_rn(invert ? -linear : linear, 32768.0f)) : 0;
+    }
+    // :1197-1201 (quirk: gated on bypass_master_eq too)
+    static __host__ __device__ bool output_eq_frozen(bool enabled, bool mute, bool bypass_master_eq) { return !(enabled && !mute && !bypass_master_eq); }
+};
+
 // Mass reconfiguration of the dynamics stages on the device (SURVEY f-1), RP2040 stores: see chain_f32.cu
 __global__ void chainq_dynamics_kernel(ChainQ d, uint32_t inst0, uint32_t n, const dspi_dynamics_config *__restrict__ cfgs, float fs)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t inst = inst0 + i;
-    const size_t Np = d.N_pad;
     const dspi_dynamics_config cfg = cfgs[i];
     uint8_t flags = d.flags[inst] & (uint8_t)~(F_XFEED | F_LEV | F_LOOKAHEAD | F_LOUD);
-    float a0, b1, ap;
-    const bool xon = dyn::crossfeed_coeffs(cfg.crossfeed, fs, a0, b1, ap);
-    const float scale = 268435456.0f;                                        // crossfeed.c:115-118
-    d.xf[0 * Np + inst] = xon ? dyn::f2i_sat(__fmul_rn(a0, scale)) : 0;
-    d.xf[1 * Np + inst] = xon ? dyn::f2i_sat(__fmul_rn(b1, scale)) : 0;
-    d.xf[4 * Np + inst] = xon ? dyn::f2i_sat(__fmul_rn(ap, scale)) : 0;
-    d.xf[2 * Np + inst] = 0; d.xf[3 * Np + inst] = 0; d.xf[5 * Np + inst] = 0; d.xf[6 * Np + inst] = 0;
+    ParamStores::crossfeed(d, inst, cfg.crossfeed, fs);
     if (cfg.crossfeed.enabled) flags |= F_XFEED;
-    float lv[9];
-    dyn::leveller_coeffs(cfg.leveller, fs, lv);
-#pragma unroll
-    for (int k = 0; k < 9; k++) d.lev_c[k * Np + inst] = lv[k];
+    ParamStores::leveller(d, inst, cfg.leveller, fs);
     if (cfg.leveller.enabled) flags |= F_LEV;
     if (cfg.leveller.lookahead) flags |= F_LOOKAHEAD;
     uint32_t row;
     const int16_t vol_mul = dyn::host_volume(cfg.volume_8_8, row);
-    float lo_db, hi_db;
-    dyn::loudness_row_gains((int)row, cfg.loudness_ref_spl, cfg.loudness_intensity_pct, lo_db, hi_db);
-    int32_t c[5];
-    bool byp;
-    uint8_t lb = 0;
-    const float lfs = fs < 1.0f ? 48000.0f : fs;
-    dyn::shelf_q28(200.0f, 0.707f, lo_db, false, lfs, c, byp);
-    if (byp) lb |= 1;
-#pragma unroll
-    for (int k = 0; k < 5; k++) d.loud_c[(0 * 5 + k) * Np + inst] = c[k];
-    dyn::shelf_q28(6000.0f, 0.707f, hi_db, true, lfs, c, byp);
-    if (byp) lb |= 2;
-#pragma unroll
-    for (int k = 0; k < 5; k++) d.loud_c[(1 * 5 + k) * Np + inst] = c[k];
-    d.loud_byp[inst] = lb;
+    ParamStores::loudness(d, inst, row, cfg.loudness_ref_spl, cfg.loudness_intensity_pct, fs);
     if (cfg.loudness_enabled) flags |= F_LOUD;
     d.flags[inst] = flags;
-    const int32_t vol_base = cfg.host_mute ? 0 : (int32_t)vol_mul;           // usb_audio.c:975
-    d.vol_base[inst] = vol_base;
-    const int32_t vmm = mul_q15(mul_q15(vol_base, d.pmg[inst]), d.vol_master[inst]);    // :979-980
-    for (int o = 0; o < kOuts; o++)
-        d.o_gain[o * Np + inst] = (d.o_flags[o * Np + inst] & O_MUTE) ? 0 : __float2int_rz(__fmul_rn(d.o_glin[o * Np + inst], (float)vmm));   // :1204-1205
+    ParamStores::host_volume(d, inst, vol_mul, cfg.host_mute != 0);
 }
 
 __device__ __forceinline__ int32_t outq_gain(int32_t v, bool enabled, int32_t gain)
@@ -815,6 +851,7 @@ struct dspi_chainq {
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     dspi::PacketSchedule sched;      // packet lengths of the current call
     dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chainq_response_*
+    dspi::bulk::Stage bulk;          // device staging of dspi_chainq_apply_bulk_device, allocated by its first call
 };
 
 namespace {
@@ -873,6 +910,7 @@ int dspi_chainq_destroy(dspi_chainq *c)
     c->st.destroy();
     c->sched.destroy();
     c->resp.destroy();
+    c->bulk.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -1027,20 +1065,17 @@ int dspi_chainq_set_params(dspi_chainq *c, uint32_t inst0, uint32_t n, const dsp
             gr[o * n + i] = xr.enabled ? dspi::h_f2i_sat((xr.phase_invert ? -xr.gain_linear : xr.gain_linear) * 32768.0f) : 0;
             gain[o * n + i] = oc.mute ? 0 : dspi::h_f2i_sat(oc.gain_linear * (float)vol_mul_master);    // :1204-1205
             glin[o * n + i] = oc.gain_linear;
-            uint8_t f = (oc.enabled ? dspi::O_ENABLED : 0) | (oc.mute ? dspi::O_MUTE : 0);
-            if (o < O - 1 && !oc.enabled && !p.matrix.outputs[o ^ 1].enabled) f |= dspi::O_PAIR_OFF;    // :1248-1251
-            oflags[o * n + i] = f;
-            skip_o[o * n + i] = (oc.enabled && !oc.mute && !p.bypass_master_eq) ? 0 : 1;                 // :1197-1201 (quirk: gated on bypass_master_eq too)
+            const bool has_pair = o < O - 1;                                                            // :1248-1251
+            oflags[o * n + i] = dspi::output_flags(oc.enabled, oc.mute, has_pair, has_pair && p.matrix.outputs[o ^ 1].enabled);
+            skip_o[o * n + i] = dspi::ParamStores::output_eq_frozen(oc.enabled, oc.mute, p.bypass_master_eq) ? 1 : 0;
             int32_t ds = oc.delay_samples;
             if (ds > DSPI_CHAINQ_MAX_DELAY) ds = DSPI_CHAINQ_MAX_DELAY;
             if (ds < 0) ds = 0;
             dly[o * n + i] = ds;
             if (ds > 0) any_delay = true;
         }
-        flags[i] = (p.bypass_master_eq ? dspi::F_BYPASS_MASTER : 0) | (p.loudness_enabled ? dspi::F_LOUD : 0) |
-                   (p.crossfeed_enabled ? dspi::F_XFEED : 0) | (p.leveller_enabled ? dspi::F_LEV : 0) |
-                   (p.leveller_lookahead ? dspi::F_LOOKAHEAD : 0) | (any_delay ? dspi::F_ANY_DELAY : 0) |
-                   (p.matrix.outputs[O - 1].enabled ? dspi::F_SUB_ON : 0);
+        flags[i] = dspi::chain_flags(p.bypass_master_eq, p.loudness_enabled, p.crossfeed_enabled, p.leveller_enabled, p.leveller_lookahead, any_delay,
+                                     p.matrix.outputs[O - 1].enabled);
         skip_m[0 * n + i] = skip_m[1 * n + i] = p.bypass_master_eq ? 1 : 0;                              // :1050-1055
         loud_byp[i] = (p.loudness[0].bypass ? 1 : 0) | (p.loudness[1].bypass ? 2 : 0);
         for (int j = 0; j < 2; j++) {
@@ -1153,6 +1188,17 @@ int dspi_chainq_set_dynamics_device(dspi_chainq *c, uint32_t inst0, uint32_t n, 
     if (e != cudaSuccess) return fail(DSPI_ECUDA, "dynamics coefficient generation: %s", cudaGetErrorString(e));
     c->launches++;
     return DSPI_OK;
+}
+
+int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
+                                  int exact_db, float sample_rate, int32_t *results)
+{
+    if (!c || !packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
+    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return dspi::bulk::apply<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, exact_db, sample_rate, results);
 }
 
 int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_biquad_q28 *biquads)

@@ -89,12 +89,14 @@ __device__ void cookbook(const dspi_eq_param &p, float A, float fs, float (&n)[3
 }
 
 __global__ void __launch_bounds__(256)
-coeff_f32_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_f32 *__restrict__ aos, uint32_t ch0, uint32_t n, float fs)
+coeff_f32_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_f32 *__restrict__ aos, uint32_t ch0, uint32_t n, float fs, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * kMaxBands) return;
+    if (i >= n * kMaxBands || (rr.reject && rr.reject[i / kMaxBands])) return;
+    recipes += (size_t)blockIdx.y * n * kMaxBands;
+    aos += ((size_t)ch0 + (size_t)blockIdx.y * rr.stride) * kMaxBands;
     dspi_eq_param p = recipes[i];
-    dspi_biquad_f32 bq = aos[(size_t)ch0 * kMaxBands + i];
+    dspi_biquad_f32 bq = aos[i];
     if (recipe_is_flat(p) || fs == 0.0f) {                                   // :62-73
         bq.bypass = 1;
         bq.use_svf = 0;
@@ -149,7 +151,7 @@ coeff_f32_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_f32 *__restric
         }
     }
     recipes[i] = p;
-    aos[(size_t)ch0 * kMaxBands + i] = bq;
+    aos[i] = bq;
 }
 
 // (int32_t) cast with the firmware's saturating semantics (:168-173 run on the RP2040's soft float)
@@ -161,12 +163,14 @@ __device__ __forceinline__ int32_t to_q28(float v)
 }
 
 __global__ void __launch_bounds__(256)
-coeff_q28_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_q28 *__restrict__ aos, uint32_t ch0, uint32_t n, float fs)
+coeff_q28_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_q28 *__restrict__ aos, uint32_t ch0, uint32_t n, float fs, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * kMaxBands) return;
+    if (i >= n * kMaxBands || (rr.reject && rr.reject[i / kMaxBands])) return;
+    recipes += (size_t)blockIdx.y * n * kMaxBands;
+    aos += ((size_t)ch0 + (size_t)blockIdx.y * rr.stride) * kMaxBands;
     dspi_eq_param p = recipes[i];
-    dspi_biquad_q28 bq = aos[(size_t)ch0 * kMaxBands + i];
+    dspi_biquad_q28 bq = aos[i];
     if (recipe_is_flat(p) || fs == 0.0f) {
         bq.bypass = 1;
         bq.b0 = 1 << 28;
@@ -184,17 +188,18 @@ coeff_q28_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_q28 *__restric
         bq.a2 = to_q28(fdiv(dd[2], dd[0]));
     }
     recipes[i] = p;
-    aos[(size_t)ch0 * kMaxBands + i] = bq;
+    aos[i] = bq;
 }
 
 }  // namespace
 
-cudaError_t launch_coeffs(bool q28, dspi_eq_param *d_recipes, void *d_aos, uint32_t ch0, uint32_t n, float fs, cudaStream_t stream)
+cudaError_t launch_coeffs(bool q28, dspi_eq_param *d_recipes, void *d_aos, uint32_t ch0, uint32_t n, float fs, cudaStream_t stream,
+                          const RoleRange &rr)
 {
     if (n == 0) return cudaSuccess;
-    const uint32_t items = n * kMaxBands;
-    if (q28) coeff_q28_kernel<<<(items + 255) / 256, 256, 0, stream>>>(d_recipes, (dspi_biquad_q28 *)d_aos, ch0, n, fs);
-    else coeff_f32_kernel<<<(items + 255) / 256, 256, 0, stream>>>(d_recipes, (dspi_biquad_f32 *)d_aos, ch0, n, fs);
+    const dim3 grid((n * kMaxBands + 255) / 256, rr.roles);
+    if (q28) coeff_q28_kernel<<<grid, 256, 0, stream>>>(d_recipes, (dspi_biquad_q28 *)d_aos, ch0, n, fs, rr);
+    else coeff_f32_kernel<<<grid, 256, 0, stream>>>(d_recipes, (dspi_biquad_f32 *)d_aos, ch0, n, fs, rr);
     return cudaGetLastError();
 }
 

@@ -68,6 +68,14 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *m
         : "memory");
 }
 
+// 1-D bulk load: `bytes` contiguous bytes global -> smem, completes on `bar`.  Both addresses and the size are multiples of 16.
+__device__ __forceinline__ void bulk_load_1d(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)), "l"(gsrc),
+                 "r"(bytes), "r"(smem_u32(bar))
+                 : "memory");
+}
+
 // 2-D tiled TMA store: smem -> box at (x, y); tracked by the issuing thread's bulk async-group
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *smem_src, int32_t x, int32_t y)
 {

@@ -517,14 +517,14 @@ static int remask(dspi_eq *e, cudaStream_t s)
     return DSPI_OK;
 }
 
-int eq_pack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s)
+int eq_pack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s, const RoleRange &rr)
 {
     if (n == 0) return DSPI_OK;
     CU_OK(cudaSetDevice(e->desc.device));
     if (e->desc.arith == DSPI_ARITH_Q28)
-        CU_OK(launch_pack_q28((const dspi_biquad_q28 *)e->d_aos, ch0, n, (int32_t *)e->d_coef, s));
+        CU_OK(launch_pack_q28((const dspi_biquad_q28 *)e->d_aos, ch0, n, (int32_t *)e->d_coef, s, rr));
     else
-        CU_OK(launch_pack_f32((const dspi_biquad_f32 *)e->d_aos, ch0, n, (float *)e->d_coef, e->d_modes, e->cpl, s));
+        CU_OK(launch_pack_f32((const dspi_biquad_f32 *)e->d_aos, ch0, n, (float *)e->d_coef, e->d_modes, e->cpl, s, rr));
     e->launches++;
     e->sig_dirty = true;
     int rc = remask(e, s);
@@ -533,14 +533,14 @@ int eq_pack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s)
     return DSPI_OK;
 }
 
-int eq_unpack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s)
+int eq_unpack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s, const RoleRange &rr)
 {
     if (n == 0) return DSPI_OK;
     CU_OK(cudaSetDevice(e->desc.device));
     if (e->desc.arith == DSPI_ARITH_Q28)
-        CU_OK(launch_unpack_q28((dspi_biquad_q28 *)e->d_aos, ch0, n, (const int32_t *)e->d_coef, s));
+        CU_OK(launch_unpack_q28((dspi_biquad_q28 *)e->d_aos, ch0, n, (const int32_t *)e->d_coef, s, rr));
     else
-        CU_OK(launch_unpack_f32((dspi_biquad_f32 *)e->d_aos, ch0, n, (const float *)e->d_coef, e->cpl, s));
+        CU_OK(launch_unpack_f32((dspi_biquad_f32 *)e->d_aos, ch0, n, (const float *)e->d_coef, e->cpl, s, rr));
     e->launches++;
     return DSPI_OK;
 }

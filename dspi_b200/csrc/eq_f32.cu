@@ -100,11 +100,11 @@ cudaError_t launch_eq_f32(const EqLaunch &a, bool fused, int cpl, cudaStream_t s
 // Biquad[n][12] (reference layout, AoS) <-> packed device store
 // ---------------------------------------------------------------------------------------
 __global__ void pack_f32_kernel(const dspi_biquad_f32 *__restrict__ aos, uint32_t ch0, uint32_t n, float *__restrict__ coef,
-                                uint64_t *__restrict__ modes, int cpl)
+                                uint64_t *__restrict__ modes, int cpl, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t ch = ch0 + i;
+    if (i >= n || (rr.reject && rr.reject[i])) return;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i;
     const uint32_t rows = 32 * cpl;
     const uint32_t g = ch / rows, r = ch % rows, lane = r & 31, h = r >> 5;
     uint64_t mw = 0;
@@ -129,11 +129,11 @@ __global__ void pack_f32_kernel(const dspi_biquad_f32 *__restrict__ aos, uint32_
     modes[(size_t)g * rows + h * 32 + lane] = mw;
 }
 
-__global__ void unpack_f32_kernel(dspi_biquad_f32 *__restrict__ aos, uint32_t ch0, uint32_t n, const float *__restrict__ coef, int cpl)
+__global__ void unpack_f32_kernel(dspi_biquad_f32 *__restrict__ aos, uint32_t ch0, uint32_t n, const float *__restrict__ coef, int cpl, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t ch = ch0 + i;
+    if (i >= n || (rr.reject && rr.reject[i])) return;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i;
     const uint32_t rows = 32 * cpl;
     const uint32_t g = ch / rows, r = ch % rows, lane = r & 31, h = r >> 5;
     for (int b = 0; b < kMaxBands; b++) {
@@ -146,10 +146,11 @@ __global__ void unpack_f32_kernel(dspi_biquad_f32 *__restrict__ aos, uint32_t ch
     }
 }
 
-cudaError_t launch_pack_f32(const dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, float *coef, uint64_t *modes, int cpl, cudaStream_t stream)
+cudaError_t launch_pack_f32(const dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, float *coef, uint64_t *modes, int cpl, cudaStream_t stream,
+                            const RoleRange &rr)
 {
     if (n == 0) return cudaSuccess;
-    pack_f32_kernel<<<(n + 127) / 128, 128, 0, stream>>>(aos, ch0, n, coef, modes, cpl);
+    pack_f32_kernel<<<dim3((n + 127) / 128, rr.roles), 128, 0, stream>>>(aos, ch0, n, coef, modes, cpl, rr);
     return cudaGetLastError();
 }
 __global__ void mask_modes_kernel(const uint64_t *__restrict__ raw, const uint8_t *__restrict__ skip, uint64_t *__restrict__ eff, uint32_t n)
@@ -163,10 +164,11 @@ cudaError_t launch_mask_modes(const uint64_t *raw, const uint8_t *skip, uint64_t
     mask_modes_kernel<<<(n + 255) / 256, 256, 0, stream>>>(raw, skip, eff, n);
     return cudaGetLastError();
 }
-cudaError_t launch_unpack_f32(dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, const float *coef, int cpl, cudaStream_t stream)
+cudaError_t launch_unpack_f32(dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, const float *coef, int cpl, cudaStream_t stream,
+                              const RoleRange &rr)
 {
     if (n == 0) return cudaSuccess;
-    unpack_f32_kernel<<<(n + 127) / 128, 128, 0, stream>>>(aos, ch0, n, coef, cpl);
+    unpack_f32_kernel<<<dim3((n + 127) / 128, rr.roles), 128, 0, stream>>>(aos, ch0, n, coef, cpl, rr);
     return cudaGetLastError();
 }
 

@@ -42,15 +42,26 @@ struct PerDeviceOnce {
 // per-thread message buffer behind dspi_last_error() (engine.cu)
 char *error_buffer(size_t *cap);
 
+// One launch over the same channel range of several roles: role r covers channels [ch0 + r * stride, ch0 + r * stride + n).
+// The chain engines keep role-major rows (channel = role * N_pad + instance), so an instance range is one such set.
+// reject[i] != 0 (device memory, [n], or nullptr) leaves channel i of every role untouched.  The default is one plain range.
+struct RoleRange {
+    uint32_t roles = 1, stride = 0;
+    const int32_t *reject = nullptr;
+};
+
 // K1 — float cascade.  cpl: channels per lane (1, or 2 held in a register pair)
 cudaError_t launch_eq_f32(const EqLaunch &a, bool fused, int cpl, cudaStream_t stream);
-cudaError_t launch_pack_f32(const dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, float *coef, uint64_t *modes, int cpl, cudaStream_t stream);
-cudaError_t launch_unpack_f32(dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, const float *coef, int cpl, cudaStream_t stream);
+cudaError_t launch_pack_f32(const dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, float *coef, uint64_t *modes, int cpl, cudaStream_t stream,
+                            const RoleRange &rr = RoleRange());
+cudaError_t launch_unpack_f32(dspi_biquad_f32 *aos, uint32_t ch0, uint32_t n, const float *coef, int cpl, cudaStream_t stream,
+                              const RoleRange &rr = RoleRange());
 
 // K2 — Q28 cascade (1 channel per lane)
 cudaError_t launch_eq_q28(const EqLaunch &a, cudaStream_t stream);
-cudaError_t launch_pack_q28(const dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, int32_t *coef, cudaStream_t stream);
-cudaError_t launch_unpack_q28(dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, const int32_t *coef, cudaStream_t stream);
+cudaError_t launch_pack_q28(const dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, int32_t *coef, cudaStream_t stream, const RoleRange &rr = RoleRange());
+cudaError_t launch_unpack_q28(dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, const int32_t *coef, cudaStream_t stream,
+                              const RoleRange &rr = RoleRange());
 
 }  // namespace dspi
 
@@ -59,8 +70,8 @@ cudaError_t launch_unpack_q28(dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, co
 struct dspi_eq;
 namespace dspi {
 void *eq_aos_mirror(dspi_eq *e);                                          // device Biquad[c_pad][12], reference layout
-int eq_pack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s);   // mirror -> packed store (coefficients and state), synchronous
-int eq_unpack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s); // packed store -> mirror (state), asynchronous on s
+int eq_pack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s, const RoleRange &rr = RoleRange());   // mirror -> packed store (coefficients and state), synchronous
+int eq_unpack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s, const RoleRange &rr = RoleRange()); // packed store -> mirror (state), asynchronous on s
 // rows with skip[ch] != 0 keep their whole cascade frozen (all bands treated as bypassed, state untouched):
 // usb_audio.c:721-728 (bypass_master_eq), :879-884 (muted / disabled outputs).  `d_skip` is [n_channels]
 // device memory owned by the caller; call again after changing it.
@@ -80,8 +91,10 @@ int eq_state_imported(dspi_eq *e, cudaStream_t s);
 int eq_geometry(const dspi_eq *e);
 size_t eq_state_bytes(const dspi_eq *e, int cpl);
 int eq_state_load(dspi_eq *e, const void *src, int cpl, cudaStream_t s);
-// coeff.cu: dsp_compute_coefficients() for channels [ch0, ch0 + n) of a mirror, recipes [n][12] on the device (clamped in place)
-cudaError_t launch_coeffs(bool q28, dspi_eq_param *d_recipes, void *d_aos, uint32_t ch0, uint32_t n, float fs, cudaStream_t stream);
+// coeff.cu: dsp_compute_coefficients() for channels [ch0, ch0 + n) of a mirror, recipes [n][12] on the device (clamped in place);
+// with a RoleRange, recipes [roles][n][12]
+cudaError_t launch_coeffs(bool q28, dspi_eq_param *d_recipes, void *d_aos, uint32_t ch0, uint32_t n, float fs, cudaStream_t stream,
+                          const RoleRange &rr = RoleRange());
 cudaError_t launch_skip_q28(int32_t *coef, const uint8_t *skip, uint32_t n, cudaStream_t stream);
 cudaError_t launch_mask_modes(const uint64_t *raw, const uint8_t *skip, uint64_t *eff, uint32_t n, cudaStream_t stream);
 // response.cu: frequency response of channels [ch0, ch0 + n) of a mirror (bands b < nb) at d_freq[nf] -> d_out [n][nf] float2

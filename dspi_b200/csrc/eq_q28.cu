@@ -276,11 +276,11 @@ cudaError_t launch_eq_q28(const EqLaunch &a, cudaStream_t stream)
     return sub == 4 ? launch_one<12, 4>(a, stream) : launch_one<12, 8>(a, stream);
 }
 
-__global__ void pack_q28_kernel(const dspi_biquad_q28 *__restrict__ aos, uint32_t ch0, uint32_t n, int32_t *__restrict__ coef)
+__global__ void pack_q28_kernel(const dspi_biquad_q28 *__restrict__ aos, uint32_t ch0, uint32_t n, int32_t *__restrict__ coef, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t ch = ch0 + i, g = ch / 32, lane = ch % 32;
+    if (i >= n || (rr.reject && rr.reject[i])) return;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i, g = ch / 32, lane = ch % 32;
     for (int b = 0; b < kMaxBands; b++) {
         const dspi_biquad_q28 &q = aos[(size_t)ch * kMaxBands + b];
         int32_t *dst = coef + ((size_t)g * kMaxBands + b) * kSlots * 32 + lane;
@@ -311,11 +311,11 @@ cudaError_t launch_skip_q28(int32_t *coef, const uint8_t *skip, uint32_t n, cuda
     return cudaGetLastError();
 }
 
-__global__ void unpack_q28_kernel(dspi_biquad_q28 *__restrict__ aos, uint32_t ch0, uint32_t n, const int32_t *__restrict__ coef)
+__global__ void unpack_q28_kernel(dspi_biquad_q28 *__restrict__ aos, uint32_t ch0, uint32_t n, const int32_t *__restrict__ coef, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t ch = ch0 + i, g = ch / 32, lane = ch % 32;
+    if (i >= n || (rr.reject && rr.reject[i])) return;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i, g = ch / 32, lane = ch % 32;
     for (int b = 0; b < kMaxBands; b++) {
         dspi_biquad_q28 &q = aos[(size_t)ch * kMaxBands + b];
         const int32_t *src = coef + ((size_t)g * kMaxBands + b) * kSlots * 32 + lane;
@@ -324,16 +324,16 @@ __global__ void unpack_q28_kernel(dspi_biquad_q28 *__restrict__ aos, uint32_t ch
     }
 }
 
-cudaError_t launch_pack_q28(const dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, int32_t *coef, cudaStream_t stream)
+cudaError_t launch_pack_q28(const dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, int32_t *coef, cudaStream_t stream, const RoleRange &rr)
 {
     if (n == 0) return cudaSuccess;
-    pack_q28_kernel<<<(n + 127) / 128, 128, 0, stream>>>(aos, ch0, n, coef);
+    pack_q28_kernel<<<dim3((n + 127) / 128, rr.roles), 128, 0, stream>>>(aos, ch0, n, coef, rr);
     return cudaGetLastError();
 }
-cudaError_t launch_unpack_q28(dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, const int32_t *coef, cudaStream_t stream)
+cudaError_t launch_unpack_q28(dspi_biquad_q28 *aos, uint32_t ch0, uint32_t n, const int32_t *coef, cudaStream_t stream, const RoleRange &rr)
 {
     if (n == 0) return cudaSuccess;
-    unpack_q28_kernel<<<(n + 127) / 128, 128, 0, stream>>>(aos, ch0, n, coef);
+    unpack_q28_kernel<<<dim3((n + 127) / 128, rr.roles), 128, 0, stream>>>(aos, ch0, n, coef, rr);
     return cudaGetLastError();
 }
 

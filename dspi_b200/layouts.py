@@ -171,3 +171,7 @@ DYNAMICS_CONFIG = np.dtype([
     ("lev_lookahead", "u1"), ("_p3", "u1", (3,)), ("lev_gate_threshold_db", "<f4"),
     ("loudness_ref_spl", "<f4"), ("loudness_intensity_pct", "<f4"), ("loudness_enabled", "u1"), ("host_mute", "u1"), ("volume_8_8", "<i2")])
 assert DYNAMICS_CONFIG.itemsize == 48
+
+# dspi_bulk_host (include/dspi_b200.h): audio_state of one device beside its bulk packet (apply_bulk_device)
+BULK_HOST = np.dtype([("volume_8_8", "<i2"), ("host_mute", "u1"), ("reserved", "u1")])
+assert BULK_HOST.itemsize == 4

@@ -541,6 +541,40 @@ int dspi_bulk_state_to_chain_f32(const dspi_bulk_state *st, float sample_rate, i
 int dspi_bulk_state_to_chain_q28(const dspi_bulk_state *st, float sample_rate, int16_t host_volume_8_8, int host_mute,
                                  dspi_chain_params_q28 *params, dspi_biquad_q28 biquads[7][DSPI_MAX_BANDS]);
 
+/* ---- bulk parameter ingest on the device (SURVEY.md 8 f-1) ------------------------------------- */
+/* audio_state of one device: the host volume and mute are USB audio-class controls, not part of the wire packet */
+typedef struct { int16_t volume_8_8; uint8_t host_mute; uint8_t reserved; } dspi_bulk_host;
+#ifdef __cplusplus
+static_assert(sizeof(dspi_bulk_host) == 4, "dspi_bulk_host");
+#else
+_Static_assert(sizeof(dspi_bulk_host) == 4, "dspi_bulk_host");
+#endif
+/* REQ_SET_ALL_PARAMS for instances [inst0, inst0+n) of a chain engine, from wire bytes to engine records ON THE GPU:
+ * packets[n], host[n] and results[n] are host memory.  Per instance this is bulk_params_apply() (bulk_params.c:178-377)
+ * followed by what the main loop derives from it (dsp_recalculate_all_filters, dsp_update_delay_samples, the crossfeed /
+ * leveller / loudness handlers, audio_set_volume), i.e. dspi_bulk_params_apply + dspi_bulk_state_to_chain_* +
+ * dspi_chain(q)_set_params + _upload_biquads, except that
+ *   - results[i] is the firmware's code (0, -1 .. -4; the platform and the channel counts are the engine's shape) and a
+ *     rejected packet changes nothing of its instance - the firmware returns before its first write.  The call still
+ *     returns DSPI_OK;
+ *   - below format version 6 the master volume in force stays (the packet has none); the preamp comes from the legacy field;
+ *   - EQ filter state is kept unless a band's topology flips, as dsp_compute_coefficients does; the crossfeed filter state
+ *     is ALWAYS cleared, as crossfeed_compute_coefficients() does after a bulk apply (the rule of _set_dynamics_device).
+ *     The host route through _set_params differs in this one point: it keeps that state when the coefficients did not change;
+ *   - leveller, loudness-shelf, delay-line and modulator state, the meters, the preset-mute gain and envelope mode and the
+ *     S/PDIF transmitter state are left alone.
+ * Gains go through the firmware's Taylor db_to_linear (exact 0 dB -> 1.0, clamped to [-60, +20] dB) unless exact_db != 0
+ * (then 10^(dB/20)); the master volume always uses the exact conversion.  Arithmetic and libm policy as
+ * dspi_eq_set_params_device: coefficients are the oracle's policy coefficients bit for bit and within the documented libm
+ * distance of the host route's.  Ordered behind process calls issued earlier on the engine stream; returns when the engine
+ * is reconfigured.  DSPI_EINVAL for a NULL pointer or a sample_rate that is not positive and finite, DSPI_ERANGE for a
+ * range past the end of the engine; nothing is written then.  Preset images take the same route:
+ * dspi_preset_slot_apply -> dspi_bulk_params_collect -> this call with exact_db = 1. */
+int dspi_chain_apply_bulk_device (dspi_chain *c,  uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
+                                  int exact_db, float sample_rate, int32_t *results);
+int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
+                                  int exact_db, float sample_rate, int32_t *results);
+
 /* ---- preset slot images (SURVEY.md 8 f-4): PresetSlot v12, flash_storage.c:139-189 ------------ */
 /* One flash sector per slot: 12-byte header (magic "DSP3", data version, slot index, CRC-32 of everything
  * after the header) + the packed DSP state.  Device preset dumps load directly into a dspi_bulk_state and
