@@ -1380,7 +1380,10 @@ static int process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uin
     const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 2 * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
     if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
     if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
-    if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream)); }
+    if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; }
+    // the modulator writes the rows of instances with a sub only; the others go back to the caller as zeros, on every call
+    // (an earlier call's bits would be there otherwise: a sub switched off since, or a longer call's [N][F][8] layout)
+    if (pdm_out) CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream));
     CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
     rc = process_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
                         pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);

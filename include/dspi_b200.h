@@ -366,8 +366,9 @@ int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len);
  *   pcm:       [n_instances][n_packets * frames_per_packet] interleaved L,R little-endian frames,
  *              bit_depth 16 (4 bytes / frame) or 24 (packed, 6 bytes / frame)      (HOST memory)
  *   spdif_out: [n_instances][4][n_frames][2] int32 - the four pico_audio producer buffers
- *   pdm_out:   [n_instances][n_frames][8] uint32 - 256 PDM bits per frame, MSB first (written only
- *              for instances whose sub output is enabled)
+ *   pdm_out:   [n_instances][n_frames][8] uint32 - 256 PDM bits per frame, MSB first; the rows of
+ *              instances whose sub output is disabled are zero.  The _device forms write the rows of
+ *              instances with the sub enabled only and leave the others as the caller left them.
  *   status:    [n_instances], peaks of the LAST packet, clip flags OR-ed in (sticky)
  * Any of the three outputs may be NULL. */
 int dspi_chain_process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t frames_per_packet,
