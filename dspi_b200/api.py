@@ -46,6 +46,7 @@ SYMBOLS = [
     "dspi_eq_response_host", "dspi_eq_response_device", "dspi_chain_response_host", "dspi_chain_response_device",
     "dspi_chainq_response_host", "dspi_chainq_response_device",
     "dspi_chain_apply_bulk_device", "dspi_chainq_apply_bulk_device",
+    "dspi_chain_collect_bulk_device", "dspi_chainq_collect_bulk_device",
 ]
 
 
@@ -143,6 +144,7 @@ def lib():
             getattr(h, pre + "_set_dynamics_device").argtypes = [vp, u32, u32, vp, C.c_float]
             getattr(h, pre + "_sm_partition").argtypes = [vp, vp, vp]
             getattr(h, pre + "_apply_bulk_device").argtypes = [vp, u32, u32, vp, vp, C.c_int, C.c_float, vp]
+            getattr(h, pre + "_collect_bulk_device").argtypes = [vp, u32, u32, vp, vp, vp]
             getattr(h, pre + "_process_packets_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_process_packets_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_set_spdif_tx").argtypes = [vp, u32, u32, vp]
@@ -404,7 +406,7 @@ def bind_host_to_device(device):
 class _ChainSpdif:
     """What both chain engines share: each instance's S/PDIF transmitter (block position + channel status) and the
     process form whose output stage writes S/PDIF subframes (``*_spdif_tx``, ``*_process_subframes_*``), and the ingest of
-    ``WireBulkParams`` packets on the GPU (``*_apply_bulk_device``)."""
+    ``WireBulkParams`` packets on the GPU (``*_apply_bulk_device``) and their read-back (``*_collect_bulk_device``)."""
 
     def apply_bulk_device(self, packets, fs, inst0=0, host=None, exact_db=False):
         """WIRE_BULK [n] -> instances [inst0, inst0+n) reconfigured on the GPU as ``bulk_params_apply`` and the firmware's main
@@ -419,6 +421,17 @@ class _ChainSpdif:
                                                                 hv.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
                                                                 res.ctypes.data_as(C.c_void_p)))
         return res
+
+    def collect_bulk_device(self, inst0=0, n=None):
+        """``REQ_GET_ALL_PARAMS`` for instances [inst0, inst0+n) (default: to the end) from the engine's configuration records:
+        (WIRE_BULK [n], BULK_HOST [n], int32 [n] of ``layouts.BULK_CURRENT`` / ``BULK_STALE`` / ``BULK_UNSET``).  A current or
+        stale packet is what ``bulk_params_collect`` returns for the host state the same calls would have left; an unset
+        instance gives zero bytes."""
+        n = self.n_instances - int(inst0) if n is None else int(n)
+        w, hv, res = np.zeros(max(n, 0), L.WIRE_BULK), np.zeros(max(n, 0), L.BULK_HOST), np.zeros(max(n, 0), np.int32)
+        _check(getattr(lib(), self._PRE + "_collect_bulk_device")(self._h, int(inst0), n, w.ctypes.data_as(C.c_void_p),
+                                                                  hv.ctypes.data_as(C.c_void_p), res.ctypes.data_as(C.c_void_p)))
+        return w, hv, res
 
     def set_spdif_tx(self, block_pos, channel_status, inst0=0):
         """Transmitter state of instances [inst0, inst0+n): ``block_pos`` an int or [n] (0..191), ``channel_status`` 5 bytes

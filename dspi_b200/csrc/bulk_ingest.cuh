@@ -12,6 +12,13 @@
 //   lane 0 crossfeed, lane 1 leveller, lane 2 host volume + the loudness row it selects, then lane 0 the output gains
 //   all lanes             the 12 x roles recipes, 16 bytes each, into the role-major recipe buffer [role][n][12]
 // The recipes then go through the coefficient kernels of coeff.cu, one launch per sub-engine over all its roles (RoleRange).
+//
+// The way back (REQ_GET_ALL_PARAMS, bulk_params_collect() bulk_params.c:62-172): every instance has a Record, the body of the
+// packet bulk_params_collect() would return for it.  The ingest warp rewrites its shared-memory copy of an accepted packet
+// into that body (record_body) and sends it out with one bulk store; record_recipes_kernel then replaces the eq section by the
+// recipes as the coefficient kernels left them (clamps written back, dsp_pipeline.c:78-81); the dynamics kernels edit their
+// fields (record_dynamics).  bulk_collect_kernel, one warp per instance again, brings the record in with a bulk copy, stamps
+// the constant header and pin count, and sends it to the staging buffer with a bulk store.
 // The engine-specific stores (float or Q28 / Q15) are the engine's ParamStores, the same functions its dynamics kernel uses.
 //
 // Same arithmetic rules as coeff.cu / dynamics.cuh: every float operation is the reference's, rounded on its own
@@ -52,6 +59,13 @@ static_assert(kPacketBytes % 16 == 0, "the bulk copy moves multiples of 16 bytes
 
 #define DSPI_WIRE_OFF(member) ((uint32_t)offsetof(dspi_wire_bulk_params, member))
 
+// The wire-visible configuration of every instance, in device memory for the life of the engine.  Not part of the state blob.
+struct Record {
+    dspi_wire_bulk_params *packets = nullptr;              // [N_pad] packet body; header and pins are stamped by the collect kernel
+    dspi_bulk_host *host = nullptr;                        // [N_pad] the host volume and mute last given
+    uint8_t *mark = nullptr;                               // [N_pad] DSPI_BULK_CURRENT / _STALE / _UNSET
+};
+
 // bulk_params.c:49-56 — the firmware's own conversion: 4-term Taylor series of exp(), clamped
 __device__ inline float db_to_linear_fw(float db)
 {
@@ -77,9 +91,71 @@ __device__ inline int32_t validate(const unsigned char *w, int platform_id, int 
     return 0;
 }
 
+// An accepted packet -> the body of the packet bulk_params_collect() returns once it is applied, in place in the warp's
+// shared-memory copy `w`: flags as 0 / 1, the preamp fields from whichever the version makes valid (:206-215, :351-359),
+// channel_delays_ms overwritten by the output delays (:242-244, :261), the leveller defaults below version 4 (:330-346),
+// rows past NC channels / NO outputs, control-plane sections and reserved bytes zero.  `master_volume_bits` is the value in
+// force after the apply.  Every word has one lane; the two cross-field copies are read before any lane writes.
+template <int NC, int NO>
+__device__ inline void record_body(unsigned char *w, int lane, uint32_t version, uint32_t master_volume_bits)
+{
+    static_assert(NC == NO + 2, "outputs are channels CH_OUT_1 = 2 onwards (config.h:310)");
+    uint32_t *W = reinterpret_cast<uint32_t *>(w);
+    constexpr uint32_t g = DSPI_WIRE_OFF(global) / 4, x = DSPI_WIRE_OFF(crossfeed) / 4, lg = DSPI_WIRE_OFF(legacy) / 4, dl = DSPI_WIRE_OFF(delays) / 4,
+                       xp = DSPI_WIRE_OFF(crosspoints) / 4, out = DSPI_WIRE_OFF(outputs) / 4, eq = DSPI_WIRE_OFF(eq) / 4,
+                       names = DSPI_WIRE_OFF(channel_names) / 4, lev = DSPI_WIRE_OFF(leveller) / 4, pre = DSPI_WIRE_OFF(preamp) / 4;
+    const uint32_t pre0 = version >= 6 ? W[pre] : W[g], pre1 = version >= 6 ? W[pre + 1] : W[g];
+    uint32_t delay = 0;
+    if (lane < NC) delay = lane >= 2 ? W[out + (lane - 2) * 3 + 2] : W[dl + lane];
+    __syncwarp();
+    auto flag = [](uint32_t word, int byte) { return ((word >> (8 * byte)) & 0xFFu) ? 1u << (8 * byte) : 0u; };
+    if (lane == 0) {
+        W[0] = W[1] = W[2] = W[3] = 0;
+        W[DSPI_WIRE_OFF(pins) / 4] = W[DSPI_WIRE_OFF(pins) / 4 + 1] = 0;
+    } else if (lane == 1) {
+        W[g] = pre0;
+        W[g + 1] = flag(W[g + 1], 0) | flag(W[g + 1], 1);
+    } else if (lane == 2) {
+        W[x] = flag(W[x], 0) | (W[x] & 0xFF00u) | flag(W[x], 2);
+        W[x + 3] = 0;
+    } else if (lane == 3) {
+        W[lg + 3] = flag(W[lg + 3], 0) | flag(W[lg + 3], 1) | flag(W[lg + 3], 2);
+    } else if (lane == 4) {
+        if (version >= 4) {
+            W[lev] = flag(W[lev], 0) | (W[lev] & 0xFF00u) | flag(W[lev], 2);
+        } else {
+            W[lev] = 1u << 16;
+            W[lev + 1] = __float_as_uint(50.0f);
+            W[lev + 2] = __float_as_uint(15.0f);
+            W[lev + 3] = __float_as_uint(-96.0f);
+        }
+    } else if (lane == 5) {
+        W[pre] = pre0;
+        W[pre + 1] = pre1;
+        W[pre + 2] = W[pre + 3] = 0;
+    } else if (lane == 6) {
+        W[pre + 4] = master_volume_bits;
+        W[pre + 5] = W[pre + 6] = W[pre + 7] = 0;
+    }
+    if (lane < DSPI_WIRE_MAX_CHANNELS) W[dl + lane] = delay;
+    if (lane < 2 * DSPI_WIRE_MAX_OUTPUTS) {
+        if (lane % DSPI_WIRE_MAX_OUTPUTS < NO) W[xp + lane * 2] &= 0xFFFFu;
+        else W[xp + lane * 2] = W[xp + lane * 2 + 1] = 0;
+    }
+    if (lane < DSPI_WIRE_MAX_OUTPUTS) {
+        if (lane < NO) W[out + lane * 3] &= 0xFFFFu;
+        else W[out + lane * 3] = W[out + lane * 3 + 1] = W[out + lane * 3 + 2] = 0;
+    }
+    for (uint32_t r = lane; r < DSPI_WIRE_MAX_CHANNELS * kMaxBands; r += 32) {
+        if (r / kMaxBands < NC) W[eq + r * 4] &= 0xFFu;
+        else reinterpret_cast<uint4 *>(W + eq)[r] = make_uint4(0, 0, 0, 0);
+    }
+    for (uint32_t k = names + lane; k < lev; k += 32) W[k] = 0;                                    // channel names and the I2S section: control plane
+}
+
 template <class S>
 __global__ void __launch_bounds__(kWarps * 32)
-bulk_ingest_kernel(typename S::Dev d, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *__restrict__ packets,
+bulk_ingest_kernel(typename S::Dev d, Record rec, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *__restrict__ packets,
                    const dspi_bulk_host *__restrict__ host, int exact_db, float fs, dspi_eq_param *__restrict__ recipes, int32_t *__restrict__ results)
 {
     constexpr int O = S::kOuts, WO = DSPI_WIRE_MAX_OUTPUTS;
@@ -188,6 +264,114 @@ bulk_ingest_kernel(typename S::Dev d, uint32_t inst0, uint32_t n, const dspi_wir
         q.x = role | b << 8 | (q.x & 0xFFu) << 16;                                                 // {channel, band, type, reserved}
         reinterpret_cast<uint4 *>(recipes)[((size_t)role * n + i) * kMaxBands + b] = q;
     }
+
+    // ---- the record: what bulk_params_collect() reads after this apply.  Below version 6 the master volume in force stays ----
+    unsigned char *rp = reinterpret_cast<unsigned char *>(rec.packets + inst);
+    const float mv_db = __shfl_sync(0xffffffffu, db, 3 * O + 2);                                   // finite, clamped to [-128, 0] (:361-368)
+    const uint32_t mv_bits = version >= 6 ? __float_as_uint(mv_db) : *reinterpret_cast<const uint32_t *>(rp + DSPI_WIRE_OFF(master_volume));
+    record_body<S::kRoles, O>(pkt_s[warp], lane, version, mv_bits);
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+        bulk_store_1d(rp, pkt_s[warp], kPacketBytes);
+        tma_store_commit();
+        rec.mark[inst] = DSPI_BULK_CURRENT;
+        tma_store_wait_all<0>();
+    } else if (lane == 1) {
+        rec.host[inst] = hv;
+    }
+}
+
+// filter_recipes[][] of instances [inst0, inst0 + n) as dsp_compute_coefficients() left them -> the eq section of their records.
+// Recipe (role, i, band) is recipes[role * role_stride + i * inst_stride + band]; reject as in RoleRange.
+static __global__ void record_recipes_kernel(Record rec, uint32_t inst0, uint32_t n, uint32_t roles, const dspi_eq_param *__restrict__ recipes,
+                                             size_t role_stride, size_t inst_stride, const int32_t *__restrict__ reject)
+{
+    const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n * roles * kMaxBands) return;
+    const uint32_t b = idx % kMaxBands, role = idx / kMaxBands % roles, i = idx / (kMaxBands * roles);
+    if (reject && reject[i]) return;
+    uint4 q = reinterpret_cast<const uint4 *>(recipes)[role * role_stride + i * inst_stride + b];
+    q.x = (q.x >> 16) & 0xFFu;                                                                     // {channel, band, type, reserved} -> {type, reserved[3]}
+    unsigned char *rp = reinterpret_cast<unsigned char *>(rec.packets + inst0 + i);
+    reinterpret_cast<uint4 *>(rp + DSPI_WIRE_OFF(eq))[role * kMaxBands + b] = q;
+}
+
+// dspi_chain(q)_set_params / _upload_biquads replaced records the packet does not describe any more
+static __global__ void mark_stale_kernel(Record rec, uint32_t inst0, uint32_t n)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && rec.mark[inst0 + i] == DSPI_BULK_CURRENT) rec.mark[inst0 + i] = DSPI_BULK_STALE;
+}
+inline cudaError_t mark_stale(const Record &rec, uint32_t inst0, uint32_t n, cudaStream_t s)
+{
+    mark_stale_kernel<<<(n + 255) / 256, 256, 0, s>>>(rec, inst0, n);
+    return cudaGetLastError();
+}
+
+// What dspi_chain(q)_set_dynamics_device changes of the firmware's globals: crossfeed_config, leveller_config, the loudness
+// settings and audio_state's volume and mute.  One instance per thread, from the engine's dynamics kernel.
+__device__ inline void record_dynamics(const Record &rec, uint32_t inst, const dspi_dynamics_config &cfg)
+{
+    unsigned char *rp = reinterpret_cast<unsigned char *>(rec.packets + inst);
+    auto put = [&](uint32_t off, uint32_t v) { *reinterpret_cast<uint32_t *>(rp + off) = v; };
+    rp[DSPI_WIRE_OFF(global.loudness_enabled)] = cfg.loudness_enabled ? 1 : 0;
+    put(DSPI_WIRE_OFF(global.loudness_ref_spl), __float_as_uint(cfg.loudness_ref_spl));
+    put(DSPI_WIRE_OFF(global.loudness_intensity_pct), __float_as_uint(cfg.loudness_intensity_pct));
+    put(DSPI_WIRE_OFF(crossfeed), (cfg.crossfeed.enabled ? 1u : 0u) | (uint32_t)cfg.crossfeed.preset << 8 | (cfg.crossfeed.itd_enabled ? 1u : 0u) << 16);
+    put(DSPI_WIRE_OFF(crossfeed.custom_fc), __float_as_uint(cfg.crossfeed.custom_fc));
+    put(DSPI_WIRE_OFF(crossfeed.custom_feed_db), __float_as_uint(cfg.crossfeed.custom_feed_db));
+    put(DSPI_WIRE_OFF(leveller), (cfg.leveller.enabled ? 1u : 0u) | (uint32_t)cfg.leveller.speed << 8 | (cfg.leveller.lookahead ? 1u : 0u) << 16);
+    put(DSPI_WIRE_OFF(leveller.amount), __float_as_uint(cfg.leveller.amount));
+    put(DSPI_WIRE_OFF(leveller.max_gain_db), __float_as_uint(cfg.leveller.max_gain_db));
+    put(DSPI_WIRE_OFF(leveller.gate_threshold_db), __float_as_uint(cfg.leveller.gate_threshold_db));
+    rec.host[inst].volume_8_8 = cfg.volume_8_8;
+    rec.host[inst].host_mute = cfg.host_mute;
+}
+
+// REQ_GET_ALL_PARAMS: record -> the packet bulk_params_collect() returns (:66-78 header, :123 pin count), one warp per instance
+template <class S>
+__global__ void __launch_bounds__(kWarps * 32)
+bulk_collect_kernel(Record rec, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *__restrict__ packets, dspi_bulk_host *__restrict__ host,
+                    int32_t *__restrict__ results)
+{
+    __shared__ alignas(16) unsigned char pkt_s[kWarps][kPacketBytes];
+    __shared__ uint64_t bar_s[kWarps];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t i = blockIdx.x * kWarps + warp;
+    if (i >= n) return;
+    const uint32_t inst = inst0 + i;
+    uint64_t *bar = &bar_s[warp];
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        fence_mbar_init();
+        mbar_arrive_expect_tx(bar, kPacketBytes);
+        bulk_load_1d(pkt_s[warp], rec.packets + inst, kPacketBytes, bar);
+    }
+    __syncwarp();
+    const uint8_t mark = rec.mark[inst];
+    mbar_wait(bar, 0);
+    uint32_t *W = reinterpret_cast<uint32_t *>(pkt_s[warp]);
+    if (mark == DSPI_BULK_UNSET) {                         // whatever set_eq_params_device / set_dynamics_device noted: not a configuration yet
+        for (uint32_t k = lane; k < kPacketBytes / 16; k += 32) reinterpret_cast<uint4 *>(W)[k] = make_uint4(0, 0, 0, 0);
+    } else if (lane == 0) {
+        W[0] = DSPI_WIRE_FORMAT_VERSION | (uint32_t)S::kPlatformId << 8 | (uint32_t)S::kRoles << 16 | (uint32_t)S::kOuts << 24;
+        W[1] = 2u | (uint32_t)kMaxBands << 8 | kPacketBytes << 16;                                 // inputs, max_bands, payload_length
+        W[2] = 1u | 1u << 16;                                                                      // firmware 1.1, config.h:273-274
+        W[3] = 0;
+        W[DSPI_WIRE_OFF(pins) / 4] = S::kPlatformId ? 5u : 3u;
+        W[DSPI_WIRE_OFF(pins) / 4 + 1] = 0;
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+        bulk_store_1d(packets + i, pkt_s[warp], kPacketBytes);
+        tma_store_commit();
+        results[i] = mark;
+        tma_store_wait_all<0>();
+    } else if (lane == 1) {
+        host[i] = mark == DSPI_BULK_UNSET ? dspi_bulk_host{0, 0, 0} : rec.host[inst];
+    }
 }
 
 // engine-owned staging of one chunk: packets, host volumes, recipes and result codes on the device
@@ -236,7 +420,7 @@ int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_b
         e = cudaMemcpyAsync(stage.packets, packets + i0, (size_t)nc * kPacketBytes, cudaMemcpyHostToDevice, s);
         if (e == cudaSuccess) e = cudaMemcpyAsync(stage.host, host + i0, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyHostToDevice, s);
         if (e != cudaSuccess) return fail_cuda(e, "packet copy");
-        bulk_ingest_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, first, nc, stage.packets, stage.host, exact_db, fs,
+        bulk_ingest_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.packets, stage.host, exact_db, fs,
                                                                                  stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "ingest kernel");
         c->launches++;
@@ -251,7 +435,10 @@ int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_b
         e = launch_coeffs(S::kQ28, stage.recipes, eq_aos_mirror(c->eq_m), first, nc, fs, s, rm);
         if (e == cudaSuccess) e = launch_coeffs(S::kQ28, stage.recipes + (size_t)2 * nc * kMaxBands, eq_aos_mirror(c->eq_o), first, nc, fs, s, ro);
         if (e != cudaSuccess) return fail_cuda(e, "coefficient kernels");
-        c->launches += 2;
+        record_recipes_kernel<<<(nc * S::kRoles * kMaxBands + 255) / 256, 256, 0, s>>>(c->rec, first, nc, S::kRoles, stage.recipes,
+                                                                                       (size_t)nc * kMaxBands, kMaxBands, stage.results);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "recipe record kernel");
+        c->launches += 3;
         rc = eq_pack_range(c->eq_m, first, nc, s, rm);
         if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, first, nc, s, ro);
         if (rc != DSPI_OK) return rc;
@@ -261,6 +448,47 @@ int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_b
     int rc = eq_set_skip(c->eq_m, c->d.skip_m, s);
     if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, s);
     return rc;
+}
+
+// The clamped recipes dspi_chain(q)_set_eq_params_device hands back ([n][roles][12], host memory) -> the records, on the
+// engine stream; returns when they are there.
+template <class S, class Engine>
+int record_recipes(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_eq_param *recipes)
+{
+    cudaError_t e = stage.ensure(S::kRoles);
+    if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
+    constexpr uint32_t per = S::kRoles * kMaxBands;
+    for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
+        const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;
+        e = cudaMemcpyAsync(stage.recipes, recipes + (size_t)i0 * per, (size_t)nc * per * sizeof(dspi_eq_param), cudaMemcpyHostToDevice, c->stream);
+        if (e != cudaSuccess) return fail_cuda(e, "recipe copy");
+        record_recipes_kernel<<<(nc * per + 255) / 256, 256, 0, c->stream>>>(c->rec, inst0 + i0, nc, S::kRoles, stage.recipes, kMaxBands, per, nullptr);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "recipe record kernel");
+        c->launches++;
+    }
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return fail_cuda(e, "recipe record");
+    return DSPI_OK;
+}
+
+// dspi_chain(q)_collect_bulk_device for checked arguments: on the engine stream, behind everything issued before; reads only.
+template <class S, class Engine>
+int collect(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
+{
+    cudaError_t e = stage.ensure(S::kRoles);
+    if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
+    cudaStream_t s = c->stream;
+    for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
+        const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;
+        bulk_collect_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->rec, inst0 + i0, nc, stage.packets, stage.host, stage.results);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "collect kernel");
+        c->launches++;
+        e = cudaMemcpyAsync(packets + i0, stage.packets, (size_t)nc * kPacketBytes, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess && host) e = cudaMemcpyAsync(host + i0, stage.host, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess && results) e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+        if (e != cudaSuccess) return fail_cuda(e, "packet copy");
+    }
+    if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return fail_cuda(e, "collect");
+    return DSPI_OK;
 }
 
 }  // namespace bulk

@@ -504,7 +504,7 @@ struct ParamStores {
 };
 
 // Mass reconfiguration of the dynamics stages on the device (SURVEY f-1), RP2040 stores: see chain_f32.cu
-__global__ void chainq_dynamics_kernel(ChainQ d, uint32_t inst0, uint32_t n, const dspi_dynamics_config *__restrict__ cfgs, float fs)
+__global__ void chainq_dynamics_kernel(ChainQ d, bulk::Record rec, uint32_t inst0, uint32_t n, const dspi_dynamics_config *__restrict__ cfgs, float fs)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -522,6 +522,7 @@ __global__ void chainq_dynamics_kernel(ChainQ d, uint32_t inst0, uint32_t n, con
     if (cfg.loudness_enabled) flags |= F_LOUD;
     d.flags[inst] = flags;
     ParamStores::host_volume(d, inst, vol_mul, cfg.host_mute != 0);
+    bulk::record_dynamics(rec, inst, cfg);
 }
 
 __device__ __forceinline__ int32_t outq_gain(int32_t v, bool enabled, int32_t gain)
@@ -851,7 +852,8 @@ struct dspi_chainq {
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     dspi::PacketSchedule sched;      // packet lengths of the current call
     dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chainq_response_*
-    dspi::bulk::Stage bulk;          // device staging of dspi_chainq_apply_bulk_device, allocated by its first call
+    dspi::bulk::Stage bulk;          // device staging of dspi_chainq_apply_bulk_device / _collect_bulk_device, allocated by the first call
+    dspi::bulk::Record rec;          // wire-visible configuration of every instance (dspi_chainq_collect_bulk_device); not part of the state blob
 };
 
 namespace {
@@ -1008,6 +1010,10 @@ int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
     TRY(dev_alloc(c, &d.pmg, Np));
     TRY(dev_alloc(c, &c->tx.bp, Np));
     TRY(dev_alloc(c, &c->tx.cs40, Np));
+    TRY(dev_alloc(c, &c->rec.packets, Np));
+    TRY(dev_alloc(c, &c->rec.host, Np));
+    TRY(dev_alloc(c, &c->rec.mark, Np));
+    TRY(cudaMemsetAsync(c->rec.mark, DSPI_BULK_UNSET, Np, c->stream));
     TRY(init_states(c));
     TRY(init_spdif_tx(c));
 #undef TRY
@@ -1115,6 +1121,7 @@ int dspi_chainq_set_params(dspi_chainq *c, uint32_t inst0, uint32_t n, const dsp
     CU_OK(put(d.o_flags, oflags.data(), O, 1));
     CU_OK(put(d.o_dly, dly.data(), O, 4));
     CU_OK(put(d.skip_m, skip_m.data(), 2, 1));
+    CU_OK(dspi::bulk::mark_stale(c->rec, inst0, n, c->stream));
     CU_OK(put(d.skip_o, skip_o.data(), O, 1));
     CU_OK(cudaStreamSynchronize(c->stream));
     int rc = dspi::eq_set_skip(c->eq_m, d.skip_m, c->stream);
@@ -1180,7 +1187,7 @@ int dspi_chainq_set_dynamics_device(dspi_chainq *c, uint32_t inst0, uint32_t n, 
     CU_OK(cudaMalloc((void **)&d_cfg, (size_t)n * sizeof(*cfgs)));
     cudaError_t e = cudaMemcpyAsync(d_cfg, cfgs, (size_t)n * sizeof(*cfgs), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) {
-        dspi::chainq_dynamics_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, inst0, n, d_cfg, sample_rate);
+        dspi::chainq_dynamics_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, c->rec, inst0, n, d_cfg, sample_rate);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -1201,6 +1208,15 @@ int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, co
     return dspi::bulk::apply<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, exact_db, sample_rate, results);
 }
 
+int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
+{
+    if (!c || !packets) return fail(DSPI_EINVAL, "null argument");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return dspi::bulk::collect<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, results);
+}
+
 int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_biquad_q28 *biquads)
 {
     if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
@@ -1219,6 +1235,7 @@ int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const
                           : dspi::eq_pack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
         if (rc) return rc;
     }
+    CU_OK(dspi::bulk::mark_stale(c->rec, inst0, n, c->stream));
     CU_OK(cudaStreamSynchronize(c->stream));
     return DSPI_OK;
 }
@@ -1243,7 +1260,7 @@ int dspi_chainq_set_eq_params_device(dspi_chainq *c, uint32_t inst0, uint32_t n,
         for (uint32_t i = 0; i < n; i++)                            // the clamps, written back like the reference does
             memcpy(&recipes[((size_t)i * dspi::kRoles + role) * DSPI_MAX_BANDS], &tmp[(size_t)i * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
     }
-    return DSPI_OK;
+    return dspi::bulk::record_recipes<dspi::ParamStores>(c, c->bulk, inst0, n, recipes);
 }
 
 int dspi_chainq_download_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_biquad_q28 *biquads)

@@ -76,6 +76,12 @@ __device__ __forceinline__ void bulk_load_1d(void *smem_dst, const void *gsrc, u
                  : "memory");
 }
 
+// 1-D bulk store: `bytes` contiguous bytes smem -> global, tracked by the issuing thread's bulk async-group.  Same multiples of 16.
+__device__ __forceinline__ void bulk_store_1d(void *gdst, const void *smem_src, uint32_t bytes)
+{
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
+}
+
 // 2-D tiled TMA store: smem -> box at (x, y); tracked by the issuing thread's bulk async-group
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *smem_src, int32_t x, int32_t y)
 {

@@ -175,3 +175,5 @@ assert DYNAMICS_CONFIG.itemsize == 48
 # dspi_bulk_host (include/dspi_b200.h): audio_state of one device beside its bulk packet (apply_bulk_device)
 BULK_HOST = np.dtype([("volume_8_8", "<i2"), ("host_mute", "u1"), ("reserved", "u1")])
 assert BULK_HOST.itemsize == 4
+# DSPI_BULK_*: what collect_bulk_device says of each instance's packet
+BULK_CURRENT, BULK_STALE, BULK_UNSET = 0, 1, 2

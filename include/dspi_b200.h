@@ -576,6 +576,39 @@ int dspi_chain_apply_bulk_device (dspi_chain *c,  uint32_t inst0, uint32_t n, co
 int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
                                   int exact_db, float sample_rate, int32_t *results);
 
+/* REQ_GET_ALL_PARAMS for instances [inst0, inst0+n) of a chain engine: what bulk_params_collect() (bulk_params.c:62-172)
+ * would read from the firmware's globals, from a configuration record the engine keeps per instance in device memory.
+ * packets[n], host[n] and results[n] are host memory; host and results may be NULL.  results[i] is one of */
+#define DSPI_BULK_CURRENT 0   /* the packet describes what the instance runs                       */
+#define DSPI_BULK_STALE   1   /* records were replaced by set_params / upload_biquads since         */
+#define DSPI_BULK_UNSET   2   /* never configured through a wire packet: packet bytes are all zero  */
+/* For a current or stale instance packets[i] is byte for byte what dspi_bulk_params_collect returns for the dspi_bulk_state
+ * the same sequence of calls would have left on the host: format version 6, the engine's platform id and channel counts,
+ * the full payload length, firmware version 1.1, pins.num_pin_outputs 5 or 3, everything else of the pins / names / I2S
+ * sections and all reserved bytes zero, rows past the shape's channel and output counts zero.  host[i] is the
+ * dspi_bulk_host the instance was last given.  Who writes the record:
+ *   - _apply_bulk_device: for an accepted packet exactly what bulk_params_apply() writes, under its version gates (legacy
+ *     preamp field first, leveller fields from version 4 and the fixed defaults below, per-side preamp and master volume
+ *     from version 6 - below 6 the master volume in force stays -, the master volume made finite and clamped to
+ *     [-128, 0] dB, channel_delays_ms overwritten by the output delays), then the recipes with the clamps
+ *     dsp_compute_coefficients() writes back (dsp_pipeline.c:78-81), as a GET_ALL_PARAMS after a SET_ALL_PARAMS shows
+ *     them.  The instance becomes DSPI_BULK_CURRENT.  A rejected packet leaves record and mark alone;
+ *   - _set_eq_params_device: the clamped recipes; _set_dynamics_device: the crossfeed, leveller and loudness fields and
+ *     the host volume / mute.  Both keep the mark the instance has;
+ *   - _set_params and _upload_biquads take derived records (linear gains, coefficients) that dB values and recipes cannot
+ *     be recovered from: they leave the record alone and turn a current instance DSPI_BULK_STALE.  An instance that never
+ *     had an accepted packet stays DSPI_BULK_UNSET whatever else it was given, and collects zero bytes and a zero host
+ *     record.
+ * The record is not part of the state blob, and _reset_state leaves it alone.  The call is ordered behind everything issued
+ * earlier on the engine stream, asynchronous process calls included, returns when the packets are in the caller's memory,
+ * and changes nothing a process call reads.  DSPI_EINVAL for a NULL engine or packets, DSPI_ERANGE for a range past the
+ * end of the engine (also one whose end wraps in 32 bits); nothing is written then.  n == 0 does nothing.
+ * The route to a preset image: this call -> dspi_bulk_params_apply(packet, st, exact_db = 1) -> dspi_preset_slot_collect. */
+int dspi_chain_collect_bulk_device (dspi_chain *c,  uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host,
+                                    int32_t *results);
+int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host,
+                                    int32_t *results);
+
 /* ---- preset slot images (SURVEY.md 8 f-4): PresetSlot v12, flash_storage.c:139-189 ------------ */
 /* One flash sector per slot: 12-byte header (magic "DSP3", data version, slot index, CRC-32 of everything
  * after the header) + the packed DSP state.  Device preset dumps load directly into a dspi_bulk_state and
