@@ -47,6 +47,8 @@ SYMBOLS = [
     "dspi_chainq_response_host", "dspi_chainq_response_device",
     "dspi_chain_apply_bulk_device", "dspi_chainq_apply_bulk_device",
     "dspi_chain_collect_bulk_device", "dspi_chainq_collect_bulk_device",
+    "dspi_chain_apply_preset_device", "dspi_chainq_apply_preset_device",
+    "dspi_chain_collect_preset_device", "dspi_chainq_collect_preset_device",
 ]
 
 
@@ -145,6 +147,8 @@ def lib():
             getattr(h, pre + "_sm_partition").argtypes = [vp, vp, vp]
             getattr(h, pre + "_apply_bulk_device").argtypes = [vp, u32, u32, vp, vp, C.c_int, C.c_float, vp]
             getattr(h, pre + "_collect_bulk_device").argtypes = [vp, u32, u32, vp, vp, vp]
+            getattr(h, pre + "_apply_preset_device").argtypes = [vp, u32, u32, vp, C.c_size_t, vp, vp, C.c_float, vp]
+            getattr(h, pre + "_collect_preset_device").argtypes = [vp, u32, u32, vp, vp, C.c_size_t, vp]
             getattr(h, pre + "_process_packets_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_process_packets_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_set_spdif_tx").argtypes = [vp, u32, u32, vp]
@@ -406,7 +410,8 @@ def bind_host_to_device(device):
 class _ChainSpdif:
     """What both chain engines share: each instance's S/PDIF transmitter (block position + channel status) and the
     process form whose output stage writes S/PDIF subframes (``*_spdif_tx``, ``*_process_subframes_*``), and the ingest of
-    ``WireBulkParams`` packets on the GPU (``*_apply_bulk_device``) and their read-back (``*_collect_bulk_device``)."""
+    ``WireBulkParams`` packets on the GPU (``*_apply_bulk_device``) and their read-back (``*_collect_bulk_device``), and the
+    same for preset slot images (``*_apply_preset_device`` / ``*_collect_preset_device``)."""
 
     def apply_bulk_device(self, packets, fs, inst0=0, host=None, exact_db=False):
         """WIRE_BULK [n] -> instances [inst0, inst0+n) reconfigured on the GPU as ``bulk_params_apply`` and the firmware's main
@@ -432,6 +437,41 @@ class _ChainSpdif:
         _check(getattr(lib(), self._PRE + "_collect_bulk_device")(self._h, int(inst0), n, w.ctypes.data_as(C.c_void_p),
                                                                   hv.ctypes.data_as(C.c_void_p), res.ctypes.data_as(C.c_void_p)))
         return w, hv, res
+
+    def apply_preset_device(self, images, fs, inst0=0, slots=0, master_volume_mode=0, dir_master_volume_db=0.0, host=None):
+        """uint8 [n, stride] slot images (stride >= ``preset_slot_size``, e.g. 4096-byte flash sectors) -> instances
+        [inst0, inst0+n) reconfigured on the GPU as ``preset_load`` and the firmware's main loop would.  ``slots``,
+        ``master_volume_mode`` and ``dir_master_volume_db`` are scalars or [n]; ``host`` BULK_HOST [n] (default: volume 0 dB,
+        not muted).  Returns int32 [n]: 0 loaded, 3 (PRESET_ERR_CRC) rejected (that instance is left exactly as it was)."""
+        img = np.ascontiguousarray(images, np.uint8)
+        if img.ndim != 2:
+            raise ValueError("images must be [n, stride] bytes")
+        n = img.shape[0]
+        ld = np.zeros(n, L.PRESET_LOAD)
+        ld["slot_index"], ld["master_volume_mode"], ld["dir_master_volume_db"] = slots, master_volume_mode, dir_master_volume_db
+        hv = np.zeros(n, L.BULK_HOST) if host is None else np.ascontiguousarray(host, L.BULK_HOST).reshape(-1)
+        if hv.shape[0] != n:
+            raise ValueError("images and host give different instance counts")
+        res = np.zeros(n, np.int32)
+        _check(getattr(lib(), self._PRE + "_apply_preset_device")(self._h, int(inst0), n, img.ctypes.data_as(C.c_void_p), C.c_size_t(img.shape[1]),
+                                                                  ld.ctypes.data_as(C.c_void_p), hv.ctypes.data_as(C.c_void_p), C.c_float(fs),
+                                                                  res.ctypes.data_as(C.c_void_p)))
+        return res
+
+    def collect_preset_device(self, slots, inst0=0, n=None):
+        """The state part of ``preset_save`` for instances [inst0, inst0+n) (default: as many as ``slots`` gives, or to the
+        end for a scalar): (uint8 [n, slot size] images, int32 [n] of ``layouts.BULK_*`` marks).  An unset instance gives zero
+        bytes."""
+        sl = np.asarray(slots, np.uint8).reshape(-1)
+        n = (self.n_instances - int(inst0) if sl.size == 1 else sl.size) if n is None else int(n)
+        sl = np.ascontiguousarray(np.broadcast_to(sl, (max(n, 0),)) if sl.size == 1 else sl)
+        if sl.size != max(n, 0):
+            raise ValueError("slots and n give different instance counts")
+        size = preset_slot_size(L.PLATFORM_RP2040 if self._PRE == "dspi_chainq" else L.PLATFORM_RP2350)
+        img, res = np.zeros((max(n, 0), size), np.uint8), np.zeros(max(n, 0), np.int32)
+        _check(getattr(lib(), self._PRE + "_collect_preset_device")(self._h, int(inst0), n, sl.ctypes.data_as(C.c_void_p), img.ctypes.data_as(C.c_void_p),
+                                                                    C.c_size_t(size), res.ctypes.data_as(C.c_void_p)))
+        return img, res
 
     def set_spdif_tx(self, block_pos, channel_status, inst0=0):
         """Transmitter state of instances [inst0, inst0+n): ``block_pos`` an int or [n] (0..191), ``channel_status`` 5 bytes

@@ -21,15 +21,23 @@
 // the constant header and pin count, and sends it to the staging buffer with a bulk store.
 // The engine-specific stores (float or Q28 / Q15) are the engine's ParamStores, the same functions its dynamics kernel uses.
 //
+// Preset slot images (preset_load() / preset_save(), flash_storage.c:464-760) reuse that machinery.  preset_decode_kernel,
+// one warp per instance, brings an image in with a bulk copy, checks magic, slot index and CRC-32 (one lane, four-table
+// CRC over the words after the header) and writes a version-6 packet with the image's version gates and master-volume mode
+// resolved, or for a rejected image a header the ingest kernel rejects; the packets then take the ingest path above with
+// the flash gain conversion.  preset_collect_kernel maps a record to the image dspi_preset_slot_collect writes.
+//
 // Same arithmetic rules as coeff.cu / dynamics.cuh: every float operation is the reference's, rounded on its own
 // (-fmad=false, divisions spelled __fdiv_rn), libm in double rounded once, float -> int32 stores saturate.
 #pragma once
 #include <cstddef>
 #include <cstdio>
+#include <type_traits>
 
 #include "dspi_common.cuh"
 #include "dynamics.cuh"
 #include "eq_kernels.cuh"
+#include "preset_slot.h"
 
 namespace dspi {
 
@@ -76,6 +84,17 @@ __device__ inline float db_to_linear_fw(float db)
     const float linear = 1.0f + x + x * x * 0.5f + x * x * x * 0.1666667f + x * x * x * x * 0.0416667f;
     return (linear < 0.0f) ? 0.0f : linear;
 }
+
+// flash_storage.c:302-306 — the conversion of preset loads
+__device__ inline float db_to_linear_flash(float db)
+{
+    if (db <= -120.0f) return 0.0f;
+    if (db >= 80.0f) db = 80.0f;
+    return dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f));
+}
+
+// how the ingest kernel turns gains in dB into linear gains: the firmware's bulk_params.c, 10^(dB/20), flash_storage.c
+enum GainMode : int { kGainTaylor = 0, kGainExact = 1, kGainFlash = 2 };
 
 // bulk_params.c:179-203
 __device__ inline int32_t validate(const unsigned char *w, int platform_id, int n_channels, int n_outputs)
@@ -156,7 +175,7 @@ __device__ inline void record_body(unsigned char *w, int lane, uint32_t version,
 template <class S>
 __global__ void __launch_bounds__(kWarps * 32)
 bulk_ingest_kernel(typename S::Dev d, Record rec, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *__restrict__ packets,
-                   const dspi_bulk_host *__restrict__ host, int exact_db, float fs, dspi_eq_param *__restrict__ recipes, int32_t *__restrict__ results)
+                   const dspi_bulk_host *__restrict__ host, int gain_mode, float fs, dspi_eq_param *__restrict__ recipes, int32_t *__restrict__ results)
 {
     constexpr int O = S::kOuts, WO = DSPI_WIRE_MAX_OUTPUTS;
     static_assert(3 * O + 3 <= 32, "one lane per gain");
@@ -201,7 +220,8 @@ bulk_ingest_kernel(typename S::Dev d, Record rec, uint32_t inst0, uint32_t n, co
         if (db > 0.0f) db = 0.0f;
         lin = db <= -128.0f ? 0.0f : dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f));
     } else if (is_xp || is_out || is_pre) {
-        lin = exact_db ? dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f)) : db_to_linear_fw(db);
+        if (gain_mode == kGainFlash) lin = db_to_linear_flash(db);
+        else lin = gain_mode == kGainExact ? dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f)) : db_to_linear_fw(db);
     }
     bool delayed = false;
     if (is_xp) {
@@ -374,6 +394,243 @@ bulk_collect_kernel(Record rec, uint32_t inst0, uint32_t n, dspi_wire_bulk_param
     }
 }
 
+// ---- preset slot images (PresetSlot v12, preset_slot.h) ----
+template <class S>
+using SlotOf = typename std::conditional<S::kPlatformId == DSPI_PLATFORM_RP2350, slot_rp2350, slot_rp2040>::type;
+static_assert(sizeof(slot_rp2350) % 16 == 0 && sizeof(slot_rp2040) % 16 == 0, "the bulk copy moves multiples of 16 bytes");
+constexpr uint32_t kSlotHeaderWords = 3;                   // magic, version | slot_index << 16, crc32; the CRC covers the rest
+
+// crc32() of flash_storage.c:282-291 (reflected 0xEDB88320, as dspi_crc32), four tables for a word at a time
+struct Crc32Tables {
+    uint32_t t[4][256];
+    constexpr Crc32Tables() : t{}
+    {
+        for (uint32_t i = 0; i < 256; i++) {
+            uint32_t c = i;
+            for (int j = 0; j < 8; j++) c = (c >> 1) ^ (0xEDB88320u & (0u - (c & 1u)));
+            t[0][i] = c;
+        }
+        for (int k = 1; k < 4; k++)
+            for (uint32_t i = 0; i < 256; i++) t[k][i] = (t[k - 1][i] >> 8) ^ t[0][t[k - 1][i] & 0xFFu];
+    }
+};
+static __device__ const Crc32Tables kCrc32;
+
+// the slot's CRC: words [kSlotHeaderWords, words) of an image in shared memory, on one lane
+__device__ inline uint32_t slot_crc32(const uint32_t *W, uint32_t words)
+{
+    uint32_t crc = 0xFFFFFFFFu;
+    for (uint32_t k = kSlotHeaderWords; k < words; k++) {
+        crc ^= W[k];
+        crc = __ldg(&kCrc32.t[3][crc & 0xFFu]) ^ __ldg(&kCrc32.t[2][(crc >> 8) & 0xFFu]) ^ __ldg(&kCrc32.t[1][(crc >> 16) & 0xFFu]) ^
+              __ldg(&kCrc32.t[0][crc >> 24]);
+    }
+    return ~crc;
+}
+
+#define DSPI_SLOT_OFF(member) ((uint32_t)offsetof(T, member))
+
+// preset_load(): image i of the chunk -> packet i of the chunk, and the preset result code.  validate_slot() (:750-760), then
+// apply_slot_to_live() (:597-744) and apply_master_volume_from_mode() (:580-590) restated as the version-6 packet
+// bulk_params_apply() gives the same fields from: the preamp per side from version 12 (the legacy field before), the leveller
+// from version 10 (the fixed defaults before), the master volume the mode selects.  Gains stay in dB; the ingest kernel
+// converts them.  A rejected image keeps the zero header, whose format version 0 the ingest kernel rejects.
+template <class S>
+__global__ void __launch_bounds__(kWarps * 32)
+preset_decode_kernel(const unsigned char *__restrict__ images, const dspi_preset_load *__restrict__ load, uint32_t n,
+                     dspi_wire_bulk_params *__restrict__ packets, int32_t *__restrict__ results)
+{
+    using T = SlotOf<S>;
+    constexpr int NC = S::kRoles, NO = S::kOuts, WO = DSPI_WIRE_MAX_OUTPUTS;
+    constexpr uint32_t kSlot = sizeof(T);
+    static_assert(NC == NO + 2, "outputs are channels CH_OUT_1 = 2 onwards (config.h:310)");
+    static_assert(DSPI_SLOT_OFF(filter_recipes) % 4 == 0 && DSPI_SLOT_OFF(preamp_db) % 4 == 0 && DSPI_SLOT_OFF(delays_ms) % 4 == 0 &&
+                  DSPI_SLOT_OFF(channel_gain_db) % 4 == 0 && DSPI_SLOT_OFF(channel_mute) % 4 == 0 && DSPI_SLOT_OFF(loudness_enabled) % 4 == 0 &&
+                  DSPI_SLOT_OFF(crossfeed_enabled) % 4 == 0 && DSPI_SLOT_OFF(matrix_crosspoints) % 4 == 0 && DSPI_SLOT_OFF(matrix_outputs) % 4 == 0 &&
+                  DSPI_SLOT_OFF(leveller_enabled) % 4 == 0 && DSPI_SLOT_OFF(preamp_db_per_ch) % 4 == 0 && DSPI_SLOT_OFF(master_volume_db) % 4 == 0,
+                  "the kernels move the image in 4-byte words");
+    static_assert(DSPI_WIRE_OFF(eq) % 16 == 0, "16-byte recipe rows in the packet");
+    __shared__ alignas(16) unsigned char img_s[kWarps][kSlot];
+    __shared__ alignas(16) unsigned char pkt_s[kWarps][kPacketBytes];
+    __shared__ uint64_t bar_s[kWarps];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t i = blockIdx.x * kWarps + warp;
+    if (i >= n) return;
+    uint64_t *bar = &bar_s[warp];
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        fence_mbar_init();
+        mbar_arrive_expect_tx(bar, kSlot);
+        bulk_load_1d(img_s[warp], images + (size_t)i * kSlot, kSlot, bar);
+    }
+    uint32_t *P = reinterpret_cast<uint32_t *>(pkt_s[warp]);
+    for (uint32_t k = lane; k < kPacketBytes / 16; k += 32) reinterpret_cast<uint4 *>(P)[k] = make_uint4(0, 0, 0, 0);
+    const dspi_preset_load ld = load[i];
+    __syncwarp();
+    mbar_wait(bar, 0);
+    const uint32_t *I = reinterpret_cast<const uint32_t *>(img_s[warp]);
+    auto iw = [&](uint32_t off) { return I[off / 4]; };
+    const uint32_t version = I[1] & 0xFFFFu;
+
+    constexpr uint32_t g = DSPI_WIRE_OFF(global) / 4, x = DSPI_WIRE_OFF(crossfeed) / 4, lg = DSPI_WIRE_OFF(legacy) / 4, dl = DSPI_WIRE_OFF(delays) / 4,
+                       xp = DSPI_WIRE_OFF(crosspoints) / 4, out = DSPI_WIRE_OFF(outputs) / 4, eq = DSPI_WIRE_OFF(eq) / 4,
+                       lev = DSPI_WIRE_OFF(leveller) / 4, pre = DSPI_WIRE_OFF(preamp) / 4, mv = DSPI_WIRE_OFF(master_volume) / 4;
+    if (lane == 0) {                                                                               // :602-620, :634-645
+        P[g] = version >= 12 ? iw(DSPI_SLOT_OFF(preamp_db_per_ch)) : iw(DSPI_SLOT_OFF(preamp_db));
+        P[g + 1] = (iw(DSPI_SLOT_OFF(bypass)) & 0xFFu) | (iw(DSPI_SLOT_OFF(loudness_enabled)) & 0xFFu) << 8;
+        P[g + 2] = iw(DSPI_SLOT_OFF(loudness_ref_spl));
+        P[g + 3] = iw(DSPI_SLOT_OFF(loudness_intensity_pct));
+        P[x] = iw(DSPI_SLOT_OFF(crossfeed_enabled)) & 0xFFFFFFu;                                   // {enabled, preset, itd_enabled} on both sides
+        P[x + 1] = iw(DSPI_SLOT_OFF(crossfeed_custom_fc));
+        P[x + 2] = iw(DSPI_SLOT_OFF(crossfeed_custom_feed_db));
+    } else if (lane == 1) {                                                                        // :626-631
+        for (int k = 0; k < 3; k++) P[lg + k] = iw(DSPI_SLOT_OFF(channel_gain_db) + 4 * k);
+        P[lg + 3] = iw(DSPI_SLOT_OFF(channel_mute)) & 0xFFFFFFu;
+    } else if (lane == 2) {                                                                        // :724-741
+        if (version >= 10) {
+            P[lev] = iw(DSPI_SLOT_OFF(leveller_enabled)) & 0xFFFFFFu;                              // {enabled, speed, lookahead} on both sides
+            for (int k = 1; k < 4; k++) P[lev + k] = iw(DSPI_SLOT_OFF(leveller_amount) + 4 * (k - 1));
+        } else {
+            P[lev] = 1u << 16;
+            P[lev + 1] = __float_as_uint(50.0f);
+            P[lev + 2] = __float_as_uint(15.0f);
+            P[lev + 3] = __float_as_uint(-96.0f);
+        }
+    } else if (lane == 3) {                                                                        // :602-617, :580-590
+        for (int k = 0; k < 2; k++) P[pre + k] = version >= 12 ? iw(DSPI_SLOT_OFF(preamp_db_per_ch) + 4 * k) : iw(DSPI_SLOT_OFF(preamp_db));
+        P[mv] = (ld.master_volume_mode == 1 && version >= 12) ? iw(DSPI_SLOT_OFF(master_volume_db)) : __float_as_uint(ld.dir_master_volume_db);
+    }
+    if (lane < NC) P[dl + lane] = iw(DSPI_SLOT_OFF(delays_ms) + 4 * lane);                         // :623
+    if (lane < 2 * NO) {                                                                           // :648-655
+        const uint32_t side = lane / NO, o = lane % NO, s = DSPI_SLOT_OFF(matrix_crosspoints) / 4 + lane * 2, d = xp + (side * WO + o) * 2;
+        P[d] = I[s] & 0xFFFFu;
+        P[d + 1] = I[s + 1];
+    } else if (lane < 3 * NO) {                                                                    // :656-663
+        const uint32_t o = lane - 2 * NO, s = DSPI_SLOT_OFF(matrix_outputs) / 4 + o * 3;
+        P[out + o * 3] = I[s] & 0xFFFFu;
+        P[out + o * 3 + 1] = I[s + 1];
+        P[out + o * 3 + 2] = I[s + 2];
+    }
+    for (uint32_t r = lane; r < (uint32_t)NC * kMaxBands; r += 32) {                               // :599, {channel, band, type, reserved} -> {type, reserved[3]}
+        const uint32_t *q = I + DSPI_SLOT_OFF(filter_recipes) / 4 + r * 4;                         // 4-byte aligned only: the recipes start at byte 12
+        reinterpret_cast<uint4 *>(P + eq)[r] = make_uint4((q[0] >> 16) & 0xFFu, q[1], q[2], q[3]);
+    }
+    __syncwarp();
+    if (lane == 0) {
+        const bool ok = I[0] == DSPI_PRESET_SLOT_MAGIC && (I[1] >> 16) == ld.slot_index && slot_crc32(I, kSlot / 4) == I[2];
+        if (ok) {
+            P[0] = 6u | (uint32_t)S::kPlatformId << 8 | (uint32_t)NC << 16 | (uint32_t)NO << 24;
+            P[1] = 2u | (uint32_t)kMaxBands << 8 | kPacketBytes << 16;
+        }
+        results[i] = ok ? DSPI_PRESET_OK : DSPI_PRESET_ERR_CRC;
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+        bulk_store_1d(packets + i, pkt_s[warp], kPacketBytes);
+        tma_store_commit();
+        tma_store_wait_all<0>();
+    }
+}
+
+// preset_save()'s state part for a record: what dspi_preset_slot_collect writes for the dspi_bulk_state
+// dspi_bulk_params_apply(packet, exact_db = 1) leaves from dspi_bulk_state_defaults, where the packet is what
+// bulk_collect_kernel returns.  An unset instance gives zero bytes.  One warp per instance.
+template <class S>
+__global__ void __launch_bounds__(kWarps * 32)
+preset_collect_kernel(Record rec, uint32_t inst0, uint32_t n, const uint8_t *__restrict__ slots, unsigned char *__restrict__ images,
+                      int32_t *__restrict__ results)
+{
+    using T = SlotOf<S>;
+    constexpr int NC = S::kRoles, NO = S::kOuts, WO = DSPI_WIRE_MAX_OUTPUTS;
+    constexpr uint32_t kSlot = sizeof(T);
+    __shared__ alignas(16) unsigned char img_s[kWarps][kSlot];
+    __shared__ alignas(16) unsigned char pkt_s[kWarps][kPacketBytes];
+    __shared__ uint64_t bar_s[kWarps];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t i = blockIdx.x * kWarps + warp;
+    if (i >= n) return;
+    const uint32_t inst = inst0 + i;
+    uint64_t *bar = &bar_s[warp];
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        fence_mbar_init();
+        mbar_arrive_expect_tx(bar, kPacketBytes);
+        bulk_load_1d(pkt_s[warp], rec.packets + inst, kPacketBytes, bar);
+    }
+    uint32_t *I = reinterpret_cast<uint32_t *>(img_s[warp]);
+    for (uint32_t k = lane; k < kSlot / 16; k += 32) reinterpret_cast<uint4 *>(I)[k] = make_uint4(0, 0, 0, 0);
+    const uint8_t mark = rec.mark[inst];
+    __syncwarp();
+    mbar_wait(bar, 0);
+    if (mark != DSPI_BULK_UNSET) {
+        const uint32_t *P = reinterpret_cast<const uint32_t *>(pkt_s[warp]);
+        auto put = [&](uint32_t off, uint32_t v) { I[off / 4] = v; };
+        auto flag = [](uint32_t word, int byte) { return ((word >> (8 * byte)) & 0xFFu) ? 1u << (8 * byte) : 0u; };
+        constexpr uint32_t g = DSPI_WIRE_OFF(global) / 4, x = DSPI_WIRE_OFF(crossfeed) / 4, lg = DSPI_WIRE_OFF(legacy) / 4,
+                           dl = DSPI_WIRE_OFF(delays) / 4, xp = DSPI_WIRE_OFF(crosspoints) / 4, out = DSPI_WIRE_OFF(outputs) / 4,
+                           eq = DSPI_WIRE_OFF(eq) / 4, lev = DSPI_WIRE_OFF(leveller) / 4, pre = DSPI_WIRE_OFF(preamp) / 4,
+                           mv = DSPI_WIRE_OFF(master_volume) / 4;
+        if (lane == 0) {
+            put(DSPI_SLOT_OFF(preamp_db), P[pre]);                                                 // preamp_db[0] after a version-6 apply
+            put(DSPI_SLOT_OFF(bypass), flag(P[g + 1], 0));
+            put(DSPI_SLOT_OFF(loudness_enabled), flag(P[g + 1], 1) >> 8);
+            put(DSPI_SLOT_OFF(loudness_ref_spl), P[g + 2]);
+            put(DSPI_SLOT_OFF(loudness_intensity_pct), P[g + 3]);
+            put(DSPI_SLOT_OFF(crossfeed_enabled), flag(P[x], 0) | (P[x] & 0xFF00u) | flag(P[x], 2));
+            put(DSPI_SLOT_OFF(crossfeed_custom_fc), P[x + 1]);
+            put(DSPI_SLOT_OFF(crossfeed_custom_feed_db), P[x + 2]);
+        } else if (lane == 1) {
+            for (int k = 0; k < 3; k++) put(DSPI_SLOT_OFF(channel_gain_db) + 4 * k, P[lg + k]);
+            put(DSPI_SLOT_OFF(channel_mute), flag(P[lg + 3], 0) | flag(P[lg + 3], 1) | flag(P[lg + 3], 2));
+        } else if (lane == 2) {
+            put(DSPI_SLOT_OFF(leveller_enabled), flag(P[lev], 0) | (P[lev] & 0xFF00u) | flag(P[lev], 2));
+            for (int k = 0; k < 3; k++) put(DSPI_SLOT_OFF(leveller_amount) + 4 * k, P[lev + 1 + k]);
+        } else if (lane == 3) {
+            for (int k = 0; k < 2; k++) put(DSPI_SLOT_OFF(preamp_db_per_ch) + 4 * k, P[pre + k]);
+            float db = __uint_as_float(P[mv]);                                                     // bulk_params.c:361-368
+            if (isnan(db) || isinf(db)) db = 0.0f;
+            if (db < -128.0f) db = -128.0f;
+            if (db > 0.0f) db = 0.0f;
+            put(DSPI_SLOT_OFF(master_volume_db), __float_as_uint(db));
+        }
+        if (lane < NC) put(DSPI_SLOT_OFF(delays_ms) + 4 * lane, lane < 2 ? P[dl + lane] : P[out + (lane - 2) * 3 + 2]);
+        if (lane < 2 * NO) {
+            const uint32_t side = lane / NO, o = lane % NO, d = DSPI_SLOT_OFF(matrix_crosspoints) / 4 + lane * 2, s = xp + (side * WO + o) * 2;
+            I[d] = P[s] & 0xFFFFu;
+            I[d + 1] = P[s + 1];
+        } else if (lane < 3 * NO) {
+            const uint32_t o = lane - 2 * NO, d = DSPI_SLOT_OFF(matrix_outputs) / 4 + o * 3;
+            I[d] = P[out + o * 3] & 0xFFFFu;
+            I[d + 1] = P[out + o * 3 + 1];
+            I[d + 2] = P[out + o * 3 + 2];
+        }
+        for (uint32_t r = lane; r < (uint32_t)NC * kMaxBands; r += 32) {                           // {type, reserved[3]} -> {channel, band, type, 0}
+            const uint4 q = reinterpret_cast<const uint4 *>(P + eq)[r];
+            uint32_t *d = I + DSPI_SLOT_OFF(filter_recipes) / 4 + r * 4;                           // 4-byte aligned only: the recipes start at byte 12
+            d[0] = r / kMaxBands | (r % kMaxBands) << 8 | (q.x & 0xFFu) << 16;
+            d[1] = q.y;
+            d[2] = q.z;
+            d[3] = q.w;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            I[0] = DSPI_PRESET_SLOT_MAGIC;
+            I[1] = DSPI_PRESET_SLOT_VERSION | (uint32_t)slots[i] << 16;
+            I[2] = slot_crc32(I, kSlot / 4);
+        }
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+        bulk_store_1d(images + (size_t)i * kSlot, img_s[warp], kSlot);
+        tma_store_commit();
+        results[i] = mark;
+        tma_store_wait_all<0>();
+    }
+}
+#undef DSPI_SLOT_OFF
+
 // engine-owned staging of one chunk: packets, host volumes, recipes and result codes on the device
 struct Stage {
     dspi_wire_bulk_params *packets = nullptr;
@@ -397,6 +654,27 @@ struct Stage {
     }
 };
 
+// engine-owned staging of the preset calls, next to Stage
+struct PresetStage {
+    unsigned char *images = nullptr;                       // [kChunk][slot size], packed
+    dspi_preset_load *load = nullptr;                      // [kChunk]; a collect call keeps its slot indices here, one byte each
+    int32_t *results = nullptr;                            // [kChunk] preset result codes, or the marks of a collect
+    cudaError_t ensure(size_t slot_bytes)
+    {
+        if (results) return cudaSuccess;
+        cudaError_t e = cudaMalloc((void **)&images, (size_t)kChunk * slot_bytes);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&load, (size_t)kChunk * sizeof(dspi_preset_load));
+        if (e == cudaSuccess) e = cudaMalloc((void **)&results, (size_t)kChunk * sizeof(int32_t));
+        if (e != cudaSuccess) destroy();
+        return e;
+    }
+    void destroy()
+    {
+        cudaFree(images); cudaFree(load); cudaFree(results);
+        images = nullptr; load = nullptr; results = nullptr;
+    }
+};
+
 inline int fail_cuda(cudaError_t e, const char *what)
 {
     size_t cap = 0;
@@ -405,11 +683,13 @@ inline int fail_cuda(cudaError_t e, const char *what)
     return e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA;
 }
 
-// The whole call for an engine (dspi_chain or dspi_chainq) whose arguments are checked.  Everything runs on the engine
-// stream, behind earlier process calls; the last step (eq_set_skip) synchronises it.
-template <class S, class Engine>
-int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host, int exact_db,
-          float fs, int32_t *results)
+// The ingest path for an engine (dspi_chain or dspi_chainq) whose arguments are checked.  Everything runs on the engine
+// stream, behind earlier process calls; the last step (eq_set_skip) synchronises it.  Per chunk, stage_packets(i0, nc) puts
+// the packets of instances [i0, i0 + nc) of the call into stage.packets on the engine stream; `codes` (device, [kChunk]) is
+// what goes back to results, stage.results (the ingest kernel's codes) when it is null.
+template <class S, class Engine, class StagePackets>
+int ingest(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_bulk_host *host, int gain_mode, float fs, int32_t *results,
+           const int32_t *codes, StagePackets &&stage_packets)
 {
     cudaError_t e = stage.ensure(S::kRoles);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
@@ -417,10 +697,11 @@ int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_b
     const uint32_t Np = c->d.N_pad;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk, first = inst0 + i0;
-        e = cudaMemcpyAsync(stage.packets, packets + i0, (size_t)nc * kPacketBytes, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(stage.host, host + i0, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyHostToDevice, s);
-        if (e != cudaSuccess) return fail_cuda(e, "packet copy");
-        bulk_ingest_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.packets, stage.host, exact_db, fs,
+        int rc = stage_packets(i0, nc);
+        if (rc != DSPI_OK) return rc;
+        if ((e = cudaMemcpyAsync(stage.host, host + i0, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyHostToDevice, s)) != cudaSuccess)
+            return fail_cuda(e, "packet copy");
+        bulk_ingest_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.packets, stage.host, gain_mode, fs,
                                                                                  stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "ingest kernel");
         c->launches++;
@@ -429,7 +710,7 @@ int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_b
         rm.roles = 2; ro.roles = S::kRoles - 2;
         rm.stride = ro.stride = Np;
         rm.reject = ro.reject = stage.results;
-        int rc = eq_unpack_range(c->eq_m, first, nc, s, rm);
+        rc = eq_unpack_range(c->eq_m, first, nc, s, rm);
         if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, first, nc, s, ro);
         if (rc != DSPI_OK) return rc;
         e = launch_coeffs(S::kQ28, stage.recipes, eq_aos_mirror(c->eq_m), first, nc, fs, s, rm);
@@ -442,12 +723,45 @@ int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_b
         rc = eq_pack_range(c->eq_m, first, nc, s, rm);
         if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, first, nc, s, ro);
         if (rc != DSPI_OK) return rc;
-        if ((e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
+        if ((e = cudaMemcpyAsync(results + i0, codes ? codes : stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
             return fail_cuda(e, "result copy");
     }
     int rc = eq_set_skip(c->eq_m, c->d.skip_m, s);
     if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, s);
     return rc;
+}
+
+// dspi_chain(q)_apply_bulk_device for checked arguments
+template <class S, class Engine>
+int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host, int exact_db,
+          float fs, int32_t *results)
+{
+    return ingest<S>(c, stage, inst0, n, host, exact_db ? kGainExact : kGainTaylor, fs, results, nullptr, [&](uint32_t i0, uint32_t nc) -> int {
+        const cudaError_t e = cudaMemcpyAsync(stage.packets, packets + i0, (size_t)nc * kPacketBytes, cudaMemcpyHostToDevice, c->stream);
+        return e == cudaSuccess ? DSPI_OK : fail_cuda(e, "packet copy");
+    });
+}
+
+// dspi_chain(q)_apply_preset_device for checked arguments: images -> packets by preset_decode_kernel, then the ingest path
+// with the flash conversion; the preset result codes go back
+template <class S, class Engine>
+int apply_preset(Engine *c, Stage &stage, PresetStage &ps, uint32_t inst0, uint32_t n, const void *images, size_t stride,
+                 const dspi_preset_load *load, const dspi_bulk_host *host, float fs, int32_t *results)
+{
+    constexpr size_t kSlot = sizeof(SlotOf<S>);
+    cudaError_t e = ps.ensure(kSlot);
+    if (e != cudaSuccess) return fail_cuda(e, "preset staging buffers");
+    return ingest<S>(c, stage, inst0, n, host, kGainFlash, fs, results, ps.results, [&](uint32_t i0, uint32_t nc) -> int {
+        cudaStream_t s = c->stream;
+        cudaError_t e = cudaMemcpy2DAsync(ps.images, kSlot, static_cast<const unsigned char *>(images) + (size_t)i0 * stride, stride, kSlot, nc,
+                                          cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ps.load, load + i0, (size_t)nc * sizeof(dspi_preset_load), cudaMemcpyHostToDevice, s);
+        if (e != cudaSuccess) return fail_cuda(e, "image copy");
+        preset_decode_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(ps.images, ps.load, nc, stage.packets, ps.results);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "preset decode kernel");
+        c->launches++;
+        return DSPI_OK;
+    });
 }
 
 // The clamped recipes dspi_chain(q)_set_eq_params_device hands back ([n][roles][12], host memory) -> the records, on the
@@ -488,6 +802,30 @@ int collect(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, dspi_wire_bulk_
         if (e != cudaSuccess) return fail_cuda(e, "packet copy");
     }
     if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return fail_cuda(e, "collect");
+    return DSPI_OK;
+}
+
+// dspi_chain(q)_collect_preset_device for checked arguments: on the engine stream, behind everything issued before; reads only
+template <class S, class Engine>
+int collect_preset(Engine *c, PresetStage &ps, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t stride,
+                   int32_t *results)
+{
+    constexpr size_t kSlot = sizeof(SlotOf<S>);
+    cudaError_t e = ps.ensure(kSlot);
+    if (e != cudaSuccess) return fail_cuda(e, "preset staging buffers");
+    cudaStream_t s = c->stream;
+    uint8_t *slots = reinterpret_cast<uint8_t *>(ps.load);
+    for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
+        const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;
+        if ((e = cudaMemcpyAsync(slots, slot_indices + i0, nc, cudaMemcpyHostToDevice, s)) != cudaSuccess) return fail_cuda(e, "slot index copy");
+        preset_collect_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->rec, inst0 + i0, nc, slots, ps.images, ps.results);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "preset collect kernel");
+        c->launches++;
+        e = cudaMemcpy2DAsync(static_cast<unsigned char *>(images) + (size_t)i0 * stride, stride, ps.images, kSlot, kSlot, nc, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess && results) e = cudaMemcpyAsync(results + i0, ps.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+        if (e != cudaSuccess) return fail_cuda(e, "image copy");
+    }
+    if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return fail_cuda(e, "preset collect");
     return DSPI_OK;
 }
 

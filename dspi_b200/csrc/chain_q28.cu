@@ -853,6 +853,7 @@ struct dspi_chainq {
     dspi::PacketSchedule sched;      // packet lengths of the current call
     dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chainq_response_*
     dspi::bulk::Stage bulk;          // device staging of dspi_chainq_apply_bulk_device / _collect_bulk_device, allocated by the first call
+    dspi::bulk::PresetStage preset;  // device staging of dspi_chainq_apply_preset_device / _collect_preset_device, allocated by the first call
     dspi::bulk::Record rec;          // wire-visible configuration of every instance (dspi_chainq_collect_bulk_device); not part of the state blob
 };
 
@@ -913,6 +914,7 @@ int dspi_chainq_destroy(dspi_chainq *c)
     c->sched.destroy();
     c->resp.destroy();
     c->bulk.destroy();
+    c->preset.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -1215,6 +1217,28 @@ int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, 
     if (n == 0) return DSPI_OK;
     CU_OK(cudaSetDevice(c->desc.device));
     return dspi::bulk::collect<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, results);
+}
+
+int dspi_chainq_apply_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride, const dspi_preset_load *load,
+                                const dspi_bulk_host *host, float sample_rate, int32_t *results)
+{
+    if (!c || !images || !load || !host || !results) return fail(DSPI_EINVAL, "null argument");
+    if (image_stride < sizeof(dspi::bulk::SlotOf<dspi::ParamStores>)) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, sizeof(dspi::bulk::SlotOf<dspi::ParamStores>));
+    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return dspi::bulk::apply_preset<dspi::ParamStores>(c, c->bulk, c->preset, inst0, n, images, image_stride, load, host, sample_rate, results);
+}
+
+int dspi_chainq_collect_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride, int32_t *results)
+{
+    if (!c || !slot_indices || !images) return fail(DSPI_EINVAL, "null argument");
+    if (image_stride < sizeof(dspi::bulk::SlotOf<dspi::ParamStores>)) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, sizeof(dspi::bulk::SlotOf<dspi::ParamStores>));
+    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return dspi::bulk::collect_preset<dspi::ParamStores>(c, c->preset, inst0, n, slot_indices, images, image_stride, results);
 }
 
 int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_biquad_q28 *biquads)

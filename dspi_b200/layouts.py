@@ -177,3 +177,6 @@ BULK_HOST = np.dtype([("volume_8_8", "<i2"), ("host_mute", "u1"), ("reserved", "
 assert BULK_HOST.itemsize == 4
 # DSPI_BULK_*: what collect_bulk_device says of each instance's packet
 BULK_CURRENT, BULK_STALE, BULK_UNSET = 0, 1, 2
+# dspi_preset_load: per instance, what preset_load() gets from its caller and the preset directory
+PRESET_LOAD = np.dtype([("slot_index", "u1"), ("master_volume_mode", "u1"), ("reserved", "u1", (2,)), ("dir_master_volume_db", "<f4")])
+assert PRESET_LOAD.itemsize == 8

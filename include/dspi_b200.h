@@ -569,8 +569,9 @@ _Static_assert(sizeof(dspi_bulk_host) == 4, "dspi_bulk_host");
  * dspi_eq_set_params_device: coefficients are the oracle's policy coefficients bit for bit and within the documented libm
  * distance of the host route's.  Ordered behind process calls issued earlier on the engine stream; returns when the engine
  * is reconfigured.  DSPI_EINVAL for a NULL pointer or a sample_rate that is not positive and finite, DSPI_ERANGE for a
- * range past the end of the engine; nothing is written then.  Preset images take the same route:
- * dspi_preset_slot_apply -> dspi_bulk_params_collect -> this call with exact_db = 1. */
+ * range past the end of the engine; nothing is written then.  Preset slot images load with _apply_preset_device below.
+ * The older route dspi_preset_slot_apply -> dspi_bulk_params_collect -> this call with exact_db = 1 differs from it for
+ * gains <= -120 dB (flash gives 0, exact gives 10^(dB/20)) and >= 80 dB (flash clamps to 80 dB). */
 int dspi_chain_apply_bulk_device (dspi_chain *c,  uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
                                   int exact_db, float sample_rate, int32_t *results);
 int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
@@ -603,7 +604,8 @@ int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, co
  * earlier on the engine stream, asynchronous process calls included, returns when the packets are in the caller's memory,
  * and changes nothing a process call reads.  DSPI_EINVAL for a NULL engine or packets, DSPI_ERANGE for a range past the
  * end of the engine (also one whose end wraps in 32 bits); nothing is written then.  n == 0 does nothing.
- * The route to a preset image: this call -> dspi_bulk_params_apply(packet, st, exact_db = 1) -> dspi_preset_slot_collect. */
+ * Preset slot images come from _collect_preset_device below, which gives the bytes of the route this call ->
+ * dspi_bulk_params_apply(packet, st, exact_db = 1) -> dspi_preset_slot_collect without a host loop. */
 int dspi_chain_collect_bulk_device (dspi_chain *c,  uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host,
                                     int32_t *results);
 int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host,
@@ -631,6 +633,51 @@ int dspi_preset_slot_apply(const void *slot, size_t len, uint8_t slot_index, uin
  * ZERO, so the image is for exchanging DSP state between hosts of this library (apply ignores those fields) - do NOT
  * flash it onto a device, which would load the zeros over its pin / name / I2S configuration. */
 int dspi_preset_slot_collect(const dspi_bulk_state *st, uint8_t slot_index, void *out, size_t cap);
+
+/* ---- preset slot images on the device: preset_load() / preset_save() for many chain instances ----- */
+/* Per instance, what preset_load() gets from its caller and the preset directory. */
+typedef struct { uint8_t slot_index, master_volume_mode, reserved[2]; float dir_master_volume_db; } dspi_preset_load;
+#ifdef __cplusplus
+static_assert(sizeof(dspi_preset_load) == 8, "dspi_preset_load");
+#else
+_Static_assert(sizeof(dspi_preset_load) == 8, "dspi_preset_load");
+#endif
+/* preset_load() for instances [inst0, inst0+n) of a chain engine, from slot images to engine records ON THE GPU.  Image i
+ * starts at images + i * image_stride (image_stride >= dspi_preset_slot_size(platform): 2864 B RP2350, 1840 B RP2040, so
+ * 4 KiB flash sectors can be passed as dumped); images, load[n], host[n] and results[n] are host memory.  Per instance this
+ * is dspi_preset_slot_apply(image, slot size, load.slot_index, load.master_volume_mode, load.dir_master_volume_db, st)
+ * followed by what the main loop derives from it, with the contract of _apply_bulk_device:
+ *   - results[i] is DSPI_PRESET_OK, or DSPI_PRESET_ERR_CRC for a wrong magic, slot index or CRC-32 (checked on the
+ *     device); a rejected image changes nothing of its instance, and the call still returns DSPI_OK;
+ *   - version gates as the host: leveller fields from version 10 (fixed defaults below), per-side preamp and the slot's
+ *     master volume from version 12; master_volume_mode 1 takes the slot's master volume from version 12, otherwise
+ *     dir_master_volume_db is used;
+ *   - every gain uses flash_storage.c's db_to_linear (powf; <= -120 dB gives 0, >= 80 dB is clamped to 80 dB); the
+ *     master volume is made finite and clamped to [-128, 0] dB;
+ *   - coefficients, arithmetic and libm policy as dspi_eq_set_params_device; running state as _apply_bulk_device (EQ
+ *     state kept unless a band's topology flips, crossfeed state cleared, everything else left alone - arming the
+ *     preset-mute fade is dspi_chain(q)_set_preset_mute's job);
+ *   - the instance becomes DSPI_BULK_CURRENT: _collect_bulk_device then returns what dspi_bulk_params_collect returns for
+ *     the state dspi_preset_slot_apply left, and host[i] is its host record.
+ * Ordered behind earlier work on the engine stream; returns when the engine is reconfigured.  DSPI_EINVAL for a NULL
+ * pointer, an image_stride below the slot size or a sample_rate that is not positive and finite, DSPI_ERANGE for a range
+ * past the end of the engine (also one whose end wraps in 32 bits); nothing is written then.  n == 0 does nothing. */
+int dspi_chain_apply_preset_device (dspi_chain *c,  uint32_t inst0, uint32_t n, const void *images, size_t image_stride,
+                                    const dspi_preset_load *load, const dspi_bulk_host *host, float sample_rate, int32_t *results);
+int dspi_chainq_apply_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride,
+                                    const dspi_preset_load *load, const dspi_bulk_host *host, float sample_rate, int32_t *results);
+/* The state part of preset_save() for instances [inst0, inst0+n): writes dspi_preset_slot_size(platform) bytes at
+ * images + i * image_stride - magic, version 12, slot_indices[i], CRC-32 - and leaves the rest of each stride as it was.
+ * For a current or stale instance the bytes are those of _collect_bulk_device -> dspi_bulk_params_apply(packet, st,
+ * exact_db = 1) on dspi_bulk_state_defaults -> dspi_preset_slot_collect(st, slot_indices[i]): pins, names, I2S fields and
+ * padding zero, recipes carrying (channel, band) = (ch, b).  An unset instance gives an all-zero image, which an apply
+ * rejects.  results[i] (results may be NULL) is the instance's DSPI_BULK_* mark.  Read-only; ordered behind everything
+ * issued earlier on the engine stream, asynchronous process calls included; returns when the images are in the caller's
+ * memory.  Argument errors as the apply call (there is no sample rate). */
+int dspi_chain_collect_preset_device (dspi_chain *c,  uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
+                                      int32_t *results);
+int dspi_chainq_collect_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
+                                      int32_t *results);
 
 /* ---- S/PDIF (IEC 60958) subframe encoder: the step after the chain -------------------------- */
 /* What stereo_to_spdif_producer_give_s32() does with every S/PDIF producer buffer
