@@ -100,34 +100,8 @@ def lib():
         h.dspi_eq_launch_count.argtypes = [vp]
         h.dspi_eq_launch_count.restype = C.c_uint64
         h.dspi_eq_kernel_info.argtypes = [vp, C.c_char_p, C.c_size_t]
-        h.dspi_chain_create.argtypes = [C.POINTER(vp), C.POINTER(_ChainDesc)]
-        h.dspi_chain_destroy.argtypes = [vp]
-        h.dspi_chain_set_params.argtypes = [vp, u32, u32, vp]
-        h.dspi_chain_upload_biquads.argtypes = [vp, u32, u32, vp]
-        h.dspi_chain_download_biquads.argtypes = [vp, u32, u32, vp]
-        h.dspi_chain_reset_state.argtypes = [vp]
-        h.dspi_chain_process_host.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp]
-        h.dspi_chain_process_device.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp]
-        h.dspi_chain_sync.argtypes = [vp]
-        h.dspi_chain_stream.argtypes = [vp]
-        h.dspi_chain_stream.restype = vp
-        h.dspi_chain_launch_count.argtypes = [vp]
-        h.dspi_chain_launch_count.restype = C.c_uint64
         h.dspi_delay_samples.argtypes = [C.c_float, C.c_float, C.c_int]
         h.dspi_delay_samples.restype = C.c_int32
-        h.dspi_chainq_create.argtypes = [C.POINTER(vp), C.POINTER(_ChainDesc)]
-        h.dspi_chainq_destroy.argtypes = [vp]
-        h.dspi_chainq_set_params.argtypes = [vp, u32, u32, vp]
-        h.dspi_chainq_upload_biquads.argtypes = [vp, u32, u32, vp]
-        h.dspi_chainq_download_biquads.argtypes = [vp, u32, u32, vp]
-        h.dspi_chainq_reset_state.argtypes = [vp]
-        h.dspi_chainq_process_host.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp]
-        h.dspi_chainq_process_device.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp]
-        h.dspi_chainq_sync.argtypes = [vp]
-        h.dspi_chainq_stream.argtypes = [vp]
-        h.dspi_chainq_stream.restype = vp
-        h.dspi_chainq_launch_count.argtypes = [vp]
-        h.dspi_chainq_launch_count.restype = C.c_uint64
         h.dspi_crossfeed_compute_coefficients_q28.argtypes = [vp, vp, C.c_float]
         h.dspi_loudness_compute_table_q28.argtypes = [vp, C.c_float, C.c_float, C.c_float]
         h.dspi_crossfeed_compute_coefficients_f32.argtypes = [vp, vp, C.c_float]
@@ -141,6 +115,21 @@ def lib():
         h.dspi_preset_mute_step.argtypes = [vp, u32, u32]
         h.dspi_preset_mute_step.restype = C.c_float
         for pre in ("dspi_chain", "dspi_chainq"):
+            getattr(h, pre + "_create").argtypes = [C.POINTER(vp), C.POINTER(_ChainDesc)]
+            getattr(h, pre + "_destroy").argtypes = [vp]
+            getattr(h, pre + "_set_params").argtypes = [vp, u32, u32, vp]
+            getattr(h, pre + "_upload_biquads").argtypes = [vp, u32, u32, vp]
+            getattr(h, pre + "_download_biquads").argtypes = [vp, u32, u32, vp]
+            getattr(h, pre + "_reset_state").argtypes = [vp]
+            getattr(h, pre + "_process_host").argtypes = [vp, vp, u32, u32, u32, vp, vp, vp]
+            getattr(h, pre + "_process_device").argtypes = [vp, vp, u32, u32, u32, vp, vp, vp]
+            getattr(h, pre + "_sync").argtypes = [vp]
+            getattr(h, pre + "_stream").argtypes = [vp]
+            getattr(h, pre + "_stream").restype = vp
+            getattr(h, pre + "_launch_count").argtypes = [vp]
+            getattr(h, pre + "_launch_count").restype = C.c_uint64
+            getattr(h, pre + "_state_size").argtypes = [vp]
+            getattr(h, pre + "_state_size").restype = C.c_size_t
             getattr(h, pre + "_set_preset_mute").argtypes = [vp, u32, u32, vp, u32]
             getattr(h, pre + "_get_preset_mute").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_set_dynamics_device").argtypes = [vp, u32, u32, vp, C.c_float]
@@ -407,11 +396,140 @@ def bind_host_to_device(device):
     return int(lib().dspi_bind_host_to_device(int(device)))
 
 
-class _ChainSpdif:
-    """What both chain engines share: each instance's S/PDIF transmitter (block position + channel status) and the
-    process form whose output stage writes S/PDIF subframes (``*_spdif_tx``, ``*_process_subframes_*``), and the ingest of
-    ``WireBulkParams`` packets on the GPU (``*_apply_bulk_device``) and their read-back (``*_collect_bulk_device``), and the
-    same for preset slot images (``*_apply_preset_device`` / ``*_collect_preset_device``)."""
+class _ChainEngine:
+    """What both chain engines share; the subclasses differ in their constructor and in their class attributes (the
+    C prefix ``_PRE``, the ``_PARAMS``, ``_BIQUAD`` and ``_STATUS`` dtypes, EQ channels ``_ROLES``, outputs ``_OUTS``, S/PDIF
+    pairs ``_PAIRS`` and the preset slot ``_PLATFORM``)."""
+
+    def _fn(self, name):
+        return getattr(lib(), self._PRE + "_" + name)
+
+    def close(self):
+        if self._h:
+            self._fn("destroy")(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_params(self, params, inst0=0):
+        p = np.ascontiguousarray(params)
+        assert p.dtype == self._PARAMS and p.ndim == 1
+        _check(self._fn("set_params")(self._h, inst0, p.shape[0], p.ctypes.data))
+
+    def upload_biquads(self, biquads, inst0=0):
+        b = np.ascontiguousarray(biquads)
+        assert b.dtype == self._BIQUAD and b.shape[1:] == (self._ROLES, L.MAX_BANDS)
+        _check(self._fn("upload_biquads")(self._h, inst0, b.shape[0], b.ctypes.data))
+
+    def set_eq_params_device(self, recipes, fs, inst0=0):
+        """EQ_PARAM [n, roles, 12] -> coefficients of all bands computed on the GPU; returns the clamped recipes."""
+        r = np.ascontiguousarray(recipes, L.EQ_PARAM).copy()
+        assert r.shape[1:] == (self._ROLES, L.MAX_BANDS)
+        _check(self._fn("set_eq_params_device")(self._h, int(inst0), int(r.shape[0]), r.ctypes.data_as(C.c_void_p), C.c_float(fs)))
+        return r
+
+    def download_biquads(self, n=None, inst0=0):
+        n = self.n_instances - inst0 if n is None else n
+        out = np.zeros((n, self._ROLES, L.MAX_BANDS), self._BIQUAD)
+        _check(self._fn("download_biquads")(self._h, inst0, n, out.ctypes.data))
+        return out
+
+    def state_export(self):
+        """Checkpoint: filter / leveller / delay / modulator state (and coefficients) as one bytes-like blob."""
+        n = int(self._fn("state_size")(self._h))
+        blob = np.zeros(n, np.uint8)
+        _check(self._fn("state_export")(self._h, blob.ctypes.data_as(C.c_void_p), C.c_size_t(n)))
+        return blob
+
+    def state_import(self, blob):
+        b = np.ascontiguousarray(blob, np.uint8)
+        _check(self._fn("state_import")(self._h, b.ctypes.data_as(C.c_void_p), C.c_size_t(b.size)))
+
+    def sm_partition(self):
+        """(SMs reserved for the modulator, SMs for every other stage); (0, 0) without a partition."""
+        a, b = C.c_uint32(), C.c_uint32()
+        _check(self._fn("sm_partition")(self._h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def set_dynamics_device(self, cfgs, fs, inst0=0):
+        """DYNAMICS_CONFIG [n]: crossfeed / leveller / loudness coefficients and the host volume generated on the GPU."""
+        cf = np.ascontiguousarray(cfgs, L.DYNAMICS_CONFIG)
+        _check(self._fn("set_dynamics_device")(self._h, int(inst0), int(cf.shape[0]), cf.ctypes.data_as(C.c_void_p), C.c_float(fs)))
+
+    def set_preset_mute(self, states, fs, inst0=0, n=None):
+        """Envelope mode for instances [inst0, inst0+n): ``states`` PRESET_MUTE [n], or None to leave envelope mode."""
+        if states is None:
+            n = self.n_instances - inst0 if n is None else n
+            _check(self._fn("set_preset_mute")(self._h, int(inst0), int(n), None, int(fs)))
+            return
+        st = np.ascontiguousarray(states, L.PRESET_MUTE)
+        _check(self._fn("set_preset_mute")(self._h, int(inst0), int(st.shape[0]), st.ctypes.data_as(C.c_void_p), int(fs)))
+
+    def get_preset_mute(self, n=None, inst0=0):
+        n = self.n_instances - inst0 if n is None else n
+        out = np.zeros(n, L.PRESET_MUTE)
+        _check(self._fn("get_preset_mute")(self._h, int(inst0), int(n), out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def reset_state(self):
+        _check(self._fn("reset_state")(self._h))
+
+    def process_host(self, pcm, bit_depth, n_packets, frames_per_packet, want_spdif=True, want_pdm=True, want_status=True):
+        """``pcm``: uint8 [n_instances, n_frames * bytes_per_frame].  Returns (spdif, pdm, status)."""
+        return self._process_host("process_host", pcm, bit_depth, n_packets * frames_per_packet, (n_packets, frames_per_packet),
+                                  want_spdif, want_pdm, want_status)
+
+    def process_device(self, pcm_ptr, bit_depth, n_packets, frames_per_packet, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
+        _check(self._fn("process_device")(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, n_packets, frames_per_packet,
+                                          C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
+                                          C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                          C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def process_packets_host(self, pcm, bit_depth, packet_frames, want_spdif=True, want_pdm=True, want_status=True):
+        """One USB packet per entry of ``packet_frames`` (its length in frames, shared by every instance).
+        ``pcm``: uint8 [n_instances, F * bytes_per_frame] with F = sum(packet_frames).  Returns (spdif, pdm, status), spdif
+        int32 [n_instances, S/PDIF pairs, F, 2]."""
+        t, F = _packet_table(packet_frames)
+        return self._process_host("process_packets_host", pcm, bit_depth, F, (t.size, t.ctypes.data), want_spdif, want_pdm, want_status)
+
+    def _process_host(self, name, pcm, bit_depth, F, schedule, want_spdif, want_pdm, want_status):
+        pcm = np.ascontiguousarray(pcm)
+        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
+        spdif = np.zeros((self.n_instances, self._PAIRS, F, 2), np.int32) if want_spdif else None
+        pdm = np.zeros((self.n_instances, F, 8), np.uint32) if want_pdm else None
+        status = np.zeros(self.n_instances, self._STATUS) if want_status else None
+        _check(self._fn(name)(self._h, pcm.ctypes.data, bit_depth, *schedule,
+                              spdif.ctypes.data if want_spdif else None, pdm.ctypes.data if want_pdm else None,
+                              status.ctypes.data if want_status else None))
+        return spdif, pdm, status
+
+    def process_packets_device(self, pcm_ptr, bit_depth, packet_frames, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
+        """``process_packets_host`` with device pointers, asynchronous on the engine stream (outputs for F = sum(packet_frames))."""
+        t, _ = _packet_table(packet_frames)
+        _check(self._fn("process_packets_device")(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
+                                                  C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
+                                                  C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                  C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def response(self, freqs, fs, inst0=0, n=None, out_ptr=0):
+        """Frequency response of instances [inst0, inst0+n): complex64 [n, outputs, 2 inputs, n_freqs]; with ``out_ptr``
+        (device memory) asynchronous on the engine stream, returning None."""
+        return _response(self._h, self._PRE, (self._OUTS, 2), self.n_instances, freqs, fs, inst0, n, out_ptr)
+
+    def sync(self):
+        _check(self._fn("sync")(self._h))
+
+    @property
+    def stream(self):
+        return self._fn("stream")(self._h)
+
+    @property
+    def launch_count(self):
+        return int(self._fn("launch_count")(self._h))
 
     def apply_bulk_device(self, packets, fs, inst0=0, host=None, exact_db=False):
         """WIRE_BULK [n] -> instances [inst0, inst0+n) reconfigured on the GPU as ``bulk_params_apply`` and the firmware's main
@@ -422,9 +540,9 @@ class _ChainSpdif:
         if hv.shape[0] != w.shape[0]:
             raise ValueError("packets and host give different instance counts")
         res = np.zeros(w.shape[0], np.int32)
-        _check(getattr(lib(), self._PRE + "_apply_bulk_device")(self._h, int(inst0), int(w.shape[0]), w.ctypes.data_as(C.c_void_p),
-                                                                hv.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
-                                                                res.ctypes.data_as(C.c_void_p)))
+        _check(self._fn("apply_bulk_device")(self._h, int(inst0), int(w.shape[0]), w.ctypes.data_as(C.c_void_p),
+                                             hv.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
+                                             res.ctypes.data_as(C.c_void_p)))
         return res
 
     def collect_bulk_device(self, inst0=0, n=None):
@@ -434,8 +552,8 @@ class _ChainSpdif:
         instance gives zero bytes."""
         n = self.n_instances - int(inst0) if n is None else int(n)
         w, hv, res = np.zeros(max(n, 0), L.WIRE_BULK), np.zeros(max(n, 0), L.BULK_HOST), np.zeros(max(n, 0), np.int32)
-        _check(getattr(lib(), self._PRE + "_collect_bulk_device")(self._h, int(inst0), n, w.ctypes.data_as(C.c_void_p),
-                                                                  hv.ctypes.data_as(C.c_void_p), res.ctypes.data_as(C.c_void_p)))
+        _check(self._fn("collect_bulk_device")(self._h, int(inst0), n, w.ctypes.data_as(C.c_void_p),
+                                               hv.ctypes.data_as(C.c_void_p), res.ctypes.data_as(C.c_void_p)))
         return w, hv, res
 
     def apply_preset_device(self, images, fs, inst0=0, slots=0, master_volume_mode=0, dir_master_volume_db=0.0, host=None):
@@ -453,9 +571,9 @@ class _ChainSpdif:
         if hv.shape[0] != n:
             raise ValueError("images and host give different instance counts")
         res = np.zeros(n, np.int32)
-        _check(getattr(lib(), self._PRE + "_apply_preset_device")(self._h, int(inst0), n, img.ctypes.data_as(C.c_void_p), C.c_size_t(img.shape[1]),
-                                                                  ld.ctypes.data_as(C.c_void_p), hv.ctypes.data_as(C.c_void_p), C.c_float(fs),
-                                                                  res.ctypes.data_as(C.c_void_p)))
+        _check(self._fn("apply_preset_device")(self._h, int(inst0), n, img.ctypes.data_as(C.c_void_p), C.c_size_t(img.shape[1]),
+                                               ld.ctypes.data_as(C.c_void_p), hv.ctypes.data_as(C.c_void_p), C.c_float(fs),
+                                               res.ctypes.data_as(C.c_void_p)))
         return res
 
     def collect_preset_device(self, slots, inst0=0, n=None):
@@ -467,10 +585,10 @@ class _ChainSpdif:
         sl = np.ascontiguousarray(np.broadcast_to(sl, (max(n, 0),)) if sl.size == 1 else sl)
         if sl.size != max(n, 0):
             raise ValueError("slots and n give different instance counts")
-        size = preset_slot_size(L.PLATFORM_RP2040 if self._PRE == "dspi_chainq" else L.PLATFORM_RP2350)
+        size = preset_slot_size(self._PLATFORM)
         img, res = np.zeros((max(n, 0), size), np.uint8), np.zeros(max(n, 0), np.int32)
-        _check(getattr(lib(), self._PRE + "_collect_preset_device")(self._h, int(inst0), n, sl.ctypes.data_as(C.c_void_p), img.ctypes.data_as(C.c_void_p),
-                                                                    C.c_size_t(size), res.ctypes.data_as(C.c_void_p)))
+        _check(self._fn("collect_preset_device")(self._h, int(inst0), n, sl.ctypes.data_as(C.c_void_p), img.ctypes.data_as(C.c_void_p),
+                                                 C.c_size_t(size), res.ctypes.data_as(C.c_void_p)))
         return img, res
 
     def set_spdif_tx(self, block_pos, channel_status, inst0=0):
@@ -487,13 +605,13 @@ class _ChainSpdif:
         rec = np.zeros(n, L.SPDIF_TX)
         rec["block_pos"] = bp
         rec["channel_status"] = cs
-        _check(getattr(lib(), self._PRE + "_set_spdif_tx")(self._h, int(inst0), int(n), rec.ctypes.data_as(C.c_void_p)))
+        _check(self._fn("set_spdif_tx")(self._h, int(inst0), int(n), rec.ctypes.data_as(C.c_void_p)))
 
     def get_spdif_tx(self, n=None, inst0=0):
         """SPDIF_TX [n]: block position of the next frame and channel status, after the last call issued."""
         n = self.n_instances - inst0 if n is None else n
         out = np.zeros(n, L.SPDIF_TX)
-        _check(getattr(lib(), self._PRE + "_get_spdif_tx")(self._h, int(inst0), int(n), out.ctypes.data_as(C.c_void_p)))
+        _check(self._fn("get_spdif_tx")(self._h, int(inst0), int(n), out.ctypes.data_as(C.c_void_p)))
         return out
 
     def process_subframes_host(self, pcm, bit_depth, packet_frames, want_subframes=True, want_pdm=True, want_status=True):
@@ -505,25 +623,25 @@ class _ChainSpdif:
         sub = np.zeros((self.n_instances, self._PAIRS, F, 2, 2), np.uint32) if want_subframes else None
         pdm = np.zeros((self.n_instances, F, 8), np.uint32) if want_pdm else None
         status = np.zeros(self.n_instances, self._STATUS) if want_status else None
-        _check(getattr(lib(), self._PRE + "_process_subframes_host")(self._h, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
-                                                                     sub.ctypes.data if want_subframes else None,
-                                                                     pdm.ctypes.data if want_pdm else None,
-                                                                     status.ctypes.data if want_status else None))
+        _check(self._fn("process_subframes_host")(self._h, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
+                                                  sub.ctypes.data if want_subframes else None,
+                                                  pdm.ctypes.data if want_pdm else None,
+                                                  status.ctypes.data if want_status else None))
         return sub, pdm, status
 
     def process_subframes_device(self, pcm_ptr, bit_depth, packet_frames, subframes_ptr=0, pdm_ptr=0, status_ptr=0):
         """``process_subframes_host`` with device pointers (subframes 16-byte aligned), asynchronous on the engine stream."""
         t, _ = _packet_table(packet_frames)
-        _check(getattr(lib(), self._PRE + "_process_subframes_device")(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
-                                                                       C.c_void_p(int(subframes_ptr)) if subframes_ptr else None,
-                                                                       C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
-                                                                       C.c_void_p(int(status_ptr)) if status_ptr else None))
+        _check(self._fn("process_subframes_device")(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
+                                                    C.c_void_p(int(subframes_ptr)) if subframes_ptr else None,
+                                                    C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                    C.c_void_p(int(status_ptr)) if status_ptr else None))
 
 
-class ChainEngine(_ChainSpdif):
+class ChainEngine(_ChainEngine):
     """Many independent DSPi device instances, whole signal chain (``dspi_chain_*``)."""
-    _PRE = "dspi_chain"
-    _PAIRS, _STATUS = 4, L.STATUS
+    _PRE, _PARAMS, _BIQUAD, _STATUS = "dspi_chain", L.CHAIN_PARAMS_F32, L.BIQUAD_F32, L.STATUS
+    _ROLES, _OUTS, _PAIRS, _PLATFORM = L.CHAIN_EQ_CHANNELS, L.CHAIN_OUTPUTS, 4, L.PLATFORM_RP2350
 
     def __init__(self, arith, n_instances, max_frames, n_bands=L.NUM_BANDS, device=0):
         self.arith = ARITH[arith] if isinstance(arith, str) else int(arith)
@@ -531,139 +649,6 @@ class ChainEngine(_ChainSpdif):
         self._h = C.c_void_p()
         desc = _ChainDesc(self.arith, self.n_instances, int(n_bands), self.device, self.max_frames)
         _check(lib().dspi_chain_create(C.byref(self._h), C.byref(desc)))
-
-    def close(self):
-        if self._h:
-            lib().dspi_chain_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_params(self, params, inst0=0):
-        p = np.ascontiguousarray(params)
-        assert p.dtype == L.CHAIN_PARAMS_F32 and p.ndim == 1
-        _check(lib().dspi_chain_set_params(self._h, inst0, p.shape[0], p.ctypes.data))
-
-    def upload_biquads(self, biquads, inst0=0):
-        b = np.ascontiguousarray(biquads)
-        assert b.dtype == L.BIQUAD_F32 and b.shape[1:] == (L.CHAIN_EQ_CHANNELS, L.MAX_BANDS)
-        _check(lib().dspi_chain_upload_biquads(self._h, inst0, b.shape[0], b.ctypes.data))
-
-    def set_eq_params_device(self, recipes, fs, inst0=0):
-        """EQ_PARAM [n, 11, 12] -> coefficients of all bands computed on the GPU; returns the clamped recipes."""
-        r = np.ascontiguousarray(recipes, L.EQ_PARAM).copy()
-        assert r.shape[1:] == (L.CHAIN_EQ_CHANNELS, L.MAX_BANDS)
-        _check(lib().dspi_chain_set_eq_params_device(self._h, int(inst0), int(r.shape[0]), r.ctypes.data_as(C.c_void_p), C.c_float(fs)))
-        return r
-
-    def download_biquads(self, n=None, inst0=0):
-        n = self.n_instances - inst0 if n is None else n
-        out = np.zeros((n, L.CHAIN_EQ_CHANNELS, L.MAX_BANDS), L.BIQUAD_F32)
-        _check(lib().dspi_chain_download_biquads(self._h, inst0, n, out.ctypes.data))
-        return out
-
-    def state_export(self):
-        """Checkpoint: filter / leveller / delay / modulator state (and coefficients) as one bytes-like blob."""
-        fn = getattr(lib(), "dspi_chain_state_size")
-        fn.restype = C.c_size_t
-        n = int(fn(self._h))
-        blob = np.zeros(n, np.uint8)
-        _check(getattr(lib(), "dspi_chain_state_export")(self._h, blob.ctypes.data_as(C.c_void_p), C.c_size_t(n)))
-        return blob
-
-    def state_import(self, blob):
-        b = np.ascontiguousarray(blob, np.uint8)
-        _check(getattr(lib(), "dspi_chain_state_import")(self._h, b.ctypes.data_as(C.c_void_p), C.c_size_t(b.size)))
-
-    def sm_partition(self):
-        """(SMs reserved for the modulator, SMs for every other stage); (0, 0) without a partition."""
-        a, b = C.c_uint32(), C.c_uint32()
-        _check(getattr(lib(), self._PRE + "_sm_partition")(self._h, C.byref(a), C.byref(b)))
-        return a.value, b.value
-
-    def set_dynamics_device(self, cfgs, fs, inst0=0):
-        """DYNAMICS_CONFIG [n]: crossfeed / leveller / loudness coefficients and the host volume generated on the GPU."""
-        cf = np.ascontiguousarray(cfgs, L.DYNAMICS_CONFIG)
-        _check(getattr(lib(), self._PRE + "_set_dynamics_device")(self._h, int(inst0), int(cf.shape[0]), cf.ctypes.data_as(C.c_void_p), C.c_float(fs)))
-
-    def set_preset_mute(self, states, fs, inst0=0, n=None):
-        """Envelope mode for instances [inst0, inst0+n): ``states`` PRESET_MUTE [n], or None to leave envelope mode."""
-        if states is None:
-            n = self.n_instances - inst0 if n is None else n
-            _check(getattr(lib(), self._PRE + "_set_preset_mute")(self._h, int(inst0), int(n), None, int(fs)))
-            return
-        st = np.ascontiguousarray(states, L.PRESET_MUTE)
-        _check(getattr(lib(), self._PRE + "_set_preset_mute")(self._h, int(inst0), int(st.shape[0]), st.ctypes.data_as(C.c_void_p), int(fs)))
-
-    def get_preset_mute(self, n=None, inst0=0):
-        n = self.n_instances - inst0 if n is None else n
-        out = np.zeros(n, L.PRESET_MUTE)
-        _check(getattr(lib(), self._PRE + "_get_preset_mute")(self._h, int(inst0), int(n), out.ctypes.data_as(C.c_void_p)))
-        return out
-
-    def reset_state(self):
-        _check(lib().dspi_chain_reset_state(self._h))
-
-    def process_host(self, pcm, bit_depth, n_packets, frames_per_packet, want_spdif=True, want_pdm=True, want_status=True):
-        """``pcm``: uint8 [n_instances, n_frames * bytes_per_frame].  Returns (spdif, pdm, status)."""
-        F = n_packets * frames_per_packet
-        pcm = np.ascontiguousarray(pcm)
-        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
-        spdif = np.zeros((self.n_instances, 4, F, 2), np.int32) if want_spdif else None
-        pdm = np.zeros((self.n_instances, F, 8), np.uint32) if want_pdm else None
-        status = np.zeros(self.n_instances, L.STATUS) if want_status else None
-        _check(lib().dspi_chain_process_host(self._h, pcm.ctypes.data, bit_depth, n_packets, frames_per_packet,
-                                             spdif.ctypes.data if want_spdif else None, pdm.ctypes.data if want_pdm else None,
-                                             status.ctypes.data if want_status else None))
-        return spdif, pdm, status
-
-    def process_device(self, pcm_ptr, bit_depth, n_packets, frames_per_packet, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
-        _check(lib().dspi_chain_process_device(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, n_packets, frames_per_packet,
-                                               C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
-                                               C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
-                                               C.c_void_p(int(status_ptr)) if status_ptr else None))
-
-    def process_packets_host(self, pcm, bit_depth, packet_frames, want_spdif=True, want_pdm=True, want_status=True):
-        """One USB packet per entry of ``packet_frames`` (its length in frames, shared by every instance).
-        ``pcm``: uint8 [n_instances, F * bytes_per_frame] with F = sum(packet_frames).  Returns (spdif, pdm, status)."""
-        t, F = _packet_table(packet_frames)
-        pcm = np.ascontiguousarray(pcm)
-        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
-        spdif = np.zeros((self.n_instances, 4, F, 2), np.int32) if want_spdif else None
-        pdm = np.zeros((self.n_instances, F, 8), np.uint32) if want_pdm else None
-        status = np.zeros(self.n_instances, L.STATUS) if want_status else None
-        _check(lib().dspi_chain_process_packets_host(self._h, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
-                                                     spdif.ctypes.data if want_spdif else None, pdm.ctypes.data if want_pdm else None,
-                                                     status.ctypes.data if want_status else None))
-        return spdif, pdm, status
-
-    def process_packets_device(self, pcm_ptr, bit_depth, packet_frames, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
-        """``process_packets_host`` with device pointers, asynchronous on the engine stream (outputs for F = sum(packet_frames))."""
-        t, _ = _packet_table(packet_frames)
-        _check(lib().dspi_chain_process_packets_device(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
-                                                       C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
-                                                       C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
-                                                       C.c_void_p(int(status_ptr)) if status_ptr else None))
-
-    def response(self, freqs, fs, inst0=0, n=None, out_ptr=0):
-        """Frequency response of instances [inst0, inst0+n): complex64 [n, 9 outputs, 2 inputs, n_freqs]; with ``out_ptr``
-        (device memory) asynchronous on the engine stream, returning None."""
-        return _response(self._h, "dspi_chain", (L.CHAIN_OUTPUTS, 2), self.n_instances, freqs, fs, inst0, n, out_ptr)
-
-    def sync(self):
-        _check(lib().dspi_chain_sync(self._h))
-
-    @property
-    def stream(self):
-        return lib().dspi_chain_stream(self._h)
-
-    @property
-    def launch_count(self):
-        return int(lib().dspi_chain_launch_count(self._h))
 
 
 def delay_samples(delay_ms, fs, is_last=False):
@@ -810,142 +795,16 @@ def master_volume(db):
     return lin.value, q.value
 
 
-class ChainEngineQ28(_ChainSpdif):
+class ChainEngineQ28(_ChainEngine):
     """Many independent RP2040-shape instances (2 in -> 5 out), Q28 arithmetic (``dspi_chainq_*``)."""
-    _PRE = "dspi_chainq"
-    _PAIRS, _STATUS = 2, L.STATUS_Q28
+    _PRE, _PARAMS, _BIQUAD, _STATUS = "dspi_chainq", L.CHAIN_PARAMS_Q28, L.BIQUAD_Q28, L.STATUS_Q28
+    _ROLES, _OUTS, _PAIRS, _PLATFORM = L.CHAINQ_EQ_CHANNELS, L.CHAINQ_OUTPUTS, 2, L.PLATFORM_RP2040
 
     def __init__(self, n_instances, max_frames, n_bands=L.NUM_BANDS, device=0):
         self.n_instances, self.max_frames, self.device = int(n_instances), int(max_frames), int(device)
         self._h = C.c_void_p()
         desc = _ChainDesc(ARITH_Q28, self.n_instances, int(n_bands), self.device, self.max_frames)
         _check(lib().dspi_chainq_create(C.byref(self._h), C.byref(desc)))
-
-    def close(self):
-        if self._h:
-            lib().dspi_chainq_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_params(self, params, inst0=0):
-        p = np.ascontiguousarray(params)
-        assert p.dtype == L.CHAIN_PARAMS_Q28 and p.ndim == 1
-        _check(lib().dspi_chainq_set_params(self._h, inst0, p.shape[0], p.ctypes.data))
-
-    def upload_biquads(self, biquads, inst0=0):
-        b = np.ascontiguousarray(biquads)
-        assert b.dtype == L.BIQUAD_Q28 and b.shape[1:] == (L.CHAINQ_EQ_CHANNELS, L.MAX_BANDS)
-        _check(lib().dspi_chainq_upload_biquads(self._h, inst0, b.shape[0], b.ctypes.data))
-
-    def set_eq_params_device(self, recipes, fs, inst0=0):
-        r = np.ascontiguousarray(recipes, L.EQ_PARAM).copy()
-        assert r.shape[1:] == (L.CHAINQ_EQ_CHANNELS, L.MAX_BANDS)
-        _check(lib().dspi_chainq_set_eq_params_device(self._h, int(inst0), int(r.shape[0]), r.ctypes.data_as(C.c_void_p), C.c_float(fs)))
-        return r
-
-    def download_biquads(self, n=None, inst0=0):
-        n = self.n_instances - inst0 if n is None else n
-        out = np.zeros((n, L.CHAINQ_EQ_CHANNELS, L.MAX_BANDS), L.BIQUAD_Q28)
-        _check(lib().dspi_chainq_download_biquads(self._h, inst0, n, out.ctypes.data))
-        return out
-
-    def state_export(self):
-        """Checkpoint: filter / leveller / delay / modulator state (and coefficients) as one bytes-like blob."""
-        fn = getattr(lib(), "dspi_chainq_state_size")
-        fn.restype = C.c_size_t
-        n = int(fn(self._h))
-        blob = np.zeros(n, np.uint8)
-        _check(getattr(lib(), "dspi_chainq_state_export")(self._h, blob.ctypes.data_as(C.c_void_p), C.c_size_t(n)))
-        return blob
-
-    def state_import(self, blob):
-        b = np.ascontiguousarray(blob, np.uint8)
-        _check(getattr(lib(), "dspi_chainq_state_import")(self._h, b.ctypes.data_as(C.c_void_p), C.c_size_t(b.size)))
-
-    def sm_partition(self):
-        """(SMs reserved for the modulator, SMs for every other stage); (0, 0) without a partition."""
-        a, b = C.c_uint32(), C.c_uint32()
-        _check(getattr(lib(), self._PRE + "_sm_partition")(self._h, C.byref(a), C.byref(b)))
-        return a.value, b.value
-
-    def set_dynamics_device(self, cfgs, fs, inst0=0):
-        """DYNAMICS_CONFIG [n]: crossfeed / leveller / loudness coefficients and the host volume generated on the GPU."""
-        cf = np.ascontiguousarray(cfgs, L.DYNAMICS_CONFIG)
-        _check(getattr(lib(), self._PRE + "_set_dynamics_device")(self._h, int(inst0), int(cf.shape[0]), cf.ctypes.data_as(C.c_void_p), C.c_float(fs)))
-
-    def set_preset_mute(self, states, fs, inst0=0, n=None):
-        """Envelope mode for instances [inst0, inst0+n): ``states`` PRESET_MUTE [n], or None to leave envelope mode."""
-        if states is None:
-            n = self.n_instances - inst0 if n is None else n
-            _check(getattr(lib(), self._PRE + "_set_preset_mute")(self._h, int(inst0), int(n), None, int(fs)))
-            return
-        st = np.ascontiguousarray(states, L.PRESET_MUTE)
-        _check(getattr(lib(), self._PRE + "_set_preset_mute")(self._h, int(inst0), int(st.shape[0]), st.ctypes.data_as(C.c_void_p), int(fs)))
-
-    def get_preset_mute(self, n=None, inst0=0):
-        n = self.n_instances - inst0 if n is None else n
-        out = np.zeros(n, L.PRESET_MUTE)
-        _check(getattr(lib(), self._PRE + "_get_preset_mute")(self._h, int(inst0), int(n), out.ctypes.data_as(C.c_void_p)))
-        return out
-
-    def reset_state(self):
-        _check(lib().dspi_chainq_reset_state(self._h))
-
-    def process_host(self, pcm, bit_depth, n_packets, frames_per_packet):
-        F = n_packets * frames_per_packet
-        pcm = np.ascontiguousarray(pcm)
-        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
-        spdif = np.zeros((self.n_instances, 2, F, 2), np.int32)
-        pdm = np.zeros((self.n_instances, F, 8), np.uint32)
-        status = np.zeros(self.n_instances, L.STATUS_Q28)
-        _check(lib().dspi_chainq_process_host(self._h, pcm.ctypes.data, bit_depth, n_packets, frames_per_packet,
-                                              spdif.ctypes.data, pdm.ctypes.data, status.ctypes.data))
-        return spdif, pdm, status
-
-    def process_device(self, pcm_ptr, bit_depth, n_packets, frames_per_packet, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
-        _check(lib().dspi_chainq_process_device(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, n_packets, frames_per_packet,
-                                                C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
-                                                C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
-                                                C.c_void_p(int(status_ptr)) if status_ptr else None))
-
-    def process_packets_host(self, pcm, bit_depth, packet_frames):
-        """As ``ChainEngine.process_packets_host``; spdif [n_instances, 2, F, 2]."""
-        t, F = _packet_table(packet_frames)
-        pcm = np.ascontiguousarray(pcm)
-        assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
-        spdif = np.zeros((self.n_instances, 2, F, 2), np.int32)
-        pdm = np.zeros((self.n_instances, F, 8), np.uint32)
-        status = np.zeros(self.n_instances, L.STATUS_Q28)
-        _check(lib().dspi_chainq_process_packets_host(self._h, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
-                                                      spdif.ctypes.data, pdm.ctypes.data, status.ctypes.data))
-        return spdif, pdm, status
-
-    def process_packets_device(self, pcm_ptr, bit_depth, packet_frames, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
-        t, _ = _packet_table(packet_frames)
-        _check(lib().dspi_chainq_process_packets_device(self._h, C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
-                                                        C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
-                                                        C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
-                                                        C.c_void_p(int(status_ptr)) if status_ptr else None))
-
-    def response(self, freqs, fs, inst0=0, n=None, out_ptr=0):
-        """Frequency response of instances [inst0, inst0+n): complex64 [n, 5 outputs, 2 inputs, n_freqs] (see ChainEngine)."""
-        return _response(self._h, "dspi_chainq", (L.CHAINQ_OUTPUTS, 2), self.n_instances, freqs, fs, inst0, n, out_ptr)
-
-    def sync(self):
-        _check(lib().dspi_chainq_sync(self._h))
-
-    @property
-    def stream(self):
-        return lib().dspi_chainq_stream(self._h)
-
-    @property
-    def launch_count(self):
-        return int(lib().dspi_chainq_launch_count(self._h))
 
 
 def crossfeed_coefficients_q28(fs, enabled=True, itd=True, preset=0, custom_fc=700.0, custom_feed_db=4.5):

@@ -31,7 +31,7 @@
 // Everything with a serial recurrence but little arithmetic keeps lane = instance; everything without
 // one runs lane = frame, fully coalesced; the EQ — 90 % of the arithmetic — runs in the kernel that is
 // tuned against the roofline.  All per-instance parameters and states are SoA arrays with the instance
-// index innermost.
+// index innermost.  The host side (engine record, launch order over the stages, staging, checkpoints) is chain_host.cuh.
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -56,7 +56,6 @@ constexpr int kOuts = DSPI_CHAIN_OUTPUTS;
 constexpr int kRoles = DSPI_CHAIN_EQ_CHANNELS;
 constexpr int kMaxDelay = DSPI_CHAIN_MAX_DELAY;
 constexpr int kLa = DSPI_LA_SAMPLES;
-constexpr int kPkt = DSPI_PACKET_MAX;
 constexpr int kXs = 33;                           // shared-memory column stride: conflict-free for lane = instance AND lane = frame
 
 struct ChainDev {
@@ -844,182 +843,102 @@ chain_response_kernel(ChainDev d, const dspi_biquad_f32 *__restrict__ m_aos, con
     }
 }
 
-int fail(int code, const char *fmt, ...)
-{
-    size_t cap = 0;
-    char *buf = error_buffer(&cap);
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, cap, fmt, ap);
-    va_end(ap);
-    return code;
-}
+}  // namespace
+}  // namespace dspi
+
+#include "chain_host.cuh"
+
+namespace dspi {
+namespace {
+
+// one kernel set per flavour: FUSED contracts a*b + c into one rounding (DSPI_ARITH_F32_FUSED), strict rounds twice
+template <bool FUSED>
+struct F32Stages {
+    static constexpr auto pre = chain_pre_kernel<FUSED>;
+    static constexpr auto post = chain_post_kernel<FUSED>;
+    static constexpr auto mix = chain_mix_kernel<FUSED>;
+    template <bool SUBFRAMES> static constexpr auto outpost = chain_outpost_kernel<SUBFRAMES>;
+    static constexpr auto ring = chain_ring_kernel;
+    static constexpr auto pdm = chain_pdm_kernel;
+    static constexpr auto env = chain_env_kernel;
+    static constexpr auto status = chain_status_kernel;
+};
+
+// what the float engine brings to the shared host code (chain_host.cuh)
+struct F32 : ParamStores {
+    using Biquad = dspi_biquad_f32;
+    using Status = dspi_status;
+    using Params = dspi_chain_params_f32;
+    using Stores = ParamStores;
+    static constexpr int kLoudRows = 12;                                     // [2 shelves][6] SVF coefficients
+    static constexpr int kXs = dspi::kXs;
+    static constexpr uint32_t kStateVersion = 2;
+    static constexpr auto scatter = chain_scatter_kernel;
+    static constexpr auto dynamics = chain_dynamics_kernel;
+    static constexpr auto response = chain_response_kernel;
+
+    template <class F>
+    static int with_stages(const dspi_chain_desc &desc, F &&f)
+    {
+        return desc.arith == DSPI_ARITH_F32_FUSED ? f(F32Stages<true>()) : f(F32Stages<false>());
+    }
+
+    static int check_desc(const dspi_chain_desc &desc)
+    {
+        if (desc.arith != DSPI_ARITH_F32_FUSED && desc.arith != DSPI_ARITH_F32_STRICT) return fail(DSPI_EINVAL, "chain engines are float (arith 0 or 1)");
+        if (desc.n_instances == 0 || desc.max_frames == 0) return fail(DSPI_EINVAL, "n_instances and max_frames must be > 0");
+        if (desc.n_bands != 10) return fail(DSPI_EINVAL, "chain engines run channel_band_counts = 10");
+        return DSPI_OK;
+    }
+
+    static cudaError_t alloc_leveller(ChainHost<F32> *c) { return dev_alloc(c, &c->d.lev_s, (size_t)5 * c->d.N_pad); }
+
+    // leveller_reset_state()
+    static cudaError_t init_leveller(ChainHost<F32> *c)
+    {
+        const size_t Np = c->d.N_pad;
+        const std::vector<float> one(Np, 1.0f);
+        cudaError_t e;
+        if ((e = cudaMemsetAsync(c->d.lev_s, 0, 5 * Np * 4, c->stream)) != cudaSuccess) return e;
+        if ((e = cudaMemcpyAsync(c->d.lev_s + 3 * Np, one.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;   // gain_linear = 1
+        return cudaMemcpyAsync(c->d.lev_s + 4 * Np, one.data(), Np * 4, cudaMemcpyHostToDevice, c->stream);                                // gain_prev_linear = 1
+    }
+
+    static void leveller_sections(ChainHost<F32> *c, Sections &v) { v.push_back({ c->d.lev_s, (size_t)5 * c->d.N_pad * 4 }); }
+
+    // volumes, preamp, loudness shelves and matrix / output gains of instance i of a set_params call
+    static void pack(const dspi_chain_params_f32 &p, uint32_t i, uint32_t n, ParamRows<F32> &r)
+    {
+        // usb_audio.c:569-571
+        float vol_mul = p.host_mute ? 0.0f : (float)p.host_vol_mul * (1.0f / 32768.0f);
+        r.vbase[i] = vol_mul;
+        r.vmaster[i] = p.master_volume_linear;
+        r.pmg[i] = p.preset_mute_gain;
+        vol_mul *= p.preset_mute_gain;
+        const float vol_mul_master = vol_mul * p.master_volume_linear;
+        r.preamp[0 * n + i] = p.preamp_linear[0];
+        r.preamp[1 * n + i] = p.preamp_linear[1];
+        for (int o = 0; o < kOuts; o++) {
+            const dspi_output_channel &oc = p.matrix.outputs[o];
+            const dspi_matrix_crosspoint &xl = p.matrix.crosspoints[0][o], &xr = p.matrix.crosspoints[1][o];
+            float a = 0.0f, b = 0.0f;                                        // :760-764
+            if (xl.enabled) a = xl.phase_invert ? -xl.gain_linear : xl.gain_linear;
+            if (xr.enabled) b = xr.phase_invert ? -xr.gain_linear : xr.gain_linear;
+            r.gl[o * n + i] = a;
+            r.gr[o * n + i] = b;
+            r.gain[o * n + i] = oc.mute ? 0.0f : oc.gain_linear * vol_mul_master;    // :886-887
+        }
+        for (int j = 0; j < 2; j++) {
+            const float v[6] = { p.loudness[j].sva1, p.loudness[j].sva2, p.loudness[j].sva3, p.loudness[j].svm0, p.loudness[j].svm1, p.loudness[j].svm2 };
+            for (int k = 0; k < 6; k++) r.loud_c[(j * 6 + k) * n + i] = v[k];
+        }
+    }
+};
 
 }  // namespace
 }  // namespace dspi
 
-using dspi::ChainDev;
-using dspi::fail;
-
-#define CU_OK(expr)                                                                                         \
-    do {                                                                                                    \
-        cudaError_t err__ = (expr);                                                                         \
-        if (err__ != cudaSuccess) return fail(DSPI_ECUDA, "%s -> %s (%s:%d)", #expr, cudaGetErrorString(err__), __FILE__, __LINE__); \
-    } while (0)
-
-struct dspi_chain {
-    dspi_chain_desc desc;
-    ChainDev d;
-    cudaStream_t stream;                  // the engine stream callers see; stages run on st.* between ev_begin and ev_done
-    dspi::ChainStreams st;
-    dspi_biquad_f32 *d_aos;          // [N_pad][11][12] instance-major mirror of filters[][]
-    dspi_eq *eq_m, *eq_o;            // K1 engines over the master rows (2 N_pad channels) and the output rows (9 N_pad)
-    std::vector<void *> allocs;
-    uint64_t launches;
-    void *d_pcm; size_t pcm_bytes;   // host-path staging
-    int32_t *d_spdif; size_t spdif_bytes;   // host-path staging of the S/PDIF output, words or subframes
-    uint32_t *d_pdmout; size_t pdmout_bytes;
-    dspi_status *d_status;
-    dspi::SpdifTx tx;                // S/PDIF transmitter state; not part of the state blob (dspi_chain_get/set_spdif_tx)
-    uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
-    uint32_t vmm_packets;            // capacity of d.vmm in packets
-    dspi::PacketSchedule sched;      // packet lengths of the current call
-    dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chain_response_*
-    dspi::bulk::Stage bulk;          // device staging of dspi_chain_apply_bulk_device / _collect_bulk_device, allocated by the first call
-    dspi::bulk::PresetStage preset;  // device staging of dspi_chain_apply_preset_device / _collect_preset_device, allocated by the first call
-    dspi::bulk::Record rec;          // wire-visible configuration of every instance (dspi_chain_collect_bulk_device); not part of the state blob
-};
-
-namespace {
-
-template <typename T>
-cudaError_t dev_alloc(dspi_chain *c, T **p, size_t count, bool zero = true)
-{
-    void *q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
-    if (e != cudaSuccess) return e;
-    c->allocs.push_back(q);
-    *p = (T *)q;
-    return zero ? cudaMemsetAsync(q, 0, count * sizeof(T), c->stream) : cudaSuccess;
-}
-
-// state that leveller_reset_state() / the PDM restart path define as non-zero
-cudaError_t init_states(dspi_chain *c)
-{
-    const uint32_t Np = c->d.N_pad;
-    std::vector<float> one(Np, 1.0f);
-    std::vector<int32_t> seed(Np, 123456789);                               // pdm_generator.c:62
-    cudaError_t e;
-    if ((e = cudaMemsetAsync(c->d.lev_s, 0, (size_t)5 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemcpyAsync(c->d.lev_s + 3 * Np, one.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;   // gain_linear = 1
-    if ((e = cudaMemcpyAsync(c->d.lev_s + 4 * Np, one.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;   // gain_prev_linear = 1
-    if ((e = cudaMemsetAsync(c->d.lev_idx, 0, (size_t)Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.lev_la, 0, (size_t)2 * dspi::kLa * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.loud_st, 0, (size_t)8 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.dline, 0, (size_t)dspi::kOuts * dspi::kMaxDelay * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.widx_in, 0, (size_t)Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.widx_out, 0, (size_t)Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.pdm, 0, (size_t)9 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemcpyAsync(c->d.pdm + 7 * Np, seed.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.peaks, 0, (size_t)dspi::kRoles * Np * 2, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.clip, 0, (size_t)Np * 2, c->stream)) != cudaSuccess) return e;
-    return cudaStreamSynchronize(c->stream);
-}
-
-// a new engine's transmitters: block position 0, the channel status init_spdif_buffer() stamps (audio_spdif.c:82-88)
-cudaError_t init_spdif_tx(dspi_chain *c)
-{
-    const std::vector<uint64_t> cs(c->d.N_pad, dspi::kSpdifDefaultCs40);
-    cudaError_t e = cudaMemsetAsync(c->tx.bp, 0, (size_t)c->d.N_pad * 4, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(c->tx.cs40, cs.data(), (size_t)c->d.N_pad * 8, cudaMemcpyHostToDevice, c->stream);
-    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
-}
-
-// one call over the schedule c->sched has checked: its offsets go to the device first, on the engine stream
-// d_spdif: words, or subframes when `subframes` is set (either may be NULL)
-template <bool FUSED>
-int launch_chain(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, void *d_spdif, bool subframes,
-                 uint32_t *d_pdm, dspi_status *d_status)
-{
-    dspi::PacketSchedule &ps = c->sched;
-    const uint32_t n_packets = ps.n_packets, F = ps.frames;
-    CU_OK(ps.upload(packet_frames, c->stream, &c->launches));
-    auto post = dspi::chain_post_kernel<FUSED>;
-    const size_t post_smem = (size_t)4 * 2 * ps.longest * dspi::kXs * 4;    // 4 warps x (longest packet + look-ahead columns)
-    static dspi::PerDeviceOnce once;                                // per instantiation (flavour)
-    int dev = 0;
-    if (once.needs(&dev)) {
-        CU_OK(cudaFuncSetAttribute(post, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)4 * 2 * dspi::kPkt * dspi::kXs * 4)));
-        once.mark(dev);
-    }
-    // Stage pipeline over packet slices on three streams (chain_streams.cuh): front stages of slice
-    // i+1 overlap the output stages of slice i and the modulator of slice i-1.
-    dspi::ChainStreams &st = c->st;
-    uint32_t slice_bounds[dspi::ChainStreams::kMaxSlices + 1];
-    const uint32_t n_slices = (uint32_t)dspi::ChainStreams::plan_slices(n_packets, slice_bounds);
-    if (c->env_instances) {                                                  // preset-mute envelope: this call's per-packet volumes
-        if (c->vmm_packets < n_packets) {
-            CU_OK(cudaStreamSynchronize(c->stream));
-            if (c->d.vmm) CU_OK(cudaFree(c->d.vmm));
-            c->d.vmm = nullptr; c->vmm_packets = 0;
-            CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(float)));
-            c->vmm_packets = n_packets;
-        }
-        dspi::chain_env_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets);
-        CU_OK(cudaGetLastError());
-        c->launches++;
-    }
-    const ChainDev d = c->d;
-    const uint32_t n_sms = st.stream_sms();
-    static const uint32_t kStreamCtas = [] { const char *e = getenv("DSPI_CHAIN_CTAS"); const int v = e ? atoi(e) : 0; return (uint32_t)(v >= 1 && v <= 8 ? v : 8); }();   // streaming CTAs (256 threads) per SM
-    CU_OK(cudaEventRecord(st.ev_begin, c->stream));
-    CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
-    for (uint32_t sl = 0; sl < n_slices; sl++) {
-        const uint32_t p0 = slice_bounds[sl], p1 = slice_bounds[sl + 1];
-        const uint32_t fb = ps.off[p0], fe = ps.off[p1];
-        int rc;
-        // ---- front: unpack + loudness -> master EQ (K1) -> leveller + crossfeed
-        dspi::chain_pre_kernel<FUSED><<<(d.N_pad / 16 + 1) / 2, 64, 0, st.s_front>>>(d, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
-        CU_OK(cudaGetLastError());
-        if ((rc = dspi::eq_process_on(c->eq_m, d.mrow + fb, fe - fb, d.ldF, st.s_front)) != DSPI_OK) return rc;
-        post<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, ps.longest);
-        CU_OK(cudaGetLastError());
-        CU_OK(cudaEventRecord(st.ev_front[sl], st.s_front));
-        // ---- outputs: matrix -> per-output EQ (K1) -> gain / delay / metering / conversion
-        CU_OK(cudaStreamWaitEvent(st.s_out, st.ev_front[sl], 0));
-        dspi::chain_mix_kernel<FUSED><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
-        CU_OK(cudaGetLastError());
-        if ((rc = dspi::eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
-        if (subframes && d_spdif)
-            dspi::chain_outpost_kernel<true><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
-        else
-            dspi::chain_outpost_kernel<false><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
-        CU_OK(cudaGetLastError());
-        CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
-        // ---- modulator
-        CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_out[sl], 0));
-        dspi::chain_pdm_kernel<<<(d.N + 127) / 128, 128, 0, st.s_pdm>>>(d, fb, fe, F, d_pdm);
-        CU_OK(cudaGetLastError());
-        c->launches += 5;
-    }
-    dspi::chain_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets, c->tx.bp);   // after the last outpost launch (stream order)
-    CU_OK(cudaGetLastError());
-    c->launches++;
-    std::swap(c->d.widx_in, c->d.widx_out);
-    CU_OK(cudaEventRecord(st.ev_aux, st.s_out));                             // ring update done
-    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_aux, 0));
-    // the last modulator launch is ordered after every other stage launch of this call
-    CU_OK(cudaEventRecord(st.ev_done, st.s_pdm));
-    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_done, 0));                    // later work on the engine stream sees all outputs
-    if (d_status) {
-        dspi::chain_status_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, d_status);
-        CU_OK(cudaGetLastError());
-        c->launches++;
-    }
-    return DSPI_OK;
-}
-
-}  // namespace
+struct dspi_chain : dspi::ChainHost<dspi::F32> {};
 
 extern "C" {
 
@@ -1033,711 +952,111 @@ int32_t dspi_delay_samples(float delay_ms, float sample_rate, int is_last)
     return s;
 }
 
-int dspi_chain_destroy(dspi_chain *c)
-{
-    if (!c) return DSPI_OK;
-    cudaSetDevice(c->desc.device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    c->st.destroy();
-    c->sched.destroy();
-    c->resp.destroy();
-    c->bulk.destroy();
-    c->preset.destroy();
-    if (c->eq_m) dspi_eq_destroy(c->eq_m);
-    if (c->eq_o) dspi_eq_destroy(c->eq_o);
-    for (void *p : c->allocs) cudaFree(p);
-    if (c->d_pcm) cudaFree(c->d_pcm);
-    if (c->d_spdif) cudaFree(c->d_spdif);
-    if (c->d_pdmout) cudaFree(c->d_pdmout);
-    if (c->d.vmm) cudaFree(c->d.vmm);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
-    cudaGetLastError();
-    return DSPI_OK;
-}
+int dspi_chain_destroy(dspi_chain *c) { return dspi::destroy(c); }
+int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc) { return dspi::create(out, desc); }
+int dspi_chain_reset_state(dspi_chain *c) { return dspi::reset_state(c); }
 
-int dspi_chain_create(dspi_chain **out, const dspi_chain_desc *desc)
-{
-    if (!out || !desc) return fail(DSPI_EINVAL, "null argument");
-    *out = nullptr;
-    if (desc->arith != DSPI_ARITH_F32_FUSED && desc->arith != DSPI_ARITH_F32_STRICT) return fail(DSPI_EINVAL, "chain engines are float (arith 0 or 1)");
-    if (desc->n_instances == 0 || desc->max_frames == 0) return fail(DSPI_EINVAL, "n_instances and max_frames must be > 0");
-    if (desc->n_bands != 10) return fail(DSPI_EINVAL, "chain engines run channel_band_counts = 10");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPI_ENODEV, "no CUDA device (there is no CPU fallback)"); }
-    if (desc->device < 0 || desc->device >= ndev) return fail(DSPI_ENODEV, "device %d out of range", desc->device);
-    int major = 0;
-    CU_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, desc->device));
-    if (major != 9) return fail(DSPI_ENODEV, "device %d is not sm_90", desc->device);
-    CU_OK(cudaSetDevice(desc->device));
-    dspi_chain *c = new (std::nothrow) dspi_chain();
-    if (!c) return fail(DSPI_ENOMEM, "host allocation failed");
-    c->stream = nullptr;
-    c->st = dspi::ChainStreams();
-    c->sched = dspi::PacketSchedule();
-    c->eq_m = c->eq_o = nullptr;
-    c->d_aos = nullptr; c->launches = 0; c->d_pcm = nullptr; c->pcm_bytes = 0; c->d_spdif = nullptr; c->spdif_bytes = 0;
-    c->d_pdmout = nullptr; c->pdmout_bytes = 0; c->d_status = nullptr;
-    c->env_instances = 0; c->vmm_packets = 0;
-    c->tx.bp = nullptr; c->tx.cs40 = nullptr;
-    c->desc = *desc;
-    ChainDev &d = c->d;
-    memset(&d, 0, sizeof(d));
-    d.N = desc->n_instances;
-    d.N_pad = (d.N + 31) / 32 * 32;
-    d.nb = desc->n_bands;
-    d.max_frames = desc->max_frames;
-    d.ldF = (d.max_frames + 3u) & ~3u;
-    const size_t Np = d.N_pad;
-    {
-        dspi_eq_desc ed;
-        memset(&ed, 0, sizeof(ed));
-        ed.arith = desc->arith; ed.n_bands = desc->n_bands; ed.device = desc->device;
-        ed.n_channels = 2 * d.N_pad;
-        int rc = dspi_eq_create(&c->eq_m, &ed);
-        ed.n_channels = dspi::kOuts * d.N_pad;
-        if (rc == DSPI_OK) rc = dspi_eq_create(&c->eq_o, &ed);
-        if (rc != DSPI_OK) { dspi_chain_destroy(c); return rc; }
-    }
-    cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = c->st.create(desc->device, desc->n_instances);
-#define TRY(x) if (e == cudaSuccess) e = (x)
-    TRY(c->sched.create(d.max_frames));
-    d.off = c->sched.d_off;
-    TRY(dev_alloc(c, &c->d_aos, Np * dspi::kRoles * DSPI_MAX_BANDS));
-    TRY(dev_alloc(c, &d.preamp, 2 * Np));
-    TRY(dev_alloc(c, &d.flags, Np));
-    TRY(dev_alloc(c, &d.loud_c, 12 * Np));
-    TRY(dev_alloc(c, &d.loud_st, 8 * Np));
-    TRY(dev_alloc(c, &d.loud_byp, Np));
-    TRY(dev_alloc(c, &d.xf, 7 * Np));
-    TRY(dev_alloc(c, &d.lev_c, 9 * Np));
-    TRY(dev_alloc(c, &d.lev_s, 5 * Np));
-    TRY(dev_alloc(c, &d.lev_idx, Np));
-    TRY(dev_alloc(c, &d.lev_la, (size_t)2 * dspi::kLa * Np));
-    TRY(dev_alloc(c, &d.o_gl, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_gr, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_gain, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_flags, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_dly, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.dline, (size_t)dspi::kOuts * dspi::kMaxDelay * Np));
-    TRY(dev_alloc(c, &d.widx_in, Np));
-    TRY(dev_alloc(c, &d.widx_out, Np));
-    TRY(dev_alloc(c, &d.pdm, 9 * Np));
-    TRY(dev_alloc(c, &d.peaks, dspi::kRoles * Np));
-    TRY(dev_alloc(c, &d.clip, Np));
-    TRY(dev_alloc(c, &d.mrow, (size_t)2 * Np * d.ldF));
-    TRY(dev_alloc(c, &d.orow, (size_t)dspi::kOuts * Np * d.ldF));
-    TRY(dev_alloc(c, &d.subq, (size_t)Np * d.ldF));
-    TRY(dev_alloc(c, &d.skip_m, 2 * Np));
-    TRY(dev_alloc(c, &d.skip_o, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &c->d_status, Np));
-    TRY(dev_alloc(c, &d.env, 5 * Np));
-    TRY(dev_alloc(c, &d.vol_base, Np));
-    TRY(dev_alloc(c, &d.vol_master, Np));
-    TRY(dev_alloc(c, &d.o_glin, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.pmg, Np));
-    TRY(dev_alloc(c, &c->tx.bp, Np));
-    TRY(dev_alloc(c, &c->tx.cs40, Np));
-    TRY(dev_alloc(c, &c->rec.packets, Np));
-    TRY(dev_alloc(c, &c->rec.host, Np));
-    TRY(dev_alloc(c, &c->rec.mark, Np));
-    TRY(cudaMemsetAsync(c->rec.mark, DSPI_BULK_UNSET, Np, c->stream));
-    TRY(init_states(c));
-    TRY(init_spdif_tx(c));
-#undef TRY
-    if (e != cudaSuccess) {
-        fail(e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA, "chain setup: %s", cudaGetErrorString(e));
-        dspi_chain_destroy(c);
-        return e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA;
-    }
-    *out = c;
-    return DSPI_OK;
-}
+int dspi_chain_set_params(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_chain_params_f32 *params) { return dspi::set_params(c, inst0, n, params); }
 
-int dspi_chain_reset_state(dspi_chain *c)
-{
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(init_states(c));
-    return DSPI_OK;
-}
-
-int dspi_chain_set_params(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_chain_params_f32 *params)
-{
-    if (!c || !params) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const ChainDev &d = c->d;
-    const size_t Np = d.N_pad;
-    std::vector<float> preamp(2 * n), loud_c(12 * n), xf(7 * n), lev_c(9 * n), gl(9 * n), gr(9 * n), gain(9 * n), glin(9 * n), vbase(n), vmaster(n), pmgv(n);
-    std::vector<uint8_t> flags(n), loud_byp(n), oflags(9 * n), skip_m(2 * n), skip_o(9 * n);
-    std::vector<int32_t> dly(9 * n);
-    std::vector<float> xf_cur(7 * n);
-    CU_OK(cudaMemcpy2DAsync(xf_cur.data(), (size_t)n * 4, d.xf + inst0, Np * 4, (size_t)n * 4, 7, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    for (uint32_t i = 0; i < n; i++) {
-        const dspi_chain_params_f32 &p = params[i];
-        // usb_audio.c:569-571
-        float vol_mul = p.host_mute ? 0.0f : (float)p.host_vol_mul * (1.0f / 32768.0f);
-        vbase[i] = vol_mul;
-        vmaster[i] = p.master_volume_linear;
-        pmgv[i] = p.preset_mute_gain;
-        vol_mul *= p.preset_mute_gain;
-        const float vol_mul_master = vol_mul * p.master_volume_linear;
-        preamp[0 * n + i] = p.preamp_linear[0];
-        preamp[1 * n + i] = p.preamp_linear[1];
-        bool any_delay = false;
-        for (int o = 0; o < dspi::kOuts; o++) {
-            const dspi_output_channel &oc = p.matrix.outputs[o];
-            const dspi_matrix_crosspoint &xl = p.matrix.crosspoints[0][o], &xr = p.matrix.crosspoints[1][o];
-            float a = 0.0f, b = 0.0f;                                        // :760-764
-            if (xl.enabled) a = xl.phase_invert ? -xl.gain_linear : xl.gain_linear;
-            if (xr.enabled) b = xr.phase_invert ? -xr.gain_linear : xr.gain_linear;
-            gl[o * n + i] = a;
-            gr[o * n + i] = b;
-            gain[o * n + i] = oc.mute ? 0.0f : oc.gain_linear * vol_mul_master;    // :886-887
-            glin[o * n + i] = oc.gain_linear;
-            const bool has_pair = o < dspi::kOuts - 1;                       // :930-933
-            oflags[o * n + i] = dspi::output_flags(oc.enabled, oc.mute, has_pair, has_pair && p.matrix.outputs[o ^ 1].enabled);
-            skip_o[o * n + i] = dspi::ParamStores::output_eq_frozen(oc.enabled, oc.mute, p.bypass_master_eq) ? 1 : 0;   // :878-884: state frozen
-            int32_t ds = oc.delay_samples;
-            if (ds > DSPI_CHAIN_MAX_DELAY) ds = DSPI_CHAIN_MAX_DELAY;
-            if (ds < 0) ds = 0;
-            dly[o * n + i] = ds;
-            if (ds > 0) any_delay = true;                                    // dsp_pipeline.c:237
-        }
-        flags[i] = dspi::chain_flags(p.bypass_master_eq, p.loudness_enabled, p.crossfeed_enabled, p.leveller_enabled, p.leveller_lookahead, any_delay,
-                                     p.matrix.outputs[dspi::kOuts - 1].enabled);
-        skip_m[0 * n + i] = skip_m[1 * n + i] = p.bypass_master_eq ? 1 : 0;   // :721-728
-        loud_byp[i] = (p.loudness[0].bypass ? 1 : 0) | (p.loudness[1].bypass ? 2 : 0);
-        for (int j = 0; j < 2; j++) {
-            const float v[6] = { p.loudness[j].sva1, p.loudness[j].sva2, p.loudness[j].sva3, p.loudness[j].svm0, p.loudness[j].svm1, p.loudness[j].svm2 };
-            for (int k = 0; k < 6; k++) loud_c[(j * 6 + k) * n + i] = v[k];
-        }
-        const float xv[7] = { p.crossfeed.lp_a0, p.crossfeed.lp_b1, p.crossfeed.lp_state_L, p.crossfeed.lp_state_R,
-                              p.crossfeed.ap_a, p.crossfeed.ap_state_L, p.crossfeed.ap_state_R };
-        // crossfeed_compute_coefficients() is the only writer of crossfeed_state in the firmware and it clears the filter
-        // state (crossfeed.c:35-127); a volume / mute / matrix update never touches it.  So the record's state rows are
-        // taken only when its coefficients differ from the ones in force; otherwise the running state is kept.
-        const bool xf_same = xv[0] == xf_cur[0 * n + i] && xv[1] == xf_cur[1 * n + i] && xv[4] == xf_cur[4 * n + i];
-        for (int k = 0; k < 7; k++) {
-            const bool is_state = k == 2 || k == 3 || k == 5 || k == 6;
-            xf[k * n + i] = (is_state && xf_same) ? xf_cur[k * n + i] : xv[k];
-        }
-        const float *lv = &p.leveller.alpha_rms;
-        for (int k = 0; k < 9; k++) lev_c[k * n + i] = lv[k];
-    }
-    auto put = [&](void *dst_base, const void *src, int rows, size_t elem) -> cudaError_t {
-        return cudaMemcpy2DAsync((char *)dst_base + (size_t)inst0 * elem, Np * elem, src, (size_t)n * elem, (size_t)n * elem, rows,
-                                 cudaMemcpyHostToDevice, c->stream);
-    };
-    CU_OK(put(d.preamp, preamp.data(), 2, 4));
-    CU_OK(put(d.flags, flags.data(), 1, 1));
-    CU_OK(put(d.loud_c, loud_c.data(), 12, 4));
-    CU_OK(put(d.loud_byp, loud_byp.data(), 1, 1));
-    CU_OK(put(d.xf, xf.data(), 7, 4));
-    CU_OK(put(d.lev_c, lev_c.data(), 9, 4));
-    CU_OK(put(d.o_gl, gl.data(), 9, 4));
-    CU_OK(put(d.o_gr, gr.data(), 9, 4));
-    CU_OK(put(d.o_gain, gain.data(), 9, 4));
-    CU_OK(put(d.o_glin, glin.data(), 9, 4));
-    CU_OK(put(d.vol_base, vbase.data(), 1, 4));
-    CU_OK(put(d.vol_master, vmaster.data(), 1, 4));
-    CU_OK(put(d.pmg, pmgv.data(), 1, 4));
-    CU_OK(put(d.o_flags, oflags.data(), 9, 1));
-    CU_OK(put(d.o_dly, dly.data(), 9, 4));
-    CU_OK(put(d.skip_m, skip_m.data(), 2, 1));
-    CU_OK(dspi::bulk::mark_stale(c->rec, inst0, n, c->stream));
-    CU_OK(put(d.skip_o, skip_o.data(), 9, 1));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    int rc = dspi::eq_set_skip(c->eq_m, d.skip_m, c->stream);
-    if (rc == DSPI_OK) rc = dspi::eq_set_skip(c->eq_o, d.skip_o, c->stream);
-    return rc;
-}
-
-/* preset-mute envelope of instances [inst0, inst0+n): states == NULL leaves envelope mode (the constant
- * preset_mute_gain of dspi_chain_set_params applies again) */
 int dspi_chain_set_preset_mute(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
 {
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t Np = c->d.N_pad;
-    std::vector<uint32_t> cur((size_t)n), rows((size_t)5 * n, 0u);
-    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    for (uint32_t i = 0; i < n; i++) {
-        if (cur[i]) c->env_instances--;
-        if (states) {
-            rows[0 * n + i] = states[i].loading ? 1u : 0u;
-            rows[1 * n + i] = states[i].counter;
-            memcpy(&rows[2 * n + i], &states[i].smooth_gain, 4);
-            rows[3 * n + i] = sample_rate_hz;
-            rows[4 * n + i] = 1u;
-            c->env_instances++;
-        }
-    }
-    CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, Np * 4, rows.data(), (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    return dspi::set_preset_mute(c, inst0, n, states, sample_rate_hz);
 }
 
-int dspi_chain_get_preset_mute(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states)
-{
-    if (!c || !states) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t Np = c->d.N_pad;
-    std::vector<uint32_t> rows((size_t)3 * n);
-    CU_OK(cudaMemcpy2DAsync(rows.data(), (size_t)n * 4, c->d.env + inst0, Np * 4, (size_t)n * 4, 3, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    for (uint32_t i = 0; i < n; i++) {
-        memset(&states[i], 0, sizeof(states[i]));
-        states[i].loading = (uint8_t)rows[0 * n + i];
-        states[i].counter = rows[1 * n + i];
-        memcpy(&states[i].smooth_gain, &rows[2 * n + i], 4);
-    }
-    return DSPI_OK;
-}
+int dspi_chain_get_preset_mute(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states) { return dspi::get_preset_mute(c, inst0, n, states); }
 
-/* crossfeed / leveller / loudness coefficients and the host volume of instances [inst0, inst0+n) generated ON THE GPU */
 int dspi_chain_set_dynamics_device(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_dynamics_config *cfgs, float sample_rate)
 {
-    if (!c || !cfgs) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    dspi_dynamics_config *d_cfg = nullptr;
-    CU_OK(cudaMalloc((void **)&d_cfg, (size_t)n * sizeof(*cfgs)));
-    cudaError_t e = cudaMemcpyAsync(d_cfg, cfgs, (size_t)n * sizeof(*cfgs), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
-        dspi::chain_dynamics_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, c->rec, inst0, n, d_cfg, sample_rate);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cudaFree(d_cfg);
-    if (e != cudaSuccess) return fail(DSPI_ECUDA, "dynamics coefficient generation: %s", cudaGetErrorString(e));
-    c->launches++;
-    return DSPI_OK;
+    return dspi::set_dynamics_device(c, inst0, n, cfgs, sample_rate);
 }
 
 int dspi_chain_apply_bulk_device(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
                                  int exact_db, float sample_rate, int32_t *results)
 {
-    if (!c || !packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
-    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::apply<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, exact_db, sample_rate, results);
+    return dspi::apply_bulk_device(c, inst0, n, packets, host, exact_db, sample_rate, results);
 }
 
 int dspi_chain_collect_bulk_device(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
 {
-    if (!c || !packets) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::collect<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, results);
+    return dspi::collect_bulk_device(c, inst0, n, packets, host, results);
 }
 
 int dspi_chain_apply_preset_device(dspi_chain *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride, const dspi_preset_load *load,
-                               const dspi_bulk_host *host, float sample_rate, int32_t *results)
+                                   const dspi_bulk_host *host, float sample_rate, int32_t *results)
 {
-    if (!c || !images || !load || !host || !results) return fail(DSPI_EINVAL, "null argument");
-    if (image_stride < sizeof(dspi::bulk::SlotOf<dspi::ParamStores>)) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, sizeof(dspi::bulk::SlotOf<dspi::ParamStores>));
-    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::apply_preset<dspi::ParamStores>(c, c->bulk, c->preset, inst0, n, images, image_stride, load, host, sample_rate, results);
+    return dspi::apply_preset_device(c, inst0, n, images, image_stride, load, host, sample_rate, results);
 }
 
-int dspi_chain_collect_preset_device(dspi_chain *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride, int32_t *results)
+int dspi_chain_collect_preset_device(dspi_chain *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
+                                     int32_t *results)
 {
-    if (!c || !slot_indices || !images) return fail(DSPI_EINVAL, "null argument");
-    if (image_stride < sizeof(dspi::bulk::SlotOf<dspi::ParamStores>)) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, sizeof(dspi::bulk::SlotOf<dspi::ParamStores>));
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::collect_preset<dspi::ParamStores>(c, c->preset, inst0, n, slot_indices, images, image_stride, results);
+    return dspi::collect_preset_device(c, inst0, n, slot_indices, images, image_stride, results);
 }
 
-int dspi_chain_upload_biquads(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_biquad_f32 *biquads)
-{
-    if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t row = (size_t)dspi::kRoles * DSPI_MAX_BANDS;
-    CU_OK(cudaMemcpyAsync(c->d_aos + inst0 * row, biquads, n * row * sizeof(dspi_biquad_f32), cudaMemcpyHostToDevice, c->stream));
-    const uint32_t Np = c->d.N_pad, items = n * dspi::kRoles * DSPI_MAX_BANDS;
-    dspi::chain_scatter_kernel<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_m),
-                                                                          (dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_o), 1);
-    CU_OK(cudaGetLastError());
-    c->launches++;
-    for (int role = 0; role < dspi::kRoles; role++) {
-        int rc = role < 2 ? dspi::eq_pack_range(c->eq_m, role * Np + inst0, n, c->stream)
-                          : dspi::eq_pack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
-        if (rc) return rc;
-    }
-    CU_OK(dspi::bulk::mark_stale(c->rec, inst0, n, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
+int dspi_chain_upload_biquads(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_biquad_f32 *biquads) { return dspi::upload_biquads(c, inst0, n, biquads); }
+int dspi_chain_download_biquads(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_biquad_f32 *biquads) { return dspi::download_biquads(c, inst0, n, biquads); }
 
 int dspi_chain_set_eq_params_device(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_eq_param *recipes, float sample_rate)
 {
-    if (!c || !recipes) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    // the sub-engines generate and pack on their own streams: everything issued on the engine stream so far (an
-    // asynchronous process_device in particular) must have finished reading the coefficient stores first
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    const uint32_t Np = c->d.N_pad;
-    std::vector<dspi_eq_param> tmp((size_t)n * DSPI_MAX_BANDS);
-    for (int role = 0; role < dspi::kRoles; role++) {               // filter_recipes[role][band] of every instance -> one engine range per role
-        for (uint32_t i = 0; i < n; i++)
-            memcpy(&tmp[(size_t)i * DSPI_MAX_BANDS], &recipes[((size_t)i * dspi::kRoles + role) * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
-        int rc = role < 2 ? dspi_eq_set_params_device(c->eq_m, role * Np + inst0, n, tmp.data(), sample_rate)
-                          : dspi_eq_set_params_device(c->eq_o, (role - 2) * Np + inst0, n, tmp.data(), sample_rate);
-        if (rc) return rc;
-        for (uint32_t i = 0; i < n; i++)                            // the clamps, written back like the reference does
-            memcpy(&recipes[((size_t)i * dspi::kRoles + role) * DSPI_MAX_BANDS], &tmp[(size_t)i * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
-    }
-    return dspi::bulk::record_recipes<dspi::ParamStores>(c, c->bulk, inst0, n, recipes);
+    return dspi::set_eq_params_device(c, inst0, n, recipes, sample_rate);
 }
 
-int dspi_chain_download_biquads(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_biquad_f32 *biquads)
-{
-    if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const uint32_t Np = c->d.N_pad, items = n * dspi::kRoles * DSPI_MAX_BANDS;
-    for (int role = 0; role < dspi::kRoles; role++) {
-        int rc = role < 2 ? dspi::eq_unpack_range(c->eq_m, role * Np + inst0, n, c->stream)
-                          : dspi::eq_unpack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
-        if (rc) return rc;
-    }
-    dspi::chain_scatter_kernel<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_m),
-                                                                          (dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_o), 0);
-    CU_OK(cudaGetLastError());
-    c->launches++;
-    const size_t row = (size_t)dspi::kRoles * DSPI_MAX_BANDS;
-    CU_OK(cudaMemcpyAsync(biquads, c->d_aos + inst0 * row, n * row * sizeof(dspi_biquad_f32), cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-static int check_process(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp)
-{
-    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
-    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
-    if (fpp == 0 || fpp > DSPI_PACKET_MAX) return fail(DSPI_EINVAL, "frames_per_packet must be 1..%d", DSPI_PACKET_MAX);
-    if (n_packets == 0) return fail(DSPI_EINVAL, "n_packets must be > 0");
-    if ((uint64_t)n_packets * fpp > c->desc.max_frames) return fail(DSPI_ERANGE, "%u frames exceed max_frames %u", n_packets * fpp, c->desc.max_frames);
-    return DSPI_OK;
-}
-
-static int check_packets(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames)
-{
-    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
-    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
-    const char *why = "";
-    const int rc = c->sched.check(n_packets, packet_frames, &why);
-    if (rc == DSPI_ERANGE) return fail(rc, "%s %u", why, c->desc.max_frames);
-    return rc ? fail(rc, "%s", why) : DSPI_OK;
-}
-
-static int process_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                          void *d_spdif, bool subframes, uint32_t *d_pdm, dspi_status *d_status)
-{
-    int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
-    if (rc) return rc;
-    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
-    CU_OK(cudaSetDevice(c->desc.device));
-    if (c->desc.arith == DSPI_ARITH_F32_FUSED) return launch_chain<true>(c, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
-    return launch_chain<false>(c, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
-}
-
-// host memory in and out, staged through the engine's device buffers
-static int process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                        void *spdif_out, bool subframes, uint32_t *pdm_out, dspi_status *status)
-{
-    int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
-    if (rc) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t N = c->desc.n_instances, F = c->sched.frames;
-    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 4 * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
-    if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
-    if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
-    if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; }
-    // the modulator writes the rows of instances with a sub only; the others go back to the caller as zeros, on every call
-    // (an earlier call's bits would be there otherwise: a sub switched off since, or a longer call's [N][F][8] layout)
-    if (pdm_out) CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream));
-    CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = process_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
-                        pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
-    if (rc) return rc;
-    if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(dspi_status), cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                      int32_t *d_spdif, uint32_t *d_pdm, dspi_status *d_status)
-{
-    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
-}
-
-int dspi_chain_process_packets_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                    int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status)
-{
-    return process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
-}
-
-int dspi_chain_process_subframes_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                        dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status *d_status)
-{
-    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
-}
-
-int dspi_chain_process_subframes_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                      dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status *status)
-{
-    return process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
-}
-
-int dspi_chain_set_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
-{
-    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    std::vector<uint32_t> bp(n);
-    std::vector<uint64_t> cs(n);
-    if (!dspi::spdif_tx_unpack(tx, n, bp.data(), cs.data())) return fail(DSPI_EINVAL, "block_pos must be 0..191");
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));   // behind earlier calls
-    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-int dspi_chain_get_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
-{
-    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    std::vector<uint32_t> bp(n);
-    std::vector<uint64_t> cs(n);
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaMemcpyAsync(bp.data(), c->tx.bp + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaMemcpyAsync(cs.data(), c->tx.cs40 + inst0, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    dspi::spdif_tx_pack(bp.data(), cs.data(), n, tx);
-    return DSPI_OK;
-}
-
-// the uniform schedule: n_packets packets of fpp frames
 int dspi_chain_process_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *d_spdif,
                               uint32_t *d_pdm, dspi_status *d_status)
 {
-    int rc = check_process(c, d_pcm, bit_depth, n_packets, fpp);
-    if (rc) return rc;
-    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
-    return dspi_chain_process_packets_device(c, d_pcm, bit_depth, n_packets, table.data(), d_spdif, d_pdm, d_status);
+    return dspi::process_uniform(c, d_pcm, bit_depth, n_packets, fpp, d_spdif, d_pdm, d_status, false);
 }
 
 int dspi_chain_process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif_out,
                             uint32_t *pdm_out, dspi_status *status)
 {
-    int rc = check_process(c, pcm, bit_depth, n_packets, fpp);
-    if (rc) return rc;
-    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
-    return dspi_chain_process_packets_host(c, pcm, bit_depth, n_packets, table.data(), spdif_out, pdm_out, status);
+    return dspi::process_uniform(c, pcm, bit_depth, n_packets, fpp, spdif_out, pdm_out, status, true);
 }
 
-
-// ---- checkpoint / resume: everything a later process call depends on besides the parameters ----------------
-static void state_sections(dspi_chain *c, std::vector<std::pair<void *, size_t>> &v, bool with_eq = true)
+int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                      int32_t *d_spdif, uint32_t *d_pdm, dspi_status *d_status)
 {
-    const size_t Np = c->d.N_pad;
-    v.push_back({ c->d.loud_st, 8 * Np * 4 });
-    v.push_back({ c->d.xf, 7 * Np * 4 });                                  // crossfeed coefficients and state (CrossfeedState)
-    v.push_back({ c->d.lev_s, 5 * Np * 4 });
-    v.push_back({ c->d.lev_idx, Np * 4 });
-    v.push_back({ c->d.lev_la, (size_t)2 * dspi::kLa * Np * 4 });
-    v.push_back({ c->d.dline, (size_t)dspi::kOuts * dspi::kMaxDelay * Np * 4 });
-    v.push_back({ c->d.widx_in, Np * 4 });
-    v.push_back({ c->d.pdm, 9 * Np * 4 });
-    v.push_back({ c->d.peaks, (size_t)dspi::kRoles * Np * 2 });
-    v.push_back({ c->d.clip, Np * 2 });
-    v.push_back({ c->d.env, 5 * Np * 4 });                                 // preset-mute envelope state and mode
-    if (!with_eq) return;
-    dspi::eq_state_sections(c->eq_m, v);
-    dspi::eq_state_sections(c->eq_o, v);
+    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
 }
 
-// Version 2 records the K1 geometry (channels per lane, DSPI_F32_CPL) that the two EQ engines' packed stores were laid out
-// for, so that a blob resumes in an engine created under either geometry.  Version 1 blobs have no such fields and are read
-// as one channel per lane.
-struct StateHeader { uint32_t magic, version, arith, n_instances, n_bands, n_sections; uint64_t bytes; uint32_t cpl_m, cpl_o; };
-static const uint32_t kStateMagic = 0x53505344u;          // "DSPS"
-static const size_t kHeaderV1 = offsetof(StateHeader, cpl_m);
-
-// blob size for this engine's shape with header `hdr` bytes and EQ stores laid out for cpl_m / cpl_o channels per lane
-static size_t state_bytes(dspi_chain *c, size_t hdr, int cpl_m, int cpl_o)
+int dspi_chain_process_packets_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                    int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status)
 {
-    std::vector<std::pair<void *, size_t>> v;
-    state_sections(c, v, false);
-    size_t n = hdr + dspi::eq_state_bytes(c->eq_m, cpl_m) + dspi::eq_state_bytes(c->eq_o, cpl_o);
-    for (auto &s : v) n += s.second;
-    return n;
+    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
 }
 
-size_t dspi_chain_state_size(dspi_chain *c)
+int dspi_chain_process_subframes_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                        dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status *d_status)
 {
-    if (!c) return 0;
-    return state_bytes(c, sizeof(StateHeader), dspi::eq_geometry(c->eq_m), dspi::eq_geometry(c->eq_o));
+    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
 }
 
-int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap)
+int dspi_chain_process_subframes_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                      dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status *status)
 {
-    if (!c || !blob) return fail(DSPI_EINVAL, "null argument");
-    const size_t need = dspi_chain_state_size(c);
-    if (cap < need) return fail(DSPI_ERANGE, "state blob needs %zu bytes, %zu given", need, cap);
-    CU_OK(cudaSetDevice(c->desc.device));
-    std::vector<std::pair<void *, size_t>> v;
-    state_sections(c, v);
-    StateHeader h = { kStateMagic, 2u, c->desc.arith, c->desc.n_instances, c->desc.n_bands, (uint32_t)v.size(), (uint64_t)need,
-                      (uint32_t)dspi::eq_geometry(c->eq_m), (uint32_t)dspi::eq_geometry(c->eq_o) };
-    memcpy(blob, &h, sizeof(h));
-    char *p = (char *)blob + sizeof(h);
-    for (auto &s : v) {
-        CU_OK(cudaMemcpyAsync(p, s.first, s.second, cudaMemcpyDeviceToHost, c->stream));
-        p += s.second;
-    }
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
 }
 
-int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len)
-{
-    if (!c || !blob) return fail(DSPI_EINVAL, "null argument");
-    std::vector<std::pair<void *, size_t>> v, all;
-    state_sections(c, v, false);
-    state_sections(c, all);
-    StateHeader h;
-    if (len < kHeaderV1) return fail(DSPI_EINVAL, "state blob too short");
-    memcpy(&h, blob, kHeaderV1);
-    h.cpl_m = h.cpl_o = 1;
-    if (h.magic != kStateMagic || (h.version != 1u && h.version != 2u))
-        return fail(DSPI_EINVAL, "not a dspi_b200 state blob (magic %08x version %u)", h.magic, h.version);
-    const size_t hdr = h.version == 1u ? kHeaderV1 : sizeof(h);
-    if (len < hdr) return fail(DSPI_EINVAL, "state blob too short");
-    memcpy(&h, blob, hdr);
-    if ((h.cpl_m != 1 && h.cpl_m != 2) || (h.cpl_o != 1 && h.cpl_o != 2))
-        return fail(DSPI_EINVAL, "state blob names an unknown K1 geometry (%u, %u channels per lane)", h.cpl_m, h.cpl_o);
-    if (h.arith != c->desc.arith || h.n_instances != c->desc.n_instances || h.n_bands != c->desc.n_bands || h.n_sections != all.size() ||
-        h.bytes != state_bytes(c, hdr, (int)h.cpl_m, (int)h.cpl_o) || len < h.bytes)
-        return fail(DSPI_EINVAL, "state blob belongs to a different engine shape (%u instances, arith %u, %llu bytes)", h.n_instances, h.arith,
-                    (unsigned long long)h.bytes);
-    CU_OK(cudaSetDevice(c->desc.device));
-    const char *p = (const char *)blob + hdr;
-    for (auto &s : v) {
-        CU_OK(cudaMemcpyAsync(s.first, p, s.second, cudaMemcpyHostToDevice, c->stream));
-        p += s.second;
-    }
-    CU_OK(cudaStreamSynchronize(c->stream));
-    int rc = dspi::eq_state_load(c->eq_m, p, (int)h.cpl_m, c->stream);
-    p += dspi::eq_state_bytes(c->eq_m, (int)h.cpl_m);
-    if (rc == DSPI_OK) rc = dspi::eq_state_load(c->eq_o, p, (int)h.cpl_o, c->stream);
-    if (rc) return rc;
-    rc = dspi::eq_state_imported(c->eq_m, c->stream);
-    if (rc == DSPI_OK) rc = dspi::eq_state_imported(c->eq_o, c->stream);
-    if (rc) return rc;
-    std::vector<uint32_t> on(c->d.N);
-    CU_OK(cudaMemcpyAsync(on.data(), c->d.env + (size_t)4 * c->d.N_pad, (size_t)c->d.N * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    c->env_instances = 0;
-    for (uint32_t v : on) c->env_instances += v ? 1u : 0u;
-    return DSPI_OK;
-}
+int dspi_chain_set_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx) { return dspi::set_spdif_tx(c, inst0, n, tx); }
+int dspi_chain_get_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx) { return dspi::get_spdif_tx(c, inst0, n, tx); }
 
-// Frequency response of instances [inst0, inst0 + n) on the engine stream; out: device [n][9][2][n_freqs] float2, or host
-// memory filled chunk by chunk through the staging buffer
-static int chain_response(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
-{
-    const char *why = "";
-    int rc = dspi::response_check_args(freqs, n_freqs, fs, out, &why);
-    if (rc) return fail(rc, "%s", why);
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(c->resp.upload(freqs, n_freqs, c->stream, &c->launches));
-    const dspi_biquad_f32 *m_aos = (const dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_m), *o_aos = (const dspi_biquad_f32 *)dspi::eq_aos_mirror(c->eq_o);
-    auto launch = [&](uint32_t i0, uint32_t m, void *dst) -> cudaError_t {
-        const dim3 grid((n_freqs + 127) / 128, m < 65535u ? m : 65535u);
-        dspi::chain_response_kernel<<<grid, 128, 0, c->stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
-        c->launches++;
-        return cudaGetLastError();
-    };
-    if (!host) {
-        CU_OK(launch(inst0, n, out));
-        return DSPI_OK;
-    }
-    const size_t row_bytes = (size_t)dspi::kOuts * 2 * n_freqs * 2 * sizeof(float);
-    uint32_t rows = 0;
-    CU_OK(c->resp.stage(row_bytes, n, c->stream, &rows));
-    for (uint32_t i = 0; i < n; i += rows) {
-        const uint32_t m = n - i < rows ? n - i : rows;
-        CU_OK(launch(inst0 + i, m, c->resp.d_stage));
-        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->stream));
-        CU_OK(cudaStreamSynchronize(c->stream));
-    }
-    return DSPI_OK;
-}
+size_t dspi_chain_state_size(dspi_chain *c) { return dspi::state_size(c); }
+int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap) { return dspi::state_export(c, blob, cap); }
+int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len) { return dspi::state_import(c, blob, len); }
 
 int dspi_chain_response_host(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
 {
-    return chain_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, out, true);
+    return dspi::response(c, inst0, n, freqs_hz, n_freqs, sample_rate, out, true);
 }
 
 int dspi_chain_response_device(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out)
 {
-    return chain_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
+    return dspi::response(c, inst0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
 }
 
-int dspi_chain_sync(dspi_chain *c)
-{
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-void *dspi_chain_stream(dspi_chain *c) { return c ? (void *)c->stream : nullptr; }
-/* SMs reserved for the modulator / left to every other stage (0, 0: no partition, see chain_streams.cuh) */
-int dspi_chain_sm_partition(dspi_chain *c, uint32_t *pdm_sms, uint32_t *rest_sms)
-{
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    if (pdm_sms) *pdm_sms = c->st.pdm_sms;
-    if (rest_sms) *rest_sms = c->st.rest_sms;
-    return DSPI_OK;
-}
-
-uint64_t dspi_chain_launch_count(dspi_chain *c)
-{
-    return c ? c->launches + dspi_eq_launch_count(c->eq_m) + dspi_eq_launch_count(c->eq_o) : 0;
-}
+int dspi_chain_sync(dspi_chain *c) { return dspi::sync(c); }
+void *dspi_chain_stream(dspi_chain *c) { return dspi::stream(c); }
+int dspi_chain_sm_partition(dspi_chain *c, uint32_t *pdm_sms, uint32_t *rest_sms) { return dspi::sm_partition(c, pdm_sms, rest_sms); }
+uint64_t dspi_chain_launch_count(dspi_chain *c) { return dspi::launch_count(c); }
 
 }  // extern "C"

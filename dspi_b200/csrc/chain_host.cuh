@@ -1,0 +1,921 @@
+// chain_host.cuh — the host half of the float and Q28 chain engines (chain_f32.cu, chain_q28.cu): engine record,
+// lifetime, argument checks, parameter uploads, the stage pipeline over packet slices, host staging, S/PDIF transmitter
+// state, checkpoints and the frequency response.  Host code only; each engine file includes it after its kernels.
+//
+// Everything here is a template over the engine's arithmetic traits A, which supply what differs between the two
+// engines: the types (A::Dev the device record, A::Biquad, A::Status, A::Params, A::Stores the device-side parameter
+// stores), the constants (A::kOuts, A::kRoles, A::kMaxDelay, A::kLoudRows coefficient rows of the loudness shelves,
+// A::kXs the post kernel's shared-memory column stride, A::kStateVersion of the blobs it writes), the kernels the host
+// launches (A::scatter, A::dynamics, A::response, and per kernel set K of A::with_stages: K::pre, K::post, K::mix,
+// K::outpost<SUBFRAMES>, K::ring, K::pdm, K::env, K::status) and the hooks
+//   A::check_desc(desc)                       arithmetic, instance / frame counts and band count of a new engine
+//   A::alloc_leveller(c), A::init_leveller(c) the leveller state arrays and their reset values
+//   A::pack(params, i, n, rows)               volumes, preamp, loudness and matrix / output gains of one instance
+//   A::leveller_sections(c, v)                the leveller state in the checkpoint
+// The code below never asks which arithmetic it serves.
+#pragma once
+#include <cstdarg>
+#include <cstddef>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <new>
+#include <type_traits>
+#include <utility>
+#include <vector>
+
+#include "bulk_ingest.cuh"
+#include "chain_schedule.cuh"
+#include "chain_streams.cuh"
+#include "eq_kernels.cuh"
+#include "response.cuh"
+#include "spdif_bmc.cuh"
+
+namespace dspi {
+namespace {
+
+int fail(int code, const char *fmt, ...)
+{
+    size_t cap = 0;
+    char *buf = error_buffer(&cap);
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, cap, fmt, ap);
+    va_end(ap);
+    return code;
+}
+
+#define CU_OK(expr)                                                                                         \
+    do {                                                                                                    \
+        cudaError_t err__ = (expr);                                                                         \
+        if (err__ != cudaSuccess) return fail(DSPI_ECUDA, "%s -> %s (%s:%d)", #expr, cudaGetErrorString(err__), __FILE__, __LINE__); \
+    } while (0)
+
+// One engine: dspi_chain and dspi_chainq are this record for their arithmetic.
+template <class A>
+struct ChainHost {
+    using Arith = A;
+    dspi_chain_desc desc;
+    typename A::Dev d;
+    cudaStream_t stream;             // the engine stream callers see; stages run on st.* between ev_begin and ev_done
+    ChainStreams st;
+    typename A::Biquad *d_aos;       // [N_pad][roles][12] instance-major mirror of filters[][]
+    dspi_eq *eq_m, *eq_o;            // EQ engines over the master rows (2 N_pad channels) and the output rows (kOuts N_pad)
+    std::vector<void *> allocs;
+    uint64_t launches;
+    void *d_pcm; size_t pcm_bytes;   // host-path staging
+    int32_t *d_spdif; size_t spdif_bytes;   // host-path staging of the S/PDIF output, words or subframes
+    uint32_t *d_pdmout; size_t pdmout_bytes;
+    typename A::Status *d_status;
+    SpdifTx tx;                      // S/PDIF transmitter state; not part of the state blob (*_get/set_spdif_tx)
+    uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
+    uint32_t vmm_packets;            // capacity of d.vmm in packets
+    PacketSchedule sched;            // packet lengths of the current call
+    ResponseBuffers resp;            // frequency table and host staging of *_response_*
+    bulk::Stage bulk;                // device staging of *_apply_bulk_device / _collect_bulk_device, allocated by the first call
+    bulk::PresetStage preset;        // device staging of *_apply_preset_device / _collect_preset_device, allocated by the first call
+    bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
+};
+
+template <class A, typename T>
+cudaError_t dev_alloc(ChainHost<A> *c, T **p, size_t count, bool zero = true)
+{
+    void *q = nullptr;
+    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
+    if (e != cudaSuccess) return e;
+    c->allocs.push_back(q);
+    *p = (T *)q;
+    return zero ? cudaMemsetAsync(q, 0, count * sizeof(T), c->stream) : cudaSuccess;
+}
+
+template <class A>
+int check_range(const ChainHost<A> *c, uint32_t inst0, uint32_t n)
+{
+    if ((uint64_t)inst0 + n > c->desc.n_instances)
+        return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    return DSPI_OK;
+}
+
+// state that leveller_reset_state() / the PDM restart path define as non-zero
+template <class A>
+cudaError_t init_states(ChainHost<A> *c)
+{
+    const size_t Np = c->d.N_pad;
+    std::vector<int32_t> seed(Np, 123456789);                               // pdm_generator.c:62
+    cudaError_t e;
+    if ((e = A::init_leveller(c)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.lev_idx, 0, Np * 4, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.lev_la, 0, (size_t)2 * DSPI_LA_SAMPLES * Np * 4, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.loud_st, 0, 8 * Np * 4, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.dline, 0, (size_t)A::kOuts * A::kMaxDelay * Np * 4, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.widx_in, 0, Np * 4, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.widx_out, 0, Np * 4, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.pdm, 0, 9 * Np * 4, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemcpyAsync(c->d.pdm + 7 * Np, seed.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.peaks, 0, (size_t)A::kRoles * Np * 2, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(c->d.clip, 0, Np * 2, c->stream)) != cudaSuccess) return e;
+    return cudaStreamSynchronize(c->stream);
+}
+
+// a new engine's transmitters: block position 0, the channel status init_spdif_buffer() stamps (audio_spdif.c:82-88)
+template <class A>
+cudaError_t init_spdif_tx(ChainHost<A> *c)
+{
+    const std::vector<uint64_t> cs(c->d.N_pad, kSpdifDefaultCs40);
+    cudaError_t e = cudaMemsetAsync(c->tx.bp, 0, (size_t)c->d.N_pad * 4, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(c->tx.cs40, cs.data(), (size_t)c->d.N_pad * 8, cudaMemcpyHostToDevice, c->stream);
+    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
+}
+
+// ---- lifetime ----------------------------------------------------------------------------------------------------------
+template <class H>
+int destroy(H *c)
+{
+    if (!c) return DSPI_OK;
+    cudaSetDevice(c->desc.device);
+    if (c->stream) cudaStreamSynchronize(c->stream);
+    c->st.destroy();
+    c->sched.destroy();
+    c->resp.destroy();
+    c->bulk.destroy();
+    c->preset.destroy();
+    if (c->eq_m) dspi_eq_destroy(c->eq_m);
+    if (c->eq_o) dspi_eq_destroy(c->eq_o);
+    for (void *p : c->allocs) cudaFree(p);
+    if (c->d_pcm) cudaFree(c->d_pcm);
+    if (c->d_spdif) cudaFree(c->d_spdif);
+    if (c->d_pdmout) cudaFree(c->d_pdmout);
+    if (c->d.vmm) cudaFree(c->d.vmm);
+    if (c->stream) cudaStreamDestroy(c->stream);
+    delete c;
+    cudaGetLastError();
+    return DSPI_OK;
+}
+
+// H: the handle type (dspi_chain / dspi_chainq), a ChainHost<H::Arith>
+template <class H>
+int create(H **out, const dspi_chain_desc *desc)
+{
+    using A = typename H::Arith;
+    if (!out || !desc) return fail(DSPI_EINVAL, "null argument");
+    *out = nullptr;
+    int rc = A::check_desc(*desc);
+    if (rc) return rc;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPI_ENODEV, "no CUDA device (there is no CPU fallback)"); }
+    if (desc->device < 0 || desc->device >= ndev) return fail(DSPI_ENODEV, "device %d out of range", desc->device);
+    int major = 0;
+    CU_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, desc->device));
+    if (major != 9) return fail(DSPI_ENODEV, "device %d is not sm_90", desc->device);
+    CU_OK(cudaSetDevice(desc->device));
+    H *c = new (std::nothrow) H();                                          // value-initialised: every pointer and count 0
+    if (!c) return fail(DSPI_ENOMEM, "host allocation failed");
+    c->desc = *desc;
+    auto &d = c->d;
+    d.N = desc->n_instances;
+    d.N_pad = (d.N + 31) / 32 * 32;
+    d.nb = desc->n_bands;
+    d.max_frames = desc->max_frames;
+    d.ldF = (d.max_frames + 3u) & ~3u;
+    const size_t Np = d.N_pad;
+    {
+        dspi_eq_desc ed;
+        memset(&ed, 0, sizeof(ed));
+        ed.arith = desc->arith; ed.n_bands = desc->n_bands; ed.device = desc->device;
+        ed.n_channels = 2 * d.N_pad;
+        rc = dspi_eq_create(&c->eq_m, &ed);
+        ed.n_channels = A::kOuts * d.N_pad;
+        if (rc == DSPI_OK) rc = dspi_eq_create(&c->eq_o, &ed);
+        if (rc != DSPI_OK) { destroy(c); return rc; }
+    }
+    cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = c->st.create(desc->device, desc->n_instances);
+#define TRY(x) if (e == cudaSuccess) e = (x)
+    TRY(c->sched.create(d.max_frames));
+    d.off = c->sched.d_off;
+    TRY(dev_alloc(c, &c->d_aos, Np * A::kRoles * DSPI_MAX_BANDS));
+    TRY(dev_alloc(c, &d.preamp, 2 * Np));
+    TRY(dev_alloc(c, &d.flags, Np));
+    TRY(dev_alloc(c, &d.loud_c, A::kLoudRows * Np));
+    TRY(dev_alloc(c, &d.loud_st, 8 * Np));
+    TRY(dev_alloc(c, &d.loud_byp, Np));
+    TRY(dev_alloc(c, &d.xf, 7 * Np));
+    TRY(dev_alloc(c, &d.lev_c, 9 * Np));
+    TRY(A::alloc_leveller(c));
+    TRY(dev_alloc(c, &d.lev_idx, Np));
+    TRY(dev_alloc(c, &d.lev_la, (size_t)2 * DSPI_LA_SAMPLES * Np));
+    TRY(dev_alloc(c, &d.o_gl, A::kOuts * Np));
+    TRY(dev_alloc(c, &d.o_gr, A::kOuts * Np));
+    TRY(dev_alloc(c, &d.o_gain, A::kOuts * Np));
+    TRY(dev_alloc(c, &d.o_flags, A::kOuts * Np));
+    TRY(dev_alloc(c, &d.o_dly, A::kOuts * Np));
+    TRY(dev_alloc(c, &d.dline, (size_t)A::kOuts * A::kMaxDelay * Np));
+    TRY(dev_alloc(c, &d.widx_in, Np));
+    TRY(dev_alloc(c, &d.widx_out, Np));
+    TRY(dev_alloc(c, &d.pdm, 9 * Np));
+    TRY(dev_alloc(c, &d.peaks, A::kRoles * Np));
+    TRY(dev_alloc(c, &d.clip, Np));
+    TRY(dev_alloc(c, &d.mrow, (size_t)2 * Np * d.ldF));
+    TRY(dev_alloc(c, &d.orow, (size_t)A::kOuts * Np * d.ldF));
+    TRY(dev_alloc(c, &d.subq, (size_t)Np * d.ldF));
+    TRY(dev_alloc(c, &d.skip_m, 2 * Np));
+    TRY(dev_alloc(c, &d.skip_o, A::kOuts * Np));
+    TRY(dev_alloc(c, &c->d_status, Np));
+    TRY(dev_alloc(c, &d.env, 5 * Np));
+    TRY(dev_alloc(c, &d.vol_base, Np));
+    TRY(dev_alloc(c, &d.vol_master, Np));
+    TRY(dev_alloc(c, &d.o_glin, A::kOuts * Np));
+    TRY(dev_alloc(c, &d.pmg, Np));
+    TRY(dev_alloc(c, &c->tx.bp, Np));
+    TRY(dev_alloc(c, &c->tx.cs40, Np));
+    TRY(dev_alloc(c, &c->rec.packets, Np));
+    TRY(dev_alloc(c, &c->rec.host, Np));
+    TRY(dev_alloc(c, &c->rec.mark, Np));
+    TRY(cudaMemsetAsync(c->rec.mark, DSPI_BULK_UNSET, Np, c->stream));
+    TRY(init_states(c));
+    TRY(init_spdif_tx(c));
+#undef TRY
+    if (e != cudaSuccess) {
+        rc = e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA;
+        fail(rc, "chain setup: %s", cudaGetErrorString(e));
+        destroy(c);
+        return rc;
+    }
+    *out = c;
+    return DSPI_OK;
+}
+
+template <class A>
+int reset_state(ChainHost<A> *c)
+{
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(init_states(c));
+    return DSPI_OK;
+}
+
+// ---- parameters --------------------------------------------------------------------------------------------------------
+// host rows of set_params, [rows][n] each, typed like the device arrays they go to
+template <class A>
+struct ParamRows {
+    template <typename P> using Rows = std::vector<std::remove_pointer_t<P>>;
+    using D = typename A::Dev;
+    Rows<decltype(D::preamp)> preamp;
+    Rows<decltype(D::loud_c)> loud_c;
+    Rows<decltype(D::xf)> xf;
+    Rows<decltype(D::o_gl)> gl, gr;
+    Rows<decltype(D::o_gain)> gain;
+    Rows<decltype(D::vol_base)> vbase;
+    Rows<decltype(D::vol_master)> vmaster;
+    Rows<decltype(D::pmg)> pmg;
+    Rows<decltype(D::lev_c)> lev_c;
+    Rows<decltype(D::o_glin)> glin;
+    Rows<decltype(D::o_dly)> dly;
+    std::vector<uint8_t> flags, loud_byp, oflags, skip_m, skip_o;
+    explicit ParamRows(uint32_t n)
+        : preamp(2 * n), loud_c(A::kLoudRows * n), xf(7 * n), gl(A::kOuts * n), gr(A::kOuts * n), gain(A::kOuts * n), vbase(n), vmaster(n),
+          pmg(n), lev_c(9 * n), glin(A::kOuts * n), dly(A::kOuts * n), flags(n), loud_byp(n), oflags(A::kOuts * n), skip_m(2 * n),
+          skip_o(A::kOuts * n)
+    {
+    }
+};
+
+template <class A>
+int set_params(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Params *params)
+{
+    if (!c || !params) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    const auto &d = c->d;
+    const size_t Np = d.N_pad;
+    constexpr int O = A::kOuts;
+    ParamRows<A> r(n);
+    decltype(r.xf) xf_cur(7 * n);
+    CU_OK(cudaMemcpy2DAsync(xf_cur.data(), (size_t)n * 4, d.xf + inst0, Np * 4, (size_t)n * 4, 7, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    for (uint32_t i = 0; i < n; i++) {
+        const typename A::Params &p = params[i];
+        A::pack(p, i, n, r);
+        bool any_delay = false;
+        for (int o = 0; o < O; o++) {
+            const dspi_output_channel &oc = p.matrix.outputs[o];
+            r.glin[o * n + i] = oc.gain_linear;
+            const bool has_pair = o < O - 1;                                 // usb_audio.c:930-933
+            r.oflags[o * n + i] = output_flags(oc.enabled, oc.mute, has_pair, has_pair && p.matrix.outputs[o ^ 1].enabled);
+            r.skip_o[o * n + i] = A::Stores::output_eq_frozen(oc.enabled, oc.mute, p.bypass_master_eq) ? 1 : 0;   // :878-884: state frozen
+            int32_t ds = oc.delay_samples;
+            if (ds > A::kMaxDelay) ds = A::kMaxDelay;
+            if (ds < 0) ds = 0;
+            r.dly[o * n + i] = ds;
+            if (ds > 0) any_delay = true;                                    // dsp_pipeline.c:237
+        }
+        r.flags[i] = chain_flags(p.bypass_master_eq, p.loudness_enabled, p.crossfeed_enabled, p.leveller_enabled, p.leveller_lookahead, any_delay,
+                                 p.matrix.outputs[O - 1].enabled);
+        r.skip_m[0 * n + i] = r.skip_m[1 * n + i] = p.bypass_master_eq ? 1 : 0;   // usb_audio.c:721-728
+        r.loud_byp[i] = (p.loudness[0].bypass ? 1 : 0) | (p.loudness[1].bypass ? 2 : 0);
+        const typename decltype(r.xf)::value_type xv[7] = { p.crossfeed.lp_a0, p.crossfeed.lp_b1, p.crossfeed.lp_state_L, p.crossfeed.lp_state_R,
+                                                            p.crossfeed.ap_a, p.crossfeed.ap_state_L, p.crossfeed.ap_state_R };
+        // crossfeed_compute_coefficients() is the only writer of crossfeed_state in the firmware and it clears the filter
+        // state (crossfeed.c:35-127); a volume / mute / matrix update never touches it.  So the record's state rows are
+        // taken only when its coefficients differ from the ones in force; otherwise the running state is kept.
+        const bool xf_same = xv[0] == xf_cur[0 * n + i] && xv[1] == xf_cur[1 * n + i] && xv[4] == xf_cur[4 * n + i];
+        for (int k = 0; k < 7; k++) {
+            const bool is_state = k == 2 || k == 3 || k == 5 || k == 6;
+            r.xf[k * n + i] = (is_state && xf_same) ? xf_cur[k * n + i] : xv[k];
+        }
+        const float *lv = &p.leveller.alpha_rms;
+        for (int k = 0; k < 9; k++) r.lev_c[k * n + i] = lv[k];
+    }
+    auto put = [&](auto *dst_base, const auto &src, int rows) -> cudaError_t {
+        const size_t elem = sizeof(*dst_base);
+        return cudaMemcpy2DAsync((char *)dst_base + (size_t)inst0 * elem, Np * elem, src.data(), (size_t)n * elem, (size_t)n * elem, rows,
+                                 cudaMemcpyHostToDevice, c->stream);
+    };
+    CU_OK(put(d.preamp, r.preamp, 2));
+    CU_OK(put(d.flags, r.flags, 1));
+    CU_OK(put(d.loud_c, r.loud_c, A::kLoudRows));
+    CU_OK(put(d.loud_byp, r.loud_byp, 1));
+    CU_OK(put(d.xf, r.xf, 7));
+    CU_OK(put(d.lev_c, r.lev_c, 9));
+    CU_OK(put(d.o_gl, r.gl, O));
+    CU_OK(put(d.o_gr, r.gr, O));
+    CU_OK(put(d.o_gain, r.gain, O));
+    CU_OK(put(d.o_glin, r.glin, O));
+    CU_OK(put(d.vol_base, r.vbase, 1));
+    CU_OK(put(d.vol_master, r.vmaster, 1));
+    CU_OK(put(d.pmg, r.pmg, 1));
+    CU_OK(put(d.o_flags, r.oflags, O));
+    CU_OK(put(d.o_dly, r.dly, O));
+    CU_OK(put(d.skip_m, r.skip_m, 2));
+    CU_OK(bulk::mark_stale(c->rec, inst0, n, c->stream));
+    CU_OK(put(d.skip_o, r.skip_o, O));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    rc = eq_set_skip(c->eq_m, d.skip_m, c->stream);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, d.skip_o, c->stream);
+    return rc;
+}
+
+// preset-mute envelope of instances [inst0, inst0+n): states == NULL leaves envelope mode (the constant preset_mute_gain of
+// set_params applies again)
+template <class A>
+int set_preset_mute(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
+{
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    const size_t Np = c->d.N_pad;
+    std::vector<uint32_t> cur((size_t)n), rows((size_t)5 * n, 0u);
+    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    for (uint32_t i = 0; i < n; i++) {
+        if (cur[i]) c->env_instances--;
+        if (states) {
+            rows[0 * n + i] = states[i].loading ? 1u : 0u;
+            rows[1 * n + i] = states[i].counter;
+            memcpy(&rows[2 * n + i], &states[i].smooth_gain, 4);
+            rows[3 * n + i] = sample_rate_hz;
+            rows[4 * n + i] = 1u;
+            c->env_instances++;
+        }
+    }
+    CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, Np * 4, rows.data(), (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+int get_preset_mute(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states)
+{
+    if (!c || !states) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    const size_t Np = c->d.N_pad;
+    std::vector<uint32_t> rows((size_t)3 * n);
+    CU_OK(cudaMemcpy2DAsync(rows.data(), (size_t)n * 4, c->d.env + inst0, Np * 4, (size_t)n * 4, 3, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    for (uint32_t i = 0; i < n; i++) {
+        memset(&states[i], 0, sizeof(states[i]));
+        states[i].loading = (uint8_t)rows[0 * n + i];
+        states[i].counter = rows[1 * n + i];
+        memcpy(&states[i].smooth_gain, &rows[2 * n + i], 4);
+    }
+    return DSPI_OK;
+}
+
+// crossfeed / leveller / loudness coefficients and the host volume of instances [inst0, inst0+n) generated ON THE GPU
+template <class A>
+int set_dynamics_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_dynamics_config *cfgs, float sample_rate)
+{
+    if (!c || !cfgs) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    dspi_dynamics_config *d_cfg = nullptr;
+    CU_OK(cudaMalloc((void **)&d_cfg, (size_t)n * sizeof(*cfgs)));
+    cudaError_t e = cudaMemcpyAsync(d_cfg, cfgs, (size_t)n * sizeof(*cfgs), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) {
+        A::dynamics<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, c->rec, inst0, n, d_cfg, sample_rate);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    cudaFree(d_cfg);
+    if (e != cudaSuccess) return fail(DSPI_ECUDA, "dynamics coefficient generation: %s", cudaGetErrorString(e));
+    c->launches++;
+    return DSPI_OK;
+}
+
+template <class A>
+int apply_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
+                      int exact_db, float sample_rate, int32_t *results)
+{
+    if (!c || !packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
+    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return bulk::apply<typename A::Stores>(c, c->bulk, inst0, n, packets, host, exact_db, sample_rate, results);
+}
+
+template <class A>
+int collect_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
+{
+    if (!c || !packets) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return bulk::collect<typename A::Stores>(c, c->bulk, inst0, n, packets, host, results);
+}
+
+template <class A>
+int apply_preset_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride, const dspi_preset_load *load,
+                        const dspi_bulk_host *host, float sample_rate, int32_t *results)
+{
+    constexpr size_t kSlot = sizeof(bulk::SlotOf<typename A::Stores>);
+    if (!c || !images || !load || !host || !results) return fail(DSPI_EINVAL, "null argument");
+    if (image_stride < kSlot) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, kSlot);
+    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return bulk::apply_preset<typename A::Stores>(c, c->bulk, c->preset, inst0, n, images, image_stride, load, host, sample_rate, results);
+}
+
+template <class A>
+int collect_preset_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
+                          int32_t *results)
+{
+    constexpr size_t kSlot = sizeof(bulk::SlotOf<typename A::Stores>);
+    if (!c || !slot_indices || !images) return fail(DSPI_EINVAL, "null argument");
+    if (image_stride < kSlot) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, kSlot);
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return bulk::collect_preset<typename A::Stores>(c, c->preset, inst0, n, slot_indices, images, image_stride, results);
+}
+
+template <class A>
+int upload_biquads(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Biquad *biquads)
+{
+    if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    using B = typename A::Biquad;
+    const size_t row = (size_t)A::kRoles * DSPI_MAX_BANDS;
+    CU_OK(cudaMemcpyAsync(c->d_aos + inst0 * row, biquads, n * row * sizeof(B), cudaMemcpyHostToDevice, c->stream));
+    const uint32_t Np = c->d.N_pad, items = n * A::kRoles * DSPI_MAX_BANDS;
+    A::scatter<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (B *)eq_aos_mirror(c->eq_m), (B *)eq_aos_mirror(c->eq_o), 1);
+    CU_OK(cudaGetLastError());
+    c->launches++;
+    for (int role = 0; role < A::kRoles; role++) {
+        rc = role < 2 ? eq_pack_range(c->eq_m, role * Np + inst0, n, c->stream) : eq_pack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
+        if (rc) return rc;
+    }
+    CU_OK(bulk::mark_stale(c->rec, inst0, n, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+int set_eq_params_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_eq_param *recipes, float sample_rate)
+{
+    if (!c || !recipes) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    // the sub-engines generate and pack on their own streams: everything issued on the engine stream so far (an
+    // asynchronous process_device in particular) must have finished reading the coefficient stores first
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    const uint32_t Np = c->d.N_pad;
+    std::vector<dspi_eq_param> tmp((size_t)n * DSPI_MAX_BANDS);
+    for (int role = 0; role < A::kRoles; role++) {                  // filter_recipes[role][band] of every instance -> one engine range per role
+        for (uint32_t i = 0; i < n; i++)
+            memcpy(&tmp[(size_t)i * DSPI_MAX_BANDS], &recipes[((size_t)i * A::kRoles + role) * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
+        rc = role < 2 ? dspi_eq_set_params_device(c->eq_m, role * Np + inst0, n, tmp.data(), sample_rate)
+                      : dspi_eq_set_params_device(c->eq_o, (role - 2) * Np + inst0, n, tmp.data(), sample_rate);
+        if (rc) return rc;
+        for (uint32_t i = 0; i < n; i++)                            // the clamps, written back like the reference does
+            memcpy(&recipes[((size_t)i * A::kRoles + role) * DSPI_MAX_BANDS], &tmp[(size_t)i * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
+    }
+    return bulk::record_recipes<typename A::Stores>(c, c->bulk, inst0, n, recipes);
+}
+
+template <class A>
+int download_biquads(ChainHost<A> *c, uint32_t inst0, uint32_t n, typename A::Biquad *biquads)
+{
+    if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    using B = typename A::Biquad;
+    const uint32_t Np = c->d.N_pad, items = n * A::kRoles * DSPI_MAX_BANDS;
+    for (int role = 0; role < A::kRoles; role++) {
+        rc = role < 2 ? eq_unpack_range(c->eq_m, role * Np + inst0, n, c->stream) : eq_unpack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
+        if (rc) return rc;
+    }
+    A::scatter<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (B *)eq_aos_mirror(c->eq_m), (B *)eq_aos_mirror(c->eq_o), 0);
+    CU_OK(cudaGetLastError());
+    c->launches++;
+    const size_t row = (size_t)A::kRoles * DSPI_MAX_BANDS;
+    CU_OK(cudaMemcpyAsync(biquads, c->d_aos + inst0 * row, n * row * sizeof(B), cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+// ---- processing --------------------------------------------------------------------------------------------------------
+template <class A>
+int check_process(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp)
+{
+    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
+    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
+    if (fpp == 0 || fpp > DSPI_PACKET_MAX) return fail(DSPI_EINVAL, "frames_per_packet must be 1..%d", DSPI_PACKET_MAX);
+    if (n_packets == 0) return fail(DSPI_EINVAL, "n_packets must be > 0");
+    if ((uint64_t)n_packets * fpp > c->desc.max_frames) return fail(DSPI_ERANGE, "%u frames exceed max_frames %u", n_packets * fpp, c->desc.max_frames);
+    return DSPI_OK;
+}
+
+template <class A>
+int check_packets(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames)
+{
+    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
+    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
+    const char *why = "";
+    const int rc = c->sched.check(n_packets, packet_frames, &why);
+    if (rc == DSPI_ERANGE) return fail(rc, "%s %u", why, c->desc.max_frames);
+    return rc ? fail(rc, "%s", why) : DSPI_OK;
+}
+
+// One call over the schedule c->sched has checked, with the kernel set K: its offsets go to the device first, on the
+// engine stream.  d_spdif: words, or subframes when `subframes` is set (either may be NULL).
+template <class A, class K>
+int run_stages(ChainHost<A> *c, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, void *d_spdif, bool subframes,
+               uint32_t *d_pdm, typename A::Status *d_status)
+{
+    PacketSchedule &ps = c->sched;
+    const uint32_t n_packets = ps.n_packets, F = ps.frames;
+    CU_OK(ps.upload(packet_frames, c->stream, &c->launches));
+    const size_t post_smem = (size_t)4 * 2 * ps.longest * A::kXs * 4;      // 4 warps x (longest packet + look-ahead columns)
+    static PerDeviceOnce once;                                              // per kernel set
+    int dev = 0;
+    if (once.needs(&dev)) {
+        CU_OK(cudaFuncSetAttribute(K::post, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)4 * 2 * DSPI_PACKET_MAX * A::kXs * 4)));
+        once.mark(dev);
+    }
+    // Stage pipeline over packet slices on three streams (chain_streams.cuh): front stages of slice
+    // i+1 overlap the output stages of slice i and the modulator of slice i-1.
+    ChainStreams &st = c->st;
+    uint32_t slice_bounds[ChainStreams::kMaxSlices + 1];
+    const uint32_t n_slices = (uint32_t)ChainStreams::plan_slices(n_packets, slice_bounds);
+    if (c->env_instances) {                                                  // preset-mute envelope: this call's per-packet volumes
+        if (c->vmm_packets < n_packets) {
+            CU_OK(cudaStreamSynchronize(c->stream));
+            if (c->d.vmm) CU_OK(cudaFree(c->d.vmm));
+            c->d.vmm = nullptr; c->vmm_packets = 0;
+            CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(*c->d.vmm)));
+            c->vmm_packets = n_packets;
+        }
+        K::env<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets);
+        CU_OK(cudaGetLastError());
+        c->launches++;
+    }
+    const typename A::Dev d = c->d;
+    const uint32_t n_sms = st.stream_sms();
+    static const uint32_t kStreamCtas = [] { const char *e = getenv("DSPI_CHAIN_CTAS"); const int v = e ? atoi(e) : 0; return (uint32_t)(v >= 1 && v <= 8 ? v : 8); }();   // streaming CTAs (256 threads) per SM
+    CU_OK(cudaEventRecord(st.ev_begin, c->stream));
+    CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
+    for (uint32_t sl = 0; sl < n_slices; sl++) {
+        const uint32_t p0 = slice_bounds[sl], p1 = slice_bounds[sl + 1];
+        const uint32_t fb = ps.off[p0], fe = ps.off[p1];
+        int rc;
+        // ---- front: unpack + loudness -> master EQ -> leveller + crossfeed
+        K::pre<<<(d.N_pad / 16 + 1) / 2, 64, 0, st.s_front>>>(d, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
+        CU_OK(cudaGetLastError());
+        if ((rc = eq_process_on(c->eq_m, d.mrow + fb, fe - fb, d.ldF, st.s_front)) != DSPI_OK) return rc;
+        K::post<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, ps.longest);
+        CU_OK(cudaGetLastError());
+        CU_OK(cudaEventRecord(st.ev_front[sl], st.s_front));
+        // ---- outputs: matrix -> per-output EQ -> gain / delay / metering / conversion
+        CU_OK(cudaStreamWaitEvent(st.s_out, st.ev_front[sl], 0));
+        K::mix<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
+        CU_OK(cudaGetLastError());
+        if ((rc = eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
+        if (subframes && d_spdif)
+            K::template outpost<true><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
+        else
+            K::template outpost<false><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
+        CU_OK(cudaGetLastError());
+        CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
+        // ---- modulator
+        CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_out[sl], 0));
+        K::pdm<<<(d.N + 127) / 128, 128, 0, st.s_pdm>>>(d, fb, fe, F, d_pdm);
+        CU_OK(cudaGetLastError());
+        c->launches += 5;
+    }
+    K::ring<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets, c->tx.bp);   // after the last outpost launch (stream order)
+    CU_OK(cudaGetLastError());
+    c->launches++;
+    std::swap(c->d.widx_in, c->d.widx_out);
+    CU_OK(cudaEventRecord(st.ev_aux, st.s_out));                             // ring update done
+    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_aux, 0));
+    // the last modulator launch is ordered after every other stage launch of this call
+    CU_OK(cudaEventRecord(st.ev_done, st.s_pdm));
+    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_done, 0));                    // later work on the engine stream sees all outputs
+    if (d_status) {
+        K::status<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, d_status);
+        CU_OK(cudaGetLastError());
+        c->launches++;
+    }
+    return DSPI_OK;
+}
+
+template <class A>
+int process_device(ChainHost<A> *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames, void *d_spdif,
+                   bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
+{
+    int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
+    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
+    CU_OK(cudaSetDevice(c->desc.device));
+    return A::with_stages(c->desc, [&](auto k) {
+        return run_stages<A, decltype(k)>(c, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
+    });
+}
+
+// host memory in and out, staged through the engine's device buffers
+template <class A>
+int process_host(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames, void *spdif_out,
+                 bool subframes, uint32_t *pdm_out, typename A::Status *status)
+{
+    int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    const size_t N = c->desc.n_instances, F = c->sched.frames, pairs = (A::kOuts - 1) / 2;   // the sub output has no S/PDIF pair
+    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * pairs * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
+    if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
+    if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
+    if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; }
+    // the modulator writes the rows of instances with a sub only; the others go back to the caller as zeros, on every call
+    // (an earlier call's bits would be there otherwise: a sub switched off since, or a longer call's [N][F][8] layout)
+    if (pdm_out) CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream));
+    CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    rc = process_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
+                        pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
+    if (rc) return rc;
+    if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
+    if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
+    if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(typename A::Status), cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+// the uniform schedule: n_packets packets of fpp frames, from device (host == false) or host memory
+template <class A>
+int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif, uint32_t *pdm,
+                    typename A::Status *status, bool host)
+{
+    int rc = check_process(c, pcm, bit_depth, n_packets, fpp);
+    if (rc) return rc;
+    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
+    return host ? process_host(c, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status)
+                : process_device(c, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status);
+}
+
+// ---- S/PDIF transmitters -----------------------------------------------------------------------------------------------
+template <class A>
+int set_spdif_tx(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
+{
+    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    std::vector<uint32_t> bp(n);
+    std::vector<uint64_t> cs(n);
+    if (!spdif_tx_unpack(tx, n, bp.data(), cs.data())) return fail(DSPI_EINVAL, "block_pos must be 0..191");
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));   // behind earlier calls
+    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+int get_spdif_tx(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
+{
+    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    std::vector<uint32_t> bp(n);
+    std::vector<uint64_t> cs(n);
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaMemcpyAsync(bp.data(), c->tx.bp + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaMemcpyAsync(cs.data(), c->tx.cs40 + inst0, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    spdif_tx_pack(bp.data(), cs.data(), n, tx);
+    return DSPI_OK;
+}
+
+// ---- checkpoint / resume: everything a later process call depends on besides the parameters ----------------------------
+using Sections = std::vector<std::pair<void *, size_t>>;
+
+template <class A>
+void state_sections(ChainHost<A> *c, Sections &v, bool with_eq = true)
+{
+    const size_t Np = c->d.N_pad;
+    v.push_back({ c->d.loud_st, 8 * Np * 4 });
+    v.push_back({ c->d.xf, 7 * Np * 4 });                                  // crossfeed coefficients and state (CrossfeedState)
+    A::leveller_sections(c, v);
+    v.push_back({ c->d.lev_idx, Np * 4 });
+    v.push_back({ c->d.lev_la, (size_t)2 * DSPI_LA_SAMPLES * Np * 4 });
+    v.push_back({ c->d.dline, (size_t)A::kOuts * A::kMaxDelay * Np * 4 });
+    v.push_back({ c->d.widx_in, Np * 4 });
+    v.push_back({ c->d.pdm, 9 * Np * 4 });
+    v.push_back({ c->d.peaks, (size_t)A::kRoles * Np * 2 });
+    v.push_back({ c->d.clip, Np * 2 });
+    v.push_back({ c->d.env, 5 * Np * 4 });                                 // preset-mute envelope state and mode
+    if (!with_eq) return;
+    eq_state_sections(c->eq_m, v);
+    eq_state_sections(c->eq_o, v);
+}
+
+// Version 2 records the K1 geometry (channels per lane, DSPI_F32_CPL) that the two EQ engines' packed stores were laid out
+// for, so that a blob resumes in an engine created under either geometry.  Version 1 blobs have no such fields and are read
+// as one channel per lane.  An engine writes version A::kStateVersion and reads versions 1 .. A::kStateVersion.
+struct StateHeader { uint32_t magic, version, arith, n_instances, n_bands, n_sections; uint64_t bytes; uint32_t cpl_m, cpl_o; };
+constexpr uint32_t kStateMagic = 0x53505344u;             // "DSPS"
+constexpr size_t kHeaderV1 = offsetof(StateHeader, cpl_m);
+inline size_t header_bytes(uint32_t version) { return version == 1u ? kHeaderV1 : sizeof(StateHeader); }
+
+// blob size for this engine's shape with header `hdr` bytes and EQ stores laid out for cpl_m / cpl_o channels per lane
+template <class A>
+size_t state_bytes(ChainHost<A> *c, size_t hdr, int cpl_m, int cpl_o)
+{
+    Sections v;
+    state_sections(c, v, false);
+    size_t n = hdr + eq_state_bytes(c->eq_m, cpl_m) + eq_state_bytes(c->eq_o, cpl_o);
+    for (auto &s : v) n += s.second;
+    return n;
+}
+
+template <class A>
+size_t state_size(ChainHost<A> *c)
+{
+    if (!c) return 0;
+    return state_bytes(c, header_bytes(A::kStateVersion), eq_geometry(c->eq_m), eq_geometry(c->eq_o));
+}
+
+template <class A>
+int state_export(ChainHost<A> *c, void *blob, size_t cap)
+{
+    if (!c || !blob) return fail(DSPI_EINVAL, "null argument");
+    const size_t need = state_size(c);
+    if (cap < need) return fail(DSPI_ERANGE, "state blob needs %zu bytes, %zu given", need, cap);
+    CU_OK(cudaSetDevice(c->desc.device));
+    Sections v;
+    state_sections(c, v);
+    const StateHeader h = { kStateMagic, A::kStateVersion, c->desc.arith, c->desc.n_instances, c->desc.n_bands, (uint32_t)v.size(), (uint64_t)need,
+                            (uint32_t)eq_geometry(c->eq_m), (uint32_t)eq_geometry(c->eq_o) };
+    const size_t hdr = header_bytes(A::kStateVersion);
+    memcpy(blob, &h, hdr);
+    char *p = (char *)blob + hdr;
+    for (auto &s : v) {
+        CU_OK(cudaMemcpyAsync(p, s.first, s.second, cudaMemcpyDeviceToHost, c->stream));
+        p += s.second;
+    }
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+int state_import(ChainHost<A> *c, const void *blob, size_t len)
+{
+    if (!c || !blob) return fail(DSPI_EINVAL, "null argument");
+    Sections v, all;
+    state_sections(c, v, false);
+    state_sections(c, all);
+    StateHeader h;
+    if (len < kHeaderV1) return fail(DSPI_EINVAL, "state blob too short");
+    memcpy(&h, blob, kHeaderV1);
+    h.cpl_m = h.cpl_o = 1;
+    if (h.magic != kStateMagic || h.version < 1u || h.version > A::kStateVersion)
+        return fail(DSPI_EINVAL, "not a dspi_b200 state blob (magic %08x version %u)", h.magic, h.version);
+    const size_t hdr = header_bytes(h.version);
+    if (len < hdr) return fail(DSPI_EINVAL, "state blob too short");
+    memcpy(&h, blob, hdr);
+    if ((h.cpl_m != 1 && h.cpl_m != 2) || (h.cpl_o != 1 && h.cpl_o != 2))
+        return fail(DSPI_EINVAL, "state blob names an unknown K1 geometry (%u, %u channels per lane)", h.cpl_m, h.cpl_o);
+    if (h.arith != c->desc.arith || h.n_instances != c->desc.n_instances || h.n_bands != c->desc.n_bands || h.n_sections != all.size() ||
+        h.bytes != state_bytes(c, hdr, (int)h.cpl_m, (int)h.cpl_o) || len < h.bytes)
+        return fail(DSPI_EINVAL, "state blob belongs to a different engine shape (%u instances, arith %u, %llu bytes)", h.n_instances, h.arith,
+                    (unsigned long long)h.bytes);
+    CU_OK(cudaSetDevice(c->desc.device));
+    const char *p = (const char *)blob + hdr;
+    for (auto &s : v) {
+        CU_OK(cudaMemcpyAsync(s.first, p, s.second, cudaMemcpyHostToDevice, c->stream));
+        p += s.second;
+    }
+    CU_OK(cudaStreamSynchronize(c->stream));
+    int rc = eq_state_load(c->eq_m, p, (int)h.cpl_m, c->stream);
+    p += eq_state_bytes(c->eq_m, (int)h.cpl_m);
+    if (rc == DSPI_OK) rc = eq_state_load(c->eq_o, p, (int)h.cpl_o, c->stream);
+    if (rc) return rc;
+    rc = eq_state_imported(c->eq_m, c->stream);
+    if (rc == DSPI_OK) rc = eq_state_imported(c->eq_o, c->stream);
+    if (rc) return rc;
+    std::vector<uint32_t> on(c->d.N);
+    CU_OK(cudaMemcpyAsync(on.data(), c->d.env + (size_t)4 * c->d.N_pad, (size_t)c->d.N * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    c->env_instances = 0;
+    for (uint32_t x : on) c->env_instances += x ? 1u : 0u;
+    return DSPI_OK;
+}
+
+// ---- queries -----------------------------------------------------------------------------------------------------------
+// Frequency response of instances [inst0, inst0 + n) on the engine stream; out: device [n][kOuts][2][n_freqs] float2, or
+// host memory filled chunk by chunk through the staging buffer
+template <class A>
+int response(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
+{
+    const char *why = "";
+    int rc = response_check_args(freqs, n_freqs, fs, out, &why);
+    if (rc) return fail(rc, "%s", why);
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(c->resp.upload(freqs, n_freqs, c->stream, &c->launches));
+    using B = typename A::Biquad;
+    const B *m_aos = (const B *)eq_aos_mirror(c->eq_m), *o_aos = (const B *)eq_aos_mirror(c->eq_o);
+    auto launch = [&](uint32_t i0, uint32_t m, void *dst) -> cudaError_t {
+        const dim3 grid((n_freqs + 127) / 128, m < 65535u ? m : 65535u);
+        A::response<<<grid, 128, 0, c->stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
+        c->launches++;
+        return cudaGetLastError();
+    };
+    if (!host) {
+        CU_OK(launch(inst0, n, out));
+        return DSPI_OK;
+    }
+    const size_t row_bytes = (size_t)A::kOuts * 2 * n_freqs * 2 * sizeof(float);
+    uint32_t rows = 0;
+    CU_OK(c->resp.stage(row_bytes, n, c->stream, &rows));
+    for (uint32_t i = 0; i < n; i += rows) {
+        const uint32_t m = n - i < rows ? n - i : rows;
+        CU_OK(launch(inst0 + i, m, c->resp.d_stage));
+        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->stream));
+        CU_OK(cudaStreamSynchronize(c->stream));
+    }
+    return DSPI_OK;
+}
+
+template <class A>
+int sync(ChainHost<A> *c)
+{
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+void *stream(ChainHost<A> *c) { return c ? (void *)c->stream : nullptr; }
+
+// SMs reserved for the modulator / left to every other stage (0, 0: no partition, see chain_streams.cuh)
+template <class A>
+int sm_partition(ChainHost<A> *c, uint32_t *pdm_sms, uint32_t *rest_sms)
+{
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    if (pdm_sms) *pdm_sms = c->st.pdm_sms;
+    if (rest_sms) *rest_sms = c->st.rest_sms;
+    return DSPI_OK;
+}
+
+template <class A>
+uint64_t launch_count(ChainHost<A> *c)
+{
+    return c ? c->launches + dspi_eq_launch_count(c->eq_m) + dspi_eq_launch_count(c->eq_o) : 0;
+}
+
+}  // namespace
+}  // namespace dspi

@@ -5,9 +5,9 @@
 // :1191-1276); fast_mul_q28 dsp_pipeline.c:47-58; fast_mul_q15 config.h:556-567; cascade
 // dsp_process_rp2040.S:225-394; crossfeed.c:161-180; leveller.c:275-389; PDM pdm_generator.c:351-397.
 //
-// Same stage-wise decomposition as chain_f32.cu: pre (unpack, preamp, loudness) -> K2 over the master rows
-// -> post (leveller, peaks, crossfeed) -> mix -> K2 over the output rows -> outpost (gain, delay, metering,
-// 24-bit words or S/PDIF subframes) -> ring update -> modulator, on three streams over packet slices.  The EQ rows run through
+// Same stage-wise decomposition as the float chain: pre (unpack, preamp, loudness) -> K2 over the master rows -> post
+// (leveller, peaks, crossfeed) -> mix -> K2 over the output rows -> outpost (gain, delay, metering, 24-bit words or S/PDIF
+// subframes) -> ring update -> modulator, run on three streams over packet slices by chain_host.cuh.  The EQ rows run through
 // the Q28 cascade kernel of the EQ engine (eq_q28.cu: TMA ring, coefficients pre-split in registers);
 // everything is integer-pipe bound (about 27 integer ops per band-sample).
 #include <cstdarg>
@@ -33,7 +33,6 @@ constexpr int kOuts = DSPI_CHAINQ_OUTPUTS;
 constexpr int kRoles = DSPI_CHAINQ_EQ_CHANNELS;
 constexpr int kMaxDelay = DSPI_CHAINQ_MAX_DELAY;
 constexpr int kLa = DSPI_LA_SAMPLES;
-constexpr int kPkt = DSPI_PACKET_MAX;
 constexpr int kXs = 33;                                       // shared-memory column stride: conflict-free for lane = instance AND lane = frame
 constexpr int32_t kUnity = 1 << 28;
 constexpr int32_t kClipThresh = (1 << 28) + 268;              // config.h:54
@@ -795,16 +794,13 @@ chainq_response_kernel(ChainQ d, const dspi_biquad_q28 *__restrict__ m_aos, cons
     }
 }
 
-int fail(int code, const char *fmt, ...)
-{
-    size_t cap = 0;
-    char *buf = error_buffer(&cap);
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, cap, fmt, ap);
-    va_end(ap);
-    return code;
-}
+}  // namespace
+}  // namespace dspi
+
+#include "chain_host.cuh"
+
+namespace dspi {
+namespace {
 
 // host copies of the firmware's integer helpers (per-packet scalars are folded on the host)
 int32_t h_mul_q15(int32_t s, int32_t g)
@@ -822,842 +818,205 @@ int32_t h_f2i_sat(float x)
     return (int32_t)x;
 }
 
-}  // namespace
-}  // namespace dspi
-
-using dspi::ChainQ;
-using dspi::fail;
-
-#define CU_OK(expr)                                                                                         \
-    do {                                                                                                    \
-        cudaError_t err__ = (expr);                                                                         \
-        if (err__ != cudaSuccess) return fail(DSPI_ECUDA, "%s -> %s (%s:%d)", #expr, cudaGetErrorString(err__), __FILE__, __LINE__); \
-    } while (0)
-
-struct dspi_chainq {
-    dspi_chain_desc desc;
-    ChainQ d;
-    cudaStream_t stream;                  // the engine stream callers see; stages run on st.* between ev_begin and ev_done
-    dspi::ChainStreams st;
-    dspi_biquad_q28 *d_aos;
-    dspi_eq *eq_m, *eq_o;            // K2 engines over the master rows (2 N_pad channels) and the output rows (5 N_pad)
-    std::vector<void *> allocs;
-    uint64_t launches;
-    void *d_pcm; size_t pcm_bytes;
-    int32_t *d_spdif; size_t spdif_bytes;   // host-path staging of the S/PDIF output, words or subframes
-    uint32_t *d_pdmout; size_t pdmout_bytes;
-    dspi_status_q28 *d_status;
-    dspi::SpdifTx tx;                // S/PDIF transmitter state; not part of the state blob (dspi_chainq_get/set_spdif_tx)
-    uint32_t env_instances;          // instances in envelope mode
-    uint32_t vmm_packets;            // capacity of d.vmm in packets
-    dspi::PacketSchedule sched;      // packet lengths of the current call
-    dspi::ResponseBuffers resp;      // frequency table and host staging of dspi_chainq_response_*
-    dspi::bulk::Stage bulk;          // device staging of dspi_chainq_apply_bulk_device / _collect_bulk_device, allocated by the first call
-    dspi::bulk::PresetStage preset;  // device staging of dspi_chainq_apply_preset_device / _collect_preset_device, allocated by the first call
-    dspi::bulk::Record rec;          // wire-visible configuration of every instance (dspi_chainq_collect_bulk_device); not part of the state blob
+struct Q28Stages {
+    static constexpr auto pre = chainq_pre_kernel;
+    static constexpr auto post = chainq_post_kernel;
+    static constexpr auto mix = chainq_mix_kernel;
+    template <bool SUBFRAMES> static constexpr auto outpost = chainq_outpost_kernel<SUBFRAMES>;
+    static constexpr auto ring = chainq_ring_kernel;
+    static constexpr auto pdm = chainq_pdm_kernel;
+    static constexpr auto env = chainq_env_kernel;
+    static constexpr auto status = chainq_status_kernel;
 };
 
-namespace {
+// what the Q28 engine brings to the shared host code (chain_host.cuh)
+struct Q28 : ParamStores {
+    using Biquad = dspi_biquad_q28;
+    using Status = dspi_status_q28;
+    using Params = dspi_chain_params_q28;
+    using Stores = ParamStores;
+    static constexpr int kLoudRows = 10;                                     // [2 shelves][5] TDF2 coefficients
+    static constexpr int kXs = dspi::kXs;
+    static constexpr uint32_t kStateVersion = 1;
+    static constexpr auto scatter = chainq_scatter_kernel;
+    static constexpr auto dynamics = chainq_dynamics_kernel;
+    static constexpr auto response = chainq_response_kernel;
 
-template <typename T>
-cudaError_t dev_alloc(dspi_chainq *c, T **p, size_t count, bool zero = true)
-{
-    void *q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
-    if (e != cudaSuccess) return e;
-    c->allocs.push_back(q);
-    *p = (T *)q;
-    return zero ? cudaMemsetAsync(q, 0, count * sizeof(T), c->stream) : cudaSuccess;
-}
+    template <class F>
+    static int with_stages(const dspi_chain_desc &, F &&f) { return f(Q28Stages()); }
 
-cudaError_t init_states(dspi_chainq *c)
-{
-    const size_t Np = c->d.N_pad;
-    std::vector<int32_t> unity(Np, 1 << 28), seed(Np, 123456789);
-    cudaError_t e;
-    if ((e = cudaMemsetAsync(c->d.lev_i, 0, 4 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemcpyAsync(c->d.lev_i + 2 * Np, unity.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;   // leveller.c:101-102
-    if ((e = cudaMemcpyAsync(c->d.lev_i + 3 * Np, unity.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.lev_f, 0, Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.lev_idx, 0, Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.lev_la, 0, (size_t)2 * dspi::kLa * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.loud_st, 0, 8 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.dline, 0, (size_t)dspi::kOuts * dspi::kMaxDelay * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.widx_in, 0, Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.widx_out, 0, Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.pdm, 0, 9 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemcpyAsync(c->d.pdm + 7 * Np, seed.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.peaks, 0, (size_t)dspi::kRoles * Np * 2, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.clip, 0, Np * 2, c->stream)) != cudaSuccess) return e;
-    return cudaStreamSynchronize(c->stream);
-}
-
-// a new engine's transmitters: block position 0, the channel status init_spdif_buffer() stamps (audio_spdif.c:82-88)
-cudaError_t init_spdif_tx(dspi_chainq *c)
-{
-    const std::vector<uint64_t> cs(c->d.N_pad, dspi::kSpdifDefaultCs40);
-    cudaError_t e = cudaMemsetAsync(c->tx.bp, 0, (size_t)c->d.N_pad * 4, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(c->tx.cs40, cs.data(), (size_t)c->d.N_pad * 8, cudaMemcpyHostToDevice, c->stream);
-    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
-}
-
-}  // namespace
-
-extern "C" {
-
-int dspi_chainq_destroy(dspi_chainq *c)
-{
-    if (!c) return DSPI_OK;
-    cudaSetDevice(c->desc.device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    c->st.destroy();
-    c->sched.destroy();
-    c->resp.destroy();
-    c->bulk.destroy();
-    c->preset.destroy();
-    if (c->eq_m) dspi_eq_destroy(c->eq_m);
-    if (c->eq_o) dspi_eq_destroy(c->eq_o);
-    for (void *p : c->allocs) cudaFree(p);
-    if (c->d_pcm) cudaFree(c->d_pcm);
-    if (c->d_spdif) cudaFree(c->d_spdif);
-    if (c->d_pdmout) cudaFree(c->d_pdmout);
-    if (c->d.vmm) cudaFree(c->d.vmm);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
-    cudaGetLastError();
-    return DSPI_OK;
-}
-
-int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc)
-{
-    if (!out || !desc) return fail(DSPI_EINVAL, "null argument");
-    *out = nullptr;
-    if (desc->arith != DSPI_ARITH_Q28) return fail(DSPI_EINVAL, "dspi_chainq engines are Q28 (arith 2)");
-    if (desc->n_instances == 0 || desc->max_frames == 0) return fail(DSPI_EINVAL, "n_instances and max_frames must be > 0");
-    if (desc->n_bands == 0 || desc->n_bands > DSPI_MAX_BANDS) return fail(DSPI_EINVAL, "n_bands must be 1..%d", DSPI_MAX_BANDS);
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(DSPI_ENODEV, "no CUDA device (there is no CPU fallback)"); }
-    if (desc->device < 0 || desc->device >= ndev) return fail(DSPI_ENODEV, "device %d out of range", desc->device);
-    int major = 0;
-    CU_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, desc->device));
-    if (major != 9) return fail(DSPI_ENODEV, "device %d is not sm_90", desc->device);
-    CU_OK(cudaSetDevice(desc->device));
-    dspi_chainq *c = new (std::nothrow) dspi_chainq();
-    if (!c) return fail(DSPI_ENOMEM, "host allocation failed");
-    c->stream = nullptr;
-    c->st = dspi::ChainStreams();
-    c->sched = dspi::PacketSchedule();
-    c->eq_m = c->eq_o = nullptr;
-    c->d_aos = nullptr; c->launches = 0; c->d_pcm = nullptr; c->pcm_bytes = 0; c->d_spdif = nullptr; c->spdif_bytes = 0;
-    c->d_pdmout = nullptr; c->pdmout_bytes = 0; c->d_status = nullptr;
-    c->env_instances = 0; c->vmm_packets = 0;
-    c->tx.bp = nullptr; c->tx.cs40 = nullptr;
-    c->desc = *desc;
-    ChainQ &d = c->d;
-    memset(&d, 0, sizeof(d));
-    d.N = desc->n_instances;
-    d.N_pad = (d.N + 31) / 32 * 32;
-    d.nb = desc->n_bands;
-    d.max_frames = desc->max_frames;
-    d.ldF = (d.max_frames + 3u) & ~3u;
-    const size_t Np = d.N_pad;
+    static int check_desc(const dspi_chain_desc &desc)
     {
-        dspi_eq_desc ed;
-        memset(&ed, 0, sizeof(ed));
-        ed.arith = DSPI_ARITH_Q28; ed.n_bands = desc->n_bands; ed.device = desc->device;
-        ed.n_channels = 2 * d.N_pad;
-        int rc = dspi_eq_create(&c->eq_m, &ed);
-        ed.n_channels = dspi::kOuts * d.N_pad;
-        if (rc == DSPI_OK) rc = dspi_eq_create(&c->eq_o, &ed);
-        if (rc != DSPI_OK) { dspi_chainq_destroy(c); return rc; }
+        if (desc.arith != DSPI_ARITH_Q28) return fail(DSPI_EINVAL, "dspi_chainq engines are Q28 (arith 2)");
+        if (desc.n_instances == 0 || desc.max_frames == 0) return fail(DSPI_EINVAL, "n_instances and max_frames must be > 0");
+        if (desc.n_bands == 0 || desc.n_bands > DSPI_MAX_BANDS) return fail(DSPI_EINVAL, "n_bands must be 1..%d", DSPI_MAX_BANDS);
+        return DSPI_OK;
     }
-    cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = c->st.create(desc->device, desc->n_instances);
-#define TRY(x) if (e == cudaSuccess) e = (x)
-    TRY(c->sched.create(d.max_frames));
-    d.off = c->sched.d_off;
-    TRY(dev_alloc(c, &c->d_aos, Np * dspi::kRoles * DSPI_MAX_BANDS));
-    TRY(dev_alloc(c, &d.preamp, 2 * Np));
-    TRY(dev_alloc(c, &d.flags, Np));
-    TRY(dev_alloc(c, &d.loud_c, 10 * Np));
-    TRY(dev_alloc(c, &d.loud_st, 8 * Np));
-    TRY(dev_alloc(c, &d.loud_byp, Np));
-    TRY(dev_alloc(c, &d.xf, 7 * Np));
-    TRY(dev_alloc(c, &d.lev_c, 9 * Np));
-    TRY(dev_alloc(c, &d.lev_i, 4 * Np));
-    TRY(dev_alloc(c, &d.lev_f, Np));
-    TRY(dev_alloc(c, &d.lev_idx, Np));
-    TRY(dev_alloc(c, &d.lev_la, (size_t)2 * dspi::kLa * Np));
-    TRY(dev_alloc(c, &d.o_gl, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_gr, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_gain, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_flags, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.o_dly, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.dline, (size_t)dspi::kOuts * dspi::kMaxDelay * Np));
-    TRY(dev_alloc(c, &d.widx_in, Np));
-    TRY(dev_alloc(c, &d.widx_out, Np));
-    TRY(dev_alloc(c, &d.pdm, 9 * Np));
-    TRY(dev_alloc(c, &d.peaks, dspi::kRoles * Np));
-    TRY(dev_alloc(c, &d.clip, Np));
-    TRY(dev_alloc(c, &d.mrow, (size_t)2 * Np * d.ldF));
-    TRY(dev_alloc(c, &d.orow, (size_t)dspi::kOuts * Np * d.ldF));
-    TRY(dev_alloc(c, &d.subq, (size_t)Np * d.ldF));
-    TRY(dev_alloc(c, &d.skip_m, 2 * Np));
-    TRY(dev_alloc(c, &d.skip_o, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &c->d_status, Np));
-    TRY(dev_alloc(c, &d.env, 5 * Np));
-    TRY(dev_alloc(c, &d.vol_base, Np));
-    TRY(dev_alloc(c, &d.vol_master, Np));
-    TRY(dev_alloc(c, &d.o_glin, dspi::kOuts * Np));
-    TRY(dev_alloc(c, &d.pmg, Np));
-    TRY(dev_alloc(c, &c->tx.bp, Np));
-    TRY(dev_alloc(c, &c->tx.cs40, Np));
-    TRY(dev_alloc(c, &c->rec.packets, Np));
-    TRY(dev_alloc(c, &c->rec.host, Np));
-    TRY(dev_alloc(c, &c->rec.mark, Np));
-    TRY(cudaMemsetAsync(c->rec.mark, DSPI_BULK_UNSET, Np, c->stream));
-    TRY(init_states(c));
-    TRY(init_spdif_tx(c));
-#undef TRY
-    if (e != cudaSuccess) {
-        fail(e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA, "chainq setup: %s", cudaGetErrorString(e));
-        dspi_chainq_destroy(c);
-        return e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA;
+
+    static cudaError_t alloc_leveller(ChainHost<Q28> *c)
+    {
+        cudaError_t e = dev_alloc(c, &c->d.lev_i, (size_t)4 * c->d.N_pad);
+        return e == cudaSuccess ? dev_alloc(c, &c->d.lev_f, (size_t)c->d.N_pad) : e;
     }
-    *out = c;
-    return DSPI_OK;
-}
 
-int dspi_chainq_reset_state(dspi_chainq *c)
-{
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(init_states(c));
-    return DSPI_OK;
-}
+    // leveller_reset_state(): env_l, env_r 0, gain, gain_prev unity (leveller.c:101-102), smooth_db 0
+    static cudaError_t init_leveller(ChainHost<Q28> *c)
+    {
+        const size_t Np = c->d.N_pad;
+        const std::vector<int32_t> unity(Np, kUnity);
+        cudaError_t e;
+        if ((e = cudaMemsetAsync(c->d.lev_i, 0, 4 * Np * 4, c->stream)) != cudaSuccess) return e;
+        if ((e = cudaMemcpyAsync(c->d.lev_i + 2 * Np, unity.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
+        if ((e = cudaMemcpyAsync(c->d.lev_i + 3 * Np, unity.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
+        return cudaMemsetAsync(c->d.lev_f, 0, Np * 4, c->stream);
+    }
 
-int dspi_chainq_set_params(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_chain_params_q28 *params)
-{
-    if (!c || !params) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const ChainQ &d = c->d;
-    const size_t Np = d.N_pad;
-    const int O = dspi::kOuts;
-    std::vector<int32_t> preamp(2 * n), loud_c(10 * n), xf(7 * n), gl(O * n), gr(O * n), gain(O * n), dly(O * n);
-    std::vector<float> lev_c(9 * n), glin(O * n);
-    std::vector<int32_t> vbase(n), vmaster(n), pmgv(n);
-    std::vector<uint8_t> flags(n), loud_byp(n), oflags(O * n), skip_m(2 * n), skip_o(O * n);
-    std::vector<int32_t> xf_cur(7 * n);
-    CU_OK(cudaMemcpy2DAsync(xf_cur.data(), (size_t)n * 4, d.xf + inst0, Np * 4, (size_t)n * 4, 7, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    for (uint32_t i = 0; i < n; i++) {
-        const dspi_chain_params_q28 &p = params[i];
+    static void leveller_sections(ChainHost<Q28> *c, Sections &v)
+    {
+        v.push_back({ c->d.lev_i, (size_t)4 * c->d.N_pad * 4 });
+        v.push_back({ c->d.lev_f, (size_t)c->d.N_pad * 4 });
+    }
+
+    // volumes, preamp, loudness shelves and matrix / output gains of instance i of a set_params call, folded to Q15 / Q28
+    static void pack(const dspi_chain_params_q28 &p, uint32_t i, uint32_t n, ParamRows<Q28> &r)
+    {
         int32_t vol_mul = p.host_mute ? 0 : (int32_t)p.host_vol_mul;                                    // usb_audio.c:975
-        vbase[i] = vol_mul;
-        vmaster[i] = p.master_volume_q15;
+        r.vbase[i] = vol_mul;
+        r.vmaster[i] = p.master_volume_q15;
         int32_t pmg = (int32_t)(p.preset_mute_gain * 32768.0f + 0.5f);                                  // :976-978
         if (pmg < 0) pmg = 0;
         if (pmg > 32768) pmg = 32768;
-        pmgv[i] = pmg;
-        vol_mul = dspi::h_mul_q15(vol_mul, pmg);                                                        // :979
-        const int32_t vol_mul_master = dspi::h_mul_q15(vol_mul, p.master_volume_q15);                   // :980
-        preamp[0 * n + i] = p.preamp_q28[0];
-        preamp[1 * n + i] = p.preamp_q28[1];
-        bool any_delay = false;
-        for (int o = 0; o < O; o++) {
+        r.pmg[i] = pmg;
+        vol_mul = h_mul_q15(vol_mul, pmg);                                                              // :979
+        const int32_t vol_mul_master = h_mul_q15(vol_mul, p.master_volume_q15);                         // :980
+        r.preamp[0 * n + i] = p.preamp_q28[0];
+        r.preamp[1 * n + i] = p.preamp_q28[1];
+        for (int o = 0; o < kOuts; o++) {
             const dspi_output_channel &oc = p.matrix.outputs[o];
             const dspi_matrix_crosspoint &xl = p.matrix.crosspoints[0][o], &xr = p.matrix.crosspoints[1][o];
-            gl[o * n + i] = xl.enabled ? dspi::h_f2i_sat((xl.phase_invert ? -xl.gain_linear : xl.gain_linear) * 32768.0f) : 0;   // :1084-1085
-            gr[o * n + i] = xr.enabled ? dspi::h_f2i_sat((xr.phase_invert ? -xr.gain_linear : xr.gain_linear) * 32768.0f) : 0;
-            gain[o * n + i] = oc.mute ? 0 : dspi::h_f2i_sat(oc.gain_linear * (float)vol_mul_master);    // :1204-1205
-            glin[o * n + i] = oc.gain_linear;
-            const bool has_pair = o < O - 1;                                                            // :1248-1251
-            oflags[o * n + i] = dspi::output_flags(oc.enabled, oc.mute, has_pair, has_pair && p.matrix.outputs[o ^ 1].enabled);
-            skip_o[o * n + i] = dspi::ParamStores::output_eq_frozen(oc.enabled, oc.mute, p.bypass_master_eq) ? 1 : 0;
-            int32_t ds = oc.delay_samples;
-            if (ds > DSPI_CHAINQ_MAX_DELAY) ds = DSPI_CHAINQ_MAX_DELAY;
-            if (ds < 0) ds = 0;
-            dly[o * n + i] = ds;
-            if (ds > 0) any_delay = true;
+            r.gl[o * n + i] = xl.enabled ? h_f2i_sat((xl.phase_invert ? -xl.gain_linear : xl.gain_linear) * 32768.0f) : 0;   // :1084-1085
+            r.gr[o * n + i] = xr.enabled ? h_f2i_sat((xr.phase_invert ? -xr.gain_linear : xr.gain_linear) * 32768.0f) : 0;
+            r.gain[o * n + i] = oc.mute ? 0 : h_f2i_sat(oc.gain_linear * (float)vol_mul_master);        // :1204-1205
         }
-        flags[i] = dspi::chain_flags(p.bypass_master_eq, p.loudness_enabled, p.crossfeed_enabled, p.leveller_enabled, p.leveller_lookahead, any_delay,
-                                     p.matrix.outputs[O - 1].enabled);
-        skip_m[0 * n + i] = skip_m[1 * n + i] = p.bypass_master_eq ? 1 : 0;                              // :1050-1055
-        loud_byp[i] = (p.loudness[0].bypass ? 1 : 0) | (p.loudness[1].bypass ? 2 : 0);
         for (int j = 0; j < 2; j++) {
             const int32_t v[5] = { p.loudness[j].b0, p.loudness[j].b1, p.loudness[j].b2, p.loudness[j].a1, p.loudness[j].a2 };
-            for (int k = 0; k < 5; k++) loud_c[(j * 5 + k) * n + i] = v[k];
+            for (int k = 0; k < 5; k++) r.loud_c[(j * 5 + k) * n + i] = v[k];
         }
-        const int32_t xv[7] = { p.crossfeed.lp_a0, p.crossfeed.lp_b1, p.crossfeed.lp_state_L, p.crossfeed.lp_state_R,
-                                p.crossfeed.ap_a, p.crossfeed.ap_state_L, p.crossfeed.ap_state_R };
-        // crossfeed_compute_coefficients() is the only writer of crossfeed_state in the firmware and it clears the filter
-        // state (crossfeed.c:35-127); a volume / mute / matrix update never touches it.  So the record's state rows are
-        // taken only when its coefficients differ from the ones in force; otherwise the running state is kept.
-        const bool xf_same = xv[0] == xf_cur[0 * n + i] && xv[1] == xf_cur[1 * n + i] && xv[4] == xf_cur[4 * n + i];
-        for (int k = 0; k < 7; k++) {
-            const bool is_state = k == 2 || k == 3 || k == 5 || k == 6;
-            xf[k * n + i] = (is_state && xf_same) ? xf_cur[k * n + i] : xv[k];
-        }
-        const float *lv = &p.leveller.alpha_rms;
-        for (int k = 0; k < 9; k++) lev_c[k * n + i] = lv[k];
     }
-    auto put = [&](void *dst_base, const void *src, int rows, size_t elem) -> cudaError_t {
-        return cudaMemcpy2DAsync((char *)dst_base + (size_t)inst0 * elem, Np * elem, src, (size_t)n * elem, (size_t)n * elem, rows,
-                                 cudaMemcpyHostToDevice, c->stream);
-    };
-    CU_OK(put(d.preamp, preamp.data(), 2, 4));
-    CU_OK(put(d.flags, flags.data(), 1, 1));
-    CU_OK(put(d.loud_c, loud_c.data(), 10, 4));
-    CU_OK(put(d.loud_byp, loud_byp.data(), 1, 1));
-    CU_OK(put(d.xf, xf.data(), 7, 4));
-    CU_OK(put(d.lev_c, lev_c.data(), 9, 4));
-    CU_OK(put(d.o_gl, gl.data(), O, 4));
-    CU_OK(put(d.o_gr, gr.data(), O, 4));
-    CU_OK(put(d.o_gain, gain.data(), O, 4));
-    CU_OK(put(d.o_glin, glin.data(), O, 4));
-    CU_OK(put(d.vol_base, vbase.data(), 1, 4));
-    CU_OK(put(d.vol_master, vmaster.data(), 1, 4));
-    CU_OK(put(d.pmg, pmgv.data(), 1, 4));
-    CU_OK(put(d.o_flags, oflags.data(), O, 1));
-    CU_OK(put(d.o_dly, dly.data(), O, 4));
-    CU_OK(put(d.skip_m, skip_m.data(), 2, 1));
-    CU_OK(dspi::bulk::mark_stale(c->rec, inst0, n, c->stream));
-    CU_OK(put(d.skip_o, skip_o.data(), O, 1));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    int rc = dspi::eq_set_skip(c->eq_m, d.skip_m, c->stream);
-    if (rc == DSPI_OK) rc = dspi::eq_set_skip(c->eq_o, d.skip_o, c->stream);
-    return rc;
-}
+};
 
-/* preset-mute envelope of instances [inst0, inst0+n): states == NULL leaves envelope mode (the constant
- * preset_mute_gain of dspi_chainq_set_params applies again) */
+}  // namespace
+}  // namespace dspi
+
+struct dspi_chainq : dspi::ChainHost<dspi::Q28> {};
+
+extern "C" {
+
+int dspi_chainq_destroy(dspi_chainq *c) { return dspi::destroy(c); }
+int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc) { return dspi::create(out, desc); }
+int dspi_chainq_reset_state(dspi_chainq *c) { return dspi::reset_state(c); }
+
+int dspi_chainq_set_params(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_chain_params_q28 *params) { return dspi::set_params(c, inst0, n, params); }
+
 int dspi_chainq_set_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
 {
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t Np = c->d.N_pad;
-    std::vector<uint32_t> cur((size_t)n), rows((size_t)5 * n, 0u);
-    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    for (uint32_t i = 0; i < n; i++) {
-        if (cur[i]) c->env_instances--;
-        if (states) {
-            rows[0 * n + i] = states[i].loading ? 1u : 0u;
-            rows[1 * n + i] = states[i].counter;
-            memcpy(&rows[2 * n + i], &states[i].smooth_gain, 4);
-            rows[3 * n + i] = sample_rate_hz;
-            rows[4 * n + i] = 1u;
-            c->env_instances++;
-        }
-    }
-    CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, Np * 4, rows.data(), (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    return dspi::set_preset_mute(c, inst0, n, states, sample_rate_hz);
 }
 
-int dspi_chainq_get_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states)
-{
-    if (!c || !states) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t Np = c->d.N_pad;
-    std::vector<uint32_t> rows((size_t)3 * n);
-    CU_OK(cudaMemcpy2DAsync(rows.data(), (size_t)n * 4, c->d.env + inst0, Np * 4, (size_t)n * 4, 3, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    for (uint32_t i = 0; i < n; i++) {
-        memset(&states[i], 0, sizeof(states[i]));
-        states[i].loading = (uint8_t)rows[0 * n + i];
-        states[i].counter = rows[1 * n + i];
-        memcpy(&states[i].smooth_gain, &rows[2 * n + i], 4);
-    }
-    return DSPI_OK;
-}
+int dspi_chainq_get_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states) { return dspi::get_preset_mute(c, inst0, n, states); }
 
-/* crossfeed / leveller / loudness coefficients and the host volume of instances [inst0, inst0+n) generated ON THE GPU */
 int dspi_chainq_set_dynamics_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_dynamics_config *cfgs, float sample_rate)
 {
-    if (!c || !cfgs) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    dspi_dynamics_config *d_cfg = nullptr;
-    CU_OK(cudaMalloc((void **)&d_cfg, (size_t)n * sizeof(*cfgs)));
-    cudaError_t e = cudaMemcpyAsync(d_cfg, cfgs, (size_t)n * sizeof(*cfgs), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
-        dspi::chainq_dynamics_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, c->rec, inst0, n, d_cfg, sample_rate);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cudaFree(d_cfg);
-    if (e != cudaSuccess) return fail(DSPI_ECUDA, "dynamics coefficient generation: %s", cudaGetErrorString(e));
-    c->launches++;
-    return DSPI_OK;
+    return dspi::set_dynamics_device(c, inst0, n, cfgs, sample_rate);
 }
 
 int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
                                   int exact_db, float sample_rate, int32_t *results)
 {
-    if (!c || !packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
-    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::apply<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, exact_db, sample_rate, results);
+    return dspi::apply_bulk_device(c, inst0, n, packets, host, exact_db, sample_rate, results);
 }
 
 int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
 {
-    if (!c || !packets) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::collect<dspi::ParamStores>(c, c->bulk, inst0, n, packets, host, results);
+    return dspi::collect_bulk_device(c, inst0, n, packets, host, results);
 }
 
 int dspi_chainq_apply_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride, const dspi_preset_load *load,
-                                const dspi_bulk_host *host, float sample_rate, int32_t *results)
+                                    const dspi_bulk_host *host, float sample_rate, int32_t *results)
 {
-    if (!c || !images || !load || !host || !results) return fail(DSPI_EINVAL, "null argument");
-    if (image_stride < sizeof(dspi::bulk::SlotOf<dspi::ParamStores>)) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, sizeof(dspi::bulk::SlotOf<dspi::ParamStores>));
-    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::apply_preset<dspi::ParamStores>(c, c->bulk, c->preset, inst0, n, images, image_stride, load, host, sample_rate, results);
+    return dspi::apply_preset_device(c, inst0, n, images, image_stride, load, host, sample_rate, results);
 }
 
-int dspi_chainq_collect_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride, int32_t *results)
+int dspi_chainq_collect_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
+                                      int32_t *results)
 {
-    if (!c || !slot_indices || !images) return fail(DSPI_EINVAL, "null argument");
-    if (image_stride < sizeof(dspi::bulk::SlotOf<dspi::ParamStores>)) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, sizeof(dspi::bulk::SlotOf<dspi::ParamStores>));
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return dspi::bulk::collect_preset<dspi::ParamStores>(c, c->preset, inst0, n, slot_indices, images, image_stride, results);
+    return dspi::collect_preset_device(c, inst0, n, slot_indices, images, image_stride, results);
 }
 
-int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_biquad_q28 *biquads)
-{
-    if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t row = (size_t)dspi::kRoles * DSPI_MAX_BANDS;
-    CU_OK(cudaMemcpyAsync(c->d_aos + inst0 * row, biquads, n * row * sizeof(dspi_biquad_q28), cudaMemcpyHostToDevice, c->stream));
-    const uint32_t Np = c->d.N_pad, items = n * dspi::kRoles * DSPI_MAX_BANDS;
-    dspi::chainq_scatter_kernel<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_m),
-                                                                           (dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_o), 1);
-    CU_OK(cudaGetLastError());
-    c->launches++;
-    for (int role = 0; role < dspi::kRoles; role++) {
-        int rc = role < 2 ? dspi::eq_pack_range(c->eq_m, role * Np + inst0, n, c->stream)
-                          : dspi::eq_pack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
-        if (rc) return rc;
-    }
-    CU_OK(dspi::bulk::mark_stale(c->rec, inst0, n, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
+int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_biquad_q28 *biquads) { return dspi::upload_biquads(c, inst0, n, biquads); }
+int dspi_chainq_download_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_biquad_q28 *biquads) { return dspi::download_biquads(c, inst0, n, biquads); }
 
 int dspi_chainq_set_eq_params_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_eq_param *recipes, float sample_rate)
 {
-    if (!c || !recipes) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    // the sub-engines generate and pack on their own streams: everything issued on the engine stream so far (an
-    // asynchronous process_device in particular) must have finished reading the coefficient stores first
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    const uint32_t Np = c->d.N_pad;
-    std::vector<dspi_eq_param> tmp((size_t)n * DSPI_MAX_BANDS);
-    for (int role = 0; role < dspi::kRoles; role++) {               // filter_recipes[role][band] of every instance -> one engine range per role
-        for (uint32_t i = 0; i < n; i++)
-            memcpy(&tmp[(size_t)i * DSPI_MAX_BANDS], &recipes[((size_t)i * dspi::kRoles + role) * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
-        int rc = role < 2 ? dspi_eq_set_params_device(c->eq_m, role * Np + inst0, n, tmp.data(), sample_rate)
-                          : dspi_eq_set_params_device(c->eq_o, (role - 2) * Np + inst0, n, tmp.data(), sample_rate);
-        if (rc) return rc;
-        for (uint32_t i = 0; i < n; i++)                            // the clamps, written back like the reference does
-            memcpy(&recipes[((size_t)i * dspi::kRoles + role) * DSPI_MAX_BANDS], &tmp[(size_t)i * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
-    }
-    return dspi::bulk::record_recipes<dspi::ParamStores>(c, c->bulk, inst0, n, recipes);
+    return dspi::set_eq_params_device(c, inst0, n, recipes, sample_rate);
 }
 
-int dspi_chainq_download_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_biquad_q28 *biquads)
-{
-    if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %u) outside engine of %u", inst0, inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t row = (size_t)dspi::kRoles * DSPI_MAX_BANDS;
-    const uint32_t Np = c->d.N_pad, items = n * dspi::kRoles * DSPI_MAX_BANDS;
-    for (int role = 0; role < dspi::kRoles; role++) {
-        int rc = role < 2 ? dspi::eq_unpack_range(c->eq_m, role * Np + inst0, n, c->stream)
-                          : dspi::eq_unpack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
-        if (rc) return rc;
-    }
-    dspi::chainq_scatter_kernel<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_m),
-                                                                           (dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_o), 0);
-    CU_OK(cudaGetLastError());
-    c->launches++;
-    CU_OK(cudaMemcpyAsync(biquads, c->d_aos + inst0 * row, n * row * sizeof(dspi_biquad_q28), cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-static int check_process(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp)
-{
-    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
-    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
-    if (fpp == 0 || fpp > DSPI_PACKET_MAX) return fail(DSPI_EINVAL, "frames_per_packet must be 1..%d", DSPI_PACKET_MAX);
-    if (n_packets == 0) return fail(DSPI_EINVAL, "n_packets must be > 0");
-    if ((uint64_t)n_packets * fpp > c->desc.max_frames) return fail(DSPI_ERANGE, "%u frames exceed max_frames %u", n_packets * fpp, c->desc.max_frames);
-    return DSPI_OK;
-}
-
-static int check_packets(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames)
-{
-    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
-    if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
-    const char *why = "";
-    const int rc = c->sched.check(n_packets, packet_frames, &why);
-    if (rc == DSPI_ERANGE) return fail(rc, "%s %u", why, c->desc.max_frames);
-    return rc ? fail(rc, "%s", why) : DSPI_OK;
-}
-
-// d_spdif: words, or subframes when `subframes` is set (either may be NULL)
-static int process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                          void *d_spdif, bool subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
-    if (rc) return rc;
-    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
-    CU_OK(cudaSetDevice(c->desc.device));
-    // the schedule's offsets go to the device first, on the engine stream
-    dspi::PacketSchedule &ps = c->sched;
-    const uint32_t F = ps.frames;
-    CU_OK(ps.upload(packet_frames, c->stream, &c->launches));
-    const size_t post_smem = (size_t)4 * 2 * ps.longest * dspi::kXs * 4;    // 4 warps x (longest packet + look-ahead columns)
-    static dspi::PerDeviceOnce once;
-    int dev = 0;
-    if (once.needs(&dev)) {
-        CU_OK(cudaFuncSetAttribute(dspi::chainq_post_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)4 * 2 * dspi::kPkt * dspi::kXs * 4)));
-        once.mark(dev);
-    }
-    // Stage pipeline over packet slices on three streams (chain_streams.cuh), stages as in chain_f32.cu.
-    dspi::ChainStreams &st = c->st;
-    uint32_t slice_bounds[dspi::ChainStreams::kMaxSlices + 1];
-    const uint32_t n_slices = (uint32_t)dspi::ChainStreams::plan_slices(n_packets, slice_bounds);
-    if (c->env_instances) {                                                  // preset-mute envelope: this call's per-packet volumes
-        if (c->vmm_packets < n_packets) {
-            CU_OK(cudaStreamSynchronize(c->stream));
-            if (c->d.vmm) CU_OK(cudaFree(c->d.vmm));
-            c->d.vmm = nullptr; c->vmm_packets = 0;
-            CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(int32_t)));
-            c->vmm_packets = n_packets;
-        }
-        dspi::chainq_env_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets);
-        CU_OK(cudaGetLastError());
-        c->launches++;
-    }
-    const ChainQ d = c->d;
-    const uint32_t n_sms = st.stream_sms();
-    static const uint32_t kStreamCtas = [] { const char *e = getenv("DSPI_CHAIN_CTAS"); const int v = e ? atoi(e) : 0; return (uint32_t)(v >= 1 && v <= 8 ? v : 8); }();   // streaming CTAs (256 threads) per SM
-    CU_OK(cudaEventRecord(st.ev_begin, c->stream));
-    CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
-    for (uint32_t sl = 0; sl < n_slices; sl++) {
-        const uint32_t p0 = slice_bounds[sl], p1 = slice_bounds[sl + 1];
-        const uint32_t fb = ps.off[p0], fe = ps.off[p1];
-        int rc;
-        dspi::chainq_pre_kernel<<<(d.N_pad / 16 + 1) / 2, 64, 0, st.s_front>>>(d, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
-        CU_OK(cudaGetLastError());
-        if ((rc = dspi::eq_process_on(c->eq_m, d.mrow + fb, fe - fb, d.ldF, st.s_front)) != DSPI_OK) return rc;
-        dspi::chainq_post_kernel<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, ps.longest);
-        CU_OK(cudaGetLastError());
-        CU_OK(cudaEventRecord(st.ev_front[sl], st.s_front));
-        CU_OK(cudaStreamWaitEvent(st.s_out, st.ev_front[sl], 0));
-        dspi::chainq_mix_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
-        CU_OK(cudaGetLastError());
-        if ((rc = dspi::eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
-        if (subframes && d_spdif)
-            dspi::chainq_outpost_kernel<true><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
-        else
-            dspi::chainq_outpost_kernel<false><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
-        CU_OK(cudaGetLastError());
-        CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
-        CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_out[sl], 0));
-        dspi::chainq_pdm_kernel<<<(d.N + 127) / 128, 128, 0, st.s_pdm>>>(d, fb, fe, F, d_pdm);
-        CU_OK(cudaGetLastError());
-        c->launches += 5;
-    }
-    dspi::chainq_ring_kernel<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets, c->tx.bp);      // after the last outpost launch (stream order)
-    CU_OK(cudaGetLastError());
-    c->launches++;
-    std::swap(c->d.widx_in, c->d.widx_out);
-    CU_OK(cudaEventRecord(st.ev_aux, st.s_out));
-    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_aux, 0));
-    CU_OK(cudaEventRecord(st.ev_done, st.s_pdm));
-    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_done, 0));
-    if (d_status) {
-        dspi::chainq_status_kernel<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, d_status);
-        CU_OK(cudaGetLastError());
-        c->launches++;
-    }
-    return DSPI_OK;
-}
-
-// host memory in and out, staged through the engine's device buffers
-static int process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                        void *spdif_out, bool subframes, uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
-    if (rc) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    const size_t N = c->desc.n_instances, F = c->sched.frames;
-    const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * 2 * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
-    if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
-    if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
-    if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; }
-    // the modulator writes the rows of instances with a sub only; the others go back to the caller as zeros, on every call
-    // (an earlier call's bits would be there otherwise: a sub switched off since, or a longer call's [N][F][8] layout)
-    if (pdm_out) CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream));
-    CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = process_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
-                        pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
-    if (rc) return rc;
-    if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(dspi_status_q28), cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                       int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
-}
-
-int dspi_chainq_process_packets_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                     int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    return process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
-}
-
-int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                         dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
-}
-
-int dspi_chainq_process_subframes_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                       dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    return process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
-}
-
-int dspi_chainq_set_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
-{
-    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    std::vector<uint32_t> bp(n);
-    std::vector<uint64_t> cs(n);
-    if (!dspi::spdif_tx_unpack(tx, n, bp.data(), cs.data())) return fail(DSPI_EINVAL, "block_pos must be 0..191");
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));   // behind earlier calls
-    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-int dspi_chainq_get_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
-{
-    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    std::vector<uint32_t> bp(n);
-    std::vector<uint64_t> cs(n);
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaMemcpyAsync(bp.data(), c->tx.bp + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaMemcpyAsync(cs.data(), c->tx.cs40 + inst0, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    dspi::spdif_tx_pack(bp.data(), cs.data(), n, tx);
-    return DSPI_OK;
-}
-
-// the uniform schedule: n_packets packets of fpp frames
 int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *d_spdif,
                                uint32_t *d_pdm, dspi_status_q28 *d_status)
 {
-    int rc = check_process(c, d_pcm, bit_depth, n_packets, fpp);
-    if (rc) return rc;
-    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
-    return dspi_chainq_process_packets_device(c, d_pcm, bit_depth, n_packets, table.data(), d_spdif, d_pdm, d_status);
+    return dspi::process_uniform(c, d_pcm, bit_depth, n_packets, fpp, d_spdif, d_pdm, d_status, false);
 }
 
 int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif_out,
                              uint32_t *pdm_out, dspi_status_q28 *status)
 {
-    int rc = check_process(c, pcm, bit_depth, n_packets, fpp);
-    if (rc) return rc;
-    const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
-    return dspi_chainq_process_packets_host(c, pcm, bit_depth, n_packets, table.data(), spdif_out, pdm_out, status);
+    return dspi::process_uniform(c, pcm, bit_depth, n_packets, fpp, spdif_out, pdm_out, status, true);
 }
 
-
-// ---- checkpoint / resume: everything a later process call depends on besides the parameters ----------------
-static void state_sections(dspi_chainq *c, std::vector<std::pair<void *, size_t>> &v)
+int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                       int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
 {
-    const size_t Np = c->d.N_pad;
-    v.push_back({ c->d.loud_st, 8 * Np * 4 });
-    v.push_back({ c->d.xf, 7 * Np * 4 });
-    v.push_back({ c->d.lev_i, 4 * Np * 4 });
-    v.push_back({ c->d.lev_f, Np * 4 });
-    v.push_back({ c->d.lev_idx, Np * 4 });
-    v.push_back({ c->d.lev_la, (size_t)2 * dspi::kLa * Np * 4 });
-    v.push_back({ c->d.dline, (size_t)dspi::kOuts * dspi::kMaxDelay * Np * 4 });
-    v.push_back({ c->d.widx_in, Np * 4 });
-    v.push_back({ c->d.pdm, 9 * Np * 4 });
-    v.push_back({ c->d.peaks, (size_t)dspi::kRoles * Np * 2 });
-    v.push_back({ c->d.clip, Np * 2 });
-    v.push_back({ c->d.env, 5 * Np * 4 });                                 // preset-mute envelope state and mode
-    dspi::eq_state_sections(c->eq_m, v);
-    dspi::eq_state_sections(c->eq_o, v);
+    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
 }
 
-struct StateHeader { uint32_t magic, version, arith, n_instances, n_bands, n_sections; uint64_t bytes; };
-static const uint32_t kStateMagic = 0x53505344u;          // "DSPS"
-
-size_t dspi_chainq_state_size(dspi_chainq *c)
+int dspi_chainq_process_packets_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                     int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
 {
-    if (!c) return 0;
-    std::vector<std::pair<void *, size_t>> v;
-    state_sections(c, v);
-    size_t n = sizeof(StateHeader);
-    for (auto &s : v) n += s.second;
-    return n;
+    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
 }
 
-int dspi_chainq_state_export(dspi_chainq *c, void *blob, size_t cap)
+int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                         dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
 {
-    if (!c || !blob) return fail(DSPI_EINVAL, "null argument");
-    const size_t need = dspi_chainq_state_size(c);
-    if (cap < need) return fail(DSPI_ERANGE, "state blob needs %zu bytes, %zu given", need, cap);
-    CU_OK(cudaSetDevice(c->desc.device));
-    std::vector<std::pair<void *, size_t>> v;
-    state_sections(c, v);
-    StateHeader h = { kStateMagic, 1u, c->desc.arith, c->desc.n_instances, c->desc.n_bands, (uint32_t)v.size(), (uint64_t)need };
-    memcpy(blob, &h, sizeof(h));
-    char *p = (char *)blob + sizeof(h);
-    for (auto &s : v) {
-        CU_OK(cudaMemcpyAsync(p, s.first, s.second, cudaMemcpyDeviceToHost, c->stream));
-        p += s.second;
-    }
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
 }
 
-int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len)
+int dspi_chainq_process_subframes_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                       dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status_q28 *status)
 {
-    if (!c || !blob) return fail(DSPI_EINVAL, "null argument");
-    std::vector<std::pair<void *, size_t>> v;
-    state_sections(c, v);
-    StateHeader h;
-    if (len < sizeof(h)) return fail(DSPI_EINVAL, "state blob too short");
-    memcpy(&h, blob, sizeof(h));
-    if (h.magic != kStateMagic || h.version != 1u) return fail(DSPI_EINVAL, "not a dspi_b200 state blob (magic %08x version %u)", h.magic, h.version);
-    if (h.arith != c->desc.arith || h.n_instances != c->desc.n_instances || h.n_bands != c->desc.n_bands || h.n_sections != v.size() ||
-        h.bytes != dspi_chainq_state_size(c) || len < h.bytes)
-        return fail(DSPI_EINVAL, "state blob belongs to a different engine shape (%u instances, arith %u, %llu bytes)", h.n_instances, h.arith,
-                    (unsigned long long)h.bytes);
-    CU_OK(cudaSetDevice(c->desc.device));
-    const char *p = (const char *)blob + sizeof(h);
-    for (auto &s : v) {
-        CU_OK(cudaMemcpyAsync(s.first, p, s.second, cudaMemcpyHostToDevice, c->stream));
-        p += s.second;
-    }
-    CU_OK(cudaStreamSynchronize(c->stream));
-    int rc = dspi::eq_state_imported(c->eq_m, c->stream);
-    if (rc == DSPI_OK) rc = dspi::eq_state_imported(c->eq_o, c->stream);
-    if (rc) return rc;
-    std::vector<uint32_t> on(c->d.N);
-    CU_OK(cudaMemcpyAsync(on.data(), c->d.env + (size_t)4 * c->d.N_pad, (size_t)c->d.N * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    c->env_instances = 0;
-    for (uint32_t v : on) c->env_instances += v ? 1u : 0u;
-    return DSPI_OK;
+    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
 }
 
-// Frequency response of instances [inst0, inst0 + n) on the engine stream (see chain_f32.cu); out [n][5][2][n_freqs] float2
-static int chainq_response(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
-{
-    const char *why = "";
-    int rc = dspi::response_check_args(freqs, n_freqs, fs, out, &why);
-    if (rc) return fail(rc, "%s", why);
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    if ((uint64_t)inst0 + n > c->desc.n_instances) return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
-    if (n == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(c->resp.upload(freqs, n_freqs, c->stream, &c->launches));
-    const dspi_biquad_q28 *m_aos = (const dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_m), *o_aos = (const dspi_biquad_q28 *)dspi::eq_aos_mirror(c->eq_o);
-    auto launch = [&](uint32_t i0, uint32_t m, void *dst) -> cudaError_t {
-        const dim3 grid((n_freqs + 127) / 128, m < 65535u ? m : 65535u);
-        dspi::chainq_response_kernel<<<grid, 128, 0, c->stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
-        c->launches++;
-        return cudaGetLastError();
-    };
-    if (!host) {
-        CU_OK(launch(inst0, n, out));
-        return DSPI_OK;
-    }
-    const size_t row_bytes = (size_t)dspi::kOuts * 2 * n_freqs * 2 * sizeof(float);
-    uint32_t rows = 0;
-    CU_OK(c->resp.stage(row_bytes, n, c->stream, &rows));
-    for (uint32_t i = 0; i < n; i += rows) {
-        const uint32_t m = n - i < rows ? n - i : rows;
-        CU_OK(launch(inst0 + i, m, c->resp.d_stage));
-        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->stream));
-        CU_OK(cudaStreamSynchronize(c->stream));
-    }
-    return DSPI_OK;
-}
+int dspi_chainq_set_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx) { return dspi::set_spdif_tx(c, inst0, n, tx); }
+int dspi_chainq_get_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx) { return dspi::get_spdif_tx(c, inst0, n, tx); }
+
+size_t dspi_chainq_state_size(dspi_chainq *c) { return dspi::state_size(c); }
+int dspi_chainq_state_export(dspi_chainq *c, void *blob, size_t cap) { return dspi::state_export(c, blob, cap); }
+int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len) { return dspi::state_import(c, blob, len); }
 
 int dspi_chainq_response_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
 {
-    return chainq_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, out, true);
+    return dspi::response(c, inst0, n, freqs_hz, n_freqs, sample_rate, out, true);
 }
 
 int dspi_chainq_response_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out)
 {
-    return chainq_response(c, inst0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
+    return dspi::response(c, inst0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
 }
 
-int dspi_chainq_sync(dspi_chainq *c)
-{
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
-}
-
-/* SMs reserved for the modulator / left to every other stage (0, 0: no partition, see chain_streams.cuh) */
-int dspi_chainq_sm_partition(dspi_chainq *c, uint32_t *pdm_sms, uint32_t *rest_sms)
-{
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    if (pdm_sms) *pdm_sms = c->st.pdm_sms;
-    if (rest_sms) *rest_sms = c->st.rest_sms;
-    return DSPI_OK;
-}
-
-void *dspi_chainq_stream(dspi_chainq *c) { return c ? (void *)c->stream : nullptr; }
-uint64_t dspi_chainq_launch_count(dspi_chainq *c)
-{
-    return c ? c->launches + dspi_eq_launch_count(c->eq_m) + dspi_eq_launch_count(c->eq_o) : 0;
-}
+int dspi_chainq_sync(dspi_chainq *c) { return dspi::sync(c); }
+void *dspi_chainq_stream(dspi_chainq *c) { return dspi::stream(c); }
+int dspi_chainq_sm_partition(dspi_chainq *c, uint32_t *pdm_sms, uint32_t *rest_sms) { return dspi::sm_partition(c, pdm_sms, rest_sms); }
+uint64_t dspi_chainq_launch_count(dspi_chainq *c) { return dspi::launch_count(c); }
 
 }  // extern "C"
