@@ -49,6 +49,8 @@ SYMBOLS = [
     "dspi_chain_collect_bulk_device", "dspi_chainq_collect_bulk_device",
     "dspi_chain_apply_preset_device", "dspi_chainq_apply_preset_device",
     "dspi_chain_collect_preset_device", "dspi_chainq_collect_preset_device",
+    "dspi_chain_instance_image_size", "dspi_chain_export_instances", "dspi_chain_import_instances", "dspi_chain_reset_instances",
+    "dspi_chainq_instance_image_size", "dspi_chainq_export_instances", "dspi_chainq_import_instances", "dspi_chainq_reset_instances",
 ]
 
 
@@ -130,6 +132,11 @@ def lib():
             getattr(h, pre + "_launch_count").restype = C.c_uint64
             getattr(h, pre + "_state_size").argtypes = [vp]
             getattr(h, pre + "_state_size").restype = C.c_size_t
+            getattr(h, pre + "_instance_image_size").argtypes = [vp]
+            getattr(h, pre + "_instance_image_size").restype = C.c_size_t
+            getattr(h, pre + "_export_instances").argtypes = [vp, u32, u32, vp, C.c_size_t]
+            getattr(h, pre + "_import_instances").argtypes = [vp, u32, u32, vp, C.c_size_t]
+            getattr(h, pre + "_reset_instances").argtypes = [vp, u32, u32]
             getattr(h, pre + "_set_preset_mute").argtypes = [vp, u32, u32, vp, u32]
             getattr(h, pre + "_get_preset_mute").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_set_dynamics_device").argtypes = [vp, u32, u32, vp, C.c_float]
@@ -448,6 +455,35 @@ class _ChainEngine:
     def state_import(self, blob):
         b = np.ascontiguousarray(blob, np.uint8)
         _check(self._fn("state_import")(self._h, b.ctypes.data_as(C.c_void_p), C.c_size_t(b.size)))
+
+    def instance_image_size(self):
+        """Bytes of one instance image (``export_instances``)."""
+        return int(self._fn("instance_image_size")(self._h))
+
+    def export_instances(self, inst0=0, n=None):
+        """Images of instances [inst0, inst0+n) (default: to the end), uint8 [n, instance_image_size]: everything of each
+        instance a later call depends on - parameters, biquads and all running state, S/PDIF transmitter, configuration
+        record.  Ordered behind earlier work on the engine stream; changes nothing."""
+        n = self.n_instances - int(inst0) if n is None else int(n)
+        size = self.instance_image_size()
+        out = np.zeros((max(n, 0), size), np.uint8)
+        _check(self._fn("export_instances")(self._h, int(inst0), n, out.ctypes.data_as(C.c_void_p), C.c_size_t(size)))
+        return out
+
+    def import_instances(self, images, inst0=0):
+        """uint8 [n, stride] images (stride >= instance_image_size) from an engine of the same arith and band count, any
+        size or device -> instances [inst0, inst0+n), from the next process call on.  All or nothing: a bad header raises
+        and writes nothing."""
+        img = np.ascontiguousarray(images, np.uint8)
+        if img.ndim != 2:
+            raise ValueError("images must be [n, stride] bytes")
+        _check(self._fn("import_instances")(self._h, int(inst0), int(img.shape[0]), img.ctypes.data_as(C.c_void_p),
+                                            C.c_size_t(img.shape[1])))
+
+    def reset_instances(self, inst0=0, n=None):
+        """``reset_state`` for instances [inst0, inst0+n) only (default: to the end); parameters are kept."""
+        n = self.n_instances - int(inst0) if n is None else int(n)
+        _check(self._fn("reset_instances")(self._h, int(inst0), n))
 
     def sm_partition(self):
         """(SMs reserved for the modulator, SMs for every other stage); (0, 0) without a partition."""

@@ -893,18 +893,11 @@ struct F32 : ParamStores {
 
     static cudaError_t alloc_leveller(ChainHost<F32> *c) { return dev_alloc(c, &c->d.lev_s, (size_t)5 * c->d.N_pad); }
 
-    // leveller_reset_state()
-    static cudaError_t init_leveller(ChainHost<F32> *c)
+    // leveller_reset_state(): envelopes and smoothed gain 0, gain_linear and gain_prev_linear (rows 3, 4) 1.0f
+    static void leveller_arrays(ChainHost<F32> *c, std::vector<InstArray> &v)
     {
-        const size_t Np = c->d.N_pad;
-        const std::vector<float> one(Np, 1.0f);
-        cudaError_t e;
-        if ((e = cudaMemsetAsync(c->d.lev_s, 0, 5 * Np * 4, c->stream)) != cudaSuccess) return e;
-        if ((e = cudaMemcpyAsync(c->d.lev_s + 3 * Np, one.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;   // gain_linear = 1
-        return cudaMemcpyAsync(c->d.lev_s + 4 * Np, one.data(), Np * 4, cudaMemcpyHostToDevice, c->stream);                                // gain_prev_linear = 1
+        v.push_back(inst_array(c->d.lev_s, 5, kInBlob | kInImage | kReset, 4, 1u << 3 | 1u << 4, 0x3f800000u));
     }
-
-    static void leveller_sections(ChainHost<F32> *c, Sections &v) { v.push_back({ c->d.lev_s, (size_t)5 * c->d.N_pad * 4 }); }
 
     // volumes, preamp, loudness shelves and matrix / output gains of instance i of a set_params call
     static void pack(const dspi_chain_params_f32 &p, uint32_t i, uint32_t n, ParamRows<F32> &r)
@@ -1043,6 +1036,17 @@ int dspi_chain_get_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_spdi
 size_t dspi_chain_state_size(dspi_chain *c) { return dspi::state_size(c); }
 int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap) { return dspi::state_export(c, blob, cap); }
 int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len) { return dspi::state_import(c, blob, len); }
+
+size_t dspi_chain_instance_image_size(dspi_chain *c) { return dspi::instance_image_size(c); }
+int dspi_chain_export_instances(dspi_chain *c, uint32_t inst0, uint32_t n, void *images, size_t image_stride)
+{
+    return dspi::export_instances(c, inst0, n, images, image_stride);
+}
+int dspi_chain_import_instances(dspi_chain *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride)
+{
+    return dspi::import_instances(c, inst0, n, images, image_stride);
+}
+int dspi_chain_reset_instances(dspi_chain *c, uint32_t inst0, uint32_t n) { return dspi::reset_instances(c, inst0, n); }
 
 int dspi_chain_response_host(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
 {

@@ -9,9 +9,9 @@
 // launches (A::scatter, A::dynamics, A::response, and per kernel set K of A::with_stages: K::pre, K::post, K::mix,
 // K::outpost<SUBFRAMES>, K::ring, K::pdm, K::env, K::status) and the hooks
 //   A::check_desc(desc)                       arithmetic, instance / frame counts and band count of a new engine
-//   A::alloc_leveller(c), A::init_leveller(c) the leveller state arrays and their reset values
+//   A::alloc_leveller(c)                      the leveller state arrays
+//   A::leveller_arrays(c, v)                  their entries in the table of per-instance arrays, with their reset values
 //   A::pack(params, i, n, rows)               volumes, preamp, loudness and matrix / output gains of one instance
-//   A::leveller_sections(c, v)                the leveller state in the checkpoint
 // The code below never asks which arithmetic it serves.
 #pragma once
 #include <cstdarg>
@@ -28,6 +28,7 @@
 #include "chain_schedule.cuh"
 #include "chain_streams.cuh"
 #include "eq_kernels.cuh"
+#include "instance_image.cuh"
 #include "response.cuh"
 #include "spdif_bmc.cuh"
 
@@ -71,7 +72,7 @@ struct ChainHost {
     uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     PacketSchedule sched;            // packet lengths of the current call
-    ResponseBuffers resp;            // frequency table and host staging of *_response_*
+    ResponseBuffers resp;            // frequency table of *_response_*; host staging of *_response_host and the instance image calls
     bulk::Stage bulk;                // device staging of *_apply_bulk_device / _collect_bulk_device, allocated by the first call
     bulk::PresetStage preset;        // device staging of *_apply_preset_device / _collect_preset_device, allocated by the first call
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
@@ -96,25 +97,132 @@ int check_range(const ChainHost<A> *c, uint32_t inst0, uint32_t n)
     return DSPI_OK;
 }
 
-// state that leveller_reset_state() / the PDM restart path define as non-zero
+// ---- the per-instance arrays -------------------------------------------------------------------------------------------
+// One table of every per-instance array of an engine, read by the state blob (state_sections), the pipeline reset
+// (reset_range) and the instance images (image_plan).  Entry: `rows` rows of N_pad elements of `elem` bytes, element
+// (r, i) at p + (r * N_pad + i) * elem; `use` says who reads it; a reset writes `one` into the rows of the mask `one_rows`
+// (4-byte elements) and 0 into every other row.
+enum : uint32_t {
+    kInBlob = 1,     // a section of the state blob, in table order
+    kInImage = 2,    // part of an instance image
+    kReset = 4,      // cleared by reset_state / _reset_instances
+};
+struct InstArray {
+    void *p;
+    uint32_t rows, elem, use, one_rows, one;
+};
+template <typename T>
+InstArray inst_array(T *p, uint32_t rows, uint32_t use, uint32_t elem = sizeof(T), uint32_t one_rows = 0, uint32_t one = 0)
+{
+    return InstArray{ (void *)p, rows, elem, use, one_rows, one };
+}
+
+template <class A>
+void instance_arrays(ChainHost<A> *c, std::vector<InstArray> &v)
+{
+    constexpr uint32_t all = kInBlob | kInImage | kReset, O = A::kOuts;
+    auto &d = c->d;
+    // the state blob's sections, in the order its format fixes
+    v.push_back(inst_array(d.loud_st, 8, all));
+    v.push_back(inst_array(d.xf, 7, kInBlob | kInImage));                 // crossfeed coefficients and state (CrossfeedState)
+    A::leveller_arrays(c, v);
+    v.push_back(inst_array(d.lev_idx, 1, all));
+    v.push_back(inst_array(d.lev_la, 2 * DSPI_LA_SAMPLES, all));
+    v.push_back(inst_array(d.dline, O, all, A::kMaxDelay * (uint32_t)sizeof(*d.dline)));   // one ring per (output, instance)
+    v.push_back(inst_array(d.widx_in, 1, all));
+    v.push_back(inst_array(d.pdm, 9, all, 4, 1u << 7, 123456789u));      // dither seed, pdm_generator.c:62
+    v.push_back(inst_array(d.peaks, A::kRoles, all));
+    v.push_back(inst_array(d.clip, 1, all));
+    v.push_back(inst_array(d.env, 5, kInBlob | kInImage));                // preset-mute envelope state and mode
+    // rewritten from widx_in by every call
+    v.push_back(inst_array(d.widx_out, 1, kReset));
+    // the parameter rows set_params, _set_dynamics_device and _apply_bulk_device write
+    v.push_back(inst_array(d.preamp, 2, kInImage));
+    v.push_back(inst_array(d.flags, 1, kInImage));
+    v.push_back(inst_array(d.loud_c, A::kLoudRows, kInImage));
+    v.push_back(inst_array(d.loud_byp, 1, kInImage));
+    v.push_back(inst_array(d.lev_c, 9, kInImage));
+    v.push_back(inst_array(d.o_gl, O, kInImage));
+    v.push_back(inst_array(d.o_gr, O, kInImage));
+    v.push_back(inst_array(d.o_gain, O, kInImage));
+    v.push_back(inst_array(d.o_glin, O, kInImage));
+    v.push_back(inst_array(d.o_flags, O, kInImage));
+    v.push_back(inst_array(d.o_dly, O, kInImage));
+    v.push_back(inst_array(d.vol_base, 1, kInImage));
+    v.push_back(inst_array(d.vol_master, 1, kInImage));
+    v.push_back(inst_array(d.pmg, 1, kInImage));
+    v.push_back(inst_array(d.skip_m, 2, kInImage));
+    v.push_back(inst_array(d.skip_o, O, kInImage));
+    // S/PDIF transmitter and the wire configuration record
+    v.push_back(inst_array(c->tx.bp, 1, kInImage));
+    v.push_back(inst_array(c->tx.cs40, 1, kInImage));
+    v.push_back(inst_array(c->rec.packets, 1, kInImage));
+    v.push_back(inst_array(c->rec.host, 1, kInImage));
+    v.push_back(inst_array(c->rec.mark, 1, kInImage));
+}
+
+// Instance images: a header, then the wide arrays (elements of 16 bytes or more: delay rings, the configuration packet,
+// the 12 biquads of each EQ channel), then the scalar arrays by falling element size, so that every array is naturally
+// aligned; each array holds its rows back to back.  The size is a multiple of 16.
+struct ImageHeader { uint32_t magic, version, arith, n_bands; uint64_t bytes; uint32_t reserved[2]; };
+static_assert(sizeof(ImageHeader) == image::kHeaderWords * 4, "image header");
+constexpr uint32_t kImageMagic = 0x49505344u;             // "DSPI"
+constexpr uint32_t kImageVersion = 1;
+
+// The launch plan over the arrays of `use` (kInImage: with the biquads of the sub-engines' mirrors; kReset); returns the
+// image size.
+template <class A>
+size_t image_plan(ChainHost<A> *c, uint32_t use, image::Plan &pl)
+{
+    using B = typename A::Biquad;
+    std::vector<InstArray> t;
+    instance_arrays(c, t);
+    if (use == kInImage) {       // channel = role * N_pad + instance in both mirrors, [12] biquads each
+        t.push_back(inst_array((B *)eq_aos_mirror(c->eq_m), 2, kInImage, DSPI_MAX_BANDS * (uint32_t)sizeof(B)));
+        t.push_back(inst_array((B *)eq_aos_mirror(c->eq_o), A::kOuts, kInImage, DSPI_MAX_BANDS * (uint32_t)sizeof(B)));
+    }
+    memset(&pl, 0, sizeof(pl));
+    pl.N_pad = c->d.N_pad;
+    size_t off = sizeof(ImageHeader);
+    for (uint32_t e : { 0u, 8u, 4u, 2u, 1u }) {               // 0: the wide arrays
+        for (const InstArray &a : t) {
+            if (!(a.use & use) || (e == 0 ? a.elem < 16 : a.elem != e)) continue;
+            if (pl.n_fields == image::kMaxFields) return 0;
+            const uint32_t fi = pl.n_fields++;
+            pl.f[fi] = image::Field{ (char *)a.p, a.rows, a.elem, (uint32_t)off, a.one_rows, a.one };
+            const uint32_t step = e == 0 ? 1 : image::kSlabRows, segs = e == 0 ? (a.elem + image::kSegBytes - 1) / image::kSegBytes : 1;
+            for (uint32_t r = 0; r < a.rows; r += step)
+                for (uint32_t s = 0; s < segs; s++) {
+                    if (pl.n_tasks == image::kMaxTasks) return 0;
+                    pl.t[pl.n_tasks++] = image::Task{ (uint8_t)fi, (uint8_t)(e == 0 ? s : (a.rows - r < step ? a.rows - r : step)), (uint16_t)r };
+                }
+            off += (size_t)a.rows * a.elem;
+        }
+    }
+    pl.used = (uint32_t)off;
+    pl.bytes = (uint32_t)((off + 15) & ~(size_t)15);
+    const ImageHeader h = { kImageMagic, kImageVersion, c->desc.arith, c->desc.n_bands, pl.bytes, { 0, 0 } };
+    memcpy(pl.header, &h, sizeof(h));
+    return pl.bytes;
+}
+
+// the pipeline reset of instances [inst0, inst0 + n) on the engine stream
+template <class A>
+cudaError_t reset_range(ChainHost<A> *c, uint32_t inst0, uint32_t n)
+{
+    image::Plan pl;
+    if (!image_plan(c, kReset, pl)) return cudaErrorInvalidValue;
+    image::instance_image_kernel<image::kReset><<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, inst0, n, nullptr);
+    c->launches++;
+    return cudaGetLastError();
+}
+
+// every instance, padding included: what a new engine starts from and reset_state returns to
 template <class A>
 cudaError_t init_states(ChainHost<A> *c)
 {
-    const size_t Np = c->d.N_pad;
-    std::vector<int32_t> seed(Np, 123456789);                               // pdm_generator.c:62
-    cudaError_t e;
-    if ((e = A::init_leveller(c)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.lev_idx, 0, Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.lev_la, 0, (size_t)2 * DSPI_LA_SAMPLES * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.loud_st, 0, 8 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.dline, 0, (size_t)A::kOuts * A::kMaxDelay * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.widx_in, 0, Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.widx_out, 0, Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.pdm, 0, 9 * Np * 4, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemcpyAsync(c->d.pdm + 7 * Np, seed.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.peaks, 0, (size_t)A::kRoles * Np * 2, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d.clip, 0, Np * 2, c->stream)) != cudaSuccess) return e;
-    return cudaStreamSynchronize(c->stream);
+    cudaError_t e = reset_range(c, 0, c->d.N_pad);
+    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
 }
 
 // a new engine's transmitters: block position 0, the channel status init_spdif_buffer() stamps (audio_spdif.c:82-88)
@@ -742,18 +850,10 @@ using Sections = std::vector<std::pair<void *, size_t>>;
 template <class A>
 void state_sections(ChainHost<A> *c, Sections &v, bool with_eq = true)
 {
-    const size_t Np = c->d.N_pad;
-    v.push_back({ c->d.loud_st, 8 * Np * 4 });
-    v.push_back({ c->d.xf, 7 * Np * 4 });                                  // crossfeed coefficients and state (CrossfeedState)
-    A::leveller_sections(c, v);
-    v.push_back({ c->d.lev_idx, Np * 4 });
-    v.push_back({ c->d.lev_la, (size_t)2 * DSPI_LA_SAMPLES * Np * 4 });
-    v.push_back({ c->d.dline, (size_t)A::kOuts * A::kMaxDelay * Np * 4 });
-    v.push_back({ c->d.widx_in, Np * 4 });
-    v.push_back({ c->d.pdm, 9 * Np * 4 });
-    v.push_back({ c->d.peaks, (size_t)A::kRoles * Np * 2 });
-    v.push_back({ c->d.clip, Np * 2 });
-    v.push_back({ c->d.env, 5 * Np * 4 });                                 // preset-mute envelope state and mode
+    std::vector<InstArray> t;
+    instance_arrays(c, t);
+    for (const InstArray &a : t)
+        if (a.use & kInBlob) v.push_back({ a.p, (size_t)a.rows * c->d.N_pad * a.elem });
     if (!with_eq) return;
     eq_state_sections(c->eq_m, v);
     eq_state_sections(c->eq_o, v);
@@ -848,6 +948,128 @@ int state_import(ChainHost<A> *c, const void *blob, size_t len)
     CU_OK(cudaStreamSynchronize(c->stream));
     c->env_instances = 0;
     for (uint32_t x : on) c->env_instances += x ? 1u : 0u;
+    return DSPI_OK;
+}
+
+// ---- per-instance lifecycle: instance images and the pipeline reset of a range -------------------------------------------
+template <class A>
+size_t instance_image_size(ChainHost<A> *c)
+{
+    if (!c) return 0;
+    image::Plan pl;
+    return image_plan(c, kInImage, pl);
+}
+
+// arguments of the image calls; *plan filled, *size the image size
+template <class A>
+int check_images(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *images, size_t stride, image::Plan *plan, size_t *size)
+{
+    if (!c || !images) return fail(DSPI_EINVAL, "null argument");
+    *size = image_plan(c, kInImage, *plan);
+    if (*size == 0) return fail(DSPI_EINVAL, "instance image plan exceeds its tables");
+    if (stride < *size) return fail(DSPI_EINVAL, "image_stride %zu below the image size %zu", stride, *size);
+    return check_range(c, inst0, n);
+}
+
+// the EQ sub-engines' ranges of instances [inst0, inst0 + n): every role of the master / output engine in one launch
+template <class A>
+void role_ranges(ChainHost<A> *c, RoleRange &rm, RoleRange &ro)
+{
+    rm.roles = 2; ro.roles = A::kOuts;
+    rm.stride = ro.stride = c->d.N_pad;
+}
+
+template <class A>
+int export_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, void *images, size_t stride)
+{
+    image::Plan pl;
+    size_t size = 0;
+    int rc = check_images(c, inst0, n, images, stride, &pl, &size);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    uint32_t chunk = 0;
+    CU_OK(c->resp.stage(size, n, c->stream, &chunk));
+    RoleRange rm, ro;
+    role_ranges(c, rm, ro);
+    rc = eq_unpack_range(c->eq_m, inst0, n, c->stream, rm);               // running EQ state into the mirrors, as download_biquads
+    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, inst0, n, c->stream, ro);
+    if (rc) return rc;
+    unsigned char *stage = (unsigned char *)c->resp.d_stage;
+    for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
+        const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
+        image::instance_image_kernel<image::kExport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, inst0 + i0, nc, stage);
+        CU_OK(cudaGetLastError());
+        c->launches++;
+        CU_OK(cudaMemcpy2DAsync((char *)images + (size_t)i0 * stride, stride, stage, size, size, nc, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CU_OK(cudaStreamSynchronize(c->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *images, size_t stride)
+{
+    image::Plan pl;
+    size_t size = 0;
+    int rc = check_images(c, inst0, n, images, stride, &pl, &size);
+    if (rc || n == 0) return rc;
+    const char *img = (const char *)images;
+    for (uint32_t i = 0; i < n; i++) {                                       // every header before anything is written
+        ImageHeader h;
+        memcpy(&h, img + (size_t)i * stride, sizeof(h));
+        if (h.magic != kImageMagic || h.version != kImageVersion)
+            return fail(DSPI_EINVAL, "image %u is not a dspi_b200 instance image (magic %08x version %u)", i, h.magic, h.version);
+        if (h.arith != c->desc.arith || h.n_bands != c->desc.n_bands || h.bytes != size)
+            return fail(DSPI_EINVAL, "image %u belongs to a different engine kind (arith %u, %u bands, %llu bytes)", i, h.arith, h.n_bands,
+                        (unsigned long long)h.bytes);
+    }
+    CU_OK(cudaSetDevice(c->desc.device));
+    // envelope-mode instances: the range's modes before (behind earlier work) and in the images (env row 4)
+    uint32_t env_off = 0;
+    for (uint32_t k = 0; k < pl.n_fields; k++)
+        if (pl.f[k].p == (char *)c->d.env) env_off = pl.f[k].off + 4 * 4;
+    const size_t Np = c->d.N_pad;
+    std::vector<uint32_t> cur((size_t)n);
+    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    uint32_t before = 0, after = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        uint32_t on;
+        memcpy(&on, img + (size_t)i * stride + env_off, 4);
+        before += cur[i] ? 1u : 0u;
+        after += on ? 1u : 0u;
+    }
+    uint32_t chunk = 0;
+    CU_OK(c->resp.stage(size, n, c->stream, &chunk));
+    unsigned char *stage = (unsigned char *)c->resp.d_stage;
+    for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
+        const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
+        CU_OK(cudaMemcpy2DAsync(stage, size, img + (size_t)i0 * stride, stride, size, nc, cudaMemcpyHostToDevice, c->stream));
+        image::instance_image_kernel<image::kImport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, inst0 + i0, nc, stage);
+        CU_OK(cudaGetLastError());
+        c->launches++;
+    }
+    c->env_instances = c->env_instances - before + after;
+    // mirrors -> packed stores of the range only (topology words, skip remask, K1 kernel choice), then the skip masks, as
+    // upload_biquads and set_params do
+    RoleRange rm, ro;
+    role_ranges(c, rm, ro);
+    rc = eq_pack_range(c->eq_m, inst0, n, c->stream, rm);
+    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, inst0, n, c->stream, ro);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->stream);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->stream);
+    return rc;
+}
+
+template <class A>
+int reset_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n)
+{
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(reset_range(c, inst0, n));
+    CU_OK(cudaStreamSynchronize(c->stream));
     return DSPI_OK;
 }
 

@@ -859,22 +859,11 @@ struct Q28 : ParamStores {
         return e == cudaSuccess ? dev_alloc(c, &c->d.lev_f, (size_t)c->d.N_pad) : e;
     }
 
-    // leveller_reset_state(): env_l, env_r 0, gain, gain_prev unity (leveller.c:101-102), smooth_db 0
-    static cudaError_t init_leveller(ChainHost<Q28> *c)
+    // leveller_reset_state(): env_l, env_r 0, gain, gain_prev (rows 2, 3) unity (leveller.c:101-102), smooth_db 0
+    static void leveller_arrays(ChainHost<Q28> *c, std::vector<InstArray> &v)
     {
-        const size_t Np = c->d.N_pad;
-        const std::vector<int32_t> unity(Np, kUnity);
-        cudaError_t e;
-        if ((e = cudaMemsetAsync(c->d.lev_i, 0, 4 * Np * 4, c->stream)) != cudaSuccess) return e;
-        if ((e = cudaMemcpyAsync(c->d.lev_i + 2 * Np, unity.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
-        if ((e = cudaMemcpyAsync(c->d.lev_i + 3 * Np, unity.data(), Np * 4, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return e;
-        return cudaMemsetAsync(c->d.lev_f, 0, Np * 4, c->stream);
-    }
-
-    static void leveller_sections(ChainHost<Q28> *c, Sections &v)
-    {
-        v.push_back({ c->d.lev_i, (size_t)4 * c->d.N_pad * 4 });
-        v.push_back({ c->d.lev_f, (size_t)c->d.N_pad * 4 });
+        v.push_back(inst_array(c->d.lev_i, 4, kInBlob | kInImage | kReset, 4, 1u << 2 | 1u << 3, (uint32_t)kUnity));
+        v.push_back(inst_array(c->d.lev_f, 1, kInBlob | kInImage | kReset));
     }
 
     // volumes, preamp, loudness shelves and matrix / output gains of instance i of a set_params call, folded to Q15 / Q28
@@ -1003,6 +992,17 @@ int dspi_chainq_get_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_sp
 size_t dspi_chainq_state_size(dspi_chainq *c) { return dspi::state_size(c); }
 int dspi_chainq_state_export(dspi_chainq *c, void *blob, size_t cap) { return dspi::state_export(c, blob, cap); }
 int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len) { return dspi::state_import(c, blob, len); }
+
+size_t dspi_chainq_instance_image_size(dspi_chainq *c) { return dspi::instance_image_size(c); }
+int dspi_chainq_export_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, void *images, size_t image_stride)
+{
+    return dspi::export_instances(c, inst0, n, images, image_stride);
+}
+int dspi_chainq_import_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride)
+{
+    return dspi::import_instances(c, inst0, n, images, image_stride);
+}
+int dspi_chainq_reset_instances(dspi_chainq *c, uint32_t inst0, uint32_t n) { return dspi::reset_instances(c, inst0, n); }
 
 int dspi_chainq_response_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
 {

@@ -362,6 +362,37 @@ int dspi_chain_get_preset_mute(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_p
 size_t dspi_chain_state_size(dspi_chain *c);
 int dspi_chain_state_export(dspi_chain *c, void *blob, size_t cap);
 int dspi_chain_state_import(dspi_chain *c, const void *blob, size_t len);
+/* Per-instance lifecycle: restart, checkpoint or move one device without touching the others.  An instance image holds
+ * everything of ONE instance that a later call depends on: its parameter rows (those _set_params, _set_dynamics_device
+ * and _apply_bulk_device write), its 11 (Q28: 7) x 12 biquads with their current state (reference layout), loudness /
+ * crossfeed / leveller state, look-ahead and delay rings with the write index, modulator state, meters, preset-mute
+ * envelope and mode, S/PDIF transmitter (block position, channel status), and the wire configuration record (packet body,
+ * host record, DSPI_BULK_* mark).  Private, versioned format (header: magic, version, arith, n_bands, size; no CRC).  It
+ * loads into any engine of the same arith and n_bands on any device, at any instance index: it does not depend on
+ * n_instances, max_frames, the K1 geometry (DSPI_F32_CPL) or the SM partition.  _instance_image_size gives its size
+ * (0 for a NULL engine): about 164 KB for the float engine, 51 KB for Q28, most of it the delay rings.
+ * images is host memory; image i is at images + i * image_stride, image_stride >= the image size (as preset images).
+ * The calls stage through a bounded device buffer in instance chunks (32 MiB, DSPI_HOST_CHUNK_MB in the environment
+ * overrides; shared with the _response_host staging), one copy kernel and one copy each way per chunk.
+ *   _export_instances: images of instances [inst0, inst0+n).  Read-only; ordered behind everything issued earlier on the
+ *     engine stream, asynchronous process calls included; returns when the images are in the caller's memory.
+ *   _import_instances: instances [inst0, inst0+n) become the instances the images were exported from, from the next
+ *     process call on (a continuation gives the bytes the source engine would have given).  All or nothing: every
+ *     header is checked first - magic, version, arith, n_bands, size - and any mismatch gives DSPI_EINVAL with nothing
+ *     written.  Ordered behind earlier work; every instance outside the range is left untouched, its EQ coefficients and
+ *     state in 32- and 64-channel groups shared with the range included.  The configuration record and its mark come
+ *     from the image (a stale or unset instance stays so).  Returns when the engine is updated.
+ *   _reset_instances: _reset_state for instances [inst0, inst0+n) only - the same fields cleared, the same kept (EQ
+ *     state, crossfeed state, preset-mute envelope, S/PDIF transmitter), and the parameters and configuration record
+ *     kept too.  Ordered behind earlier work; returns when done.
+ * A freed slot returns to power-on state by importing an image exported from a freshly created engine of the same arith
+ * and n_bands: parameters, state and transmitter of a new engine's instance, mark DSPI_BULK_UNSET.
+ * Errors: DSPI_EINVAL for a NULL pointer or an image_stride below the image size; DSPI_ERANGE for a range past the end of
+ * the engine (also one whose end wraps in 32 bits); nothing is written then.  n == 0 does nothing. */
+size_t dspi_chain_instance_image_size(dspi_chain *c);
+int dspi_chain_export_instances(dspi_chain *c, uint32_t inst0, uint32_t n, void *images, size_t image_stride);
+int dspi_chain_import_instances(dspi_chain *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride);
+int dspi_chain_reset_instances(dspi_chain *c, uint32_t inst0, uint32_t n);
 /* n_packets USB packets of frames_per_packet (<= 192) frames for every instance.
  *   pcm:       [n_instances][n_packets * frames_per_packet] interleaved L,R little-endian frames,
  *              bit_depth 16 (4 bytes / frame) or 24 (packed, 6 bytes / frame)      (HOST memory)
@@ -458,6 +489,11 @@ int dspi_chainq_get_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi
 size_t dspi_chainq_state_size(dspi_chainq *c);
 int dspi_chainq_state_export(dspi_chainq *c, void *blob, size_t cap);
 int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len);   /* + dspi_chainq_set_spdif_tx, as dspi_chain_* */
+/* per-instance images and reset, as dspi_chain_* */
+size_t dspi_chainq_instance_image_size(dspi_chainq *c);
+int dspi_chainq_export_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, void *images, size_t image_stride);
+int dspi_chainq_import_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride);
+int dspi_chainq_reset_instances(dspi_chainq *c, uint32_t inst0, uint32_t n);
 /* pcm as for dspi_chain_process_host; spdif_out [n_instances][2][n_frames][2]; pdm_out [n_instances][n_frames][8] */
 int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t frames_per_packet,
                              int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status);
