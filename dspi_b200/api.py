@@ -51,6 +51,10 @@ SYMBOLS = [
     "dspi_chain_collect_preset_device", "dspi_chainq_collect_preset_device",
     "dspi_chain_instance_image_size", "dspi_chain_export_instances", "dspi_chain_import_instances", "dspi_chain_reset_instances",
     "dspi_chainq_instance_image_size", "dspi_chainq_export_instances", "dspi_chainq_import_instances", "dspi_chainq_reset_instances",
+    "dspi_chain_process_packets_range_host", "dspi_chain_process_packets_range_device",
+    "dspi_chain_process_subframes_range_host", "dspi_chain_process_subframes_range_device",
+    "dspi_chainq_process_packets_range_host", "dspi_chainq_process_packets_range_device",
+    "dspi_chainq_process_subframes_range_host", "dspi_chainq_process_subframes_range_device",
 ]
 
 
@@ -151,6 +155,9 @@ def lib():
             getattr(h, pre + "_get_spdif_tx").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_process_subframes_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_process_subframes_device").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
+            for form in ("packets", "subframes"):
+                for where in ("host", "device"):
+                    getattr(h, "%s_process_%s_range_%s" % (pre, form, where)).argtypes = [vp, u32, u32, vp, u32, u32, vp, vp, vp, vp]
         for pre in ("dspi_eq", "dspi_chain", "dspi_chainq"):
             getattr(h, pre + "_response_host").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
             getattr(h, pre + "_response_device").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
@@ -532,6 +539,30 @@ class _ChainEngine:
         t, F = _packet_table(packet_frames)
         return self._process_host("process_packets_host", pcm, bit_depth, F, (t.size, t.ctypes.data), want_spdif, want_pdm, want_status)
 
+    def process_packets_range_host(self, inst0, pcm, bit_depth, packet_frames, want_spdif=True, want_pdm=True, want_status=True):
+        """``process_packets_host`` over instances [inst0, inst0 + n) only, n = ``pcm.shape[0]`` (inst0 a multiple of 64),
+        with this call's own ``packet_frames``.  Every array has n rows, row i for instance inst0 + i; nothing outside the
+        range changes.  Returns (spdif, pdm, status)."""
+        t, F = _packet_table(packet_frames)
+        pcm = np.ascontiguousarray(pcm)
+        n = pcm.shape[0]
+        assert pcm.dtype == np.uint8 and pcm.shape == (n, F * (6 if bit_depth == 24 else 4))
+        spdif = np.zeros((n, self._PAIRS, F, 2), np.int32) if want_spdif else None
+        pdm = np.zeros((n, F, 8), np.uint32) if want_pdm else None
+        status = np.zeros(n, self._STATUS) if want_status else None
+        _check(self._fn("process_packets_range_host")(self._h, int(inst0), n, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
+                                                      spdif.ctypes.data if want_spdif else None, pdm.ctypes.data if want_pdm else None,
+                                                      status.ctypes.data if want_status else None))
+        return spdif, pdm, status
+
+    def process_packets_range_device(self, inst0, n, pcm_ptr, bit_depth, packet_frames, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
+        """``process_packets_range_host`` with device pointers to n-row buffers, asynchronous on the engine stream."""
+        t, _ = _packet_table(packet_frames)
+        _check(self._fn("process_packets_range_device")(self._h, int(inst0), int(n), C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
+                                                        C.c_void_p(int(spdif_ptr)) if spdif_ptr else None,
+                                                        C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                        C.c_void_p(int(status_ptr)) if status_ptr else None))
+
     def _process_host(self, name, pcm, bit_depth, F, schedule, want_spdif, want_pdm, want_status):
         pcm = np.ascontiguousarray(pcm)
         assert pcm.dtype == np.uint8 and pcm.shape == (self.n_instances, F * (6 if bit_depth == 24 else 4))
@@ -664,6 +695,30 @@ class _ChainEngine:
                                                   pdm.ctypes.data if want_pdm else None,
                                                   status.ctypes.data if want_status else None))
         return sub, pdm, status
+
+    def process_subframes_range_host(self, inst0, pcm, bit_depth, packet_frames, want_subframes=True, want_pdm=True, want_status=True):
+        """``process_subframes_host`` over instances [inst0, inst0 + n) only, n = ``pcm.shape[0]``, as
+        ``process_packets_range_host``.  Returns (subframes, pdm, status) with n rows each."""
+        t, F = _packet_table(packet_frames)
+        pcm = np.ascontiguousarray(pcm)
+        n = pcm.shape[0]
+        assert pcm.dtype == np.uint8 and pcm.shape == (n, F * (6 if bit_depth == 24 else 4))
+        sub = np.zeros((n, self._PAIRS, F, 2, 2), np.uint32) if want_subframes else None
+        pdm = np.zeros((n, F, 8), np.uint32) if want_pdm else None
+        status = np.zeros(n, self._STATUS) if want_status else None
+        _check(self._fn("process_subframes_range_host")(self._h, int(inst0), n, pcm.ctypes.data, bit_depth, t.size, t.ctypes.data,
+                                                        sub.ctypes.data if want_subframes else None,
+                                                        pdm.ctypes.data if want_pdm else None,
+                                                        status.ctypes.data if want_status else None))
+        return sub, pdm, status
+
+    def process_subframes_range_device(self, inst0, n, pcm_ptr, bit_depth, packet_frames, subframes_ptr=0, pdm_ptr=0, status_ptr=0):
+        """``process_subframes_range_host`` with device pointers (subframes 16-byte aligned), asynchronous on the engine stream."""
+        t, _ = _packet_table(packet_frames)
+        _check(self._fn("process_subframes_range_device")(self._h, int(inst0), int(n), C.c_void_p(int(pcm_ptr)), bit_depth, t.size, t.ctypes.data,
+                                                          C.c_void_p(int(subframes_ptr)) if subframes_ptr else None,
+                                                          C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                          C.c_void_p(int(status_ptr)) if status_ptr else None))
 
     def process_subframes_device(self, pcm_ptr, bit_depth, packet_frames, subframes_ptr=0, pdm_ptr=0, status_ptr=0):
         """``process_subframes_host`` with device pointers (subframes 16-byte aligned), asynchronous on the engine stream."""

@@ -111,7 +111,8 @@ __device__ __forceinline__ float gain_computer(float x_db, float threshold, floa
 // ---------------------------------------------------------------------------------------------
 template <bool FUSED>
 __global__ void __launch_bounds__(64)
-chain_pre_kernel(ChainDev d, const uint8_t *__restrict__ pcm, uint32_t bit_depth, uint32_t f_begin, uint32_t f_end, uint32_t F)
+chain_pre_kernel(ChainDev d, uint32_t inst0, uint32_t n, const uint8_t *__restrict__ pcm, uint32_t bit_depth, uint32_t f_begin, uint32_t f_end,
+                 uint32_t F)
 {
     // warp = 16 instances x {L, R}: lane l handles side l >> 4 of instance inst16 + (l & 15).  The two sides of an
     // instance share nothing in this stage (separate shelf states, usb_audio.c:696 / :707), so splitting them over two
@@ -119,11 +120,13 @@ chain_pre_kernel(ChainDev d, const uint8_t *__restrict__ pcm, uint32_t bit_depth
     __shared__ float tile_s[2][32][kXs];                  // per warp: [frame][row = side * 16 + instance]
     __shared__ uint32_t pcm_s[2][2][16][49];              // per warp, double-buffered: 16 instances x 32 frames x <= 6 bytes (rows padded to 49 words)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t inst16 = (blockIdx.x * 2 + warp) * 16;
-    if (inst16 >= d.N_pad) return;
+    // instances [inst0, inst0 + n) of the engine, PCM rows and warps counted from inst0; warps cover n rounded up to 32
+    // instances, the lanes past n are not live and leave every state alone
+    const uint32_t local16 = (blockIdx.x * 2 + warp) * 16;
+    if (local16 >= ((n + 31) & ~31u)) return;
     const uint32_t side = lane >> 4, li = lane & 15;
-    const uint32_t inst = inst16 + li;
-    const bool live = inst < d.N;
+    const uint32_t inst16 = inst0 + local16, inst = inst16 + li;
+    const bool live = local16 + li < n;
     const uint32_t Np = d.N_pad;
     float (*tile)[kXs] = tile_s[warp];
 
@@ -145,8 +148,8 @@ chain_pre_kernel(ChainDev d, const uint8_t *__restrict__ pcm, uint32_t bit_depth
     // a 4-byte boundary the warp fetches the 16 tiles of its instances with coalesced word loads into shared
     // memory and every lane then decodes its own side from there, otherwise lanes read their bytes directly.
     const bool words_ok = ((reinterpret_cast<uintptr_t>(pcm) | ((size_t)F * bpf) | ((size_t)f_begin * bpf)) & 3u) == 0;
-    const uint8_t *my_pcm = pcm + (size_t)inst * F * bpf;
-    const uint32_t n_inst = min(16u, d.N > inst16 ? d.N - inst16 : 0u);
+    const uint8_t *my_pcm = pcm + (size_t)(local16 + li) * F * bpf;
+    const uint32_t n_inst = min(16u, n > local16 ? n - local16 : 0u);
     // asynchronous fetch of the tile starting at frame f0 into buffer `buf` (one commit group per call).  A last
     // word may run <= 2 bytes past a ragged tile: still inside the PCM buffer, because the very end of the
     // buffer is word-aligned (F * bpf is) and so is every tile start.
@@ -154,7 +157,7 @@ chain_pre_kernel(ChainDev d, const uint8_t *__restrict__ pcm, uint32_t bit_depth
         if (words_ok && f0 < f_end) {
             const uint32_t nwords = (min(32u, f_end - f0) * bpf + 3) / 4;
             for (uint32_t i = 0; i < n_inst; i++) {
-                const uint32_t *src = reinterpret_cast<const uint32_t *>(pcm + ((size_t)(inst16 + i) * F + f0) * bpf);
+                const uint32_t *src = reinterpret_cast<const uint32_t *>(pcm + ((size_t)(local16 + i) * F + f0) * bpf);
                 for (uint32_t w = lane; w < nwords; w += 32) cp_async_4(&pcm_s[warp][buf][i][w], src + w);
             }
         }
@@ -218,6 +221,7 @@ chain_pre_kernel(ChainDev d, const uint8_t *__restrict__ pcm, uint32_t bit_depth
         }
         __syncwarp();
     }
+    if (!live) return;
 #pragma unroll
     for (int j = 0; j < 2; j++) {
         d.loud_st[((side * 2 + j) * 2 + 0) * Np + inst] = ls[j][0];
@@ -230,20 +234,21 @@ chain_pre_kernel(ChainDev d, const uint8_t *__restrict__ pcm, uint32_t bit_depth
 // ---------------------------------------------------------------------------------------------
 template <bool FUSED>
 __global__ void __launch_bounds__(128)
-chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t longest)
+chain_post_kernel(ChainDev d, uint32_t inst0, uint32_t n, uint32_t p0, uint32_t n_packets, uint32_t longest)
 {
     extern __shared__ float smem[];                       // per warp: packet columns [longest][33] + look-ahead reads [longest][33]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t side = lane >> 4;
-    const uint32_t inst16 = (blockIdx.x * (blockDim.x >> 5) + warp) * 16;
-    if (inst16 >= d.N_pad) return;
-    const uint32_t inst = inst16 + (lane & 15);
+    const uint32_t local16 = (blockIdx.x * (blockDim.x >> 5) + warp) * 16;      // instances [inst0, inst0 + n): see chain_pre_kernel
+    if (local16 >= ((n + 31) & ~31u)) return;
+    const uint32_t inst16 = inst0 + local16, inst = inst16 + (lane & 15);
+    const bool live = local16 + (lane & 15) < n;
     const uint32_t Np = d.N_pad;
     float *xw = smem + (size_t)warp * 2 * longest * kXs;  // xw[t * 33 + r]: column r of this warp
     float *xs = xw + lane;                                // own column
     float *hs = xw + (size_t)longest * kXs + lane;        // held look-ahead samples, own column
 
-    const uint8_t flags = d.flags[inst];
+    const uint8_t flags = live ? d.flags[inst] : 0;       // lanes past the range run with every stage off
     const bool lev_on = flags & F_LEV, xf_on = flags & F_XFEED, lookahead = flags & F_LOOKAHEAD;
     // crossfeed: this lane owns its side's lowpass / all-pass state
     const float xf_a0 = d.xf[0 * Np + inst], xf_b1 = d.xf[1 * Np + inst], xf_ap = d.xf[4 * Np + inst];
@@ -374,6 +379,8 @@ chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t longest)
     }
 
     // ---- state back ----
+    const uint16_t clip_other = (uint16_t)__shfl_xor_sync(0xffffffffu, (uint32_t)clip, 16);
+    if (!live) return;
     d.xf[(2 + side) * Np + inst] = xf_lp;
     d.xf[(5 + side) * Np + inst] = xf_as;
     d.lev_s[side * Np + inst] = env;
@@ -385,7 +392,6 @@ chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t longest)
     }
     d.peaks[side * Np + inst] = (uint16_t)__fmul_rn(fminf(1.0f, peak_in), 32767.0f);    // usb_audio.c:963-964
     // clip_flags bits 0/1: the two sides of one instance sit in lanes l and l+16; two instances share a 32-bit word
-    const uint16_t clip_other = (uint16_t)__shfl_xor_sync(0xffffffffu, (uint32_t)clip, 16);
     if (side == 0 && (clip | clip_other)) atomicOr(reinterpret_cast<unsigned int *>(d.clip + (inst & ~1u)), (unsigned int)(clip | clip_other) << (16 * (inst & 1)));
 }
 
@@ -394,15 +400,15 @@ chain_post_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t longest)
 // ---------------------------------------------------------------------------------------------
 template <bool FUSED>
 __global__ void __launch_bounds__(256)
-chain_mix_kernel(ChainDev d, uint32_t f_begin, uint32_t f_end)
+chain_mix_kernel(ChainDev d, uint32_t inst0, uint32_t n, uint32_t f_begin, uint32_t f_end)
 {
     const int lane = threadIdx.x & 31;
     constexpr int kB = 4;                                  // frames per lane per unit: kB independent loads in flight
     const uint32_t n_tiles = (f_end - f_begin + 32 * kB - 1) / (32 * kB);
-    const uint64_t units = (uint64_t)d.N * n_tiles;
+    const uint64_t units = (uint64_t)n * n_tiles;
     const uint32_t Np = d.N_pad;
     for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
-        const uint32_t inst = (uint32_t)(u / n_tiles), tile = (uint32_t)(u % n_tiles);
+        const uint32_t inst = inst0 + (uint32_t)(u / n_tiles), tile = (uint32_t)(u % n_tiles);
         const uint32_t fbase = f_begin + tile * 32 * kB + lane;
         float l[kB], r[kB];
 #pragma unroll
@@ -436,11 +442,11 @@ chain_mix_kernel(ChainDev d, uint32_t f_begin, uint32_t f_end)
 // update_preset_mute_envelope() (usb_audio.c:466-498) for every packet of the call, one instance per thread, and the
 // volume chain of :569-571 that depends on it: vmm[p] = (vol_base * g_p) * master_volume_linear.  Same operations, same
 // order as dspi_preset_mute_step() on the host.
-__global__ void chain_env_kernel(ChainDev d, uint32_t n_packets)
+__global__ void chain_env_kernel(ChainDev d, uint32_t inst0, uint32_t n, uint32_t n_packets)
 {
-    const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, inst = inst0 + i;
     const uint32_t Np = d.N_pad;
-    if (inst >= d.N || !d.env[4 * Np + inst]) return;
+    if (i >= n || !d.env[4 * Np + inst]) return;
     uint32_t loading = d.env[0 * Np + inst], counter = d.env[1 * Np + inst];
     float g = __uint_as_float(d.env[2 * Np + inst]);
     const uint32_t fs = d.env[3 * Np + inst];
@@ -625,17 +631,18 @@ __device__ __forceinline__ float warp_max(float v)
     return v;
 }
 
-// SUBFRAMES = false: spdif_out is [N][4][F][2] int32 words.  SUBFRAMES = true: it is [N][4][F] uint4 subframe pairs
+// Instances [inst0, inst0 + n); the caller's rows are counted from inst0.
+// SUBFRAMES = false: spdif_out is [n][4][F][2] int32 words.  SUBFRAMES = true: it is [n][4][F] uint4 subframe pairs
 // {l, h, l, h}, each instance's frames encoded at its own block position and channel status (spdif_bmc.cuh) - what
 // dspi_spdif_encode_* makes of the words, without the words buffer.
 template <bool SUBFRAMES>
 __global__ void __launch_bounds__(256)
-chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out, SpdifTx tx)
+chain_outpost_kernel(ChainDev d, uint32_t inst0, uint32_t n, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out, SpdifTx tx)
 {
     const int lane = threadIdx.x & 31;
-    const uint64_t units = (uint64_t)d.N * n_packets;
+    const uint64_t units = (uint64_t)(inst0 + n) * n_packets;              // units (instance, packet) of the range
     const uint32_t Np = d.N_pad;
-    for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
+    for (uint64_t u = (uint64_t)inst0 * n_packets + blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
         const uint32_t inst = (uint32_t)(u / n_packets), p = p0 + (uint32_t)(u % n_packets);
         const uint32_t f0 = d.off[p], count = d.off[p + 1] - f0;
         const bool last = p == p0 + n_packets - 1;
@@ -675,9 +682,9 @@ chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, in
                         }
                         if (SUBFRAMES) {                                      // 16 bytes per lane: 512 contiguous bytes per warp store
                             const uint32_t pos = (bp + T) % 192u;
-                            reinterpret_cast<uint4 *>(spdif_out)[((size_t)inst * 4 + k) * F + T] = encode_frame(w, spdif_pre_left(pos), spdif_cs_bit(pos, cs40));
+                            reinterpret_cast<uint4 *>(spdif_out)[((size_t)(inst - inst0) * 4 + k) * F + T] = encode_frame(w, spdif_pre_left(pos), spdif_cs_bit(pos, cs40));
                         } else {
-                            *reinterpret_cast<int2 *>(spdif_out + (((size_t)inst * 4 + k) * F + T) * 2) = w;
+                            *reinterpret_cast<int2 *>(spdif_out + (((size_t)(inst - inst0) * 4 + k) * F + T) * 2) = w;
                         }
                     }
                 }
@@ -699,17 +706,18 @@ chain_outpost_kernel(ChainDev d, uint32_t p0, uint32_t n_packets, uint32_t F, in
     }
 }
 
-// once per call, after every outpost launch of the call: the delay rings take the last <= 4096 post-gain
-// samples (older writes of this call would have been overwritten anyway), the shared write index advances, and so
-// does the S/PDIF block position - by all F frames whatever the call copied out (the transmitter sends every frame)
+// once per call, after every outpost launch of the call: the delay rings of instances [inst0, inst0 + n) take the last
+// <= 4096 post-gain samples (older writes of this call would have been overwritten anyway), the shared write index advances
+// (into widx_out), and so does the S/PDIF block position - by all F frames whatever the call copied out (the transmitter
+// sends every frame)
 __global__ void __launch_bounds__(256)
-chain_ring_kernel(ChainDev d, uint32_t F, uint32_t n_packets, uint32_t *__restrict__ spdif_bp)
+chain_ring_kernel(ChainDev d, uint32_t inst0, uint32_t n, uint32_t F, uint32_t n_packets, uint32_t *__restrict__ spdif_bp)
 {
     const int lane = threadIdx.x & 31;
-    const uint64_t units = (uint64_t)d.N * kOuts;
+    const uint64_t units = (uint64_t)n * kOuts;
     const uint32_t Np = d.N_pad;
     for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
-        const uint32_t inst = (uint32_t)(u / kOuts), o = (uint32_t)(u % kOuts);
+        const uint32_t inst = inst0 + (uint32_t)(u / kOuts), o = (uint32_t)(u % kOuts);
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
         const OutCfg c = out_cfg(d, o, inst, any_delay);
@@ -729,12 +737,12 @@ chain_ring_kernel(ChainDev d, uint32_t F, uint32_t n_packets, uint32_t *__restri
 // delta-sigma PDM (chain_pdm.cuh): one instance per lane
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
-chain_pdm_kernel(ChainDev d, uint32_t f_begin, uint32_t f_end, uint32_t F, uint32_t *__restrict__ pdm_out)
+chain_pdm_kernel(ChainDev d, uint32_t inst0, uint32_t n, uint32_t f_begin, uint32_t f_end, uint32_t F, uint32_t *__restrict__ pdm_out)
 {
-    const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
-    if (inst >= d.N) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, inst = inst0 + i;
+    if (i >= n) return;
     if (!(d.flags[inst] & F_SUB_ON)) return;                                 // usb_audio.c:944
-    pdm_modulate_frames(d.pdm, d.subq + (size_t)inst * d.ldF, 1, d.N_pad, inst, f_begin, f_end, F, pdm_out);
+    pdm_modulate_frames(d.pdm, d.subq + (size_t)inst * d.ldF, 1, d.N_pad, inst, f_begin, f_end, pdm_out ? pdm_out + (size_t)i * F * 8 : nullptr);
 }
 
 // filters[][] of n instances (instance-major AoS) <-> the mirrors of the two EQ engines (channel = role' * N_pad + inst)
@@ -750,16 +758,16 @@ __global__ void chain_scatter_kernel(const dspi_biquad_f32 *__restrict__ aos, ui
     else *chain_q = *eng_q;
 }
 
-__global__ void chain_status_kernel(ChainDev d, dspi_status *__restrict__ out)
+__global__ void chain_status_kernel(ChainDev d, uint32_t inst0, uint32_t n, dspi_status *__restrict__ out)
 {
-    const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
-    if (inst >= d.N) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, inst = inst0 + i;
+    if (i >= n) return;
     dspi_status s;
     for (int r = 0; r < kRoles; r++) s.peaks[r] = d.peaks[r * d.N_pad + inst];
     s.cpu0_load = 0;
     s.cpu1_load = 0;
     s.clip_flags = d.clip[inst];
-    out[inst] = s;
+    out[i] = s;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1009,25 +1017,49 @@ int dspi_chain_process_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, 
 int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                       int32_t *d_spdif, uint32_t *d_pdm, dspi_status *d_status)
 {
-    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
+    return dspi::process_device(c, 0, dspi::all_instances(c), d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
 }
 
 int dspi_chain_process_packets_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                     int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status)
 {
-    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
+    return dspi::process_host(c, 0, dspi::all_instances(c), pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
 }
 
 int dspi_chain_process_subframes_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                         dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status *d_status)
 {
-    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
+    return dspi::process_device(c, 0, dspi::all_instances(c), d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
 }
 
 int dspi_chain_process_subframes_host(dspi_chain *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                       dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status *status)
 {
-    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
+    return dspi::process_host(c, 0, dspi::all_instances(c), pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
+}
+
+int dspi_chain_process_packets_range_device(dspi_chain *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                    const uint16_t *packet_frames, int32_t *d_spdif, uint32_t *d_pdm, dspi_status *d_status)
+{
+    return dspi::process_device(c, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
+}
+
+int dspi_chain_process_packets_range_host(dspi_chain *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                                  const uint16_t *packet_frames, int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status)
+{
+    return dspi::process_host(c, inst0, n, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
+}
+
+int dspi_chain_process_subframes_range_device(dspi_chain *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                      const uint16_t *packet_frames, dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status *d_status)
+{
+    return dspi::process_device(c, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
+}
+
+int dspi_chain_process_subframes_range_host(dspi_chain *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                                    const uint16_t *packet_frames, dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status *status)
+{
+    return dspi::process_host(c, inst0, n, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
 }
 
 int dspi_chain_set_spdif_tx(dspi_chain *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx) { return dspi::set_spdif_tx(c, inst0, n, tx); }

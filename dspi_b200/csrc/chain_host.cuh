@@ -676,11 +676,28 @@ int check_packets(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t
     return rc ? fail(rc, "%s", why) : DSPI_OK;
 }
 
-// One call over the schedule c->sched has checked, with the kernel set K: its offsets go to the device first, on the
-// engine stream.  d_spdif: words, or subframes when `subframes` is set (either may be NULL).
+// The EQ stage of one slice over the rows of `roles` roles (row = role * N_pad + instance) of instances [inst0, inst0 + n):
+// one launch over every row for the whole engine, else one launch per role over that role's rows.
+template <class A>
+int eq_stage(ChainHost<A> *c, dspi_eq *eq, uint32_t roles, void *rows, uint32_t fb, uint32_t fe, uint32_t inst0, uint32_t n, cudaStream_t s)
+{
+    const auto &d = c->d;
+    using T = std::remove_pointer_t<decltype(d.mrow)>;
+    if (inst0 == 0 && n == d.N) return eq_process_on(eq, (T *)rows + fb, fe - fb, d.ldF, s);
+    for (uint32_t r = 0; r < roles; r++) {
+        const uint32_t ch0 = r * d.N_pad + inst0;
+        const int rc = eq_process_range_on(eq, (T *)rows + (size_t)ch0 * d.ldF + fb, fe - fb, d.ldF, ch0, n, s);
+        if (rc) return rc;
+    }
+    return DSPI_OK;
+}
+
+// One call over instances [inst0, inst0 + n) and the schedule c->sched has checked, with the kernel set K: its offsets go
+// to the device first, on the engine stream.  The caller's buffers hold rows for the n instances.  d_spdif: words, or
+// subframes when `subframes` is set (either may be NULL).
 template <class A, class K>
-int run_stages(ChainHost<A> *c, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, void *d_spdif, bool subframes,
-               uint32_t *d_pdm, typename A::Status *d_status)
+int run_stages(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, void *d_spdif,
+               bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
 {
     PacketSchedule &ps = c->sched;
     const uint32_t n_packets = ps.n_packets, F = ps.frames;
@@ -705,13 +722,18 @@ int run_stages(ChainHost<A> *c, const void *d_pcm, uint32_t bit_depth, const uin
             CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(*c->d.vmm)));
             c->vmm_packets = n_packets;
         }
-        K::env<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, n_packets);
+        K::env<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, inst0, n, n_packets);
         CU_OK(cudaGetLastError());
         c->launches++;
     }
     const typename A::Dev d = c->d;
     const uint32_t n_sms = st.stream_sms();
     static const uint32_t kStreamCtas = [] { const char *e = getenv("DSPI_CHAIN_CTAS"); const int v = e ? atoi(e) : 0; return (uint32_t)(v >= 1 && v <= 8 ? v : 8); }();   // streaming CTAs (256 threads) per SM
+    auto stream_grid = [&](uint64_t units) {                                 // grid-stride kernels: no more CTAs than 8-warp units
+        const uint64_t ctas = (units + 7) / 8;
+        return (uint32_t)(ctas < (uint64_t)n_sms * kStreamCtas ? (ctas ? ctas : 1) : (uint64_t)n_sms * kStreamCtas);
+    };
+    const uint32_t n_warps16 = ((n + 31) & ~31u) / 16;                       // pre / post: 16 instances per warp
     CU_OK(cudaEventRecord(st.ev_begin, c->stream));
     CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
     for (uint32_t sl = 0; sl < n_slices; sl++) {
@@ -719,68 +741,89 @@ int run_stages(ChainHost<A> *c, const void *d_pcm, uint32_t bit_depth, const uin
         const uint32_t fb = ps.off[p0], fe = ps.off[p1];
         int rc;
         // ---- front: unpack + loudness -> master EQ -> leveller + crossfeed
-        K::pre<<<(d.N_pad / 16 + 1) / 2, 64, 0, st.s_front>>>(d, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
+        K::pre<<<(n_warps16 + 1) / 2, 64, 0, st.s_front>>>(d, inst0, n, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
         CU_OK(cudaGetLastError());
-        if ((rc = eq_process_on(c->eq_m, d.mrow + fb, fe - fb, d.ldF, st.s_front)) != DSPI_OK) return rc;
-        K::post<<<(d.N_pad / 16 + 3) / 4, 128, post_smem, st.s_front>>>(d, p0, p1 - p0, ps.longest);
+        if ((rc = eq_stage(c, c->eq_m, 2, d.mrow, fb, fe, inst0, n, st.s_front)) != DSPI_OK) return rc;
+        K::post<<<(n_warps16 + 3) / 4, 128, post_smem, st.s_front>>>(d, inst0, n, p0, p1 - p0, ps.longest);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_front[sl], st.s_front));
         // ---- outputs: matrix -> per-output EQ -> gain / delay / metering / conversion
         CU_OK(cudaStreamWaitEvent(st.s_out, st.ev_front[sl], 0));
-        K::mix<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, fb, fe);
+        K::mix<<<stream_grid((uint64_t)n * ((fe - fb + 127) / 128)), 256, 0, st.s_out>>>(d, inst0, n, fb, fe);
         CU_OK(cudaGetLastError());
-        if ((rc = eq_process_on(c->eq_o, d.orow + fb, fe - fb, d.ldF, st.s_out)) != DSPI_OK) return rc;
+        if ((rc = eq_stage(c, c->eq_o, A::kOuts, d.orow, fb, fe, inst0, n, st.s_out)) != DSPI_OK) return rc;
+        const uint32_t out_grid = stream_grid((uint64_t)n * (p1 - p0));
         if (subframes && d_spdif)
-            K::template outpost<true><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
+            K::template outpost<true><<<out_grid, 256, 0, st.s_out>>>(d, inst0, n, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
         else
-            K::template outpost<false><<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
+            K::template outpost<false><<<out_grid, 256, 0, st.s_out>>>(d, inst0, n, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
         // ---- modulator
         CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_out[sl], 0));
-        K::pdm<<<(d.N + 127) / 128, 128, 0, st.s_pdm>>>(d, fb, fe, F, d_pdm);
+        K::pdm<<<(n + 127) / 128, 128, 0, st.s_pdm>>>(d, inst0, n, fb, fe, F, d_pdm);
         CU_OK(cudaGetLastError());
         c->launches += 5;
     }
-    K::ring<<<n_sms * kStreamCtas, 256, 0, st.s_out>>>(d, F, n_packets, c->tx.bp);   // after the last outpost launch (stream order)
+    K::ring<<<stream_grid((uint64_t)n * A::kOuts), 256, 0, st.s_out>>>(d, inst0, n, F, n_packets, c->tx.bp);   // after the last outpost launch (stream order)
     CU_OK(cudaGetLastError());
     c->launches++;
-    std::swap(c->d.widx_in, c->d.widx_out);
+    // The ring kernel wrote the advanced write index of the call's instances into widx_out (the outpost and ring kernels read
+    // widx_in until the end of the call).  A whole-engine call swaps the two buffers; a range call copies its instances'
+    // indices back, so that every other instance keeps the index it has in widx_in.
+    if (inst0 == 0 && n == d.N) std::swap(c->d.widx_in, c->d.widx_out);
+    else CU_OK(cudaMemcpyAsync(d.widx_in + inst0, d.widx_out + inst0, (size_t)n * sizeof(*d.widx_in), cudaMemcpyDeviceToDevice, st.s_out));
     CU_OK(cudaEventRecord(st.ev_aux, st.s_out));                             // ring update done
     CU_OK(cudaStreamWaitEvent(c->stream, st.ev_aux, 0));
     // the last modulator launch is ordered after every other stage launch of this call
     CU_OK(cudaEventRecord(st.ev_done, st.s_pdm));
     CU_OK(cudaStreamWaitEvent(c->stream, st.ev_done, 0));                    // later work on the engine stream sees all outputs
     if (d_status) {
-        K::status<<<(c->d.N + 127) / 128, 128, 0, c->stream>>>(c->d, d_status);
+        K::status<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, inst0, n, d_status);
         CU_OK(cudaGetLastError());
         c->launches++;
     }
     return DSPI_OK;
 }
 
+// Instances [inst0, inst0 + n) of a call: inst0 on a 64-instance boundary, so that the pre and post stages' 16-instance
+// warps and every vector access of the SoA arrays stay aligned.  Checked after the arguments check_packets covers.
 template <class A>
-int process_device(ChainHost<A> *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames, void *d_spdif,
-                   bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
+int check_window(const ChainHost<A> *c, uint32_t inst0, uint32_t n)
+{
+    if (inst0 % 64u) return fail(DSPI_EINVAL, "first instance %u is not a multiple of 64", inst0);
+    return check_range(c, inst0, n);
+}
+
+// the window of a whole-engine call (a NULL handle is refused by the checks that follow)
+template <class A>
+uint32_t all_instances(const ChainHost<A> *c) { return c ? c->desc.n_instances : 0; }
+
+// instances [inst0, inst0 + n), every buffer laid out for the n instances (the whole engine: 0, n_instances)
+template <class A>
+int process_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                   const uint16_t *packet_frames, void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
 {
     int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
     if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
+    if ((rc = check_window(c, inst0, n)) || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     return A::with_stages(c->desc, [&](auto k) {
-        return run_stages<A, decltype(k)>(c, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
+        return run_stages<A, decltype(k)>(c, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
     });
 }
 
 // host memory in and out, staged through the engine's device buffers
 template <class A>
-int process_host(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames, void *spdif_out,
-                 bool subframes, uint32_t *pdm_out, typename A::Status *status)
+int process_host(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                 const uint16_t *packet_frames, void *spdif_out, bool subframes, uint32_t *pdm_out, typename A::Status *status)
 {
     int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
+    if ((rc = check_window(c, inst0, n)) || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    const size_t N = c->desc.n_instances, F = c->sched.frames, pairs = (A::kOuts - 1) / 2;   // the sub output has no S/PDIF pair
+    const size_t N = n, F = c->sched.frames, pairs = (A::kOuts - 1) / 2;   // the sub output has no S/PDIF pair
     const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * pairs * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
     if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
     if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
@@ -789,7 +832,7 @@ int process_host(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t 
     // (an earlier call's bits would be there otherwise: a sub switched off since, or a longer call's [N][F][8] layout)
     if (pdm_out) CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream));
     CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = process_device(c, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
+    rc = process_device(c, inst0, n, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
                         pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
     if (rc) return rc;
     if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
@@ -807,8 +850,9 @@ int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32
     int rc = check_process(c, pcm, bit_depth, n_packets, fpp);
     if (rc) return rc;
     const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
-    return host ? process_host(c, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status)
-                : process_device(c, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status);
+    const uint32_t n = c->desc.n_instances;
+    return host ? process_host(c, 0, n, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status)
+                : process_device(c, 0, n, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status);
 }
 
 // ---- S/PDIF transmitters -----------------------------------------------------------------------------------------------

@@ -10,9 +10,9 @@ namespace dspi {
 // state words (SoA, [9][Np]): err1 err2 x1 x2 y1 y2 err_acc rng fade_in_pos.
 // Modulates frames [f_begin, f_end) of instance `inst`: Q28 samples at subq[f * frame_stride] (the
 // caller offsets `subq` to this instance), 8 words (256 bits, MSB first) per frame to
-// pdm_out[(inst * F + f) * 8 ..].
+// pdm_out[f * 8 ..] (the caller offsets `pdm_out` to this instance's row).
 __device__ __forceinline__ void pdm_modulate_frames(int32_t *__restrict__ pdm, const int32_t *__restrict__ subq, size_t frame_stride, uint32_t Np,
-                                                    uint32_t inst, uint32_t f_begin, uint32_t f_end, uint32_t F, uint32_t *__restrict__ pdm_out)
+                                                    uint32_t inst, uint32_t f_begin, uint32_t f_end, uint32_t *__restrict__ pdm_out)
 {
     int32_t err1 = pdm[0 * Np + inst], err2 = pdm[1 * Np + inst];
     int32_t x1 = pdm[2 * Np + inst], x2 = pdm[3 * Np + inst], y1 = pdm[4 * Np + inst], y2 = pdm[5 * Np + inst];
@@ -67,7 +67,7 @@ __device__ __forceinline__ void pdm_modulate_frames(int32_t *__restrict__ pdm, c
         err1 -= err1 >> 16;                                                  // :396-397
         err2 -= err2 >> 16;
         if (pdm_out) {
-            uint4 *dst = reinterpret_cast<uint4 *>(pdm_out + ((size_t)inst * F + f) * 8);
+            uint4 *dst = reinterpret_cast<uint4 *>(pdm_out + (size_t)f * 8);
             dst[0] = make_uint4(words[0], words[1], words[2], words[3]);
             dst[1] = make_uint4(words[4], words[5], words[6], words[7]);
         }

@@ -98,17 +98,19 @@ __device__ __forceinline__ float gain_computer(float x_db, float threshold, floa
 // pre: PCM unpack + preamp (usb_audio.c:997-1015), loudness TDF2 shelves (:1018-1047) -> master rows
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(64)
-chainq_pre_kernel(ChainQ d, const uint8_t *__restrict__ pcm, uint32_t bit_depth, uint32_t f_begin, uint32_t f_end, uint32_t F)
+chainq_pre_kernel(ChainQ d, uint32_t inst0, uint32_t n, const uint8_t *__restrict__ pcm, uint32_t bit_depth, uint32_t f_begin, uint32_t f_end,
+                  uint32_t F)
 {
-    // warp = 16 instances x {L, R}, lane l = side l >> 4 of instance inst16 + (l & 15): see chain_pre_kernel (chain_f32.cu)
+    // warp = 16 instances x {L, R}, lane l = side l >> 4 of instance inst16 + (l & 15), instances [inst0, inst0 + n):
+    // see chain_pre_kernel (chain_f32.cu)
     __shared__ int32_t tile_s[2][32][kXs];                // per warp: [frame][row = side * 16 + instance]
     __shared__ uint32_t pcm_s[2][2][16][49];              // per warp, double-buffered: 16 instances x 32 frames x <= 6 bytes (rows padded to 49 words)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t inst16 = (blockIdx.x * 2 + warp) * 16;
-    if (inst16 >= d.N_pad) return;
+    const uint32_t local16 = (blockIdx.x * 2 + warp) * 16;
+    if (local16 >= ((n + 31) & ~31u)) return;
     const uint32_t side = lane >> 4, li = lane & 15;
-    const uint32_t inst = inst16 + li;
-    const bool live = inst < d.N;
+    const uint32_t inst16 = inst0 + local16, inst = inst16 + li;
+    const bool live = local16 + li < n;
     const size_t Np = d.N_pad;
     int32_t (*tile)[kXs] = tile_s[warp];
 
@@ -125,13 +127,13 @@ chainq_pre_kernel(ChainQ d, const uint8_t *__restrict__ pcm, uint32_t bit_depth,
     const int32_t preamp = d.preamp[side * Np + inst];
     const uint32_t bpf = bit_depth == 24 ? 6u : 4u;
     const bool words_ok = ((reinterpret_cast<uintptr_t>(pcm) | ((size_t)F * bpf) | ((size_t)f_begin * bpf)) & 3u) == 0;
-    const uint8_t *my_pcm = pcm + (size_t)inst * F * bpf;
-    const uint32_t n_inst = min(16u, d.N > inst16 ? d.N - inst16 : 0u);
+    const uint8_t *my_pcm = pcm + (size_t)(local16 + li) * F * bpf;
+    const uint32_t n_inst = min(16u, n > local16 ? n - local16 : 0u);
     auto fetch = [&](uint32_t f0, int buf) {               // see chain_pre_kernel (chain_f32.cu)
         if (words_ok && f0 < f_end) {
             const uint32_t nwords = (min(32u, f_end - f0) * bpf + 3) / 4;
             for (uint32_t i = 0; i < n_inst; i++) {
-                const uint32_t *src = reinterpret_cast<const uint32_t *>(pcm + ((size_t)(inst16 + i) * F + f0) * bpf);
+                const uint32_t *src = reinterpret_cast<const uint32_t *>(pcm + ((size_t)(local16 + i) * F + f0) * bpf);
                 for (uint32_t w = lane; w < nwords; w += 32) cp_async_4(&pcm_s[warp][buf][i][w], src + w);
             }
         }
@@ -182,6 +184,7 @@ chainq_pre_kernel(ChainQ d, const uint8_t *__restrict__ pcm, uint32_t bit_depth,
         }
         __syncwarp();
     }
+    if (!live) return;
 #pragma unroll
     for (int j = 0; j < 2; j++) {
         d.loud_st[((side * 2 + j) * 2 + 0) * Np + inst] = ls[j][0];
@@ -193,20 +196,21 @@ chainq_pre_kernel(ChainQ d, const uint8_t *__restrict__ pcm, uint32_t bit_depth,
 // post: Q28 leveller (leveller.c:275-389), input peaks, crossfeed (crossfeed.c:161-180), per packet
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
-chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t longest)
+chainq_post_kernel(ChainQ d, uint32_t inst0, uint32_t n, uint32_t p0, uint32_t n_packets, uint32_t longest)
 {
     extern __shared__ int32_t smem_q[];                    // per warp: packet columns [longest][33] + look-ahead reads [longest][33]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t side = lane >> 4;
-    const uint32_t inst16 = (blockIdx.x * (blockDim.x >> 5) + warp) * 16;
-    if (inst16 >= d.N_pad) return;
-    const uint32_t inst = inst16 + (lane & 15);
+    const uint32_t local16 = (blockIdx.x * (blockDim.x >> 5) + warp) * 16;      // instances [inst0, inst0 + n): see chain_pre_kernel
+    if (local16 >= ((n + 31) & ~31u)) return;
+    const uint32_t inst16 = inst0 + local16, inst = inst16 + (lane & 15);
+    const bool live = local16 + (lane & 15) < n;
     const size_t Np = d.N_pad;
     int32_t *xw = smem_q + (size_t)warp * 2 * longest * kXs;
     int32_t *xs = xw + lane;
     int32_t *hs = xw + (size_t)longest * kXs + lane;
 
-    const uint8_t flags = d.flags[inst];
+    const uint8_t flags = live ? d.flags[inst] : 0;       // lanes past the range run with every stage off
     const bool lev_on = flags & F_LEV, xf_on = flags & F_XFEED, lookahead = flags & F_LOOKAHEAD;
     const int32_t xf_a0 = d.xf[0 * Np + inst], xf_b1 = d.xf[1 * Np + inst], xf_ap = d.xf[4 * Np + inst];
     int32_t xf_lp = d.xf[(2 + side) * Np + inst], xf_as = d.xf[(5 + side) * Np + inst];
@@ -343,6 +347,8 @@ chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t longest)
         __syncwarp();
     }
 
+    const uint16_t clip_other = (uint16_t)__shfl_xor_sync(0xffffffffu, (uint32_t)clip, 16);
+    if (!live) return;
     d.xf[(2 + side) * Np + inst] = xf_lp;
     d.xf[(5 + side) * Np + inst] = xf_as;
     d.lev_i[side * Np + inst] = env;
@@ -353,7 +359,6 @@ chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t longest)
         d.lev_idx[inst] = la_idx;
     }
     d.peaks[side * Np + inst] = (uint16_t)(peak_last >> 13);                                              // :1279-1280
-    const uint16_t clip_other = (uint16_t)__shfl_xor_sync(0xffffffffu, (uint32_t)clip, 16);
     if (side == 0 && (clip | clip_other)) atomicOr(reinterpret_cast<unsigned int *>(d.clip + (inst & ~1u)), (unsigned int)(clip | clip_other) << (16 * (inst & 1)));
 }
 
@@ -361,15 +366,15 @@ chainq_post_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t longest)
 // matrix mix in Q15 (usb_audio.c:1076-1100): lane = frame
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-chainq_mix_kernel(ChainQ d, uint32_t f_begin, uint32_t f_end)
+chainq_mix_kernel(ChainQ d, uint32_t inst0, uint32_t n, uint32_t f_begin, uint32_t f_end)
 {
     const int lane = threadIdx.x & 31;
     constexpr int kB = 4;
     const uint32_t n_tiles = (f_end - f_begin + 32 * kB - 1) / (32 * kB);
-    const uint64_t units = (uint64_t)d.N * n_tiles;
+    const uint64_t units = (uint64_t)n * n_tiles;
     const size_t Np = d.N_pad;
     for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
-        const uint32_t inst = (uint32_t)(u / n_tiles), tile = (uint32_t)(u % n_tiles);
+        const uint32_t inst = inst0 + (uint32_t)(u / n_tiles), tile = (uint32_t)(u % n_tiles);
         const uint32_t fbase = f_begin + tile * 32 * kB + lane;
         int32_t l[kB], r[kB];
 #pragma unroll
@@ -402,11 +407,11 @@ chainq_mix_kernel(ChainQ d, uint32_t f_begin, uint32_t f_end)
 // ---------------------------------------------------------------------------------------------
 // update_preset_mute_envelope() (usb_audio.c:466-498) for every packet of the call, one instance per thread, then the Q15
 // volume chain of :976-980: pmg = (int32)(g * 32768 + 0.5) clamped, vmm[p] = mul_q15(mul_q15(vol_base, pmg), master_q15)
-__global__ void chainq_env_kernel(ChainQ d, uint32_t n_packets)
+__global__ void chainq_env_kernel(ChainQ d, uint32_t inst0, uint32_t n, uint32_t n_packets)
 {
-    const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, inst = inst0 + i;
     const size_t Np = d.N_pad;
-    if (inst >= d.N || !d.env[4 * Np + inst]) return;
+    if (i >= n || !d.env[4 * Np + inst]) return;
     uint32_t loading = d.env[0 * Np + inst], counter = d.env[1 * Np + inst];
     float g = __uint_as_float(d.env[2 * Np + inst]);
     const uint32_t fs = d.env[3 * Np + inst];
@@ -582,18 +587,18 @@ __device__ __forceinline__ int32_t outq_sample(const OutCfgQ &c, uint32_t T, uin
 
 __device__ __forceinline__ int32_t clip_s24(int32_t w) { return w > 0x7FFFFF ? 0x7FFFFF : (w < -0x800000 ? -0x800000 : w); }   // config.h:547-551
 
-// SUBFRAMES = false: spdif_out is [N][2][F][2] int32 words; true: [N][2][F] uint4 subframe pairs at each instance's
-// block position and channel status (as chain_f32.cu)
+// Instances [inst0, inst0 + n), the caller's rows counted from inst0.  SUBFRAMES = false: spdif_out is [n][2][F][2] int32
+// words; true: [n][2][F] uint4 subframe pairs at each instance's block position and channel status (as chain_f32.cu)
 template <bool SUBFRAMES>
 __global__ void __launch_bounds__(256)
-chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out, SpdifTx tx)
+chainq_outpost_kernel(ChainQ d, uint32_t inst0, uint32_t n, uint32_t p0, uint32_t n_packets, uint32_t F, int32_t *__restrict__ spdif_out, SpdifTx tx)
 {
     const int lane = threadIdx.x & 31;
-    const uint64_t units = (uint64_t)d.N * n_packets;
+    const uint64_t units = (uint64_t)n * n_packets;
     const size_t Np = d.N_pad;
     constexpr int kPairs = (kOuts - 1) / 2;
     for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
-        const uint32_t inst = (uint32_t)(u / n_packets), p = p0 + (uint32_t)(u % n_packets);
+        const uint32_t local = (uint32_t)(u / n_packets), inst = inst0 + local, p = p0 + (uint32_t)(u % n_packets);
         const uint32_t f0 = d.off[p], count = d.off[p + 1] - f0;
         const bool last = p == p0 + n_packets - 1;
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
@@ -629,9 +634,9 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int
                         if (!ca.pair_off) { w.x = clip_s24((xa[j] + 32) >> 6); w.y = clip_s24((xb[j] + 32) >> 6); }   // :1254-1255
                         if (SUBFRAMES) {                                      // 16 bytes per lane: 512 contiguous bytes per warp store
                             const uint32_t pos = (bp + T) % 192u;
-                            reinterpret_cast<uint4 *>(spdif_out)[((size_t)inst * kPairs + k) * F + T] = encode_frame(w, spdif_pre_left(pos), spdif_cs_bit(pos, cs40));
+                            reinterpret_cast<uint4 *>(spdif_out)[((size_t)local * kPairs + k) * F + T] = encode_frame(w, spdif_pre_left(pos), spdif_cs_bit(pos, cs40));
                         } else {
-                            *reinterpret_cast<int2 *>(spdif_out + (((size_t)inst * kPairs + k) * F + T) * 2) = w;
+                            *reinterpret_cast<int2 *>(spdif_out + (((size_t)local * kPairs + k) * F + T) * 2) = w;
                         }
                     }
                 }
@@ -655,13 +660,13 @@ chainq_outpost_kernel(ChainQ d, uint32_t p0, uint32_t n_packets, uint32_t F, int
 }
 
 __global__ void __launch_bounds__(256)
-chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t n_packets, uint32_t *__restrict__ spdif_bp)
+chainq_ring_kernel(ChainQ d, uint32_t inst0, uint32_t n, uint32_t F, uint32_t n_packets, uint32_t *__restrict__ spdif_bp)
 {
     const int lane = threadIdx.x & 31;
-    const uint64_t units = (uint64_t)d.N * kOuts;
+    const uint64_t units = (uint64_t)n * kOuts;
     const size_t Np = d.N_pad;
     for (uint64_t u = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); u < units; u += (uint64_t)gridDim.x * (blockDim.x >> 5)) {
-        const uint32_t inst = (uint32_t)(u / kOuts), o = (uint32_t)(u % kOuts);
+        const uint32_t inst = inst0 + (uint32_t)(u / kOuts), o = (uint32_t)(u % kOuts);
         const bool any_delay = d.flags[inst] & F_ANY_DELAY;
         const uint32_t widx0 = d.widx_in[inst];
         const OutCfgQ c = outq_cfg(d, o, inst, any_delay);
@@ -678,12 +683,12 @@ chainq_ring_kernel(ChainQ d, uint32_t F, uint32_t n_packets, uint32_t *__restric
 }
 
 __global__ void __launch_bounds__(128)
-chainq_pdm_kernel(ChainQ d, uint32_t f_begin, uint32_t f_end, uint32_t F, uint32_t *__restrict__ pdm_out)
+chainq_pdm_kernel(ChainQ d, uint32_t inst0, uint32_t n, uint32_t f_begin, uint32_t f_end, uint32_t F, uint32_t *__restrict__ pdm_out)
 {
-    const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
-    if (inst >= d.N) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, inst = inst0 + i;
+    if (i >= n) return;
     if (!(d.flags[inst] & F_SUB_ON)) return;                                                              // usb_audio.c:1261
-    pdm_modulate_frames(d.pdm, d.subq + (size_t)inst * d.ldF, 1, d.N_pad, inst, f_begin, f_end, F, pdm_out);
+    pdm_modulate_frames(d.pdm, d.subq + (size_t)inst * d.ldF, 1, d.N_pad, inst, f_begin, f_end, pdm_out ? pdm_out + (size_t)i * F * 8 : nullptr);
 }
 
 // filters[][] of n instances (instance-major AoS, 32-byte records) <-> the mirrors of the two EQ engines
@@ -699,16 +704,16 @@ __global__ void chainq_scatter_kernel(const dspi_biquad_q28 *__restrict__ aos, u
     else *chain_q = *eng_q;
 }
 
-__global__ void chainq_status_kernel(ChainQ d, dspi_status_q28 *__restrict__ out)
+__global__ void chainq_status_kernel(ChainQ d, uint32_t inst0, uint32_t n, dspi_status_q28 *__restrict__ out)
 {
-    const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
-    if (inst >= d.N) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, inst = inst0 + i;
+    if (i >= n) return;
     dspi_status_q28 s;
     for (int r = 0; r < kRoles; r++) s.peaks[r] = d.peaks[r * d.N_pad + inst];
     s.cpu0_load = 0;
     s.cpu1_load = 0;
     s.clip_flags = d.clip[inst];
-    out[inst] = s;
+    out[i] = s;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -965,25 +970,49 @@ int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth
 int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                        int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
 {
-    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
+    return dspi::process_device(c, 0, dspi::all_instances(c), d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
 }
 
 int dspi_chainq_process_packets_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                      int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
 {
-    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
+    return dspi::process_host(c, 0, dspi::all_instances(c), pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
 }
 
 int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                          dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
 {
-    return dspi::process_device(c, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
+    return dspi::process_device(c, 0, dspi::all_instances(c), d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
 }
 
 int dspi_chainq_process_subframes_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                        dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status_q28 *status)
 {
-    return dspi::process_host(c, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
+    return dspi::process_host(c, 0, dspi::all_instances(c), pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
+}
+
+int dspi_chainq_process_packets_range_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                    const uint16_t *packet_frames, int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
+{
+    return dspi::process_device(c, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
+}
+
+int dspi_chainq_process_packets_range_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                                  const uint16_t *packet_frames, int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
+{
+    return dspi::process_host(c, inst0, n, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
+}
+
+int dspi_chainq_process_subframes_range_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                      const uint16_t *packet_frames, dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
+{
+    return dspi::process_device(c, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
+}
+
+int dspi_chainq_process_subframes_range_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                                    const uint16_t *packet_frames, dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status_q28 *status)
+{
+    return dspi::process_host(c, inst0, n, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
 }
 
 int dspi_chainq_set_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx) { return dspi::set_spdif_tx(c, inst0, n, tx); }

@@ -442,9 +442,10 @@ static int refresh_kernel_choice(dspi_eq *e)
     return DSPI_OK;
 }
 
-// launch over groups [g0, g0 + ng) of the engine on `stream`; d_samples points at the first row of
-// group g0 and holds `n_rows` valid rows
-static int launch_eq(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, uint32_t g0, uint32_t ng, uint32_t n_rows, cudaStream_t stream)
+// launch over groups [g0, g0 + ng) of the engine on `stream`; d_samples points at row row_lo of group g0 (the first row
+// of the launch) and holds `n_rows` valid rows
+static int launch_eq(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, uint32_t g0, uint32_t ng, uint32_t n_rows, cudaStream_t stream,
+                     uint32_t row_lo = 0)
 {
     dspi::EqLaunch a;
     memset(&a, 0, sizeof(a));
@@ -468,6 +469,7 @@ static int launch_eq(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, uint3
     a.sched = e->d_sched;
     a.n_sms = e->n_sms;
     a.n_rows = n_rows;
+    a.row_lo = row_lo;
     a.T = T;
     a.n_bands = e->desc.n_bands;
     a.use_tma = tma_ok ? 1u : 0u;
@@ -632,13 +634,15 @@ int eq_process_on(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, cudaStre
 }
 
 // channels [ch0, ch0 + n) on a stream of the caller's choosing (launches over disjoint channel ranges may run concurrently:
-// they touch disjoint parts of the coefficient / state store)
+// they touch disjoint parts of the coefficient / state store).  ch0 is a multiple of 32; in the 64-row geometry the range
+// may begin half-way into a group, whose other rows K1 then leaves alone.
 int eq_process_range_on(dspi_eq *e, void *d_rows, uint32_t T, uint32_t ld, uint32_t ch0, uint32_t n, cudaStream_t s)
 {
     if (T == 0 || n == 0) return DSPI_OK;
-    if (ch0 % range_unit(e)) return fail(DSPI_EINVAL, "first channel %u is not a multiple of %u", ch0, range_unit(e));
+    if (ch0 % 32u) return fail(DSPI_EINVAL, "first channel %u is not a multiple of 32", ch0);
     CU_OK(cudaSetDevice(e->desc.device));
-    return launch_eq(e, d_rows, T, ld, ch0 / e->rows, (n + e->rows - 1) / e->rows, n, s);
+    const uint32_t row_lo = ch0 % e->rows;
+    return launch_eq(e, d_rows, T, ld, ch0 / e->rows, (row_lo + n + e->rows - 1) / e->rows, n, s, row_lo);
 }
 
 }  // namespace dspi

@@ -310,12 +310,11 @@ struct EqBank {
         all_tdf2 = __all_sync(0xffffffffu, mine);
     }
 
-    // `halves`: how many of this lane's CPL channels belong to the launch (0..CPL; channel lane + 32 h
-    // for h < halves).  The others are rows past the end of a range call, i.e. channels outside it:
-    // their state words are left as they are.
-    __device__ __forceinline__ void store(V *base, int halves, bool shared_state = false) const
+    // This lane's channels lane + 32 h with h in [h_lo, h_hi) belong to the launch.  The others are rows outside a range
+    // call (past its end, or below its start in a group it shares with another range): their state words are left as they are.
+    __device__ __forceinline__ void store(V *base, int h_lo, int h_hi, bool shared_state = false) const
     {
-        if (halves >= CPL) {
+        if (h_lo == 0 && h_hi >= CPL) {
 #pragma unroll
             for (int b = 0; b < NB; b++) {
                 if (shared_state) {
@@ -327,17 +326,19 @@ struct EqBank {
                 }
             }
         } else if constexpr (CPL == 2) {
-            if (halves == 1) {                                  // channel lane only: the low float of each pair
+#pragma unroll
+            for (int h = 0; h < 2; h++) {                       // one float of each pair: channel lane (h = 0) or lane + 32
+                if (h < h_lo || h >= h_hi) continue;
 #pragma unroll
                 for (int b = 0; b < NB; b++) {
-                    float *s0 = reinterpret_cast<float *>(base + (b * 8 + 6) * 32);
-                    float *s1 = reinterpret_cast<float *>(base + (b * 8 + 7) * 32);
+                    float *s0 = reinterpret_cast<float *>(base + (b * 8 + 6) * 32) + h;
+                    float *s1 = reinterpret_cast<float *>(base + (b * 8 + 7) * 32) + h;
                     if (shared_state) {
-                        st_cg(s0, Lanes<V>::get(st[b][0], 0));
-                        st_cg(s1, Lanes<V>::get(st[b][1], 0));
+                        st_cg(s0, Lanes<V>::get(st[b][0], h));
+                        st_cg(s1, Lanes<V>::get(st[b][1], h));
                     } else {
-                        *s0 = Lanes<V>::get(st[b][0], 0);
-                        *s1 = Lanes<V>::get(st[b][1], 0);
+                        *s0 = Lanes<V>::get(st[b][0], h);
+                        *s1 = Lanes<V>::get(st[b][1], h);
                     }
                 }
             }

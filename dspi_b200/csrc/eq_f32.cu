@@ -36,10 +36,10 @@ using k1::kWarps;
 template <typename V, bool FUSED, int NB, bool DYN>
 __global__ void __launch_bounds__(kWarps * 32, 1)
 eq_f32_kernel(const __grid_constant__ CUtensorMap tmap, float *__restrict__ samples, uint32_t ld, V *__restrict__ coef,
-              const uint64_t *__restrict__ modes, uint32_t n_groups, uint32_t n_rows, uint32_t T, uint32_t nb_active, uint32_t use_tma, uint32_t dbg,
-              unsigned long long nz_bits, uint32_t slice_tiles, uint32_t *__restrict__ sched)
+              const uint64_t *__restrict__ modes, uint32_t n_groups, uint32_t n_rows, uint32_t row_lo, uint32_t T, uint32_t nb_active, uint32_t use_tma,
+              uint32_t dbg, unsigned long long nz_bits, uint32_t slice_tiles, uint32_t *__restrict__ sched)
 {
-    k1::eq_f32_body<V, FUSED, NB, DYN, k1::NoSig>(tmap, samples, ld, coef, modes, n_groups, n_rows, T, nb_active, use_tma, dbg, nz_bits, slice_tiles, sched);
+    k1::eq_f32_body<V, FUSED, NB, DYN, k1::NoSig>(tmap, samples, ld, coef, modes, n_groups, n_rows, row_lo, T, nb_active, use_tma, dbg, nz_bits, slice_tiles, sched);
 }
 
 template <typename V, bool FUSED, int NB>
@@ -73,10 +73,10 @@ cudaError_t launch_one(const EqLaunch &a, cudaStream_t stream)
         if (e != cudaSuccess) return e;
     }
     if (sched)
-        kern_dyn<<<grid, kWarps * 32, smem, stream>>>(a.tmap, (float *)a.samples, a.ld, (V *)a.coef, a.modes, n_groups, a.n_rows, a.T, a.n_bands, a.use_tma,
+        kern_dyn<<<grid, kWarps * 32, smem, stream>>>(a.tmap, (float *)a.samples, a.ld, (V *)a.coef, a.modes, n_groups, a.n_rows, a.row_lo, a.T, a.n_bands, a.use_tma,
                                                       a.dbg, 0x8000000080000000ull, slice_tiles, sched);
     else
-        kern<<<grid, kWarps * 32, smem, stream>>>(a.tmap, (float *)a.samples, a.ld, (V *)a.coef, a.modes, n_groups, a.n_rows, a.T, a.n_bands, a.use_tma,
+        kern<<<grid, kWarps * 32, smem, stream>>>(a.tmap, (float *)a.samples, a.ld, (V *)a.coef, a.modes, n_groups, a.n_rows, a.row_lo, a.T, a.n_bands, a.use_tma,
                                                   a.dbg, 0x8000000080000000ull, 0u, nullptr);
     return cudaGetLastError();
 }

@@ -16,9 +16,9 @@ typedef float JitV;
 
 extern "C" __global__ void __launch_bounds__(dspi::k1::kWarps * 32, 1)
 eq_f32_jit(const __grid_constant__ CUtensorMap tmap, float *__restrict__ samples, uint32_t ld, JitV *__restrict__ coef,
-           const uint64_t *__restrict__ modes, uint32_t n_groups, uint32_t n_rows, uint32_t T, uint32_t nb_active, uint32_t use_tma, uint32_t dbg,
+           const uint64_t *__restrict__ modes, uint32_t n_groups, uint32_t n_rows, uint32_t row_lo, uint32_t T, uint32_t nb_active, uint32_t use_tma, uint32_t dbg,
            unsigned long long nz_bits, uint32_t slice_tiles, uint32_t *__restrict__ sched)
 {
     dspi::k1::eq_f32_body<JitV, (DSPI_JIT_FUSED) != 0, DSPI_JIT_NB, false, dspi::k1::SigWord<(DSPI_JIT_SIG)>>(
-        tmap, samples, ld, coef, modes, n_groups, n_rows, T, nb_active, use_tma, dbg, nz_bits, slice_tiles, sched);
+        tmap, samples, ld, coef, modes, n_groups, n_rows, row_lo, T, nb_active, use_tma, dbg, nz_bits, slice_tiles, sched);
 }

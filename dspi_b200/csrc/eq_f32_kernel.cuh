@@ -34,7 +34,7 @@ template <unsigned long long W> struct SigWord { static constexpr bool enabled =
 
 template <typename V, bool FUSED, int NB, bool DYN, typename SIG>
 __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__restrict__ samples, uint32_t ld, V *__restrict__ coef,
-              const uint64_t *__restrict__ modes, uint32_t n_groups, uint32_t n_rows, uint32_t T, uint32_t nb_active, uint32_t use_tma, uint32_t dbg, unsigned long long nz_bits, uint32_t slice_tiles, uint32_t *__restrict__ sched)
+              const uint64_t *__restrict__ modes, uint32_t n_groups, uint32_t n_rows, uint32_t row_lo, uint32_t T, uint32_t nb_active, uint32_t use_tma, uint32_t dbg, unsigned long long nz_bits, uint32_t slice_tiles, uint32_t *__restrict__ sched)
 {
     constexpr int CPL = Lanes<V>::CPL;
     constexpr int kRows = 32 * CPL;
@@ -98,7 +98,13 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
             tile_begin = 0;
             tile_end = ntiles;
         }
-        const int c0 = g * kRows;                               // first channel (row) of this group
+        // first channel (row) of this group, counted from `samples`: group 0 starts row_lo rows before it (a range that
+        // begins half-way into a 64-row group).  Rows from n_rows on belong to other launches: TMA clips them (zero-filled
+        // loads, dropped stores).  A group that starts below row 0 takes the plain path, which skips the rows outside the
+        // launch both ways, so that a TMA box never starts at a negative row.  No state is stored for rows outside.
+        const int c0 = (int)(g * kRows) - (int)row_lo;
+        const bool tma = use_tma && c0 >= 0;
+        const uint32_t tcount0 = tcount;
 
         // boxes of a tile that start inside the row (a box wholly past T is neither loaded nor stored)
         auto n_boxes = [&](uint32_t tile) { return kHalves == 1 || tile * kTileT + 32 < T ? kHalves : 1; };
@@ -111,7 +117,7 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
         };
         if (use_tma && mem_on && lane == 0) {
             if constexpr (DYN) tma_store_wait_read<0>();        // ring buffers of the previous item are drained
-            for (uint32_t j = 0; j + 1 < kStages && tile_begin + j < tile_end; j++) issue_load(tile_begin + j, tcount + j);
+            for (uint32_t j = 0; tma && j + 1 < kStages && tile_begin + j < tile_end; j++) issue_load(tile_begin + j, tcount + j);
         }
 
         // ---- coefficients, state and topology of every band -> registers ----------------------
@@ -132,11 +138,11 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
         for (uint32_t tile = tile_begin; tile < tile_end; tile++, tcount++) {
             const uint32_t s = tcount % kStages;
             uint8_t *buf = my_smem + s * kStageBytes;
-            if (use_tma) {
+            if (tma) {
                 if (mem_on) mbar_wait(&full[s], (tcount / kStages) & 1);
             } else {                                                // plain-load fallback (odd strides / unaligned bases)
                 for (int r = 0; r < kRows; r++) {
-                    const uint32_t ch = c0 + r;
+                    const uint32_t ch = c0 + r;                 // rows below the launch wrap past n_rows
                     for (int h = 0; h < kHalves; h++) {
                         const uint32_t t = tile * kTileT + h * 32 + lane;
                         float v = 0.0f;
@@ -224,7 +230,7 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
                             make_float4(back[h][4 * k], back[h][4 * k + 1], back[h][4 * k + 2], back[h][4 * k + 3]);
             }
 
-            if (use_tma) {
+            if (tma) {
                 fence_proxy_async_smem();                           // my smem writes -> async proxy
                 __syncwarp();
                 if (lane == 0 && mem_on) {
@@ -252,10 +258,14 @@ __device__ __forceinline__ void eq_f32_body(const CUtensorMap &tmap, float *__re
         }
 
 
-        int halves = 0;                                         // rows >= n_rows are channels outside a range call
+        if (!tma) tcount = tcount0;                             // the TMA ring's stage / parity sequence only counts TMA tiles
+        int h_lo = 0, h_hi = 0;                                 // this lane's channels lane + 32 h, h in [h_lo, h_hi), are in the launch
 #pragma unroll
-        for (int h = 0; h < CPL; h++) halves += (uint32_t)(c0 + 32 * h + lane) < n_rows ? 1 : 0;
-        bank.store(my_coef, halves, DYN);                       // filter state back to the coefficient store
+        for (int h = 0; h < CPL; h++) {
+            if (c0 + 32 * h + lane < 0) h_lo = h + 1;
+            if ((uint32_t)(c0 + 32 * h + lane) < n_rows) h_hi = h + 1;
+        }
+        bank.store(my_coef, h_lo, h_hi, DYN);                   // filter state back to the coefficient store
         if constexpr (!DYN) break;
         __threadfence();                                        // state visible before the slice counter moves
         __syncwarp();

@@ -18,6 +18,7 @@ struct EqLaunch {
     const uint64_t *modes; // f32 only
     uint32_t n_groups;     // groups of (32 * channels-per-lane) channels
     uint32_t n_rows;       // valid channel rows in `samples`
+    uint32_t row_lo;       // rows of the first group that lie before `samples` (K1 range launches half-way into a 64-row group; else 0)
     uint32_t T;
     uint32_t n_bands;
     uint32_t use_tma;

@@ -423,6 +423,28 @@ int dspi_chain_process_packets_host  (dspi_chain *c, const void *pcm, uint32_t b
                                       int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status);
 int dspi_chain_process_packets_device(dspi_chain *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                       int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status *d_status);
+/* dspi_chain_process_packets_* over the instances [inst0, inst0 + n) only, with this call's own packet_frames: a host packs
+ * its connected devices (or each group of devices on one clock) into contiguous ranges with the instance image calls and
+ * serves each range as its packets arrive, so idle slots cost nothing and a 44.1 kHz group, a 48 kHz group and a
+ * feedback-paced group share one engine.  The schedule stays one per call (see above).
+ *   Layout: every buffer is laid out for n instances - pcm [n][F * bytes per frame], spdif_out [n][4][F][2], pdm_out
+ *   [n][F][8], status [n] - and row i belongs to instance inst0 + i.  F = sum of packet_frames <= max_frames.  PDM rows as
+ *   for the whole engine: _host zeroes the rows of instances whose sub is off, _device leaves them as they were.
+ *   Inside the range everything happens as in a whole-engine call: filter, loudness, crossfeed and leveller state, the
+ *   look-ahead and delay rings and their write index, modulator state, meters, the preset-mute envelope step per packet,
+ *   the S/PDIF block position advancing by F.
+ *   Outside the range nothing changes: state, envelope, transmitter, meters, and the EQ coefficients and state of
+ *   instances that share a K1 / K2 channel group with the range.  A later call on them gives the bytes it would have given
+ *   without this call.
+ *   Rules: inst0 is a multiple of 64 (DSPI_EINVAL otherwise); n is any count and n == 0 does nothing; a range past the end
+ *   of the engine (also one whose end wraps in 32 bits) is DSPI_ERANGE; the table, bit depth and NULL checks are those of
+ *   dspi_chain_process_packets_*.  Nothing is written on any error.
+ *   The _device form is asynchronous on the engine stream and never waits for the device; consecutive calls on one engine
+ *   run in issue order.  The whole-engine calls are this call with inst0 = 0, n = n_instances. */
+int dspi_chain_process_packets_range_host  (dspi_chain *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                                            const uint16_t *packet_frames, int32_t *spdif_out, uint32_t *pdm_out, dspi_status *status);
+int dspi_chain_process_packets_range_device(dspi_chain *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                            const uint16_t *packet_frames, int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status *d_status);
 int dspi_chain_sync(dspi_chain *c);
 void *dspi_chain_stream(dspi_chain *c);
 uint64_t dspi_chain_launch_count(dspi_chain *c);
@@ -504,6 +526,11 @@ int dspi_chainq_process_packets_host  (dspi_chainq *c, const void *pcm, uint32_t
                                        int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status);
 int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                        int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
+/* instances [inst0, inst0 + n) only, as dspi_chain_process_packets_range_*; spdif_out [n][2][F][2] */
+int dspi_chainq_process_packets_range_host  (dspi_chainq *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                                             const uint16_t *packet_frames, int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status);
+int dspi_chainq_process_packets_range_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                             const uint16_t *packet_frames, int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
 int dspi_chainq_sync(dspi_chainq *c);
 void *dspi_chainq_stream(dspi_chainq *c);
 uint64_t dspi_chainq_launch_count(dspi_chainq *c);
@@ -771,6 +798,16 @@ int dspi_chainq_process_subframes_host  (dspi_chainq *c, const void *pcm,   uint
                                          dspi_spdif_subframe *subframes,   uint32_t *pdm_out,   dspi_status_q28 *status);
 int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
                                          dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
+/* instances [inst0, inst0 + n) only, as dspi_chain(q)_process_packets_range_*: subframes [n][4 (Q28: 2)][F][2], row i for
+ * instance inst0 + i; each instance encoded at its own block position and channel status; d_subframes 16-byte aligned */
+int dspi_chain_process_subframes_range_host   (dspi_chain *c,  uint32_t inst0, uint32_t n, const void *pcm,   uint32_t bit_depth, uint32_t n_packets,
+                                               const uint16_t *packet_frames, dspi_spdif_subframe *subframes,   uint32_t *pdm_out,   dspi_status *status);
+int dspi_chain_process_subframes_range_device (dspi_chain *c,  uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                               const uint16_t *packet_frames, dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status *d_status);
+int dspi_chainq_process_subframes_range_host  (dspi_chainq *c, uint32_t inst0, uint32_t n, const void *pcm,   uint32_t bit_depth, uint32_t n_packets,
+                                               const uint16_t *packet_frames, dspi_spdif_subframe *subframes,   uint32_t *pdm_out,   dspi_status_q28 *status);
+int dspi_chainq_process_subframes_range_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                                               const uint16_t *packet_frames, dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
 
 /* ---- frequency response of EQ channels and chain instances ------------------------------------ */
 /* The complex transfer function H(e^{j omega}) of the linear, time-invariant part of the path the NEXT process call applies,
