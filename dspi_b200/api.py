@@ -47,6 +47,7 @@ SYMBOLS = [
     "dspi_chainq_response_host", "dspi_chainq_response_device",
     "dspi_chain_apply_bulk_device", "dspi_chainq_apply_bulk_device",
     "dspi_chain_collect_bulk_device", "dspi_chainq_collect_bulk_device",
+    "dspi_chain_set_rate_device", "dspi_chainq_set_rate_device",
     "dspi_chain_apply_preset_device", "dspi_chainq_apply_preset_device",
     "dspi_chain_collect_preset_device", "dspi_chainq_collect_preset_device",
     "dspi_chain_instance_image_size", "dspi_chain_export_instances", "dspi_chain_import_instances", "dspi_chain_reset_instances",
@@ -147,6 +148,7 @@ def lib():
             getattr(h, pre + "_sm_partition").argtypes = [vp, vp, vp]
             getattr(h, pre + "_apply_bulk_device").argtypes = [vp, u32, u32, vp, vp, C.c_int, C.c_float, vp]
             getattr(h, pre + "_collect_bulk_device").argtypes = [vp, u32, u32, vp, vp, vp]
+            getattr(h, pre + "_set_rate_device").argtypes = [vp, u32, u32, vp, vp]
             getattr(h, pre + "_apply_preset_device").argtypes = [vp, u32, u32, vp, C.c_size_t, vp, vp, C.c_float, vp]
             getattr(h, pre + "_collect_preset_device").argtypes = [vp, u32, u32, vp, vp, C.c_size_t, vp]
             getattr(h, pre + "_process_packets_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
@@ -610,6 +612,16 @@ class _ChainEngine:
         _check(self._fn("apply_bulk_device")(self._h, int(inst0), int(w.shape[0]), w.ctypes.data_as(C.c_void_p),
                                              hv.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
                                              res.ctypes.data_as(C.c_void_p)))
+        return res
+
+    def set_rate_device(self, rates, inst0=0):
+        """The USB host switched instances [inst0, inst0+n) to ``rates`` (float [n], one rate per instance, or a scalar for
+        one instance): every rate-dependent record re-derived on the GPU from each instance's configuration record, as
+        ``perform_rate_change`` does.  Returns int32 [n] of ``layouts.BULK_*`` marks; only ``BULK_CURRENT`` instances switched,
+        the others are left exactly as they were."""
+        r = np.ascontiguousarray(np.asarray(rates, np.float32).reshape(-1))
+        res = np.zeros(r.size, np.int32)
+        _check(self._fn("set_rate_device")(self._h, int(inst0), int(r.size), r.ctypes.data_as(C.c_void_p), res.ctypes.data_as(C.c_void_p)))
         return res
 
     def collect_bulk_device(self, inst0=0, n=None):

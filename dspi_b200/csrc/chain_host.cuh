@@ -548,6 +548,19 @@ int apply_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_wi
 }
 
 template <class A>
+int set_rate_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results)
+{
+    if (!c || !sample_rates) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);                     // before the rates are read: n counts them
+    if (rc) return rc;
+    for (uint32_t i = 0; i < n; i++)
+        if (!(sample_rates[i] > 0.0f) || sample_rates[i] > 3.4e38f) return fail(DSPI_EINVAL, "sample_rates[%u] must be positive and finite", i);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return bulk::set_rate<typename A::Stores>(c, c->bulk, inst0, n, sample_rates, results);
+}
+
+template <class A>
 int collect_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
 {
     if (!c || !packets) return fail(DSPI_EINVAL, "null argument");

@@ -930,6 +930,11 @@ int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, co
     return dspi::apply_bulk_device(c, inst0, n, packets, host, exact_db, sample_rate, results);
 }
 
+int dspi_chainq_set_rate_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results)
+{
+    return dspi::set_rate_device(c, inst0, n, sample_rates, results);
+}
+
 int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
 {
     return dspi::collect_bulk_device(c, inst0, n, packets, host, results);

@@ -93,6 +93,7 @@ coeff_f32_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_f32 *__restric
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n * kMaxBands || (rr.reject && rr.reject[i / kMaxBands])) return;
+    if (rr.fs) fs = rr.fs[i / kMaxBands];
     recipes += (size_t)blockIdx.y * n * kMaxBands;
     aos += ((size_t)ch0 + (size_t)blockIdx.y * rr.stride) * kMaxBands;
     dspi_eq_param p = recipes[i];
@@ -167,6 +168,7 @@ coeff_q28_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_q28 *__restric
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n * kMaxBands || (rr.reject && rr.reject[i / kMaxBands])) return;
+    if (rr.fs) fs = rr.fs[i / kMaxBands];
     recipes += (size_t)blockIdx.y * n * kMaxBands;
     aos += ((size_t)ch0 + (size_t)blockIdx.y * rr.stride) * kMaxBands;
     dspi_eq_param p = recipes[i];

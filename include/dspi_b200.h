@@ -674,6 +674,35 @@ int dspi_chain_collect_bulk_device (dspi_chain *c,  uint32_t inst0, uint32_t n, 
 int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host,
                                     int32_t *results);
 
+/* perform_rate_change() (main.c:132-171) for instances [inst0, inst0+n) ON THE GPU, from each instance's configuration
+ * record: the USB host switched those devices to new sample rates.  sample_rates[n] (host memory) gives each instance its
+ * own rate fs_i; results[n] (host memory, may be NULL) gets each instance's DSPI_BULK_* mark.
+ *   - Only DSPI_BULK_CURRENT instances switch.  A DSPI_BULK_STALE or DSPI_BULK_UNSET instance is left exactly as it was:
+ *     its derived records came from _set_params / _upload_biquads, which the record cannot reproduce.  The call still
+ *     returns DSPI_OK.
+ *   - A switched instance gets, at fs_i: dsp_recalculate_all_filters(fs_i) over all 11 (Q28: 7) x 12 bands from the
+ *     record's recipes, the clamps written back into the record (dsp_pipeline.c:78-81: a band a 44.1 kHz switch clamped to
+ *     19845 Hz stays there after a switch back to 96 kHz), filter state kept unless a band's topology flips (SVF below
+ *     fs / 7.5, TDF2 above); dsp_update_delay_samples(fs_i) from the record's output delays in ms (the sub's
+ *     SUB_ALIGN_SAMPLES term, the clamp to [0, MAX], dly == MAX still aliasing to no delay) and the any_delay bit of its
+ *     flag word recomputed, delay-line contents and write index kept; crossfeed_compute_coefficients(cfg, fs_i) with the
+ *     crossfeed filter state cleared; leveller_compute_coefficients(cfg, fs_i) with leveller state kept; the loudness row
+ *     loudness_recompute_table(ref_spl, intensity, fs_i) selects for the record's host volume, shelf state kept.
+ *   - Left alone: every gain (preamp, matrix crosspoints, output gains, master volume, vol_mul), the flags and skip rows
+ *     that do not depend on the rate, modulator state, meters, the preset-mute envelope, the S/PDIF transmitter (block
+ *     position and channel status), the mark and the host record.  Of the record only the eq section changes: the
+ *     recipes, clamped at fs_i.
+ *   - The rest of a rate change is the caller's, through the calls that do it: channel-status byte 3 (the rate code) with
+ *     _set_spdif_tx, a fade with _set_preset_mute, a pipeline reset with _reset_instances.  Whether perform_rate_change()
+ *     does any of these was not checked against main.c; this call does none of them.
+ * Arithmetic and libm policy as dspi_eq_set_params_device / _set_dynamics_device: coefficients are the oracle's policy
+ * coefficients bit for bit.  Ordered behind everything issued earlier on the engine stream, asynchronous process calls
+ * included; returns when the engine is reconfigured.  DSPI_EINVAL for a NULL engine or sample_rates, or any rate that is
+ * not positive and finite (every rate is checked before the first write); DSPI_ERANGE for a range past the end of the
+ * engine (also one whose end wraps in 32 bits); nothing is written then.  n == 0 does nothing. */
+int dspi_chain_set_rate_device (dspi_chain *c,  uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results);
+int dspi_chainq_set_rate_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results);
+
 /* ---- preset slot images (SURVEY.md 8 f-4): PresetSlot v12, flash_storage.c:139-189 ------------ */
 /* One flash sector per slot: 12-byte header (magic "DSP3", data version, slot index, CRC-32 of everything
  * after the header) + the packed DSP state.  Device preset dumps load directly into a dspi_bulk_state and
