@@ -52,6 +52,7 @@ SYMBOLS = [
     "dspi_chain_collect_preset_device", "dspi_chainq_collect_preset_device",
     "dspi_chain_instance_image_size", "dspi_chain_export_instances", "dspi_chain_import_instances", "dspi_chain_reset_instances",
     "dspi_chainq_instance_image_size", "dspi_chainq_export_instances", "dspi_chainq_import_instances", "dspi_chainq_reset_instances",
+    "dspi_chain_copy_instances", "dspi_chainq_copy_instances",
     "dspi_chain_process_packets_range_host", "dspi_chain_process_packets_range_device",
     "dspi_chain_process_subframes_range_host", "dspi_chain_process_subframes_range_device",
     "dspi_chainq_process_packets_range_host", "dspi_chainq_process_packets_range_device",
@@ -142,6 +143,7 @@ def lib():
             getattr(h, pre + "_export_instances").argtypes = [vp, u32, u32, vp, C.c_size_t]
             getattr(h, pre + "_import_instances").argtypes = [vp, u32, u32, vp, C.c_size_t]
             getattr(h, pre + "_reset_instances").argtypes = [vp, u32, u32]
+            getattr(h, pre + "_copy_instances").argtypes = [vp, u32, vp, vp]
             getattr(h, pre + "_set_preset_mute").argtypes = [vp, u32, u32, vp, u32]
             getattr(h, pre + "_get_preset_mute").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_set_dynamics_device").argtypes = [vp, u32, u32, vp, C.c_float]
@@ -488,6 +490,19 @@ class _ChainEngine:
             raise ValueError("images must be [n, stride] bytes")
         _check(self._fn("import_instances")(self._h, int(inst0), int(img.shape[0]), img.ctypes.data_as(C.c_void_p),
                                             C.c_size_t(img.shape[1])))
+
+    def copy_instances(self, src, dst):
+        """Instance ``src[k]`` -> instance ``dst[k]`` on the GPU, as ``export_instances(src[k], 1)`` then
+        ``import_instances(..., dst[k])`` would, with no image leaving the device.  ``src`` may repeat; ``dst`` must be
+        distinct and share no index with ``src``.  Ordered behind earlier work; returns when the engine is updated."""
+        s = np.ascontiguousarray(np.asarray(src, np.int64).reshape(-1))
+        d = np.ascontiguousarray(np.asarray(dst, np.int64).reshape(-1))
+        if s.shape != d.shape:
+            raise ValueError("src and dst give different copy counts")
+        if s.size and (min(s.min(), d.min()) < 0 or max(s.max(), d.max()) > 0xFFFFFFFF):
+            raise ValueError("instance indices must be 0 .. 2**32 - 1")
+        s, d = s.astype(np.uint32), d.astype(np.uint32)
+        _check(self._fn("copy_instances")(self._h, int(s.size), s.ctypes.data_as(C.c_void_p), d.ctypes.data_as(C.c_void_p)))
 
     def reset_instances(self, inst0=0, n=None):
         """``reset_state`` for instances [inst0, inst0+n) only (default: to the end); parameters are kept."""

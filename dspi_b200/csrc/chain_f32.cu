@@ -1084,6 +1084,10 @@ int dspi_chain_import_instances(dspi_chain *c, uint32_t inst0, uint32_t n, const
     return dspi::import_instances(c, inst0, n, images, image_stride);
 }
 int dspi_chain_reset_instances(dspi_chain *c, uint32_t inst0, uint32_t n) { return dspi::reset_instances(c, inst0, n); }
+int dspi_chain_copy_instances(dspi_chain *c, uint32_t n, const uint32_t *src, const uint32_t *dst)
+{
+    return dspi::copy_instances(c, n, src, dst);
+}
 
 int dspi_chain_response_host(dspi_chain *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
 {

@@ -14,6 +14,7 @@
 //   A::pack(params, i, n, rows)               volumes, preamp, loudness and matrix / output gains of one instance
 // The code below never asks which arithmetic it serves.
 #pragma once
+#include <algorithm>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -52,6 +53,26 @@ int fail(int code, const char *fmt, ...)
         if (err__ != cudaSuccess) return fail(DSPI_ECUDA, "%s -> %s (%s:%d)", #expr, cudaGetErrorString(err__), __FILE__, __LINE__); \
     } while (0)
 
+// device copy of the instance lists of *_copy_instances (sources, then destinations); grows to the largest call
+struct IndexLists {
+    uint32_t *d = nullptr;
+    uint32_t cap = 0;                // pairs
+    cudaError_t ensure(uint32_t n)
+    {
+        if (n <= cap) return cudaSuccess;
+        cudaFree(d);
+        d = nullptr; cap = 0;
+        cudaError_t e = cudaMalloc((void **)&d, (size_t)2 * n * sizeof(uint32_t));
+        if (e == cudaSuccess) cap = n;
+        return e;
+    }
+    void destroy()
+    {
+        cudaFree(d);
+        d = nullptr; cap = 0;
+    }
+};
+
 // One engine: dspi_chain and dspi_chainq are this record for their arithmetic.
 template <class A>
 struct ChainHost {
@@ -76,6 +97,7 @@ struct ChainHost {
     bulk::Stage bulk;                // device staging of *_apply_bulk_device / _collect_bulk_device, allocated by the first call
     bulk::PresetStage preset;        // device staging of *_apply_preset_device / _collect_preset_device, allocated by the first call
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
+    IndexLists copy_lists;           // device instance lists of *_copy_instances, allocated by the first call
 };
 
 template <class A, typename T>
@@ -247,6 +269,7 @@ int destroy(H *c)
     c->resp.destroy();
     c->bulk.destroy();
     c->preset.destroy();
+    c->copy_lists.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -1113,6 +1136,67 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
     role_ranges(c, rm, ro);
     rc = eq_pack_range(c->eq_m, inst0, n, c->stream, rm);
     if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, inst0, n, c->stream, ro);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->stream);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->stream);
+    return rc;
+}
+
+// Instance src[k] becomes what export_instances(src[k], 1) then import_instances(dst[k], 1) would make of dst[k], with
+// the data moving engine to engine: running EQ state of the sources into the mirrors, every array of the image plan
+// (mirror rows included) from source to destination, then the destinations' mirror rows into the packed stores.
+template <class A>
+int copy_instances(ChainHost<A> *c, uint32_t n, const uint32_t *src, const uint32_t *dst)
+{
+    if (!c || !src || !dst) return fail(DSPI_EINVAL, "null argument");
+    const uint32_t N = c->desc.n_instances;
+    uint32_t lo = N, hi = 0;                                                // span of every index named, for the envelope count
+    for (uint32_t k = 0; k < n; k++) {
+        if (src[k] >= N || dst[k] >= N)
+            return fail(DSPI_ERANGE, "copy %u names instance %u, outside engine of %u", k, src[k] >= N ? src[k] : dst[k], N);
+        lo = std::min(lo, std::min(src[k], dst[k]));
+        hi = std::max(hi, std::max(src[k], dst[k]));
+    }
+    if (n == 0) return DSPI_OK;
+    std::vector<uint8_t> seen((size_t)hi - lo + 1, 0);                     // 1: a source, 2: a destination
+    for (uint32_t k = 0; k < n; k++) seen[src[k] - lo] |= 1;
+    for (uint32_t k = 0; k < n; k++) {
+        uint8_t &s = seen[dst[k] - lo];
+        if (s & 2) return fail(DSPI_EINVAL, "instance %u is a destination twice", dst[k]);
+        if (s & 1) return fail(DSPI_EINVAL, "instance %u is both a source and a destination", dst[k]);
+        s |= 2;
+    }
+    image::Plan pl;
+    if (!image_plan(c, kInImage, pl)) return fail(DSPI_EINVAL, "instance image plan exceeds its tables");
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(c->copy_lists.ensure(n));
+    const uint32_t *d_src = c->copy_lists.d, *d_dst = c->copy_lists.d + n;
+    std::vector<uint32_t> lists((size_t)2 * n);
+    memcpy(lists.data(), src, (size_t)n * 4);
+    memcpy(lists.data() + n, dst, (size_t)n * 4);
+    CU_OK(cudaMemcpyAsync(c->copy_lists.d, lists.data(), (size_t)2 * n * 4, cudaMemcpyHostToDevice, c->stream));
+    // envelope-mode instances: the modes (env row 4) of sources and destinations, behind earlier work
+    std::vector<uint32_t> mode((size_t)hi - lo + 1);
+    CU_OK(cudaMemcpyAsync(mode.data(), c->d.env + (size_t)4 * c->d.N_pad + lo, mode.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_OK(cudaStreamSynchronize(c->stream));
+    uint32_t before = 0, after = 0;
+    for (uint32_t k = 0; k < n; k++) {
+        before += mode[dst[k] - lo] ? 1u : 0u;
+        after += mode[src[k] - lo] ? 1u : 0u;
+    }
+    RoleRange rm, ro;
+    role_ranges(c, rm, ro);
+    rm.inst = ro.inst = d_src;
+    int rc = eq_unpack_range(c->eq_m, 0, n, c->stream, rm);               // running EQ state into the mirrors, as export
+    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, 0, n, c->stream, ro);
+    if (rc) return rc;
+    image::instance_copy_kernel<<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, n, d_src, d_dst);
+    CU_OK(cudaGetLastError());
+    c->launches++;
+    c->env_instances = c->env_instances - before + after;
+    // the destinations' mirror rows -> packed stores, then the skip masks, as import
+    rm.inst = ro.inst = d_dst;
+    rc = eq_pack_range(c->eq_m, 0, n, c->stream, rm);
+    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, 0, n, c->stream, ro);
     if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->stream);
     if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->stream);
     return rc;

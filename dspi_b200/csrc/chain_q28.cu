@@ -1037,6 +1037,10 @@ int dspi_chainq_import_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, con
     return dspi::import_instances(c, inst0, n, images, image_stride);
 }
 int dspi_chainq_reset_instances(dspi_chainq *c, uint32_t inst0, uint32_t n) { return dspi::reset_instances(c, inst0, n); }
+int dspi_chainq_copy_instances(dspi_chainq *c, uint32_t n, const uint32_t *src, const uint32_t *dst)
+{
+    return dspi::copy_instances(c, n, src, dst);
+}
 
 int dspi_chainq_response_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
 {

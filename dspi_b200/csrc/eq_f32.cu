@@ -104,7 +104,7 @@ __global__ void pack_f32_kernel(const dspi_biquad_f32 *__restrict__ aos, uint32_
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || (rr.reject && rr.reject[i])) return;
-    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + (rr.inst ? rr.inst[i] : i);
     const uint32_t rows = 32 * cpl;
     const uint32_t g = ch / rows, r = ch % rows, lane = r & 31, h = r >> 5;
     uint64_t mw = 0;
@@ -133,7 +133,7 @@ __global__ void unpack_f32_kernel(dspi_biquad_f32 *__restrict__ aos, uint32_t ch
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || (rr.reject && rr.reject[i])) return;
-    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + (rr.inst ? rr.inst[i] : i);
     const uint32_t rows = 32 * cpl;
     const uint32_t g = ch / rows, r = ch % rows, lane = r & 31, h = r >> 5;
     for (int b = 0; b < kMaxBands; b++) {

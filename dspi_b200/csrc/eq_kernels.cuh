@@ -47,11 +47,13 @@ char *error_buffer(size_t *cap);
 // The chain engines keep role-major rows (channel = role * N_pad + instance), so an instance range is one such set.
 // reject[i] != 0 (device memory, [n], or nullptr) leaves channel i of every role untouched.  fs (device memory, [n], or
 // nullptr) gives channel i of every role its own sample rate in the coefficient kernels, in place of their scalar one.
-// The default is one plain range.
+// inst (device memory, [n], or nullptr) turns the range into a list: channel i of role r is ch0 + r * stride + inst[i]
+// (pack / unpack kernels only; the chain engines' copy of scattered instances).  The default is one plain range.
 struct RoleRange {
     uint32_t roles = 1, stride = 0;
     const int32_t *reject = nullptr;
     const float *fs = nullptr;
+    const uint32_t *inst = nullptr;
 };
 
 // K1 — float cascade.  cpl: channels per lane (1, or 2 held in a register pair)

@@ -280,7 +280,7 @@ __global__ void pack_q28_kernel(const dspi_biquad_q28 *__restrict__ aos, uint32_
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || (rr.reject && rr.reject[i])) return;
-    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i, g = ch / 32, lane = ch % 32;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + (rr.inst ? rr.inst[i] : i), g = ch / 32, lane = ch % 32;
     for (int b = 0; b < kMaxBands; b++) {
         const dspi_biquad_q28 &q = aos[(size_t)ch * kMaxBands + b];
         int32_t *dst = coef + ((size_t)g * kMaxBands + b) * kSlots * 32 + lane;
@@ -315,7 +315,7 @@ __global__ void unpack_q28_kernel(dspi_biquad_q28 *__restrict__ aos, uint32_t ch
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || (rr.reject && rr.reject[i])) return;
-    const uint32_t ch = ch0 + blockIdx.y * rr.stride + i, g = ch / 32, lane = ch % 32;
+    const uint32_t ch = ch0 + blockIdx.y * rr.stride + (rr.inst ? rr.inst[i] : i), g = ch / 32, lane = ch % 32;
     for (int b = 0; b < kMaxBands; b++) {
         dspi_biquad_q28 &q = aos[(size_t)ch * kMaxBands + b];
         const int32_t *src = coef + ((size_t)g * kMaxBands + b) * kSlots * 32 + lane;

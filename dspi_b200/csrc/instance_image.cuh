@@ -1,7 +1,8 @@
 // instance_image.cuh — the one kernel behind dspi_chain(q)_export_instances / _import_instances / _reset_instances (and
 // the engines' reset_state): it moves the per-instance arrays of an instance range between the engine and instance
-// images in a device staging buffer, or writes their reset values.  The host side (which arrays, the image layout, the
-// staging and the EQ sub-engines' pack / unpack around it) is chain_host.cuh.
+// images in a device staging buffer, or writes their reset values.  Its sibling behind _copy_instances moves the same
+// arrays from listed instances to listed instances of the same engine.  The host side (which arrays, the image layout,
+// the staging and the EQ sub-engines' pack / unpack around it) is chain_host.cuh.
 //
 // Every array is `rows` rows of N_pad elements with the instance index innermost, element (r, i) at p + (r N_pad + i) elem:
 //   scalar fields (elem 1, 2, 4 or 8): a CTA takes 32 instances x up to 32 rows, reads them lane = instance (coalesced)
@@ -130,6 +131,48 @@ __global__ void __launch_bounds__(256) instance_image_kernel(const __grid_consta
         __syncthreads();
         if (g0 + lane < n)
             for (uint32_t r = warp; r < S; r += 8) store_elem(dev_at(r, g0 + lane), E, tile[r][lane]);
+    }
+}
+
+// Instance src[k] -> instance dst[k] for k < n, engine to engine with no image in between (dspi_chain(q)_copy_instances):
+// the same plan and grid as above, with the lists in place of (inst0, n).  No index of dst appears in src, so no copy
+// reads an element another copy writes; src may repeat.  Scalar fields: one thread per (row, k), element (r, src[k]) to
+// (r, dst[k]); wide fields: one warp per (k, segment) in 16-byte vectors.
+__global__ void __launch_bounds__(256) instance_copy_kernel(const __grid_constant__ Plan plan, uint32_t n, const uint32_t *__restrict__ src,
+                                                            const uint32_t *__restrict__ dst)
+{
+    const uint32_t g0 = blockIdx.x * 32, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const Task t = plan.t[blockIdx.y];
+    const Field &f = plan.f[t.field];
+    const size_t Np = plan.N_pad;
+    if (f.elem >= 16) {
+        const uint32_t seg = (uint32_t)t.count * kSegBytes, rest = f.elem - seg;
+        const uint32_t nv = (rest < kSegBytes ? rest : kSegBytes) / 16;
+        for (uint32_t k = warp; k < 32 && g0 + k < n; k += 8) {
+            const size_t row = (size_t)t.first * Np;
+            const uint4 *from = reinterpret_cast<const uint4 *>(f.p + (row + src[g0 + k]) * f.elem + seg);
+            uint4 *to = reinterpret_cast<uint4 *>(f.p + (row + dst[g0 + k]) * f.elem + seg);
+            for (uint32_t w0 = 0; w0 < nv; w0 += 4 * 32) {                           // four 16-byte loads in flight per lane
+                uint4 v[4];
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const uint32_t w = w0 + j * 32 + lane;
+                    if (w < nv) v[j] = from[w];
+                }
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const uint32_t w = w0 + j * 32 + lane;
+                    if (w < nv) to[w] = v[j];
+                }
+            }
+        }
+        return;
+    }
+    if (g0 + lane >= n) return;
+    const size_t s = src[g0 + lane], d = dst[g0 + lane];
+    for (uint32_t r = warp; r < t.count; r += 8) {
+        const size_t row = (size_t)(t.first + r) * Np;
+        store_elem(f.p + (row + d) * f.elem, f.elem, load_elem(f.p + (row + s) * f.elem, f.elem));
     }
 }
 

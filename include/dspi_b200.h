@@ -393,6 +393,25 @@ size_t dspi_chain_instance_image_size(dspi_chain *c);
 int dspi_chain_export_instances(dspi_chain *c, uint32_t inst0, uint32_t n, void *images, size_t image_stride);
 int dspi_chain_import_instances(dspi_chain *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride);
 int dspi_chain_reset_instances(dspi_chain *c, uint32_t inst0, uint32_t n);
+/* Copy instances within one engine on the GPU, so a host can repack its clock groups into contiguous ranges (or clone
+ * one configured device into many slots) without sending images over the bus.
+ *   src[n] and dst[n] are host memory, read during the call.  After it, instance dst[k] is, byte for byte, what
+ *   _export_instances(src[k], 1) followed by _import_instances(dst[k], 1) would have made of it: everything an instance
+ *   image holds (parameter rows, the 11 (Q28: 7) x 12 biquads with their current state, loudness / crossfeed / leveller
+ *   state, look-ahead and delay rings with the write index, modulator state, meters, preset-mute envelope and mode,
+ *   S/PDIF transmitter, configuration record, host record and DSPI_BULK_* mark).  A later process call on dst[k] gives
+ *   the bytes the source would have given.  The data moves device to device; no image is formed.
+ *   Sources are left exactly as they were, and so is every instance not in dst, its EQ coefficients and state in 32- and
+ *   64-channel groups shared with a destination included.
+ *   src may repeat (one instance cloned into many slots).  dst entries must be distinct and no index may be in both
+ *   lists, so every copy reads a source no copy of the call writes.  To shift a group onto slots that overlap its own,
+ *   call in steps whose sources and destinations do not overlap (e.g. through free slots, or one block at a time).
+ *   Ordered behind everything issued earlier on the engine stream, asynchronous process calls included; returns when
+ *   the engine is updated.  The engine's count of envelope-mode instances follows the copied modes.
+ * Errors: DSPI_EINVAL for a NULL engine, src or dst, a destination named twice, or an index in both lists; DSPI_ERANGE
+ * for an index at or above n_instances.  Every check runs before anything is written, and nothing is written on an
+ * error.  n == 0 does nothing. */
+int dspi_chain_copy_instances(dspi_chain *c, uint32_t n, const uint32_t *src, const uint32_t *dst);
 /* n_packets USB packets of frames_per_packet (<= 192) frames for every instance.
  *   pcm:       [n_instances][n_packets * frames_per_packet] interleaved L,R little-endian frames,
  *              bit_depth 16 (4 bytes / frame) or 24 (packed, 6 bytes / frame)      (HOST memory)
@@ -516,6 +535,7 @@ size_t dspi_chainq_instance_image_size(dspi_chainq *c);
 int dspi_chainq_export_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, void *images, size_t image_stride);
 int dspi_chainq_import_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride);
 int dspi_chainq_reset_instances(dspi_chainq *c, uint32_t inst0, uint32_t n);
+int dspi_chainq_copy_instances(dspi_chainq *c, uint32_t n, const uint32_t *src, const uint32_t *dst);
 /* pcm as for dspi_chain_process_host; spdif_out [n_instances][2][n_frames][2]; pdm_out [n_instances][n_frames][8] */
 int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t frames_per_packet,
                              int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status);
