@@ -48,6 +48,7 @@ SYMBOLS = [
     "dspi_chain_apply_bulk_device", "dspi_chainq_apply_bulk_device",
     "dspi_chain_collect_bulk_device", "dspi_chainq_collect_bulk_device",
     "dspi_chain_set_rate_device", "dspi_chainq_set_rate_device",
+    "dspi_chain_edit_bulk_device", "dspi_chainq_edit_bulk_device",
     "dspi_chain_apply_preset_device", "dspi_chainq_apply_preset_device",
     "dspi_chain_collect_preset_device", "dspi_chainq_collect_preset_device",
     "dspi_chain_instance_image_size", "dspi_chain_export_instances", "dspi_chain_import_instances", "dspi_chain_reset_instances",
@@ -151,6 +152,7 @@ def lib():
             getattr(h, pre + "_apply_bulk_device").argtypes = [vp, u32, u32, vp, vp, C.c_int, C.c_float, vp]
             getattr(h, pre + "_collect_bulk_device").argtypes = [vp, u32, u32, vp, vp, vp]
             getattr(h, pre + "_set_rate_device").argtypes = [vp, u32, u32, vp, vp]
+            getattr(h, pre + "_edit_bulk_device").argtypes = [vp, u32, vp, C.c_int, C.c_float, vp]
             getattr(h, pre + "_apply_preset_device").argtypes = [vp, u32, u32, vp, C.c_size_t, vp, vp, C.c_float, vp]
             getattr(h, pre + "_collect_preset_device").argtypes = [vp, u32, u32, vp, vp, C.c_size_t, vp]
             getattr(h, pre + "_process_packets_host").argtypes = [vp, vp, u32, u32, vp, vp, vp, vp]
@@ -637,6 +639,16 @@ class _ChainEngine:
         r = np.ascontiguousarray(np.asarray(rates, np.float32).reshape(-1))
         res = np.zeros(r.size, np.int32)
         _check(self._fn("set_rate_device")(self._h, int(inst0), int(r.size), r.ctypes.data_as(C.c_void_p), res.ctypes.data_as(C.c_void_p)))
+        return res
+
+    def edit_bulk_device(self, edits, fs, exact_db=False):
+        """BULK_EDIT [n] (see ``layouts.bulk_edit``) -> single fields of current instances edited on the GPU, in list order,
+        as collect + patch + ``apply_bulk_device(fs, exact_db)`` would leave them, with only the touched fields re-derived.
+        Returns int32 [n]: the ``layouts.BULK_*`` mark of each edit's instance; stale and unset instances are left alone."""
+        e = np.ascontiguousarray(edits, L.BULK_EDIT).reshape(-1)
+        res = np.zeros(e.shape[0], np.int32)
+        _check(self._fn("edit_bulk_device")(self._h, int(e.shape[0]), e.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
+                                            res.ctypes.data_as(C.c_void_p)))
         return res
 
     def collect_bulk_device(self, inst0=0, n=None):

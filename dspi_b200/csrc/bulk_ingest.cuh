@@ -34,9 +34,12 @@
 // Same arithmetic rules as coeff.cu / dynamics.cuh: every float operation is the reference's, rounded on its own
 // (-fmad=false, divisions spelled __fdiv_rn), libm in double rounded once, float -> int32 stores saturate.
 #pragma once
+#include <algorithm>
 #include <cstddef>
 #include <cstdio>
+#include <cstring>
 #include <type_traits>
+#include <vector>
 
 #include "dspi_common.cuh"
 #include "dynamics.cuh"
@@ -188,17 +191,100 @@ __device__ __forceinline__ int32_t delay_samples(float delay_ms, uint32_t o, flo
     return ds;
 }
 
-// filter_recipes[][] (bulk_params.c:291-300) of instance i of n from the eq section of a packet or record in shared memory
-// `w` -> the role-major recipe buffer [role][n][12] of the coefficient kernels; all lanes of the warp
+// recipe r = role * 12 + band (bulk_params.c:291-300) of instance i of n from the eq section of a packet or record in shared
+// memory `w` -> the role-major recipe buffer [role][n][12] of the coefficient kernels
+__device__ __forceinline__ void stage_recipe(const unsigned char *w, uint32_t r, uint32_t i, uint32_t n, dspi_eq_param *__restrict__ recipes)
+{
+    const uint32_t role = r / kMaxBands, b = r % kMaxBands;
+    uint4 q = *reinterpret_cast<const uint4 *>(w + DSPI_WIRE_OFF(eq) + r * 16);                     // {type, reserved[3]}, freq, q, gain_db
+    q.x = role | b << 8 | (q.x & 0xFFu) << 16;                                                     // {channel, band, type, reserved}
+    reinterpret_cast<uint4 *>(recipes)[((size_t)role * n + i) * kMaxBands + b] = q;
+}
+
+// filter_recipes[][] of instance i of n, every role and band; all lanes of the warp
 template <class S>
 __device__ __forceinline__ void stage_recipes(const unsigned char *w, int lane, uint32_t i, uint32_t n, dspi_eq_param *__restrict__ recipes)
 {
-    for (uint32_t r = lane; r < (uint32_t)S::kRoles * kMaxBands; r += 32) {
-        const uint32_t role = r / kMaxBands, b = r % kMaxBands;
-        uint4 q = *reinterpret_cast<const uint4 *>(w + DSPI_WIRE_OFF(eq) + r * 16);                 // {type, reserved[3]}, freq, q, gain_db
-        q.x = role | b << 8 | (q.x & 0xFFu) << 16;                                                 // {channel, band, type, reserved}
-        reinterpret_cast<uint4 *>(recipes)[((size_t)role * n + i) * kMaxBands + b] = q;
-    }
+    for (uint32_t r = lane; r < (uint32_t)S::kRoles * kMaxBands; r += 32) stage_recipe(w, r, i, n, recipes);
+}
+
+// ---- lane bodies of the ingest, rate and edit kernels: each reads a packet or record in shared memory `w` ----
+__device__ __forceinline__ float wire_f32(const unsigned char *w, uint32_t off) { return *reinterpret_cast<const float *>(w + off); }
+
+// a crosspoint, output or preamp gain in dB -> linear (:206-215, :247-264) under the ingest's gain mode
+__device__ __forceinline__ float gain_linear(float db, int gain_mode)
+{
+    if (gain_mode == kGainFlash) return db_to_linear_flash(db);
+    return gain_mode == kGainExact ? dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f)) : db_to_linear_fw(db);
+}
+
+// the master volume (:361-374): `db` made finite and clamped to [-128, 0] in place, then always the exact conversion
+__device__ __forceinline__ float master_linear(float &db)
+{
+    if (isnan(db) || isinf(db)) db = 0.0f;
+    if (db < -128.0f) db = -128.0f;
+    if (db > 0.0f) db = 0.0f;
+    return db <= -128.0f ? 0.0f : dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f));
+}
+
+// output o's flag word (the S/PDIF pair-off bit reads its partner's enable) and its EQ skip row (usb_audio.c:878-884)
+template <class S>
+__device__ __forceinline__ void output_flag_rows(const typename S::Dev &d, const unsigned char *w, uint32_t inst, uint32_t o, bool bypass_master)
+{
+    const uint32_t Np = d.N_pad, off = DSPI_WIRE_OFF(outputs) + o * 12;
+    const bool enabled = w[off] != 0, mute = w[off + 1] != 0;
+    const bool partner = w[DSPI_WIRE_OFF(outputs) + (o ^ 1u) * 12] != 0;
+    d.o_flags[o * Np + inst] = output_flags(enabled, mute, o < (uint32_t)S::kOuts - 1, partner);
+    d.skip_o[o * Np + inst] = S::output_eq_frozen(enabled, mute, bypass_master) ? 1 : 0;
+}
+
+// output o's delay in samples at fs (dsp_update_delay_samples()); returns it
+template <class S>
+__device__ __forceinline__ int32_t output_delay_row(const typename S::Dev &d, const unsigned char *w, uint32_t inst, uint32_t o, float fs)
+{
+    const int32_t ds = delay_samples<S>(wire_f32(w, DSPI_WIRE_OFF(outputs) + o * 12 + 8), o, fs);
+    d.o_dly[o * d.N_pad + inst] = ds;
+    return ds;
+}
+
+// crossfeed_config (:225-230); S::crossfeed clears the filter state (crossfeed.c:110-126)
+__device__ __forceinline__ dspi_crossfeed_config crossfeed_config(const unsigned char *w)
+{
+    dspi_crossfeed_config xf;
+    xf.enabled = w[DSPI_WIRE_OFF(crossfeed.enabled)] != 0;
+    xf.itd_enabled = w[DSPI_WIRE_OFF(crossfeed.itd_enabled)] != 0;
+    xf.preset = w[DSPI_WIRE_OFF(crossfeed.preset)];
+    xf.custom_fc = wire_f32(w, DSPI_WIRE_OFF(crossfeed.custom_fc));
+    xf.custom_feed_db = wire_f32(w, DSPI_WIRE_OFF(crossfeed.custom_feed_db));
+    return xf;
+}
+
+// leveller_config (:330-346): the fixed defaults below format version 4 (a record holds the version gates' result)
+__device__ __forceinline__ dspi_leveller_config leveller_config(const unsigned char *w, uint32_t version)
+{
+    dspi_leveller_config lev;
+    lev.enabled = version >= 4 ? (w[DSPI_WIRE_OFF(leveller.enabled)] != 0) : 0;
+    lev.speed = version >= 4 ? w[DSPI_WIRE_OFF(leveller.speed)] : 0;
+    lev.lookahead = version >= 4 ? (w[DSPI_WIRE_OFF(leveller.lookahead)] != 0) : 1;
+    lev.amount = version >= 4 ? wire_f32(w, DSPI_WIRE_OFF(leveller.amount)) : 50.0f;
+    lev.max_gain_db = version >= 4 ? wire_f32(w, DSPI_WIRE_OFF(leveller.max_gain_db)) : 15.0f;
+    lev.gate_threshold_db = version >= 4 ? wire_f32(w, DSPI_WIRE_OFF(leveller.gate_threshold_db)) : -96.0f;
+    return lev;
+}
+
+// the loudness row audio_set_volume() selected (`row`), at fs
+template <class S>
+__device__ __forceinline__ void loudness_row(const typename S::Dev &d, const unsigned char *w, uint32_t inst, uint32_t row, float fs)
+{
+    S::loudness(d, inst, row, wire_f32(w, DSPI_WIRE_OFF(global.loudness_ref_spl)), wire_f32(w, DSPI_WIRE_OFF(global.loudness_intensity_pct)), fs);
+}
+
+// the instance's flag word
+template <class S>
+__device__ __forceinline__ uint8_t instance_flags(const unsigned char *w, const dspi_leveller_config &lev, bool any_delay)
+{
+    return chain_flags(w[DSPI_WIRE_OFF(global.bypass)] != 0, w[DSPI_WIRE_OFF(global.loudness_enabled)] != 0, w[DSPI_WIRE_OFF(crossfeed.enabled)] != 0,
+                       lev.enabled, lev.lookahead, any_delay, w[DSPI_WIRE_OFF(outputs) + (S::kOuts - 1) * 12] != 0);
 }
 
 template <class S>
@@ -228,7 +314,6 @@ bulk_ingest_kernel(typename S::Dev d, Record rec, uint32_t inst0, uint32_t n, co
     if (lane == 0) results[i] = rc;
     if (rc != 0) return;
 
-    auto f32 = [&](uint32_t off) { return *reinterpret_cast<const float *>(w + off); };
     const uint32_t inst = inst0 + i, Np = d.N_pad;
     const uint32_t version = w[DSPI_WIRE_OFF(header.format_version)];
     const bool bypass_master = w[DSPI_WIRE_OFF(global.bypass)] != 0;                               // :217
@@ -238,32 +323,20 @@ bulk_ingest_kernel(typename S::Dev d, Record rec, uint32_t inst0, uint32_t n, co
     const uint32_t side = is_xp ? lane / O : (uint32_t)(lane - 3 * O), o = is_xp ? lane % O : (uint32_t)(lane - 2 * O);
     const uint32_t xp_off = DSPI_WIRE_OFF(crosspoints) + (side * WO + o) * 8, out_off = DSPI_WIRE_OFF(outputs) + o * 12;
     float db = 0.0f;
-    if (is_xp) db = f32(xp_off + 4);
-    else if (is_out) db = f32(out_off + 4);
-    else if (is_pre) db = version >= 6 ? f32(DSPI_WIRE_OFF(preamp.preamp_db) + side * 4) : f32(DSPI_WIRE_OFF(global.preamp_gain_db));
-    else if (is_mv) db = f32(DSPI_WIRE_OFF(master_volume.master_volume_db));
+    if (is_xp) db = wire_f32(w, xp_off + 4);
+    else if (is_out) db = wire_f32(w, out_off + 4);
+    else if (is_pre) db = version >= 6 ? wire_f32(w, DSPI_WIRE_OFF(preamp.preamp_db) + side * 4) : wire_f32(w, DSPI_WIRE_OFF(global.preamp_gain_db));
+    else if (is_mv) db = wire_f32(w, DSPI_WIRE_OFF(master_volume.master_volume_db));
     float lin = 0.0f;
-    if (is_mv) {                                                                                   // :361-374: always the exact conversion
-        if (isnan(db) || isinf(db)) db = 0.0f;
-        if (db < -128.0f) db = -128.0f;
-        if (db > 0.0f) db = 0.0f;
-        lin = db <= -128.0f ? 0.0f : dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f));
-    } else if (is_xp || is_out || is_pre) {
-        if (gain_mode == kGainFlash) lin = db_to_linear_flash(db);
-        else lin = gain_mode == kGainExact ? dyn::pow_f(10.0f, dyn::fdiv(db, 20.0f)) : db_to_linear_fw(db);
-    }
+    if (is_mv) lin = master_linear(db);
+    else if (is_xp || is_out || is_pre) lin = gain_linear(db, gain_mode);
     bool delayed = false;
     if (is_xp) {
         S::crosspoint(d, inst, side, o, w[xp_off] != 0, w[xp_off + 1] != 0, lin);
     } else if (is_out) {
-        const bool enabled = w[out_off] != 0, mute = w[out_off + 1] != 0;
-        const bool partner = w[DSPI_WIRE_OFF(outputs) + (o ^ 1u) * 12] != 0;
         d.o_glin[o * Np + inst] = lin;
-        d.o_flags[o * Np + inst] = output_flags(enabled, mute, o < (uint32_t)O - 1, partner);
-        d.skip_o[o * Np + inst] = S::output_eq_frozen(enabled, mute, bypass_master) ? 1 : 0;
-        const int32_t ds = delay_samples<S>(f32(out_off + 8), o, fs);
-        d.o_dly[o * Np + inst] = ds;
-        delayed = ds > 0;
+        output_flag_rows<S>(d, w, inst, o, bypass_master);
+        delayed = output_delay_row<S>(d, w, inst, o, fs) > 0;
     } else if (is_pre) {
         S::preamp(d, inst, side, lin);
     } else if (is_mv && version >= 6) {
@@ -272,32 +345,18 @@ bulk_ingest_kernel(typename S::Dev d, Record rec, uint32_t inst0, uint32_t n, co
     const bool any_delay = __ballot_sync(0xffffffffu, delayed) != 0;                               // dsp_pipeline.c:237
 
     // ---- the pending-flag handlers of the main loop (main.c:868-900), one generator per lane ----
-    dspi_leveller_config lev;                                                                      // :330-346: defaults below v4
-    lev.enabled = version >= 4 ? (w[DSPI_WIRE_OFF(leveller.enabled)] != 0) : 0;
-    lev.speed = version >= 4 ? w[DSPI_WIRE_OFF(leveller.speed)] : 0;
-    lev.lookahead = version >= 4 ? (w[DSPI_WIRE_OFF(leveller.lookahead)] != 0) : 1;
-    lev.amount = version >= 4 ? f32(DSPI_WIRE_OFF(leveller.amount)) : 50.0f;
-    lev.max_gain_db = version >= 4 ? f32(DSPI_WIRE_OFF(leveller.max_gain_db)) : 15.0f;
-    lev.gate_threshold_db = version >= 4 ? f32(DSPI_WIRE_OFF(leveller.gate_threshold_db)) : -96.0f;
-    const bool xf_enabled = w[DSPI_WIRE_OFF(crossfeed.enabled)] != 0, loud_enabled = w[DSPI_WIRE_OFF(global.loudness_enabled)] != 0;
+    const dspi_leveller_config lev = leveller_config(w, version);
     const dspi_bulk_host hv = host[i];
     uint32_t row;
     const int16_t vol_mul = dyn::host_volume(hv.volume_8_8, row);
     if (lane == 0) {
-        dspi_crossfeed_config xf;                                                                  // :225-230; the filter state is cleared (crossfeed.c:110-126)
-        xf.enabled = xf_enabled;
-        xf.itd_enabled = w[DSPI_WIRE_OFF(crossfeed.itd_enabled)] != 0;
-        xf.preset = w[DSPI_WIRE_OFF(crossfeed.preset)];
-        xf.custom_fc = f32(DSPI_WIRE_OFF(crossfeed.custom_fc));
-        xf.custom_feed_db = f32(DSPI_WIRE_OFF(crossfeed.custom_feed_db));
-        S::crossfeed(d, inst, xf, fs);
-        d.flags[inst] = chain_flags(bypass_master, loud_enabled, xf_enabled, lev.enabled, lev.lookahead, any_delay,
-                                    w[DSPI_WIRE_OFF(outputs) + (O - 1) * 12] != 0);
+        S::crossfeed(d, inst, crossfeed_config(w), fs);
+        d.flags[inst] = instance_flags<S>(w, lev, any_delay);
         d.skip_m[inst] = d.skip_m[Np + inst] = bypass_master ? 1 : 0;                              // usb_audio.c:721-728
     } else if (lane == 1) {
         S::leveller(d, inst, lev, fs);
     } else if (lane == 2) {
-        S::loudness(d, inst, row, f32(DSPI_WIRE_OFF(global.loudness_ref_spl)), f32(DSPI_WIRE_OFF(global.loudness_intensity_pct)), fs);
+        loudness_row<S>(d, w, inst, row, fs);
     }
     __syncwarp();                                          // the gain rows of this instance are written: audio_set_volume() reads them
     if (lane == 0) S::host_volume(d, inst, vol_mul, hv.host_mute != 0);
@@ -355,52 +414,177 @@ rate_kernel(typename S::Dev d, Record rec, uint32_t inst0, uint32_t n, const flo
     if (lane == 0) results[i] = mark;
     if (mark != DSPI_BULK_CURRENT) return;
 
-    auto f32 = [&](uint32_t off) { return *reinterpret_cast<const float *>(w + off); };
     bool delayed = false;
-    if (lane < O) {                                                                                // dsp_update_delay_samples()
-        const int32_t ds = delay_samples<S>(f32(DSPI_WIRE_OFF(outputs) + lane * 12 + 8), lane, fs);
-        d.o_dly[lane * Np + inst] = ds;
-        delayed = ds > 0;
-    }
+    if (lane < O) delayed = output_delay_row<S>(d, w, inst, lane, fs) > 0;                        // dsp_update_delay_samples()
     const bool any_delay = __ballot_sync(0xffffffffu, delayed) != 0;                               // dsp_pipeline.c:237
     if (lane == 0) {
-        dspi_crossfeed_config xf;
-        xf.enabled = w[DSPI_WIRE_OFF(crossfeed.enabled)] != 0;
-        xf.itd_enabled = w[DSPI_WIRE_OFF(crossfeed.itd_enabled)] != 0;
-        xf.preset = w[DSPI_WIRE_OFF(crossfeed.preset)];
-        xf.custom_fc = f32(DSPI_WIRE_OFF(crossfeed.custom_fc));
-        xf.custom_feed_db = f32(DSPI_WIRE_OFF(crossfeed.custom_feed_db));
-        S::crossfeed(d, inst, xf, fs);
+        S::crossfeed(d, inst, crossfeed_config(w), fs);
         d.flags[inst] = (uint8_t)((d.flags[inst] & ~F_ANY_DELAY) | (any_delay ? F_ANY_DELAY : 0));
     } else if (lane == 1) {
-        dspi_leveller_config lev;                                                                  // the record holds the version gates' result
-        lev.enabled = w[DSPI_WIRE_OFF(leveller.enabled)] != 0;
-        lev.speed = w[DSPI_WIRE_OFF(leveller.speed)];
-        lev.lookahead = w[DSPI_WIRE_OFF(leveller.lookahead)] != 0;
-        lev.amount = f32(DSPI_WIRE_OFF(leveller.amount));
-        lev.max_gain_db = f32(DSPI_WIRE_OFF(leveller.max_gain_db));
-        lev.gate_threshold_db = f32(DSPI_WIRE_OFF(leveller.gate_threshold_db));
-        S::leveller(d, inst, lev, fs);
+        S::leveller(d, inst, leveller_config(w, DSPI_WIRE_FORMAT_VERSION), fs);                    // the record holds the version gates' result
     } else if (lane == 2) {
         uint32_t row;
         dyn::host_volume(rec.host[inst].volume_8_8, row);
-        S::loudness(d, inst, row, f32(DSPI_WIRE_OFF(global.loudness_ref_spl)), f32(DSPI_WIRE_OFF(global.loudness_intensity_pct)), fs);
+        loudness_row<S>(d, w, inst, row, fs);
     }
     stage_recipes<S>(w, lane, i, n, recipes);
 }
 
+// One edit of dspi_chain(q)_edit_bulk_device, and the edit address space: the record, then the host record
+constexpr uint32_t kEditSpace = kPacketBytes + (uint32_t)sizeof(dspi_bulk_host);
+constexpr uint32_t kEditChunk = 65536;                     // edits per staged chunk: 2 MiB; at most kChunk distinct instances
+static_assert(sizeof(dspi_bulk_edit) == 32, "dspi_bulk_edit");
+
+// any byte of [off, off + len) written by an edit; len <= 32, `hit` one bit per byte of the edit space and a spare word
+__device__ __forceinline__ bool touched(const uint32_t *hit, uint32_t off, uint32_t len)
+{
+    const uint64_t bits = (uint64_t)hit[off >> 5] | (uint64_t)hit[(off >> 5) + 1] << 32;
+    return ((bits >> (off & 31)) & ((1ull << len) - 1)) != 0;
+}
+
+// Sparse edits of current instances (dspi_chain(q)_edit_bulk_device): one warp per distinct instance, segment s of the
+// chunk, whose edits are edits[seg_off[s] .. seg_off[s + 1]) in list order.  Lane 0 brings the record in with a bulk copy
+// and the host record beside it; the mark goes to marks[s] and only a DSPI_BULK_CURRENT instance goes on.  The edits are
+// written over the shared-memory copy in order, each byte noting itself in a bitmap; the copy is normalised by record_body
+// (version 6); then the lanes re-derive the rows of touched fields only, with the ingest kernel's lane bodies, and stage
+// the touched bands' recipes with a per-(role, segment) band mask for the coefficient kernels.  reject[s] != 0 keeps the
+// segment out of the filter recalculation (no touched band, or not current).
+template <class S>
+__global__ void __launch_bounds__(kWarps * 32)
+edit_kernel(typename S::Dev d, Record rec, uint32_t nseg, const dspi_bulk_edit *__restrict__ edits, const uint32_t *__restrict__ seg_off,
+            const uint32_t *__restrict__ seg_inst, int gain_mode, float fs, dspi_eq_param *__restrict__ recipes, uint16_t *__restrict__ band_mask,
+            int32_t *__restrict__ reject, int32_t *__restrict__ marks)
+{
+    constexpr int O = S::kOuts, NC = S::kRoles, WO = DSPI_WIRE_MAX_OUTPUTS;
+    constexpr uint32_t kHitWords = (kEditSpace + 31) / 32 + 1;
+    static_assert(3 * O + 3 <= 32 && NC <= 32, "one lane per gain and per role");
+    __shared__ alignas(16) unsigned char pkt_s[kWarps][kPacketBytes + 16];
+    __shared__ uint32_t hit_s[kWarps][kHitWords];
+    __shared__ uint64_t bar_s[kWarps];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t s = blockIdx.x * kWarps + warp;
+    if (s >= nseg) return;
+    const uint32_t inst = seg_inst[s], Np = d.N_pad;
+    unsigned char *w = pkt_s[warp];
+    uint32_t *hit = hit_s[warp];
+    uint64_t *bar = &bar_s[warp];
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        fence_mbar_init();
+        mbar_arrive_expect_tx(bar, kPacketBytes);
+        bulk_load_1d(w, rec.packets + inst, kPacketBytes, bar);
+        *reinterpret_cast<dspi_bulk_host *>(w + kPacketBytes) = rec.host[inst];
+    }
+    for (uint32_t k = lane; k < kHitWords; k += 32) hit[k] = 0;
+    const uint8_t mark = rec.mark[inst];
+    __syncwarp();
+    mbar_wait(bar, 0);
+    if (lane == 0) marks[s] = mark;
+    if (mark != DSPI_BULK_CURRENT) {
+        if (lane < NC) band_mask[lane * nseg + s] = 0;
+        if (lane == 0) reject[s] = 1;
+        return;
+    }
+
+    // ---- the edits in list order: the last write to a byte wins ----
+    for (uint32_t k = seg_off[s], end = seg_off[s + 1]; k < end; k++) {
+        const uint32_t off = edits[k].offset, len = edits[k].length;
+        if ((uint32_t)lane < len) {
+            w[off + lane] = edits[k].bytes[lane];
+            atomicOr(&hit[(off + lane) >> 5], 1u << ((off + lane) & 31));
+        }
+        __syncwarp();
+    }
+
+    // ---- normalised as the ingest leaves a record (version 6; the master volume made finite and clamped) ----
+    float mv_db = wire_f32(w, DSPI_WIRE_OFF(master_volume.master_volume_db));
+    const float mv_lin = master_linear(mv_db);
+    __syncwarp();
+    record_body<NC, O>(w, lane, DSPI_WIRE_FORMAT_VERSION, __float_as_uint(mv_db));
+    __syncwarp();
+    const dspi_bulk_host hv = *reinterpret_cast<const dspi_bulk_host *>(w + kPacketBytes);
+    const bool bypass_master = w[DSPI_WIRE_OFF(global.bypass)] != 0;
+    const bool bypass_t = touched(hit, DSPI_WIRE_OFF(global.bypass), 1), mv_t = touched(hit, DSPI_WIRE_OFF(master_volume.master_volume_db), 4);
+    const bool vol_t = touched(hit, kPacketBytes, 2), host_t = touched(hit, kPacketBytes, 3);
+    const bool xf_t = touched(hit, DSPI_WIRE_OFF(crossfeed), 16), lev_t = touched(hit, DSPI_WIRE_OFF(leveller), 16);
+    const bool loud_t = touched(hit, DSPI_WIRE_OFF(global.loudness_enabled), 1) || touched(hit, DSPI_WIRE_OFF(global.loudness_ref_spl), 8);
+
+    // ---- gains, output rows and delays: the ingest's lane layout ----
+    const bool is_xp = lane < 2 * O, is_out = !is_xp && lane < 3 * O, is_pre = lane == 3 * O || lane == 3 * O + 1, is_mv = lane == 3 * O + 2;
+    const uint32_t side = is_xp ? lane / O : (uint32_t)(lane - 3 * O), o = is_xp ? lane % O : (uint32_t)(lane - 2 * O);
+    const uint32_t xp_off = DSPI_WIRE_OFF(crosspoints) + (side * WO + o) * 8, out_off = DSPI_WIRE_OFF(outputs) + o * 12;
+    const bool out_en_t = is_out && touched(hit, out_off, 4), out_gain_t = is_out && touched(hit, out_off + 4, 4);
+    const bool out_dly_t = is_out && touched(hit, out_off + 8, 4);
+    const bool flags_t = __ballot_sync(0xffffffffu, out_en_t) != 0 || bypass_t;                   // every output: pair-off bits and skip rows
+    const bool gains_t = __ballot_sync(0xffffffffu, out_en_t || out_gain_t) != 0 || mv_t || host_t;
+    const bool dly_t = __ballot_sync(0xffffffffu, out_dly_t) != 0;
+    if (is_xp) {
+        if (touched(hit, xp_off, 8)) S::crosspoint(d, inst, side, o, w[xp_off] != 0, w[xp_off + 1] != 0, gain_linear(wire_f32(w, xp_off + 4), gain_mode));
+    } else if (is_out) {
+        if (out_gain_t) d.o_glin[o * Np + inst] = gain_linear(wire_f32(w, out_off + 4), gain_mode);
+        if (flags_t) output_flag_rows<S>(d, w, inst, o, bypass_master);
+        if (out_dly_t) output_delay_row<S>(d, w, inst, o, fs);
+    } else if (is_pre) {
+        if (touched(hit, DSPI_WIRE_OFF(preamp.preamp_db) + side * 4, 4)) S::preamp(d, inst, side, gain_linear(wire_f32(w, DSPI_WIRE_OFF(preamp.preamp_db) + side * 4), gain_mode));
+    } else if (is_mv) {
+        if (mv_t) S::master_volume(d, inst, mv_lin);
+    }
+    __syncwarp();
+    const bool delayed = is_out && d.o_dly[o * Np + inst] > 0;                                     // the delays in force, touched or not
+    const bool any_delay = __ballot_sync(0xffffffffu, delayed) != 0;
+
+    // ---- the pending-flag handlers of the touched sections ----
+    const dspi_leveller_config lev = leveller_config(w, DSPI_WIRE_FORMAT_VERSION);
+    uint32_t row;
+    const int16_t vol_mul = dyn::host_volume(hv.volume_8_8, row);
+    if (lane == 0) {
+        if (xf_t) S::crossfeed(d, inst, crossfeed_config(w), fs);
+        if (flags_t || dly_t || xf_t || lev_t || loud_t) d.flags[inst] = instance_flags<S>(w, lev, any_delay);
+        if (bypass_t) d.skip_m[inst] = d.skip_m[Np + inst] = bypass_master ? 1 : 0;
+    } else if (lane == 1) {
+        if (lev_t) S::leveller(d, inst, lev, fs);
+    } else if (lane == 2) {
+        if (loud_t || vol_t) loudness_row<S>(d, w, inst, row, fs);
+    }
+    __syncwarp();
+    if (lane == 0 && gains_t) S::host_volume(d, inst, vol_mul, hv.host_mute != 0);
+
+    // ---- the touched bands' recipes and their masks ----
+    uint32_t m = 0;
+    if (lane < NC)
+        for (uint32_t b = 0; b < kMaxBands; b++)
+            if (touched(hit, DSPI_WIRE_OFF(eq) + (lane * kMaxBands + b) * 16, 16)) m |= 1u << b;
+    if (lane < NC) band_mask[lane * nseg + s] = (uint16_t)m;
+    const bool any_band = __ballot_sync(0xffffffffu, m != 0) != 0;
+    for (uint32_t r = lane; r < (uint32_t)NC * kMaxBands; r += 32)
+        if (touched(hit, DSPI_WIRE_OFF(eq) + r * 16, 16)) stage_recipe(w, r, s, nseg, recipes);
+    if (lane == 0) reject[s] = any_band ? 0 : 1;
+
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+        bulk_store_1d(rec.packets + inst, w, kPacketBytes);
+        tma_store_commit();
+        tma_store_wait_all<0>();
+    } else if (lane == 1) {
+        rec.host[inst] = hv;
+    }
+}
+
 // filter_recipes[][] of instances [inst0, inst0 + n) as dsp_compute_coefficients() left them -> the eq section of their records.
-// Recipe (role, i, band) is recipes[role * role_stride + i * inst_stride + band]; reject as in RoleRange.
+// Recipe (role, i, band) is recipes[role * role_stride + i * inst_stride + band]; reject, inst and band_mask as in RoleRange.
 static __global__ void record_recipes_kernel(Record rec, uint32_t inst0, uint32_t n, uint32_t roles, const dspi_eq_param *__restrict__ recipes,
-                                             size_t role_stride, size_t inst_stride, const int32_t *__restrict__ reject)
+                                             size_t role_stride, size_t inst_stride, const int32_t *__restrict__ reject,
+                                             const uint32_t *__restrict__ inst = nullptr, const uint16_t *__restrict__ band_mask = nullptr)
 {
     const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= n * roles * kMaxBands) return;
     const uint32_t b = idx % kMaxBands, role = idx / kMaxBands % roles, i = idx / (kMaxBands * roles);
     if (reject && reject[i]) return;
+    if (band_mask && !((band_mask[role * n + i] >> b) & 1u)) return;
     uint4 q = reinterpret_cast<const uint4 *>(recipes)[role * role_stride + i * inst_stride + b];
     q.x = (q.x >> 16) & 0xFFu;                                                                     // {channel, band, type, reserved} -> {type, reserved[3]}
-    unsigned char *rp = reinterpret_cast<unsigned char *>(rec.packets + inst0 + i);
+    unsigned char *rp = reinterpret_cast<unsigned char *>(rec.packets + inst0 + (inst ? inst[i] : i));
     reinterpret_cast<uint4 *>(rp + DSPI_WIRE_OFF(eq))[role * kMaxBands + b] = q;
 }
 
@@ -764,6 +948,37 @@ struct PresetStage {
     }
 };
 
+// engine-owned staging of the edit calls, next to Stage: one chunk of edits grouped by instance with its segment table, as
+// uploaded in one copy, and the band masks and marks of edit_kernel.  The host side keeps the upload image and, per
+// instance, 1 + its segment in the chunk being grouped (0 outside it).
+struct EditStage {
+    unsigned char *d_in = nullptr;                         // [E] edits, [nseg + 1] segment offsets, [nseg] instances
+    uint16_t *band_mask = nullptr;                         // [roles][kChunk]
+    int32_t *marks = nullptr;                              // [kChunk]
+    std::vector<unsigned char> h_in;
+    std::vector<uint32_t> seg, last, count, inst;
+    static constexpr size_t kInBytes = (size_t)kEditChunk * sizeof(dspi_bulk_edit) + (size_t)(2 * kChunk + 1) * sizeof(uint32_t);
+    cudaError_t ensure(int roles, uint32_t n_instances)
+    {
+        if (seg.size() < n_instances) seg.assign(n_instances, 0);
+        if (last.size() < n_instances) last.resize(n_instances);
+        if (marks) return cudaSuccess;
+        h_in.resize(kInBytes);
+        count.resize(kChunk);
+        inst.reserve(kChunk);
+        cudaError_t e = cudaMalloc((void **)&d_in, kInBytes);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&band_mask, (size_t)roles * kChunk * sizeof(uint16_t));
+        if (e == cudaSuccess) e = cudaMalloc((void **)&marks, (size_t)kChunk * sizeof(int32_t));
+        if (e != cudaSuccess) destroy();
+        return e;
+    }
+    void destroy()
+    {
+        cudaFree(d_in); cudaFree(band_mask); cudaFree(marks);
+        d_in = nullptr; band_mask = nullptr; marks = nullptr;
+    }
+};
+
 inline int fail_cuda(cudaError_t e, const char *what)
 {
     size_t cap = 0;
@@ -774,9 +989,11 @@ inline int fail_cuda(cudaError_t e, const char *what)
 
 // dsp_recalculate_all_filters() for instances [first, first + nc) whose recipes are in stage.recipes and whose code in
 // stage.results is 0 (the others are left alone): state into the mirrors, coefficients from the recipes at fs (or at
-// rates[i] when rates is not null), the clamped recipes into the records, mirrors back into the packed stores.
+// rates[i] when rates is not null), the clamped recipes into the records, mirrors back into the packed stores.  With `inst`
+// (device, [nc]) instance i is first + inst[i]; with `band_mask` (device, [roles][nc]) only the masked bands are computed.
 template <class S, class Engine>
-int recalculate_filters(Engine *c, Stage &stage, uint32_t first, uint32_t nc, float fs, const float *rates)
+int recalculate_filters(Engine *c, Stage &stage, uint32_t first, uint32_t nc, float fs, const float *rates, const uint32_t *inst = nullptr,
+                        const uint16_t *band_mask = nullptr)
 {
     cudaStream_t s = c->stream;
     RoleRange rm, ro;
@@ -784,6 +1001,9 @@ int recalculate_filters(Engine *c, Stage &stage, uint32_t first, uint32_t nc, fl
     rm.stride = ro.stride = c->d.N_pad;
     rm.reject = ro.reject = stage.results;
     rm.fs = ro.fs = rates;
+    rm.inst = ro.inst = inst;
+    rm.band_mask = band_mask;
+    ro.band_mask = band_mask ? band_mask + (size_t)2 * nc : nullptr;
     int rc = eq_unpack_range(c->eq_m, first, nc, s, rm);
     if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, first, nc, s, ro);
     if (rc != DSPI_OK) return rc;
@@ -791,7 +1011,7 @@ int recalculate_filters(Engine *c, Stage &stage, uint32_t first, uint32_t nc, fl
     if (e == cudaSuccess) e = launch_coeffs(S::kQ28, stage.recipes + (size_t)2 * nc * kMaxBands, eq_aos_mirror(c->eq_o), first, nc, fs, s, ro);
     if (e != cudaSuccess) return fail_cuda(e, "coefficient kernels");
     record_recipes_kernel<<<(nc * S::kRoles * kMaxBands + 255) / 256, 256, 0, s>>>(c->rec, first, nc, S::kRoles, stage.recipes,
-                                                                                   (size_t)nc * kMaxBands, kMaxBands, stage.results);
+                                                                                   (size_t)nc * kMaxBands, kMaxBands, stage.results, inst, band_mask);
     if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "recipe record kernel");
     c->launches += 3;
     rc = eq_pack_range(c->eq_m, first, nc, s, rm);
@@ -858,6 +1078,100 @@ int set_rate(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const float *r
             return fail_cuda(e, "result copy");
     }
     return finish_skip(c);
+}
+
+// dspi_chain(q)_edit_bulk_device for checked arguments.  Edits of different instances commute, so the list is cut into
+// chunks by instance: a chunk takes the pending edits of the first kChunk instances it meets, at most kEditChunk edits, and
+// leaves the others for later chunks; an instance's edits keep their list order within and across chunks.  Per chunk the
+// edits are grouped by instance on the host - a stable counting pass, segments in order of first appearance - and uploaded
+// with their segment table in one copy; edit_kernel applies them, and when an edit of the chunk lies in the eq section the
+// touched bands go through the filter recalculation by instance list and band mask.  eq_set_skip at the end follows the
+// skip rows and synchronises.  results (host, may be null) gets the mark of each edit's instance.
+template <class S, class Engine>
+int edit(Engine *c, Stage &stage, EditStage &es, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float fs, int32_t *results)
+{
+    cudaError_t e = stage.ensure(S::kRoles);
+    if (e == cudaSuccess) e = es.ensure(S::kRoles, c->desc.n_instances);
+    if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
+    cudaStream_t s = c->stream;
+    constexpr uint32_t eq0 = DSPI_WIRE_OFF(eq), eq1 = DSPI_WIRE_OFF(eq) + S::kRoles * kMaxBands * 16;
+    std::vector<int32_t> marks;                            // per segment of the call (never more than the edits)
+    std::vector<uint32_t> seg_of(results ? n_edits : 0);   // per edit: its segment
+    if (results) marks.reserve(n_edits);
+    // per instance its last edit, so that a chunk holding kChunk instances stops scanning after their last edit
+    for (uint32_t k = 0; k < n_edits; k++) es.last[edits[k].instance] = k;
+    std::vector<uint32_t> pending(n_edits), taken, later;
+    for (uint32_t k = 0; k < n_edits; k++) pending[k] = k;
+    taken.reserve(n_edits < kEditChunk ? n_edits : kEditChunk);
+    while (!pending.empty()) {
+        // the chunk: in list order, every pending edit of the first kChunk instances met, at most kEditChunk edits; the
+        // edits of other instances wait for a later chunk, so each instance's edits keep their order
+        uint32_t nseg = 0, stop = 0;
+        bool bands = false;
+        es.inst.clear();
+        taken.clear();
+        later.clear();
+        size_t p = 0;
+        for (; p < pending.size(); p++) {
+            const uint32_t k = pending[p];
+            if (taken.size() == kEditChunk || (nseg == kChunk && k > stop)) break;
+            const dspi_bulk_edit &ed = edits[k];
+            uint32_t &sl = es.seg[ed.instance];
+            if (!sl) {
+                if (nseg == kChunk) {
+                    later.push_back(k);
+                    continue;
+                }
+                es.inst.push_back(ed.instance);
+                es.count[nseg] = 0;
+                sl = ++nseg;
+                stop = std::max(stop, es.last[ed.instance]);
+            }
+            es.count[sl - 1]++;
+            taken.push_back(k);
+            bands |= ed.offset < eq1 && ed.offset + ed.length > eq0;
+        }
+        later.insert(later.end(), pending.begin() + p, pending.end());
+        pending.swap(later);
+        const uint32_t E = (uint32_t)taken.size();
+        // upload image: edits grouped by segment, then the segment offsets, then the segments' instances
+        dspi_bulk_edit *ed_h = reinterpret_cast<dspi_bulk_edit *>(es.h_in.data());
+        uint32_t *off_h = reinterpret_cast<uint32_t *>(es.h_in.data() + (size_t)E * sizeof(dspi_bulk_edit));
+        for (uint32_t g = 0, acc = 0; g <= nseg; g++) {
+            off_h[g] = acc;
+            if (g < nseg) acc += es.count[g];
+        }
+        memcpy(es.count.data(), off_h, (size_t)nseg * sizeof(uint32_t));                          // now each segment's write cursor
+        const size_t base = marks.size();
+        for (const uint32_t k : taken) {
+            const uint32_t g = es.seg[edits[k].instance] - 1;
+            ed_h[es.count[g]++] = edits[k];
+            if (results) seg_of[k] = (uint32_t)base + g;
+        }
+        for (uint32_t g = 0; g < nseg; g++) es.seg[es.inst[g]] = 0;
+        memcpy(off_h + nseg + 1, es.inst.data(), (size_t)nseg * sizeof(uint32_t));
+        const size_t bytes = (size_t)E * sizeof(dspi_bulk_edit) + (size_t)(2 * nseg + 1) * sizeof(uint32_t);
+        if ((e = cudaMemcpyAsync(es.d_in, es.h_in.data(), bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return fail_cuda(e, "edit copy");
+        const dspi_bulk_edit *d_edits = reinterpret_cast<const dspi_bulk_edit *>(es.d_in);
+        const uint32_t *d_off = reinterpret_cast<const uint32_t *>(es.d_in + (size_t)E * sizeof(dspi_bulk_edit)), *d_inst = d_off + nseg + 1;
+        edit_kernel<S><<<(nseg + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, nseg, d_edits, d_off, d_inst, exact_db ? kGainExact : kGainTaylor,
+                                                                           fs, stage.recipes, es.band_mask, stage.results, es.marks);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "edit kernel");
+        c->launches++;
+        if (bands) {
+            const int rc = recalculate_filters<S>(c, stage, 0, nseg, fs, nullptr, d_inst, es.band_mask);
+            if (rc != DSPI_OK) return rc;
+        }
+        if (results) {
+            marks.resize(base + nseg);
+            if ((e = cudaMemcpyAsync(marks.data() + base, es.marks, (size_t)nseg * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
+                return fail_cuda(e, "mark copy");
+        }
+    }
+    const int rc = finish_skip(c);
+    if (rc != DSPI_OK) return rc;
+    for (uint32_t k = 0; results && k < n_edits; k++) results[k] = marks[seg_of[k]];
+    return DSPI_OK;
 }
 
 // dspi_chain(q)_apply_bulk_device for checked arguments

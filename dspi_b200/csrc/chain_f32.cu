@@ -982,6 +982,11 @@ int dspi_chain_set_rate_device(dspi_chain *c, uint32_t inst0, uint32_t n, const 
     return dspi::set_rate_device(c, inst0, n, sample_rates, results);
 }
 
+int dspi_chain_edit_bulk_device(dspi_chain *c, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results)
+{
+    return dspi::edit_bulk_device(c, n_edits, edits, exact_db, sample_rate, results);
+}
+
 int dspi_chain_collect_bulk_device(dspi_chain *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
 {
     return dspi::collect_bulk_device(c, inst0, n, packets, host, results);

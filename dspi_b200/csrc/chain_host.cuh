@@ -96,6 +96,7 @@ struct ChainHost {
     ResponseBuffers resp;            // frequency table of *_response_*; host staging of *_response_host and the instance image calls
     bulk::Stage bulk;                // device staging of *_apply_bulk_device / _collect_bulk_device, allocated by the first call
     bulk::PresetStage preset;        // device staging of *_apply_preset_device / _collect_preset_device, allocated by the first call
+    bulk::EditStage bulk_edit;       // staging of *_edit_bulk_device, allocated by the first call
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
     IndexLists copy_lists;           // device instance lists of *_copy_instances, allocated by the first call
 };
@@ -269,6 +270,7 @@ int destroy(H *c)
     c->resp.destroy();
     c->bulk.destroy();
     c->preset.destroy();
+    c->bulk_edit.destroy();
     c->copy_lists.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
@@ -581,6 +583,30 @@ int set_rate_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *sa
     if (n == 0) return DSPI_OK;
     CU_OK(cudaSetDevice(c->desc.device));
     return bulk::set_rate<typename A::Stores>(c, c->bulk, inst0, n, sample_rates, results);
+}
+
+template <class A>
+int edit_bulk_device(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results)
+{
+    if (!c || !edits) return fail(DSPI_EINVAL, "null argument");
+    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
+    // control-plane sections: the record keeps them zero and the collect kernel stamps them
+    static const uint32_t kPlane[][2] = { { 0, 16 },
+                                          { offsetof(dspi_wire_bulk_params, pins), offsetof(dspi_wire_bulk_params, eq) },
+                                          { offsetof(dspi_wire_bulk_params, channel_names), offsetof(dspi_wire_bulk_params, leveller) } };
+    for (uint32_t k = 0; k < n_edits; k++) {
+        const dspi_bulk_edit &e = edits[k];
+        const uint32_t lo = e.offset, hi = (uint32_t)e.offset + e.length;
+        if (e.length == 0 || e.length > sizeof(e.bytes) || e.reserved)
+            return fail(DSPI_EINVAL, "edit %u: length %u (1 .. 24) or reserved %u (0)", k, e.length, e.reserved);
+        if (hi > bulk::kEditSpace) return fail(DSPI_EINVAL, "edit %u: bytes [%u, %u) past the %u-byte configuration", k, lo, hi, bulk::kEditSpace);
+        for (const auto &p : kPlane)
+            if (lo < p[1] && hi > p[0]) return fail(DSPI_EINVAL, "edit %u: bytes [%u, %u) touch a control-plane section", k, lo, hi);
+        if (e.instance >= c->desc.n_instances) return fail(DSPI_ERANGE, "edit %u names instance %u, outside engine of %u", k, e.instance, c->desc.n_instances);
+    }
+    if (n_edits == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    return bulk::edit<typename A::Stores>(c, c->bulk, c->bulk_edit, n_edits, edits, exact_db, sample_rate, results);
 }
 
 template <class A>

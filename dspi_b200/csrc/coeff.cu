@@ -88,16 +88,29 @@ __device__ void cookbook(const dspi_eq_param &p, float A, float fs, float (&n)[3
     }
 }
 
+// thread i = channel * 12 + band of role blockIdx.y: inside the range, not rejected, and in the band mask if there is one
+__device__ __forceinline__ bool band_selected(uint32_t i, uint32_t n, const RoleRange &rr)
+{
+    if (i >= n * kMaxBands || (rr.reject && rr.reject[i / kMaxBands])) return false;
+    return !rr.band_mask || ((rr.band_mask[(size_t)blockIdx.y * n + i / kMaxBands] >> (i % kMaxBands)) & 1u);
+}
+// its biquad in the role's rows: channel i / 12 of the range, or inst[i / 12] of a list
+__device__ __forceinline__ size_t band_index(uint32_t i, const RoleRange &rr)
+{
+    return rr.inst ? (size_t)rr.inst[i / kMaxBands] * kMaxBands + i % kMaxBands : (size_t)i;
+}
+
 __global__ void __launch_bounds__(256)
 coeff_f32_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_f32 *__restrict__ aos, uint32_t ch0, uint32_t n, float fs, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * kMaxBands || (rr.reject && rr.reject[i / kMaxBands])) return;
+    if (!band_selected(i, n, rr)) return;
     if (rr.fs) fs = rr.fs[i / kMaxBands];
     recipes += (size_t)blockIdx.y * n * kMaxBands;
     aos += ((size_t)ch0 + (size_t)blockIdx.y * rr.stride) * kMaxBands;
     dspi_eq_param p = recipes[i];
-    dspi_biquad_f32 bq = aos[i];
+    dspi_biquad_f32 &dst = aos[band_index(i, rr)];
+    dspi_biquad_f32 bq = dst;
     if (recipe_is_flat(p) || fs == 0.0f) {                                   // :62-73
         bq.bypass = 1;
         bq.use_svf = 0;
@@ -152,7 +165,7 @@ coeff_f32_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_f32 *__restric
         }
     }
     recipes[i] = p;
-    aos[i] = bq;
+    dst = bq;
 }
 
 // (int32_t) cast with the firmware's saturating semantics (:168-173 run on the RP2040's soft float)
@@ -167,12 +180,13 @@ __global__ void __launch_bounds__(256)
 coeff_q28_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_q28 *__restrict__ aos, uint32_t ch0, uint32_t n, float fs, RoleRange rr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * kMaxBands || (rr.reject && rr.reject[i / kMaxBands])) return;
+    if (!band_selected(i, n, rr)) return;
     if (rr.fs) fs = rr.fs[i / kMaxBands];
     recipes += (size_t)blockIdx.y * n * kMaxBands;
     aos += ((size_t)ch0 + (size_t)blockIdx.y * rr.stride) * kMaxBands;
     dspi_eq_param p = recipes[i];
-    dspi_biquad_q28 bq = aos[i];
+    dspi_biquad_q28 &dst = aos[band_index(i, rr)];
+    dspi_biquad_q28 bq = dst;
     if (recipe_is_flat(p) || fs == 0.0f) {
         bq.bypass = 1;
         bq.b0 = 1 << 28;
@@ -190,7 +204,7 @@ coeff_q28_kernel(dspi_eq_param *__restrict__ recipes, dspi_biquad_q28 *__restric
         bq.a2 = to_q28(fdiv(dd[2], dd[0]));
     }
     recipes[i] = p;
-    aos[i] = bq;
+    dst = bq;
 }
 
 }  // namespace

@@ -48,12 +48,15 @@ char *error_buffer(size_t *cap);
 // reject[i] != 0 (device memory, [n], or nullptr) leaves channel i of every role untouched.  fs (device memory, [n], or
 // nullptr) gives channel i of every role its own sample rate in the coefficient kernels, in place of their scalar one.
 // inst (device memory, [n], or nullptr) turns the range into a list: channel i of role r is ch0 + r * stride + inst[i]
-// (pack / unpack kernels only; the chain engines' copy of scattered instances).  The default is one plain range.
+// (pack / unpack and coefficient kernels; the chain engines' copy and edit of scattered instances).  band_mask (device
+// memory, [roles][n], or nullptr): the coefficient kernels compute band b of channel i of role r only where bit b of
+// band_mask[r * n + i] is set, and leave the other bands and their recipes alone.  The default is one plain range.
 struct RoleRange {
     uint32_t roles = 1, stride = 0;
     const int32_t *reject = nullptr;
     const float *fs = nullptr;
     const uint32_t *inst = nullptr;
+    const uint16_t *band_mask = nullptr;
 };
 
 // K1 — float cascade.  cpl: channels per lane (1, or 2 held in a register pair)

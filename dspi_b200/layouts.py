@@ -180,3 +180,44 @@ BULK_CURRENT, BULK_STALE, BULK_UNSET = 0, 1, 2
 # dspi_preset_load: per instance, what preset_load() gets from its caller and the preset directory
 PRESET_LOAD = np.dtype([("slot_index", "u1"), ("master_volume_mode", "u1"), ("reserved", "u1", (2,)), ("dir_master_volume_db", "<f4")])
 assert PRESET_LOAD.itemsize == 8
+
+# dspi_bulk_edit (include/dspi_b200.h): `length` bytes at `offset` of one instance's configuration, in the address space
+# WIRE_BULK [0, 2896) followed by BULK_HOST [2896, 2900) (edit_bulk_device)
+BULK_EDIT = np.dtype([("instance", "<u4"), ("offset", "<u2"), ("length", "u1"), ("reserved", "u1"), ("bytes", "u1", (24,))])
+assert BULK_EDIT.itemsize == 32
+BULK_EDIT_SPACE = WIRE_BULK.itemsize + BULK_HOST.itemsize
+
+
+def edit_field(path):
+    """(offset, dtype) of a field of the edit address space, from its path through WIRE_BULK, or through BULK_HOST after
+    "host": ``("outputs", 3, "gain_db")``, ``("eq", ch, b)``, ``("crosspoints", side, o)``, ``("host", "volume_8_8")``.
+    Integers index array dimensions in order; the offsets are the dtypes' own."""
+    path = tuple(path)
+    dt, off = (BULK_HOST, WIRE_BULK.itemsize) if path[:1] == ("host",) else (WIRE_BULK, 0)
+    shape = ()
+    for p in path[1:] if path[:1] == ("host",) else path:
+        if isinstance(p, str):
+            if shape:
+                raise ValueError(f"{path}: {p!r} needs the array index first")
+            sub, o = dt.fields[p][:2]
+            off += o
+            dt, shape = (sub.base, sub.shape) if sub.subdtype else (sub, ())
+        else:
+            if not shape or not 0 <= int(p) < shape[0]:
+                raise ValueError(f"{path}: index {p} out of range")
+            shape = shape[1:]
+            off += int(p) * int(np.prod(shape, dtype=np.int64)) * dt.itemsize
+    return off, (np.dtype((dt, shape)) if shape else dt)
+
+
+def bulk_edit(instance, path, value):
+    """BULK_EDIT [1]: write ``value`` (in the field's own dtype, or raw bytes) into the field at ``path`` (see
+    ``edit_field``) of ``instance``."""
+    off, dt = edit_field(path)
+    raw = bytes(value) if isinstance(value, (bytes, bytearray)) else np.asarray(value, dt).tobytes()
+    if not 1 <= len(raw) <= 24 or (not isinstance(value, (bytes, bytearray)) and len(raw) != dt.itemsize):
+        raise ValueError(f"{path}: {len(raw)} bytes; an edit carries 1 .. 24 bytes of one field")
+    e = np.zeros(1, BULK_EDIT)
+    e["instance"], e["offset"], e["length"] = instance, off, len(raw)
+    e["bytes"][0, :len(raw)] = np.frombuffer(raw, np.uint8)
+    return e

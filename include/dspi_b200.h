@@ -723,6 +723,60 @@ int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, 
 int dspi_chain_set_rate_device (dspi_chain *c,  uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results);
 int dspi_chainq_set_rate_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results);
 
+/* One edit: `length` bytes at `offset` of an instance's configuration, in the address space
+ *   [0, 2896)      dspi_wire_bulk_params (the packet _collect_bulk_device returns)
+ *   [2896, 2900)   dspi_bulk_host        (host volume_8_8, host_mute) */
+typedef struct { uint32_t instance; uint16_t offset; uint8_t length; uint8_t reserved; uint8_t bytes[24]; } dspi_bulk_edit;  /* 32 B */
+#ifdef __cplusplus
+static_assert(sizeof(dspi_bulk_edit) == 32, "dspi_bulk_edit");
+#else
+_Static_assert(sizeof(dspi_bulk_edit) == 32, "dspi_bulk_edit");
+#endif
+/* Single fields of many instances' configuration, edited ON THE GPU: what a DSPi Console sends while a user drags an EQ
+ * band, a fader, an output gain, a mute or a crosspoint.  edits[n_edits] and results[n_edits] are host memory; results
+ * may be NULL.
+ *   - Reference semantics.  Take a DSPI_BULK_CURRENT instance, P the packet _collect_bulk_device returns for it and H its
+ *     host record.  Write the call's edits for that instance over (P, H) in list order (the last write to a byte wins).
+ *     The instance's configuration record, host record and mark then become exactly what _apply_bulk_device(P', H',
+ *     exact_db, sample_rate) would leave, and so do its derived rows for every field an edit touched.
+ *   - A field is touched when any edit writes any byte of it, whatever the value.  The record is normalised as
+ *     _apply_bulk_device leaves it: flags 0 / 1, reserved bytes zero, global.preamp_gain_db mirroring preamp_db[0],
+ *     channel_delays_ms following the output delays, the master volume finite and clamped to [-128, 0] dB, rows past the
+ *     shape's channel and output counts zero.
+ *   - What a touched field re-derives (the rows bulk_params_apply() and the main loop's handlers write from it):
+ *       crosspoint                          its gain row
+ *       output enabled / mute               every output's flags (the partner's pair-off bit), the sub-on flag bit, skip rows
+ *       output gain_db                      its linear gain
+ *       output delay_ms                     its delay in samples at sample_rate, the any_delay flag bit
+ *       preamp_db[side]                     that preamp row
+ *       master_volume_db                    the master gain, always with the exact conversion
+ *       output enable / mute / gain, master volume, host volume or mute:   the output gain rows (audio_set_volume())
+ *       host volume_8_8                     also the loudness row it selects
+ *       global.bypass                       its flag bit, the master skip rows and the output skip rows
+ *       loudness enabled / ref / intensity  its flag bit and the loudness row
+ *       any crossfeed byte                  coefficients at sample_rate with the filter state cleared, its flag bit
+ *       any leveller byte                   coefficients at sample_rate, its flag bits
+ *       eq[ch][b]                           that band's coefficients at sample_rate, its clamped recipe written back
+ *     Legacy fields and the master channels' delays.delay_ms[0..1] change the record only, as an apply does with them.
+ *   - A field no edit touched is not re-derived: gains keep the values they have, whichever conversion made them (Taylor,
+ *     exact or preset flash), and untouched bands keep coefficients and state byte for byte, even when sample_rate differs
+ *     from the rate they were computed at.
+ *   - Running state: EQ state is kept unless a touched band flips between SVF and TDF2; the crossfeed filter state is
+ *     cleared only when a crossfeed byte is touched, so unlike _apply_bulk_device and _set_dynamics_device a host-volume or
+ *     gain edit keeps it; leveller, loudness-shelf, delay-line and modulator state, the meters, the preset-mute gain,
+ *     envelope and mode and the S/PDIF transmitter are left alone.
+ *   - Edits for a DSPI_BULK_STALE or DSPI_BULK_UNSET instance change nothing of it; results[k] is the mark of edit k's
+ *     instance at the call's point in the stream.  The call still returns DSPI_OK.
+ *   - Errors, all checked before anything is written: DSPI_EINVAL for a NULL engine or edits, a sample_rate that is not
+ *     positive and finite, a length of 0 or above 24, a non-zero reserved byte, a span past 2900 bytes, or a span that
+ *     touches the header, pins, channel_names or i2s_config (control plane: the record keeps them zero and collect stamps
+ *     them); DSPI_ERANGE for an instance at or above n_instances.  n_edits == 0 does nothing.
+ * Arithmetic and libm policy as _apply_bulk_device.  One sample_rate per call: a farm issues one call per clock group.
+ * Ordered behind everything issued earlier on the engine stream, asynchronous process calls included; returns when the
+ * engine is updated, and edits can be reused then. */
+int dspi_chain_edit_bulk_device (dspi_chain *c,  uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results);
+int dspi_chainq_edit_bulk_device(dspi_chainq *c, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results);
+
 /* ---- preset slot images (SURVEY.md 8 f-4): PresetSlot v12, flash_storage.c:139-189 ------------ */
 /* One flash sector per slot: 12-byte header (magic "DSP3", data version, slot index, CRC-32 of everything
  * after the header) + the packed DSP state.  Device preset dumps load directly into a dspi_bulk_state and
