@@ -58,6 +58,10 @@ SYMBOLS = [
     "dspi_chain_process_subframes_range_host", "dspi_chain_process_subframes_range_device",
     "dspi_chainq_process_packets_range_host", "dspi_chainq_process_packets_range_device",
     "dspi_chainq_process_subframes_range_host", "dspi_chainq_process_subframes_range_device",
+    "dspi_chain_lane_open", "dspi_chain_lane_close", "dspi_chain_lane_process_packets_device", "dspi_chain_lane_process_subframes_device",
+    "dspi_chain_lane_stream", "dspi_chain_lane_sync",
+    "dspi_chainq_lane_open", "dspi_chainq_lane_close", "dspi_chainq_lane_process_packets_device", "dspi_chainq_lane_process_subframes_device",
+    "dspi_chainq_lane_stream", "dspi_chainq_lane_sync",
 ]
 
 
@@ -164,6 +168,12 @@ def lib():
             for form in ("packets", "subframes"):
                 for where in ("host", "device"):
                     getattr(h, "%s_process_%s_range_%s" % (pre, form, where)).argtypes = [vp, u32, u32, vp, u32, u32, vp, vp, vp, vp]
+                getattr(h, "%s_lane_process_%s_device" % (pre, form)).argtypes = [vp, u32, u32, u32, vp, u32, u32, vp, vp, vp, vp]
+            getattr(h, pre + "_lane_open").argtypes = [vp, u32, u32, vp]
+            getattr(h, pre + "_lane_close").argtypes = [vp, u32]
+            getattr(h, pre + "_lane_stream").argtypes = [vp, u32]
+            getattr(h, pre + "_lane_stream").restype = vp
+            getattr(h, pre + "_lane_sync").argtypes = [vp, u32]
         for pre in ("dspi_eq", "dspi_chain", "dspi_chainq"):
             getattr(h, pre + "_response_host").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
             getattr(h, pre + "_response_device").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
@@ -766,6 +776,39 @@ class _ChainEngine:
                                                     C.c_void_p(int(subframes_ptr)) if subframes_ptr else None,
                                                     C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
                                                     C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def lane_open(self, inst0, n):
+        """Open a lane over instances [inst0, inst0+n) (inst0 a multiple of 64, no overlap with an open lane's window): an issue
+        queue whose calls run concurrently with other lanes' calls.  Returns the lane id."""
+        lane = C.c_uint32()
+        _check(self._fn("lane_open")(self._h, int(inst0), int(n), C.byref(lane)))
+        return lane.value
+
+    def lane_close(self, lane):
+        """Wait for the lane's calls and free its streams."""
+        _check(self._fn("lane_close")(self._h, int(lane)))
+
+    def _lane_process(self, form, lane, inst0, n, pcm_ptr, bit_depth, packet_frames, out_ptr, pdm_ptr, status_ptr):
+        t, _ = _packet_table(packet_frames)
+        _check(self._fn("lane_process_%s_device" % form)(self._h, int(lane), int(inst0), int(n), C.c_void_p(int(pcm_ptr)), bit_depth, t.size,
+                                                         t.ctypes.data, C.c_void_p(int(out_ptr)) if out_ptr else None,
+                                                         C.c_void_p(int(pdm_ptr)) if pdm_ptr else None,
+                                                         C.c_void_p(int(status_ptr)) if status_ptr else None))
+
+    def lane_process_packets_device(self, lane, inst0, n, pcm_ptr, bit_depth, packet_frames, spdif_ptr=0, pdm_ptr=0, status_ptr=0):
+        """``process_packets_range_device`` issued on a lane (the range inside its window), asynchronous on ``lane_stream(lane)``."""
+        self._lane_process("packets", lane, inst0, n, pcm_ptr, bit_depth, packet_frames, spdif_ptr, pdm_ptr, status_ptr)
+
+    def lane_process_subframes_device(self, lane, inst0, n, pcm_ptr, bit_depth, packet_frames, subframes_ptr=0, pdm_ptr=0, status_ptr=0):
+        """``process_subframes_range_device`` issued on a lane (the range inside its window), asynchronous on ``lane_stream(lane)``."""
+        self._lane_process("subframes", lane, inst0, n, pcm_ptr, bit_depth, packet_frames, subframes_ptr, pdm_ptr, status_ptr)
+
+    def lane_stream(self, lane):
+        """The stream where the lane's outputs become visible (None for a lane that is not open)."""
+        return self._fn("lane_stream")(self._h, int(lane))
+
+    def lane_sync(self, lane):
+        _check(self._fn("lane_sync")(self._h, int(lane)))
 
 
 class ChainEngine(_ChainEngine):

@@ -73,6 +73,26 @@ struct IndexLists {
     }
 };
 
+// Where a process call is issued: its stage streams and events, its packet schedule, and the stream it starts from and
+// joins back to.  The engine's own calls issue on the engine context (c->stream, c->st, c->sched), a lane's on the lane's.
+struct Issue {
+    cudaStream_t stream;
+    ChainStreams &st;
+    PacketSchedule &sched;
+};
+
+// A lane (dspi_chain_lane_*): an issue queue of its own, bound to the instance window [inst0, inst0 + n).  Its calls start
+// behind the engine stream as it was when they were issued (ev_engine) and end with ev_last, which engine-level calls
+// wait for (join_lanes).
+struct Lane {
+    bool open = false;
+    uint32_t inst0 = 0, n = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev_engine = nullptr, ev_last = nullptr;
+    ChainStreams st;
+    PacketSchedule sched;
+};
+
 // One engine: dspi_chain and dspi_chainq are this record for their arithmetic.
 template <class A>
 struct ChainHost {
@@ -80,6 +100,7 @@ struct ChainHost {
     dspi_chain_desc desc;
     typename A::Dev d;
     cudaStream_t stream;             // the engine stream callers see; stages run on st.* between ev_begin and ev_done
+    SmPartition part;                // the modulator's SMs and the rest, shared by the engine's and the lanes' stage streams
     ChainStreams st;
     typename A::Biquad *d_aos;       // [N_pad][roles][12] instance-major mirror of filters[][]
     dspi_eq *eq_m, *eq_o;            // EQ engines over the master rows (2 N_pad channels) and the output rows (kOuts N_pad)
@@ -99,7 +120,48 @@ struct ChainHost {
     bulk::EditStage bulk_edit;       // staging of *_edit_bulk_device, allocated by the first call
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
     IndexLists copy_lists;           // device instance lists of *_copy_instances, allocated by the first call
+    Lane lanes[DSPI_CHAIN_MAX_LANES];
+    uint32_t open_lanes;
 };
+
+// Engine-level calls run after every lane call issued before them: the engine stream waits for each open lane's last
+// call.  Every engine-level entry point passes its handle through here; with no lane open it does nothing.
+template <class H>
+H *join_lanes(H *c)
+{
+    if (!c || !c->open_lanes) return c;
+    cudaSetDevice(c->desc.device);
+    for (Lane &l : c->lanes)
+        if (l.open && cudaStreamWaitEvent(c->stream, l.ev_last, 0) != cudaSuccess) {
+            cudaGetLastError();
+            cudaStreamSynchronize(l.stream);                                // the same order, from the host
+        }
+    return c;
+}
+
+// everything issued so far, on the engine stream and on every lane, has finished (before engine-owned buffers that lane
+// calls read are reallocated)
+template <class A>
+cudaError_t drain(ChainHost<A> *c)
+{
+    for (Lane &l : c->lanes)
+        if (l.open) {
+            const cudaError_t e = cudaStreamSynchronize(l.stream);
+            if (e != cudaSuccess) return e;
+        }
+    return cudaStreamSynchronize(c->stream);
+}
+
+void lane_release(Lane &l)
+{
+    if (l.stream) cudaStreamSynchronize(l.stream);
+    l.st.destroy();
+    l.sched.destroy();
+    for (cudaEvent_t *ev : { &l.ev_engine, &l.ev_last })
+        if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
+    if (l.stream) { cudaStreamDestroy(l.stream); l.stream = nullptr; }
+    l.open = false;
+}
 
 template <class A, typename T>
 cudaError_t dev_alloc(ChainHost<A> *c, T **p, size_t count, bool zero = true)
@@ -265,7 +327,10 @@ int destroy(H *c)
     if (!c) return DSPI_OK;
     cudaSetDevice(c->desc.device);
     if (c->stream) cudaStreamSynchronize(c->stream);
+    for (Lane &l : c->lanes) lane_release(l);
+    c->open_lanes = 0;
     c->st.destroy();
+    c->part.destroy();
     c->sched.destroy();
     c->resp.destroy();
     c->bulk.destroy();
@@ -322,7 +387,14 @@ int create(H **out, const dspi_chain_desc *desc)
         if (rc != DSPI_OK) { destroy(c); return rc; }
     }
     cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = c->st.create(desc->device, desc->n_instances);
+    if (e == cudaSuccess) e = c->part.create(desc->device, desc->n_instances);
+    if (e == cudaSuccess) e = c->st.create(c->part);
+    if (e != cudaSuccess && c->part.g_pdm) {                                // no streams in the partition: run without one
+        cudaGetLastError();
+        c->st.destroy();
+        c->part.destroy();
+        e = c->st.create(c->part);
+    }
 #define TRY(x) if (e == cudaSuccess) e = (x)
     TRY(c->sched.create(d.max_frames));
     d.off = c->sched.d_off;
@@ -728,12 +800,12 @@ int check_process(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t
 }
 
 template <class A>
-int check_packets(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames)
+int check_packets(ChainHost<A> *c, PacketSchedule &ps, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames)
 {
-    if (!c || !pcm) return fail(DSPI_EINVAL, "null argument");
+    if (!pcm) return fail(DSPI_EINVAL, "null argument");
     if (bit_depth != 16 && bit_depth != 24) return fail(DSPI_EINVAL, "bit_depth must be 16 or 24");
     const char *why = "";
-    const int rc = c->sched.check(n_packets, packet_frames, &why);
+    const int rc = ps.check(n_packets, packet_frames, &why);
     if (rc == DSPI_ERANGE) return fail(rc, "%s %u", why, c->desc.max_frames);
     return rc ? fail(rc, "%s", why) : DSPI_OK;
 }
@@ -754,16 +826,16 @@ int eq_stage(ChainHost<A> *c, dspi_eq *eq, uint32_t roles, void *rows, uint32_t 
     return DSPI_OK;
 }
 
-// One call over instances [inst0, inst0 + n) and the schedule c->sched has checked, with the kernel set K: its offsets go
-// to the device first, on the engine stream.  The caller's buffers hold rows for the n instances.  d_spdif: words, or
-// subframes when `subframes` is set (either may be NULL).
+// One call over instances [inst0, inst0 + n) and the schedule x.sched has checked, with the kernel set K, issued on the
+// context x: its offsets go to the device first, on x.stream, where the call also ends.  The caller's buffers hold rows for
+// the n instances.  d_spdif: words, or subframes when `subframes` is set (either may be NULL).
 template <class A, class K>
-int run_stages(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames, void *d_spdif,
-               bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
+int run_stages(ChainHost<A> *c, const Issue &x, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames,
+               void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
 {
-    PacketSchedule &ps = c->sched;
+    PacketSchedule &ps = x.sched;
     const uint32_t n_packets = ps.n_packets, F = ps.frames;
-    CU_OK(ps.upload(packet_frames, c->stream, &c->launches));
+    CU_OK(ps.upload(packet_frames, x.stream, &c->launches));
     const size_t post_smem = (size_t)4 * 2 * ps.longest * A::kXs * 4;      // 4 warps x (longest packet + look-ahead columns)
     static PerDeviceOnce once;                                              // per kernel set
     int dev = 0;
@@ -773,30 +845,31 @@ int run_stages(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *d_pcm, u
     }
     // Stage pipeline over packet slices on three streams (chain_streams.cuh): front stages of slice
     // i+1 overlap the output stages of slice i and the modulator of slice i-1.
-    ChainStreams &st = c->st;
+    ChainStreams &st = x.st;
     uint32_t slice_bounds[ChainStreams::kMaxSlices + 1];
     const uint32_t n_slices = (uint32_t)ChainStreams::plan_slices(n_packets, slice_bounds);
+    if (c->env_instances && c->vmm_packets < n_packets) {                    // the table every context's calls read
+        CU_OK(drain(c));
+        if (c->d.vmm) CU_OK(cudaFree(c->d.vmm));
+        c->d.vmm = nullptr; c->vmm_packets = 0;
+        CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(*c->d.vmm)));
+        c->vmm_packets = n_packets;
+    }
+    typename A::Dev d = c->d;
+    d.off = ps.d_off;
     if (c->env_instances) {                                                  // preset-mute envelope: this call's per-packet volumes
-        if (c->vmm_packets < n_packets) {
-            CU_OK(cudaStreamSynchronize(c->stream));
-            if (c->d.vmm) CU_OK(cudaFree(c->d.vmm));
-            c->d.vmm = nullptr; c->vmm_packets = 0;
-            CU_OK(cudaMalloc((void **)&c->d.vmm, (size_t)n_packets * c->d.N_pad * sizeof(*c->d.vmm)));
-            c->vmm_packets = n_packets;
-        }
-        K::env<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, inst0, n, n_packets);
+        K::env<<<(n + 127) / 128, 128, 0, x.stream>>>(d, inst0, n, n_packets);
         CU_OK(cudaGetLastError());
         c->launches++;
     }
-    const typename A::Dev d = c->d;
-    const uint32_t n_sms = st.stream_sms();
+    const uint32_t n_sms = c->part.stream_sms();
     static const uint32_t kStreamCtas = [] { const char *e = getenv("DSPI_CHAIN_CTAS"); const int v = e ? atoi(e) : 0; return (uint32_t)(v >= 1 && v <= 8 ? v : 8); }();   // streaming CTAs (256 threads) per SM
     auto stream_grid = [&](uint64_t units) {                                 // grid-stride kernels: no more CTAs than 8-warp units
         const uint64_t ctas = (units + 7) / 8;
         return (uint32_t)(ctas < (uint64_t)n_sms * kStreamCtas ? (ctas ? ctas : 1) : (uint64_t)n_sms * kStreamCtas);
     };
     const uint32_t n_warps16 = ((n + 31) & ~31u) / 16;                       // pre / post: 16 instances per warp
-    CU_OK(cudaEventRecord(st.ev_begin, c->stream));
+    CU_OK(cudaEventRecord(st.ev_begin, x.stream));
     CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
     for (uint32_t sl = 0; sl < n_slices; sl++) {
         const uint32_t p0 = slice_bounds[sl], p1 = slice_bounds[sl + 1];
@@ -836,12 +909,12 @@ int run_stages(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *d_pcm, u
     if (inst0 == 0 && n == d.N) std::swap(c->d.widx_in, c->d.widx_out);
     else CU_OK(cudaMemcpyAsync(d.widx_in + inst0, d.widx_out + inst0, (size_t)n * sizeof(*d.widx_in), cudaMemcpyDeviceToDevice, st.s_out));
     CU_OK(cudaEventRecord(st.ev_aux, st.s_out));                             // ring update done
-    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_aux, 0));
+    CU_OK(cudaStreamWaitEvent(x.stream, st.ev_aux, 0));
     // the last modulator launch is ordered after every other stage launch of this call
     CU_OK(cudaEventRecord(st.ev_done, st.s_pdm));
-    CU_OK(cudaStreamWaitEvent(c->stream, st.ev_done, 0));                    // later work on the engine stream sees all outputs
+    CU_OK(cudaStreamWaitEvent(x.stream, st.ev_done, 0));                     // later work on x.stream sees all outputs
     if (d_status) {
-        K::status<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, inst0, n, d_status);
+        K::status<<<(n + 127) / 128, 128, 0, x.stream>>>(c->d, inst0, n, d_status);
         CU_OK(cudaGetLastError());
         c->launches++;
     }
@@ -861,19 +934,36 @@ int check_window(const ChainHost<A> *c, uint32_t inst0, uint32_t n)
 template <class A>
 uint32_t all_instances(const ChainHost<A> *c) { return c ? c->desc.n_instances : 0; }
 
+// the checks of a call over instances [inst0, inst0 + n) with the schedule ps
+template <class A>
+int check_call(ChainHost<A> *c, PacketSchedule &ps, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+               const uint16_t *packet_frames, const void *d_spdif, bool subframes)
+{
+    int rc = check_packets(c, ps, d_pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
+    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
+    return check_window(c, inst0, n);
+}
+
+template <class A>
+int issue_call(ChainHost<A> *c, const Issue &x, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames,
+               void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
+{
+    return A::with_stages(c->desc, [&](auto k) {
+        return run_stages<A, decltype(k)>(c, x, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
+    });
+}
+
 // instances [inst0, inst0 + n), every buffer laid out for the n instances (the whole engine: 0, n_instances)
 template <class A>
 int process_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
                    const uint16_t *packet_frames, void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
 {
-    int rc = check_packets(c, d_pcm, bit_depth, n_packets, packet_frames);
-    if (rc) return rc;
-    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
-    if ((rc = check_window(c, inst0, n)) || n == 0) return rc;
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_call(c, c->sched, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, subframes);
+    if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return A::with_stages(c->desc, [&](auto k) {
-        return run_stages<A, decltype(k)>(c, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
-    });
+    return issue_call(c, Issue{ c->stream, c->st, c->sched }, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
 }
 
 // host memory in and out, staged through the engine's device buffers
@@ -881,7 +971,8 @@ template <class A>
 int process_host(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
                  const uint16_t *packet_frames, void *spdif_out, bool subframes, uint32_t *pdm_out, typename A::Status *status)
 {
-    int rc = check_packets(c, pcm, bit_depth, n_packets, packet_frames);
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_packets(c, c->sched, pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
     if ((rc = check_window(c, inst0, n)) || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
@@ -915,6 +1006,98 @@ int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32
     const uint32_t n = c->desc.n_instances;
     return host ? process_host(c, 0, n, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status)
                 : process_device(c, 0, n, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status);
+}
+
+// ---- lanes: issue queues of one engine over disjoint instance windows, whose calls run concurrently -------------------
+template <class A>
+int lane_open(ChainHost<A> *c, uint32_t inst0, uint32_t n, uint32_t *lane)
+{
+    if (!c || !lane) return fail(DSPI_EINVAL, "null argument");
+    if (inst0 % 64u) return fail(DSPI_EINVAL, "first instance %u is not a multiple of 64", inst0);
+    if (n == 0) return fail(DSPI_EINVAL, "a lane's window holds at least one instance");
+    int rc = check_range(c, inst0, n);
+    if (rc) return rc;
+    for (const Lane &l : c->lanes)
+        if (l.open && inst0 < l.inst0 + l.n && l.inst0 < inst0 + n)
+            return fail(DSPI_EINVAL, "window [%u, %u) overlaps the open lane window [%u, %u)", inst0, inst0 + n, l.inst0, l.inst0 + l.n);
+    uint32_t id = 0;
+    while (id < DSPI_CHAIN_MAX_LANES && c->lanes[id].open) id++;
+    if (id == DSPI_CHAIN_MAX_LANES) return fail(DSPI_ERANGE, "%d lanes are open already", DSPI_CHAIN_MAX_LANES);
+    CU_OK(cudaSetDevice(c->desc.device));
+    Lane &l = c->lanes[id];
+    cudaError_t e = cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&l.ev_engine, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&l.ev_last, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = l.st.create(c->part);
+    if (e == cudaSuccess) e = l.sched.create(c->desc.max_frames);
+    if (e != cudaSuccess) {
+        lane_release(l);
+        cudaGetLastError();
+        return fail(e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA, "lane setup: %s", cudaGetErrorString(e));
+    }
+    l.open = true;
+    l.inst0 = inst0;
+    l.n = n;
+    c->open_lanes++;
+    *lane = id;
+    return DSPI_OK;
+}
+
+// the open lane `lane` of c, or NULL with the error set
+template <class A>
+Lane *lane_of(ChainHost<A> *c, uint32_t lane)
+{
+    if (!c) { fail(DSPI_EINVAL, "null argument"); return nullptr; }
+    if (lane >= DSPI_CHAIN_MAX_LANES || !c->lanes[lane].open) { fail(DSPI_EINVAL, "lane %u is not open", lane); return nullptr; }
+    return &c->lanes[lane];
+}
+
+template <class A>
+int lane_close(ChainHost<A> *c, uint32_t lane)
+{
+    Lane *l = lane_of(c, lane);
+    if (!l) return DSPI_EINVAL;
+    CU_OK(cudaSetDevice(c->desc.device));
+    lane_release(*l);                                                       // waits for the lane's calls
+    c->open_lanes--;
+    return DSPI_OK;
+}
+
+// process_device on a lane: the range call's checks, then a window check; issued behind the engine stream as it is now
+template <class A>
+int lane_process(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+                 const uint16_t *packet_frames, void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
+{
+    Lane *l = lane_of(c, lane);
+    if (!l) return DSPI_EINVAL;
+    int rc = check_call(c, l->sched, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, subframes);
+    if (rc) return rc;
+    if (inst0 < l->inst0 || (uint64_t)inst0 + n > (uint64_t)l->inst0 + l->n)
+        return fail(DSPI_ERANGE, "instances [%u, %llu) outside lane %u's window [%u, %u)", inst0, (unsigned long long)inst0 + n, lane, l->inst0,
+                    l->inst0 + l->n);
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaEventRecord(l->ev_engine, c->stream));
+    CU_OK(cudaStreamWaitEvent(l->stream, l->ev_engine, 0));
+    rc = issue_call(c, Issue{ l->stream, l->st, l->sched }, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
+    CU_OK(cudaEventRecord(l->ev_last, l->stream));
+    return rc;
+}
+
+template <class A>
+void *lane_stream(ChainHost<A> *c, uint32_t lane)
+{
+    return c && lane < DSPI_CHAIN_MAX_LANES && c->lanes[lane].open ? (void *)c->lanes[lane].stream : nullptr;
+}
+
+template <class A>
+int lane_sync(ChainHost<A> *c, uint32_t lane)
+{
+    Lane *l = lane_of(c, lane);
+    if (!l) return DSPI_EINVAL;
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(cudaStreamSynchronize(l->stream));
+    return DSPI_OK;
 }
 
 // ---- S/PDIF transmitters -----------------------------------------------------------------------------------------------
@@ -1295,8 +1478,8 @@ template <class A>
 int sm_partition(ChainHost<A> *c, uint32_t *pdm_sms, uint32_t *rest_sms)
 {
     if (!c) return fail(DSPI_EINVAL, "null argument");
-    if (pdm_sms) *pdm_sms = c->st.pdm_sms;
-    if (rest_sms) *rest_sms = c->st.rest_sms;
+    if (pdm_sms) *pdm_sms = c->part.pdm_sms;
+    if (rest_sms) *rest_sms = c->part.rest_sms;
     return DSPI_OK;
 }
 

@@ -54,6 +54,80 @@ struct GreenApi {
     }
 };
 
+// The engine's split of the GPU, made once per engine: every set of stage streams (the engine's own and each lane's,
+// chain_host.cuh) is created in these two contexts with the same priorities, so that the modulator keeps its SMs to
+// itself however many lanes run.
+struct SmPartition {
+    CUgreenCtx g_pdm = nullptr, g_rest = nullptr;
+    unsigned pdm_sms = 0, rest_sms = 0;                       // 0: no partition (priority streams on the whole GPU)
+    unsigned all_sms = 0;                                     // SM count of the device
+    int prio_hi = 0, prio_mid = 0, prio_lo = 0;               // numerically lower = higher priority
+
+    // SMs the streaming stages run on
+    unsigned stream_sms() const { return rest_sms ? rest_sms : all_sms; }
+
+    // modulator CTAs are 128 threads (one warp per sub-partition): ceil(instances / 128) SMs, in the partition granularity of 8,
+    // at most 48.  On a 132-SM H100 SXM at 8192 instances, 48 modulator SMs beat 56 and 64 by 1-3 % per call (both chains)
+    // and 72 or 80 lose 10-25 %: the other stages need the SMs more.
+    static unsigned wanted_pdm_sms(unsigned n_instances)
+    {
+        if (const char *e = getenv("DSPI_PDM_SMS")) return (unsigned)atoi(e);
+        unsigned want = ((n_instances + 127u) / 128u + 7u) / 8u * 8u;
+        return want > 48u ? 48u : want;
+    }
+
+    bool create_partition(int device, unsigned want)
+    {
+        const GreenApi &ga = GreenApi::get();
+        if (!ga.ok || want == 0) return false;
+        CUdevResource sm, part, rest;
+        unsigned groups = 1;
+        if (ga.DeviceGetDevResource((CUdevice)device, &sm, CU_DEV_RESOURCE_TYPE_SM) != CUDA_SUCCESS) return false;
+        if (want + 8 > sm.sm.smCount) return false;
+        if (ga.DevSmResourceSplitByCount(&part, &groups, &sm, &rest, 0, want) != CUDA_SUCCESS || groups != 1 || rest.sm.smCount == 0) return false;
+        CUdevResourceDesc d_part, d_rest;
+        if (ga.DevResourceGenerateDesc(&d_part, &part, 1) != CUDA_SUCCESS || ga.DevResourceGenerateDesc(&d_rest, &rest, 1) != CUDA_SUCCESS) return false;
+        if (ga.GreenCtxCreate(&g_pdm, d_part, (CUdevice)device, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) { g_pdm = nullptr; return false; }
+        if (ga.GreenCtxCreate(&g_rest, d_rest, (CUdevice)device, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) { g_rest = nullptr; destroy(); return false; }
+        pdm_sms = part.sm.smCount; rest_sms = rest.sm.smCount;
+        return true;
+    }
+
+    // the priorities, the SM count and, for n_instances > 0, the split (none when the driver cannot make one)
+    cudaError_t create(int device = 0, unsigned n_instances = 0)
+    {
+        int lo = 0, hi = 0;
+        cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+        int n_sms = 0;
+        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device);
+        all_sms = (unsigned)n_sms;
+        // the modulator is the longest serial chain: its few CTAs are placed first whenever an SM frees a
+        // slot; then the front; the many output CTAs fill what is left
+        prio_hi = hi; prio_mid = hi < lo ? hi + 1 : lo; prio_lo = lo;
+        if (e == cudaSuccess && n_instances && !create_partition(device, wanted_pdm_sms(n_instances))) cudaGetLastError();
+        return e;
+    }
+
+    // a stream of priority `prio` in green context g (a plain priority stream when there is no partition)
+    cudaError_t stream(CUgreenCtx g, cudaStream_t *s, int prio) const
+    {
+        if (!g) return cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, prio);
+        CUstream cs = nullptr;
+        if (GreenApi::get().GreenCtxStreamCreate(&cs, g, CU_STREAM_NON_BLOCKING, prio) != CUDA_SUCCESS) return cudaErrorUnknown;
+        *s = (cudaStream_t)cs;
+        return cudaSuccess;
+    }
+
+    void destroy()
+    {
+        const GreenApi &ga = GreenApi::get();
+        if (g_pdm) { ga.GreenCtxDestroy(g_pdm); g_pdm = nullptr; }
+        if (g_rest) { ga.GreenCtxDestroy(g_rest); g_rest = nullptr; }
+        pdm_sms = rest_sms = 0;
+    }
+};
+
+// The stage streams and events of one issue context (an engine's or a lane's).
 struct ChainStreams {
     static constexpr int kMaxSlices = 16;
 
@@ -95,74 +169,13 @@ struct ChainStreams {
     }
     cudaStream_t s_front = nullptr, s_out = nullptr, s_pdm = nullptr;
     cudaEvent_t ev_begin = nullptr, ev_done = nullptr, ev_aux = nullptr, ev_front[kMaxSlices] = {}, ev_out[kMaxSlices] = {};
-    CUgreenCtx g_pdm = nullptr, g_rest = nullptr;
-    unsigned pdm_sms = 0, rest_sms = 0;                       // 0: no partition (priority streams on the whole GPU)
-    unsigned all_sms = 0;                                     // SM count of the device
 
-    // SMs the streaming stages run on
-    unsigned stream_sms() const { return rest_sms ? rest_sms : all_sms; }
-
-    // modulator CTAs are 128 threads (one warp per sub-partition): ceil(instances / 128) SMs, in the partition granularity of 8,
-    // at most 48.  On a 132-SM H100 SXM at 8192 instances, 48 modulator SMs beat 56 and 64 by 1-3 % per call (both chains)
-    // and 72 or 80 lose 10-25 %: the other stages need the SMs more.
-    static unsigned wanted_pdm_sms(unsigned n_instances)
+    // the three stage streams in the partition's contexts (or priority streams without one), and the events
+    cudaError_t create(const SmPartition &p)
     {
-        if (const char *e = getenv("DSPI_PDM_SMS")) return (unsigned)atoi(e);
-        unsigned want = ((n_instances + 127u) / 128u + 7u) / 8u * 8u;
-        return want > 48u ? 48u : want;
-    }
-
-    bool create_partition(int device, unsigned want, int prio_hi, int prio_mid, int prio_lo)
-    {
-        const GreenApi &ga = GreenApi::get();
-        if (!ga.ok || want == 0) return false;
-        CUdevResource sm, part, rest;
-        unsigned groups = 1;
-        if (ga.DeviceGetDevResource((CUdevice)device, &sm, CU_DEV_RESOURCE_TYPE_SM) != CUDA_SUCCESS) return false;
-        if (want + 8 > sm.sm.smCount) return false;
-        if (ga.DevSmResourceSplitByCount(&part, &groups, &sm, &rest, 0, want) != CUDA_SUCCESS || groups != 1 || rest.sm.smCount == 0) return false;
-        CUdevResourceDesc d_part, d_rest;
-        if (ga.DevResourceGenerateDesc(&d_part, &part, 1) != CUDA_SUCCESS || ga.DevResourceGenerateDesc(&d_rest, &rest, 1) != CUDA_SUCCESS) return false;
-        if (ga.GreenCtxCreate(&g_pdm, d_part, (CUdevice)device, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) { g_pdm = nullptr; return false; }
-        if (ga.GreenCtxCreate(&g_rest, d_rest, (CUdevice)device, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) { g_rest = nullptr; destroy_partition(); return false; }
-        CUstream a = nullptr, b = nullptr, c = nullptr;
-        if (ga.GreenCtxStreamCreate(&a, g_pdm, CU_STREAM_NON_BLOCKING, prio_hi) != CUDA_SUCCESS || ga.GreenCtxStreamCreate(&b, g_rest, CU_STREAM_NON_BLOCKING, prio_mid) != CUDA_SUCCESS ||
-            ga.GreenCtxStreamCreate(&c, g_rest, CU_STREAM_NON_BLOCKING, prio_lo) != CUDA_SUCCESS) {
-            for (CUstream st : { a, b, c }) if (st) cudaStreamDestroy((cudaStream_t)st);
-            destroy_partition();
-            return false;
-        }
-        s_pdm = (cudaStream_t)a; s_front = (cudaStream_t)b; s_out = (cudaStream_t)c;
-        pdm_sms = part.sm.smCount; rest_sms = rest.sm.smCount;
-        return true;
-    }
-
-    void destroy_partition()
-    {
-        const GreenApi &ga = GreenApi::get();
-        if (g_pdm) { ga.GreenCtxDestroy(g_pdm); g_pdm = nullptr; }
-        if (g_rest) { ga.GreenCtxDestroy(g_rest); g_rest = nullptr; }
-        pdm_sms = rest_sms = 0;
-    }
-
-    cudaError_t create(int device = 0, unsigned n_instances = 0)
-    {
-        int lo = 0, hi = 0;                                   // numerically lower = higher priority
-        cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        int n_sms = 0;
-        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device);
-        all_sms = (unsigned)n_sms;
-        // the modulator is the longest serial chain: its few CTAs are placed first whenever an SM frees a
-        // slot; then the front; the many output CTAs fill what is left
-        const int mid = hi < lo ? hi + 1 : lo;
-        if (e == cudaSuccess && n_instances && create_partition(device, wanted_pdm_sms(n_instances), hi, mid, lo)) {
-            // streams live in the two green contexts
-        } else {
-            cudaGetLastError();
-            if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&s_pdm, cudaStreamNonBlocking, hi);
-            if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&s_front, cudaStreamNonBlocking, mid);
-            if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&s_out, cudaStreamNonBlocking, lo);
-        }
+        cudaError_t e = p.stream(p.g_pdm, &s_pdm, p.prio_hi);
+        if (e == cudaSuccess) e = p.stream(p.g_rest, &s_front, p.prio_mid);
+        if (e == cudaSuccess) e = p.stream(p.g_rest, &s_out, p.prio_lo);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_begin, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_done, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_aux, cudaEventDisableTiming);
@@ -177,7 +190,6 @@ struct ChainStreams {
     {
         for (cudaStream_t *s : { &s_front, &s_out, &s_pdm })
             if (*s) { cudaStreamSynchronize(*s); cudaStreamDestroy(*s); *s = nullptr; }
-        destroy_partition();
         for (cudaEvent_t *ev : { &ev_begin, &ev_done, &ev_aux })
             if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
         for (int i = 0; i < kMaxSlices; i++) {

@@ -79,7 +79,7 @@ struct dspi_eq {
     uint64_t *d_modes;       // float only: per-channel topology words as packed from the coefficient structs
     uint64_t *d_modes_eff;   // with the caller's skip mask applied (chain engines), else nullptr
     const uint8_t *d_skip;   // not owned
-    uint32_t *d_sched;       // float only: dynamic scheduler words
+    uint32_t *d_sched;       // float only: dynamic scheduler words (sched_words)
     int n_sms;
     size_t aos_elem;
     uint64_t launches;
@@ -97,6 +97,12 @@ struct dspi_eq {
     char kinfo[320];
     dspi::ResponseBuffers resp;   // frequency table and host staging of dspi_eq_response_*
 };
+
+// Scheduler words of K1's dynamic schedule (DSPI_DBG=8): a launch over groups [g0, g0 + ng) starting at row row_lo of g0
+// uses 1 + ng words from word 2 h, h = (g0 * rows + row_lo) / 32 its first 32-row block.  A launch spans at least ng such
+// blocks, so launches over disjoint channel ranges, which may share a 64-row group at their boundary, use disjoint words
+// and may run concurrently; a whole-engine launch uses words 0 .. n_groups, as a single counter block would.
+static size_t sched_words(const dspi_eq *e) { return 2 * (size_t)(e->c_pad / 32) + 1; }
 
 extern "C" {
 
@@ -245,7 +251,7 @@ int dspi_eq_create(dspi_eq **out, const dspi_eq_desc *desc)
     if ((err = cudaMemsetAsync(e->d_coef, 0, coef_bytes, e->stream)) != cudaSuccess) goto cuda_fail;
     if (!q28) {
         if ((err = cudaMalloc(&e->d_modes, (size_t)e->c_pad * 8)) != cudaSuccess) goto cuda_fail;
-        if ((err = cudaMalloc(&e->d_sched, (size_t)(1 + e->n_groups) * 4)) != cudaSuccess) goto cuda_fail;
+        if ((err = cudaMalloc(&e->d_sched, sched_words(e) * 4)) != cudaSuccess) goto cuda_fail;
         if ((err = cudaDeviceGetAttribute(&e->n_sms, cudaDevAttrMultiProcessorCount, desc->device)) != cudaSuccess) goto cuda_fail;
         if ((err = cudaMemsetAsync(e->d_modes, 0, (size_t)e->c_pad * 8, e->stream)) != cudaSuccess) goto cuda_fail;
     }
@@ -466,7 +472,7 @@ static int launch_eq(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, uint3
     const uint64_t *modes = e->d_modes_eff ? e->d_modes_eff : e->d_modes;
     a.modes = modes ? modes + (size_t)g0 * e->rows : nullptr;
     a.n_groups = ng;
-    a.sched = e->d_sched;
+    a.sched = e->d_sched + 2 * (((size_t)g0 * e->rows + row_lo) / 32);
     a.n_sms = e->n_sms;
     a.n_rows = n_rows;
     a.row_lo = row_lo;

@@ -912,6 +912,57 @@ int dspi_chainq_process_subframes_range_host  (dspi_chainq *c, uint32_t inst0, u
 int dspi_chainq_process_subframes_range_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
                                                const uint16_t *packet_frames, dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
 
+/* ---- lanes: range calls of several clock groups running side by side ------------------------------ */
+/* A lane is an issue queue of one engine, bound to a window of instances, with stage streams and a packet schedule of its
+ * own.  Calls on different lanes run concurrently on the GPU: a farm opens one lane per clock group and serves each group's
+ * packets on its lane, so that the small calls of several groups share the GPU instead of adding their times.  The lanes'
+ * stage streams run in the engine's own SM partition (dspi_chain_sm_partition).
+ *   Window.  _lane_open reserves instances [inst0, inst0 + n) and returns the lane's id in *lane.  inst0 is a multiple of 64,
+ *   n > 0, and the window overlaps no open lane's window.  At most DSPI_CHAIN_MAX_LANES lanes are open at once; a closed
+ *   lane's id may be handed out again.
+ *   Calls.  _lane_process_packets_device / _lane_process_subframes_device run over any [inst0, inst0 + n) inside the lane's
+ *   window (inst0 a multiple of 64, n == 0 does nothing).  Arguments, buffer layout and results are exactly those of
+ *   dspi_chain(q)_process_packets_range_device / _process_subframes_range_device over that range.
+ *   Ordering.  Calls on one lane run in issue order.  A lane call runs after every engine-level call issued before it, and
+ *   every engine-level call runs after every lane call issued before it.  An engine-level call is any call taking the
+ *   engine that is not a lane call: process, range process, set / edit / apply / collect, copy / export / import / reset,
+ *   response, state, the S/PDIF and preset-mute getters and setters, dspi_chain_sync and destroy.  So engine-level calls
+ *   are barriers across lanes, and lane calls are ordered only against them, never against other lanes.
+ *   _lane_stream is where a lane's outputs (S/PDIF, PDM, status) become visible; dspi_chain_stream does not carry lane
+ *   work.  _lane_sync waits for the lane's calls.
+ *   Result.  Outputs, state, meters, envelope, S/PDIF transmitter and configuration record are byte for byte those of the
+ *   same calls issued in the same order as range calls on the engine stream.
+ *   No lane open.  Every other call issues exactly the work it issues without lanes (dspi_chain_launch_count included).
+ *   Close.  _lane_close waits for the lane's calls and frees its streams; destroying the engine closes its lanes.
+ *   Threads.  One host thread issues the calls of an engine and its lanes.  Lane calls do not wait for the device, with one
+ *   exception: a call with more packets than any envelope-mode call before it grows the envelope table, and first waits
+ *   for every lane and the engine stream.
+ *   Errors (nothing is written on any error): DSPI_EINVAL for a NULL engine or lane pointer, a misaligned inst0, n == 0 or an
+ *   overlapping window at _lane_open, an unknown or closed lane id, and every check of the range calls; DSPI_ERANGE for a
+ *   window past the end of the engine (also one whose end wraps in 32 bits), a call range outside its lane's window, or a
+ *   lane beyond DSPI_CHAIN_MAX_LANES.  _lane_stream returns NULL for an unknown or closed lane. */
+#define DSPI_CHAIN_MAX_LANES 16
+int   dspi_chain_lane_open (dspi_chain *c, uint32_t inst0, uint32_t n, uint32_t *lane);
+int   dspi_chain_lane_close(dspi_chain *c, uint32_t lane);
+int   dspi_chain_lane_process_packets_device  (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm,
+                                               uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                               int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status *d_status);
+int   dspi_chain_lane_process_subframes_device(dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm,
+                                               uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                               dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status *d_status);
+void *dspi_chain_lane_stream(dspi_chain *c, uint32_t lane);
+int   dspi_chain_lane_sync  (dspi_chain *c, uint32_t lane);
+int   dspi_chainq_lane_open (dspi_chainq *c, uint32_t inst0, uint32_t n, uint32_t *lane);
+int   dspi_chainq_lane_close(dspi_chainq *c, uint32_t lane);
+int   dspi_chainq_lane_process_packets_device  (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm,
+                                                uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                                int32_t *d_spdif_out, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
+int   dspi_chainq_lane_process_subframes_device(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm,
+                                                uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
+                                                dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
+void *dspi_chainq_lane_stream(dspi_chainq *c, uint32_t lane);
+int   dspi_chainq_lane_sync  (dspi_chainq *c, uint32_t lane);
+
 /* ---- frequency response of EQ channels and chain instances ------------------------------------ */
 /* The complex transfer function H(e^{j omega}) of the linear, time-invariant part of the path the NEXT process call applies,
  * read from the engine's device-resident coefficients and parameters at the point of the engine stream where the call is
