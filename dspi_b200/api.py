@@ -62,6 +62,8 @@ SYMBOLS = [
     "dspi_chain_lane_stream", "dspi_chain_lane_sync",
     "dspi_chainq_lane_open", "dspi_chainq_lane_close", "dspi_chainq_lane_process_packets_device", "dspi_chainq_lane_process_subframes_device",
     "dspi_chainq_lane_stream", "dspi_chainq_lane_sync",
+    "dspi_chain_lane_edit_bulk_device", "dspi_chain_lane_set_preset_mute", "dspi_chain_lane_set_spdif_tx", "dspi_chain_lane_reset_instances",
+    "dspi_chainq_lane_edit_bulk_device", "dspi_chainq_lane_set_preset_mute", "dspi_chainq_lane_set_spdif_tx", "dspi_chainq_lane_reset_instances",
 ]
 
 
@@ -174,6 +176,10 @@ def lib():
             getattr(h, pre + "_lane_stream").argtypes = [vp, u32]
             getattr(h, pre + "_lane_stream").restype = vp
             getattr(h, pre + "_lane_sync").argtypes = [vp, u32]
+            getattr(h, pre + "_lane_edit_bulk_device").argtypes = [vp, u32, u32, vp, C.c_int, C.c_float, vp]
+            getattr(h, pre + "_lane_set_preset_mute").argtypes = [vp, u32, u32, u32, vp, u32]
+            getattr(h, pre + "_lane_set_spdif_tx").argtypes = [vp, u32, u32, u32, vp]
+            getattr(h, pre + "_lane_reset_instances").argtypes = [vp, u32, u32, u32]
         for pre in ("dspi_eq", "dspi_chain", "dspi_chainq"):
             getattr(h, pre + "_response_host").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
             getattr(h, pre + "_response_device").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
@@ -710,6 +716,11 @@ class _ChainEngine:
     def set_spdif_tx(self, block_pos, channel_status, inst0=0):
         """Transmitter state of instances [inst0, inst0+n): ``block_pos`` an int or [n] (0..191), ``channel_status`` 5 bytes
         or uint8 [n, 5]; a single value on either side applies to all n.  Takes effect from the next process call."""
+        rec = self._spdif_records(block_pos, channel_status)
+        _check(self._fn("set_spdif_tx")(self._h, int(inst0), int(rec.size), rec.ctypes.data_as(C.c_void_p)))
+
+    @staticmethod
+    def _spdif_records(block_pos, channel_status):
         bp = np.asarray(block_pos, np.int64).reshape(-1)
         cs = np.frombuffer(bytes(channel_status), np.uint8) if isinstance(channel_status, (bytes, bytearray)) else np.asarray(channel_status, np.uint8)
         cs = cs.reshape(-1, 5)
@@ -721,7 +732,7 @@ class _ChainEngine:
         rec = np.zeros(n, L.SPDIF_TX)
         rec["block_pos"] = bp
         rec["channel_status"] = cs
-        _check(self._fn("set_spdif_tx")(self._h, int(inst0), int(n), rec.ctypes.data_as(C.c_void_p)))
+        return rec
 
     def get_spdif_tx(self, n=None, inst0=0):
         """SPDIF_TX [n]: block position of the next frame and channel status, after the last call issued."""
@@ -809,6 +820,32 @@ class _ChainEngine:
 
     def lane_sync(self, lane):
         _check(self._fn("lane_sync")(self._h, int(lane)))
+
+    def lane_edit_bulk_device(self, lane, edits, fs, exact_db=False, results_ptr=0):
+        """``edit_bulk_device`` issued on a lane (every edit's instance inside its window), asynchronous on
+        ``lane_stream(lane)``: returns without waiting.  ``results_ptr`` (device memory, int32 [n], or 0) receives the
+        ``layouts.BULK_*`` mark of each edit's instance there."""
+        e = np.ascontiguousarray(edits, L.BULK_EDIT).reshape(-1)
+        _check(self._fn("lane_edit_bulk_device")(self._h, int(lane), int(e.shape[0]), e.ctypes.data_as(C.c_void_p), int(bool(exact_db)),
+                                                 C.c_float(fs), C.c_void_p(int(results_ptr)) if results_ptr else None))
+
+    def lane_set_preset_mute(self, lane, states, fs, inst0, n=None):
+        """``set_preset_mute`` issued on a lane ([inst0, inst0+n) inside its window): ``states`` PRESET_MUTE [n] arms the
+        fades, None (with ``n``) leaves envelope mode.  Asynchronous on ``lane_stream(lane)``."""
+        if states is None:
+            _check(self._fn("lane_set_preset_mute")(self._h, int(lane), int(inst0), int(n), None, int(fs)))
+            return
+        st = np.ascontiguousarray(states, L.PRESET_MUTE).reshape(-1)
+        _check(self._fn("lane_set_preset_mute")(self._h, int(lane), int(inst0), int(st.shape[0]), st.ctypes.data_as(C.c_void_p), int(fs)))
+
+    def lane_set_spdif_tx(self, lane, block_pos, channel_status, inst0):
+        """``set_spdif_tx`` issued on a lane ([inst0, inst0+n) inside its window), asynchronous on ``lane_stream(lane)``."""
+        rec = self._spdif_records(block_pos, channel_status)
+        _check(self._fn("lane_set_spdif_tx")(self._h, int(lane), int(inst0), int(rec.size), rec.ctypes.data_as(C.c_void_p)))
+
+    def lane_reset_instances(self, lane, inst0, n):
+        """``reset_instances`` issued on a lane ([inst0, inst0+n) inside its window), asynchronous on ``lane_stream(lane)``."""
+        _check(self._fn("lane_reset_instances")(self._h, int(lane), int(inst0), int(n)))
 
 
 class ChainEngine(_ChainEngine):

@@ -956,8 +956,9 @@ struct EditStage {
     uint16_t *band_mask = nullptr;                         // [roles][kChunk]
     int32_t *marks = nullptr;                              // [kChunk]
     std::vector<unsigned char> h_in;
-    std::vector<uint32_t> seg, last, count, inst;
-    static constexpr size_t kInBytes = (size_t)kEditChunk * sizeof(dspi_bulk_edit) + (size_t)(2 * kChunk + 1) * sizeof(uint32_t);
+    std::vector<uint32_t> seg, last, count, inst;          // seg, last: per instance of the engine, or of a lane's window
+    // with a lane edit's device results, each grouped edit's position in the call and its segment follow: [E] + [E]
+    static constexpr size_t kInBytes = (size_t)kEditChunk * (sizeof(dspi_bulk_edit) + 2 * sizeof(uint32_t)) + (size_t)(2 * kChunk + 1) * sizeof(uint32_t);
     cudaError_t ensure(int roles, uint32_t n_instances)
     {
         if (seg.size() < n_instances) seg.assign(n_instances, 0);
@@ -979,6 +980,60 @@ struct EditStage {
     }
 };
 
+// Pinned host staging of a lane's control calls (edits, fade rows, transmitter rows): kSlots buffers taken in turn.  Each
+// is guarded by an event recorded behind the copies that read it, so the host writes a buffer again only once those
+// copies are done: with fewer than kSlots uploads in flight on the lane, taking one never waits.  A buffer grows to the
+// largest upload it has carried; growing is a pinned allocation, which may wait for the device.
+struct HostRing {
+    static constexpr int kSlots = 8;
+    unsigned char *buf[kSlots] = {};
+    size_t cap[kSlots] = {};
+    cudaEvent_t ev[kSlots] = {};
+    int next = 0, cur = 0;
+    cudaError_t take(size_t bytes, unsigned char **out)
+    {
+        const int k = next;
+        cudaError_t e = ev[k] ? cudaEventSynchronize(ev[k]) : cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming);
+        if (e == cudaSuccess && bytes > cap[k]) {
+            cudaFreeHost(buf[k]);
+            buf[k] = nullptr; cap[k] = 0;
+            e = cudaHostAlloc((void **)&buf[k], bytes, cudaHostAllocDefault);
+            if (e == cudaSuccess) cap[k] = bytes;
+        }
+        if (e != cudaSuccess) return e;
+        next = (k + 1) % kSlots;
+        cur = k;
+        *out = buf[k];
+        return cudaSuccess;
+    }
+    // the copies reading the buffer taken last are issued on s
+    cudaError_t done(cudaStream_t s) { return cudaEventRecord(ev[cur], s); }
+    void destroy()
+    {
+        for (int k = 0; k < kSlots; k++) {
+            if (ev[k]) cudaEventSynchronize(ev[k]), cudaEventDestroy(ev[k]);
+            cudaFreeHost(buf[k]);
+            buf[k] = nullptr; cap[k] = 0; ev[k] = nullptr;
+        }
+        next = cur = 0;
+    }
+};
+
+// The scope of a lane control call (chain_host.cuh, Lane): the instance window it may touch and the pinned ring its uploads
+// go through.  Engine-level calls pass none: they touch every row, stage through pageable memory and synchronise.
+struct LaneScope {
+    uint32_t inst0, n;
+    HostRing &ring;
+};
+
+// d_results of a lane edit: grouped edit j of a chunk is edit pos[j] of the call, whose instance is segment seg[j]
+static __global__ void edit_marks_kernel(const int32_t *__restrict__ marks, const uint32_t *__restrict__ pos, const uint32_t *__restrict__ seg,
+                                         uint32_t n, int32_t *__restrict__ out)
+{
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < n) out[pos[j]] = marks[seg[j]];
+}
+
 inline int fail_cuda(cudaError_t e, const char *what)
 {
     size_t cap = 0;
@@ -991,11 +1046,11 @@ inline int fail_cuda(cudaError_t e, const char *what)
 // stage.results is 0 (the others are left alone): state into the mirrors, coefficients from the recipes at fs (or at
 // rates[i] when rates is not null), the clamped recipes into the records, mirrors back into the packed stores.  With `inst`
 // (device, [nc]) instance i is first + inst[i]; with `band_mask` (device, [roles][nc]) only the masked bands are computed.
+// Issued on s; an engine-level call's pack synchronises, a lane's (lane != null) packs and remasks its window's rows only.
 template <class S, class Engine>
-int recalculate_filters(Engine *c, Stage &stage, uint32_t first, uint32_t nc, float fs, const float *rates, const uint32_t *inst = nullptr,
-                        const uint16_t *band_mask = nullptr)
+int recalculate_filters(Engine *c, cudaStream_t s, Stage &stage, const LaneScope *lane, uint32_t first, uint32_t nc, float fs, const float *rates,
+                        const uint32_t *inst = nullptr, const uint16_t *band_mask = nullptr)
 {
-    cudaStream_t s = c->stream;
     RoleRange rm, ro;
     rm.roles = 2; ro.roles = S::kRoles - 2;
     rm.stride = ro.stride = c->d.N_pad;
@@ -1014,17 +1069,29 @@ int recalculate_filters(Engine *c, Stage &stage, uint32_t first, uint32_t nc, fl
                                                                                    (size_t)nc * kMaxBands, kMaxBands, stage.results, inst, band_mask);
     if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "recipe record kernel");
     c->launches += 3;
+    if (lane) {
+        rc = eq_pack_rows(c->eq_m, first, nc, s, rm, lane->inst0, lane->n);
+        return rc == DSPI_OK ? eq_pack_rows(c->eq_o, first, nc, s, ro, lane->inst0, lane->n) : rc;
+    }
     rc = eq_pack_range(c->eq_m, first, nc, s, rm);
     if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, first, nc, s, ro);
     return rc;
 }
 
-// The skip rows into the sub-engines' effective modes after the last chunk: synchronises the engine stream.
+// The skip rows into the sub-engines' effective modes after the last chunk, on s: every row, synchronising (engine
+// level), or the rows of a lane's window (lane != null; eq_skip_set must hold for both sub-engines).
 template <class Engine>
-int finish_skip(Engine *c)
+int finish_skip(Engine *c, cudaStream_t s, const LaneScope *lane)
 {
-    int rc = eq_set_skip(c->eq_m, c->d.skip_m, c->stream);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->stream);
+    if (lane) {
+        RoleRange rm, ro;
+        rm.roles = 2; ro.roles = Engine::Arith::kOuts;
+        rm.stride = ro.stride = c->d.N_pad;
+        const int rc = eq_remask_rows(c->eq_m, lane->inst0, lane->n, rm, s);
+        return rc == DSPI_OK ? eq_remask_rows(c->eq_o, lane->inst0, lane->n, ro, s) : rc;
+    }
+    int rc = eq_set_skip(c->eq_m, c->d.skip_m, s);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, s);
     return rc;
 }
 
@@ -1049,11 +1116,11 @@ int ingest(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_bulk_
                                                                                  stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "ingest kernel");
         c->launches++;
-        if ((rc = recalculate_filters<S>(c, stage, first, nc, fs, nullptr)) != DSPI_OK) return rc;
+        if ((rc = recalculate_filters<S>(c, s, stage, nullptr, first, nc, fs, nullptr)) != DSPI_OK) return rc;
         if ((e = cudaMemcpyAsync(results + i0, codes ? codes : stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
             return fail_cuda(e, "result copy");
     }
-    return finish_skip(c);
+    return finish_skip(c, s, nullptr);
 }
 
 // dspi_chain(q)_set_rate_device for checked arguments: per chunk the rates go to stage.rates, rate_kernel re-derives the
@@ -1072,12 +1139,12 @@ int set_rate(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const float *r
         rate_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.rates, stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "rate kernel");
         c->launches++;
-        int rc = recalculate_filters<S>(c, stage, first, nc, 0.0f, stage.rates);
+        int rc = recalculate_filters<S>(c, s, stage, nullptr, first, nc, 0.0f, stage.rates);
         if (rc != DSPI_OK) return rc;
         if (results && (e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
             return fail_cuda(e, "result copy");
     }
-    return finish_skip(c);
+    return finish_skip(c, s, nullptr);
 }
 
 // dspi_chain(q)_edit_bulk_device for checked arguments.  Edits of different instances commute, so the list is cut into
@@ -1087,19 +1154,23 @@ int set_rate(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const float *r
 // with their segment table in one copy; edit_kernel applies them, and when an edit of the chunk lies in the eq section the
 // touched bands go through the filter recalculation by instance list and band mask.  eq_set_skip at the end follows the
 // skip rows and synchronises.  results (host, may be null) gets the mark of each edit's instance.
+// Everything is issued on s with the stages given.  A lane edit (lane != null, every instance inside its window) uploads
+// through the lane's pinned ring, remasks its window's rows only and does not synchronise; d_results (device, may be
+// null) gets the marks there.
 template <class S, class Engine>
-int edit(Engine *c, Stage &stage, EditStage &es, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float fs, int32_t *results)
+int edit(Engine *c, cudaStream_t s, Stage &stage, EditStage &es, const LaneScope *lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db,
+         float fs, int32_t *results, int32_t *d_results = nullptr)
 {
+    const uint32_t base = lane ? lane->inst0 : 0;          // es.seg and es.last are indexed by instance - base
     cudaError_t e = stage.ensure(S::kRoles);
-    if (e == cudaSuccess) e = es.ensure(S::kRoles, c->desc.n_instances);
+    if (e == cudaSuccess) e = es.ensure(S::kRoles, lane ? lane->n : c->desc.n_instances);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
-    cudaStream_t s = c->stream;
     constexpr uint32_t eq0 = DSPI_WIRE_OFF(eq), eq1 = DSPI_WIRE_OFF(eq) + S::kRoles * kMaxBands * 16;
     std::vector<int32_t> marks;                            // per segment of the call (never more than the edits)
     std::vector<uint32_t> seg_of(results ? n_edits : 0);   // per edit: its segment
     if (results) marks.reserve(n_edits);
     // per instance its last edit, so that a chunk holding kChunk instances stops scanning after their last edit
-    for (uint32_t k = 0; k < n_edits; k++) es.last[edits[k].instance] = k;
+    for (uint32_t k = 0; k < n_edits; k++) es.last[edits[k].instance - base] = k;
     std::vector<uint32_t> pending(n_edits), taken, later;
     for (uint32_t k = 0; k < n_edits; k++) pending[k] = k;
     taken.reserve(n_edits < kEditChunk ? n_edits : kEditChunk);
@@ -1116,7 +1187,7 @@ int edit(Engine *c, Stage &stage, EditStage &es, uint32_t n_edits, const dspi_bu
             const uint32_t k = pending[p];
             if (taken.size() == kEditChunk || (nseg == kChunk && k > stop)) break;
             const dspi_bulk_edit &ed = edits[k];
-            uint32_t &sl = es.seg[ed.instance];
+            uint32_t &sl = es.seg[ed.instance - base];
             if (!sl) {
                 if (nseg == kChunk) {
                     later.push_back(k);
@@ -1125,7 +1196,7 @@ int edit(Engine *c, Stage &stage, EditStage &es, uint32_t n_edits, const dspi_bu
                 es.inst.push_back(ed.instance);
                 es.count[nseg] = 0;
                 sl = ++nseg;
-                stop = std::max(stop, es.last[ed.instance]);
+                stop = std::max(stop, es.last[ed.instance - base]);
             }
             es.count[sl - 1]++;
             taken.push_back(k);
@@ -1134,41 +1205,53 @@ int edit(Engine *c, Stage &stage, EditStage &es, uint32_t n_edits, const dspi_bu
         later.insert(later.end(), pending.begin() + p, pending.end());
         pending.swap(later);
         const uint32_t E = (uint32_t)taken.size();
-        // upload image: edits grouped by segment, then the segment offsets, then the segments' instances
-        dspi_bulk_edit *ed_h = reinterpret_cast<dspi_bulk_edit *>(es.h_in.data());
-        uint32_t *off_h = reinterpret_cast<uint32_t *>(es.h_in.data() + (size_t)E * sizeof(dspi_bulk_edit));
+        // upload image: edits grouped by segment, then the segment offsets, then the segments' instances (then, for
+        // d_results, each grouped edit's position in the call and its segment)
+        const size_t bytes = (size_t)E * sizeof(dspi_bulk_edit) + (size_t)(2 * nseg + 1) * sizeof(uint32_t) + (d_results ? (size_t)2 * E * sizeof(uint32_t) : 0);
+        unsigned char *img = es.h_in.data();
+        if (lane && (e = lane->ring.take(bytes, &img)) != cudaSuccess) return fail_cuda(e, "edit staging");
+        dspi_bulk_edit *ed_h = reinterpret_cast<dspi_bulk_edit *>(img);
+        uint32_t *off_h = reinterpret_cast<uint32_t *>(img + (size_t)E * sizeof(dspi_bulk_edit));
+        uint32_t *pos_h = off_h + 2 * nseg + 1;
         for (uint32_t g = 0, acc = 0; g <= nseg; g++) {
             off_h[g] = acc;
             if (g < nseg) acc += es.count[g];
         }
         memcpy(es.count.data(), off_h, (size_t)nseg * sizeof(uint32_t));                          // now each segment's write cursor
-        const size_t base = marks.size();
+        const size_t done = marks.size();
         for (const uint32_t k : taken) {
-            const uint32_t g = es.seg[edits[k].instance] - 1;
-            ed_h[es.count[g]++] = edits[k];
-            if (results) seg_of[k] = (uint32_t)base + g;
+            const uint32_t g = es.seg[edits[k].instance - base] - 1, j = es.count[g]++;
+            ed_h[j] = edits[k];
+            if (results) seg_of[k] = (uint32_t)done + g;
+            if (d_results) { pos_h[j] = k; pos_h[E + j] = g; }
         }
-        for (uint32_t g = 0; g < nseg; g++) es.seg[es.inst[g]] = 0;
+        for (uint32_t g = 0; g < nseg; g++) es.seg[es.inst[g] - base] = 0;
         memcpy(off_h + nseg + 1, es.inst.data(), (size_t)nseg * sizeof(uint32_t));
-        const size_t bytes = (size_t)E * sizeof(dspi_bulk_edit) + (size_t)(2 * nseg + 1) * sizeof(uint32_t);
-        if ((e = cudaMemcpyAsync(es.d_in, es.h_in.data(), bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return fail_cuda(e, "edit copy");
+        if ((e = cudaMemcpyAsync(es.d_in, img, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return fail_cuda(e, "edit copy");
+        if (lane && (e = lane->ring.done(s)) != cudaSuccess) return fail_cuda(e, "edit staging");
         const dspi_bulk_edit *d_edits = reinterpret_cast<const dspi_bulk_edit *>(es.d_in);
         const uint32_t *d_off = reinterpret_cast<const uint32_t *>(es.d_in + (size_t)E * sizeof(dspi_bulk_edit)), *d_inst = d_off + nseg + 1;
         edit_kernel<S><<<(nseg + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, nseg, d_edits, d_off, d_inst, exact_db ? kGainExact : kGainTaylor,
                                                                            fs, stage.recipes, es.band_mask, stage.results, es.marks);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "edit kernel");
         c->launches++;
+        if (d_results) {
+            const uint32_t *d_pos = d_inst + nseg;
+            edit_marks_kernel<<<(E + 255) / 256, 256, 0, s>>>(es.marks, d_pos, d_pos + E, E, d_results);
+            if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "edit mark kernel");
+            c->launches++;
+        }
         if (bands) {
-            const int rc = recalculate_filters<S>(c, stage, 0, nseg, fs, nullptr, d_inst, es.band_mask);
+            const int rc = recalculate_filters<S>(c, s, stage, lane, 0, nseg, fs, nullptr, d_inst, es.band_mask);
             if (rc != DSPI_OK) return rc;
         }
         if (results) {
-            marks.resize(base + nseg);
-            if ((e = cudaMemcpyAsync(marks.data() + base, es.marks, (size_t)nseg * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
+            marks.resize(done + nseg);
+            if ((e = cudaMemcpyAsync(marks.data() + done, es.marks, (size_t)nseg * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
                 return fail_cuda(e, "mark copy");
         }
     }
-    const int rc = finish_skip(c);
+    const int rc = finish_skip(c, s, lane);
     if (rc != DSPI_OK) return rc;
     for (uint32_t k = 0; results && k < n_edits; k++) results[k] = marks[seg_of[k]];
     return DSPI_OK;

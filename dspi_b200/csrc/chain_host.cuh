@@ -83,7 +83,8 @@ struct Issue {
 
 // A lane (dspi_chain_lane_*): an issue queue of its own, bound to the instance window [inst0, inst0 + n).  Its calls start
 // behind the engine stream as it was when they were issued (ev_engine) and end with ev_last, which engine-level calls
-// wait for (join_lanes).
+// wait for (join_lanes).  Its control calls stage through a device staging of its own, allocated by its first edit, and
+// a ring of pinned host buffers.
 struct Lane {
     bool open = false;
     uint32_t inst0 = 0, n = 0;
@@ -91,6 +92,9 @@ struct Lane {
     cudaEvent_t ev_engine = nullptr, ev_last = nullptr;
     ChainStreams st;
     PacketSchedule sched;
+    bulk::Stage bulk;                // recipes and reject codes of the lane's edits
+    bulk::EditStage bulk_edit;
+    bulk::HostRing ring;             // edits, fade rows and transmitter rows on their way to the device
 };
 
 // One engine: dspi_chain and dspi_chainq are this record for their arithmetic.
@@ -112,6 +116,7 @@ struct ChainHost {
     typename A::Status *d_status;
     SpdifTx tx;                      // S/PDIF transmitter state; not part of the state blob (*_get/set_spdif_tx)
     uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
+    std::vector<uint8_t> env_mode;   // [N] each instance's envelope-mode flag (env row 4 != 0), as the calls issued so far leave it
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     PacketSchedule sched;            // packet lengths of the current call
     ResponseBuffers resp;            // frequency table of *_response_*; host staging of *_response_host and the instance image calls
@@ -125,17 +130,26 @@ struct ChainHost {
 };
 
 // Engine-level calls run after every lane call issued before them: the engine stream waits for each open lane's last
-// call.  Every engine-level entry point passes its handle through here; with no lane open it does nothing.
+// call.  Every engine-level entry point passes its handle through here.  After lane control calls re-packed EQ rows,
+// the K1 kernel choice is stale (eq_choice_stale): the first engine-level call waits for that work and re-selects it.
+// With no lane open and no lane control call since the last such call it does nothing.
 template <class H>
 H *join_lanes(H *c)
 {
-    if (!c || !c->open_lanes) return c;
+    if (!c) return c;
+    const bool stale = eq_choice_stale(c->eq_m) || eq_choice_stale(c->eq_o);
+    if (!c->open_lanes && !stale) return c;
     cudaSetDevice(c->desc.device);
     for (Lane &l : c->lanes)
         if (l.open && cudaStreamWaitEvent(c->stream, l.ev_last, 0) != cudaSuccess) {
             cudaGetLastError();
             cudaStreamSynchronize(l.stream);                                // the same order, from the host
         }
+    if (stale && cudaStreamSynchronize(c->stream) == cudaSuccess) {         // a failed choice leaves the ahead-of-time kernels
+        if (eq_choice_stale(c->eq_m)) eq_refresh_choice(c->eq_m);
+        if (eq_choice_stale(c->eq_o)) eq_refresh_choice(c->eq_o);
+    }
+    cudaGetLastError();
     return c;
 }
 
@@ -157,6 +171,9 @@ void lane_release(Lane &l)
     if (l.stream) cudaStreamSynchronize(l.stream);
     l.st.destroy();
     l.sched.destroy();
+    l.bulk.destroy();
+    l.bulk_edit.destroy();
+    l.ring.destroy();
     for (cudaEvent_t *ev : { &l.ev_engine, &l.ev_last })
         if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
     if (l.stream) { cudaStreamDestroy(l.stream); l.stream = nullptr; }
@@ -291,13 +308,13 @@ size_t image_plan(ChainHost<A> *c, uint32_t use, image::Plan &pl)
     return pl.bytes;
 }
 
-// the pipeline reset of instances [inst0, inst0 + n) on the engine stream
+// the pipeline reset of instances [inst0, inst0 + n) on the engine stream, or on s
 template <class A>
-cudaError_t reset_range(ChainHost<A> *c, uint32_t inst0, uint32_t n)
+cudaError_t reset_range(ChainHost<A> *c, uint32_t inst0, uint32_t n, cudaStream_t s = nullptr)
 {
     image::Plan pl;
     if (!image_plan(c, kReset, pl)) return cudaErrorInvalidValue;
-    image::instance_image_kernel<image::kReset><<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, inst0, n, nullptr);
+    image::instance_image_kernel<image::kReset><<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, s ? s : c->stream>>>(pl, inst0, n, nullptr);
     c->launches++;
     return cudaGetLastError();
 }
@@ -369,6 +386,7 @@ int create(H **out, const dspi_chain_desc *desc)
     H *c = new (std::nothrow) H();                                          // value-initialised: every pointer and count 0
     if (!c) return fail(DSPI_ENOMEM, "host allocation failed");
     c->desc = *desc;
+    c->env_mode.assign(desc->n_instances, 0);
     auto &d = c->d;
     d.N = desc->n_instances;
     d.N_pad = (d.N + 31) / 32 * 32;
@@ -561,6 +579,28 @@ int set_params(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Pa
     return rc;
 }
 
+// The envelope rows [5][n] of instances [inst0, inst0+n) that states (or NULL: leave envelope mode) give; env_instances and
+// the mode mirror follow.  Every writer of env row 4 is a call issued from the host (create, _set_preset_mute,
+// _copy_instances, _import_instances, _state_import and the lane fade calls), so the mirror is exact at issue time.
+template <class A>
+void preset_rows(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz, uint32_t *rows)
+{
+    memset(rows, 0, (size_t)5 * n * 4);
+    for (uint32_t i = 0; i < n; i++) {
+        uint8_t &on = c->env_mode[inst0 + i];
+        if (on) c->env_instances--;
+        on = states ? 1 : 0;
+        if (states) {
+            rows[0 * n + i] = states[i].loading ? 1u : 0u;
+            rows[1 * n + i] = states[i].counter;
+            memcpy(&rows[2 * n + i], &states[i].smooth_gain, 4);
+            rows[3 * n + i] = sample_rate_hz;
+            rows[4 * n + i] = 1u;
+            c->env_instances++;
+        }
+    }
+}
+
 // preset-mute envelope of instances [inst0, inst0+n): states == NULL leaves envelope mode (the constant preset_mute_gain of
 // set_params applies again)
 template <class A>
@@ -571,20 +611,8 @@ int set_preset_mute(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_pres
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     const size_t Np = c->d.N_pad;
-    std::vector<uint32_t> cur((size_t)n), rows((size_t)5 * n, 0u);
-    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    for (uint32_t i = 0; i < n; i++) {
-        if (cur[i]) c->env_instances--;
-        if (states) {
-            rows[0 * n + i] = states[i].loading ? 1u : 0u;
-            rows[1 * n + i] = states[i].counter;
-            memcpy(&rows[2 * n + i], &states[i].smooth_gain, 4);
-            rows[3 * n + i] = sample_rate_hz;
-            rows[4 * n + i] = 1u;
-            c->env_instances++;
-        }
-    }
+    std::vector<uint32_t> rows((size_t)5 * n);
+    preset_rows(c, inst0, n, states, sample_rate_hz, rows.data());
     CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, Np * 4, rows.data(), (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, c->stream));
     CU_OK(cudaStreamSynchronize(c->stream));
     return DSPI_OK;
@@ -657,10 +685,11 @@ int set_rate_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *sa
     return bulk::set_rate<typename A::Stores>(c, c->bulk, inst0, n, sample_rates, results);
 }
 
+// the argument checks of *_edit_bulk_device (c not NULL)
 template <class A>
-int edit_bulk_device(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results)
+int check_edits(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *edits, float sample_rate)
 {
-    if (!c || !edits) return fail(DSPI_EINVAL, "null argument");
+    if (!edits) return fail(DSPI_EINVAL, "null argument");
     if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
     // control-plane sections: the record keeps them zero and the collect kernel stamps them
     static const uint32_t kPlane[][2] = { { 0, 16 },
@@ -676,9 +705,17 @@ int edit_bulk_device(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *ed
             if (lo < p[1] && hi > p[0]) return fail(DSPI_EINVAL, "edit %u: bytes [%u, %u) touch a control-plane section", k, lo, hi);
         if (e.instance >= c->desc.n_instances) return fail(DSPI_ERANGE, "edit %u names instance %u, outside engine of %u", k, e.instance, c->desc.n_instances);
     }
-    if (n_edits == 0) return DSPI_OK;
+    return DSPI_OK;
+}
+
+template <class A>
+int edit_bulk_device(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results)
+{
+    if (!c) return fail(DSPI_EINVAL, "null argument");
+    const int rc = check_edits(c, n_edits, edits, sample_rate);
+    if (rc || n_edits == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::edit<typename A::Stores>(c, c->bulk, c->bulk_edit, n_edits, edits, exact_db, sample_rate, results);
+    return bulk::edit<typename A::Stores>(c, c->stream, c->bulk, c->bulk_edit, nullptr, n_edits, edits, exact_db, sample_rate, results);
 }
 
 template <class A>
@@ -1052,6 +1089,22 @@ Lane *lane_of(ChainHost<A> *c, uint32_t lane)
     return &c->lanes[lane];
 }
 
+// instances [inst0, inst0 + n) inside lane l's window, and where its calls start
+int check_lane_window(const Lane *l, uint32_t lane, uint32_t inst0, uint32_t n)
+{
+    if (inst0 < l->inst0 || (uint64_t)inst0 + n > (uint64_t)l->inst0 + l->n)
+        return fail(DSPI_ERANGE, "instances [%u, %llu) outside lane %u's window [%u, %u)", inst0, (unsigned long long)inst0 + n, lane, l->inst0,
+                    l->inst0 + l->n);
+    return DSPI_OK;
+}
+
+template <class A>
+cudaError_t lane_begin(ChainHost<A> *c, Lane &l)
+{
+    cudaError_t e = cudaEventRecord(l.ev_engine, c->stream);
+    return e == cudaSuccess ? cudaStreamWaitEvent(l.stream, l.ev_engine, 0) : e;
+}
+
 template <class A>
 int lane_close(ChainHost<A> *c, uint32_t lane)
 {
@@ -1071,14 +1124,9 @@ int lane_process(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n, con
     Lane *l = lane_of(c, lane);
     if (!l) return DSPI_EINVAL;
     int rc = check_call(c, l->sched, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, subframes);
-    if (rc) return rc;
-    if (inst0 < l->inst0 || (uint64_t)inst0 + n > (uint64_t)l->inst0 + l->n)
-        return fail(DSPI_ERANGE, "instances [%u, %llu) outside lane %u's window [%u, %u)", inst0, (unsigned long long)inst0 + n, lane, l->inst0,
-                    l->inst0 + l->n);
-    if (n == 0) return DSPI_OK;
+    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaEventRecord(l->ev_engine, c->stream));
-    CU_OK(cudaStreamWaitEvent(l->stream, l->ev_engine, 0));
+    CU_OK(lane_begin(c, *l));
     rc = issue_call(c, Issue{ l->stream, l->st, l->sched }, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
     CU_OK(cudaEventRecord(l->ev_last, l->stream));
     return rc;
@@ -1097,6 +1145,91 @@ int lane_sync(ChainHost<A> *c, uint32_t lane)
     if (!l) return DSPI_EINVAL;
     CU_OK(cudaSetDevice(c->desc.device));
     CU_OK(cudaStreamSynchronize(l->stream));
+    return DSPI_OK;
+}
+
+// ---- lane control calls: the engine-level control calls a running clock group needs, issued on its lane ---------------
+// Each takes the engine-level call's checks, then requires every instance it names inside the lane's window.  It is issued
+// like a lane process call (behind the engine stream as it is now, ending with ev_last) and does not wait for the device.
+
+template <class A>
+int lane_edit_bulk_device(ChainHost<A> *c, uint32_t lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate,
+                          int32_t *d_results)
+{
+    Lane *l = lane_of(c, lane);
+    if (!l) return DSPI_EINVAL;
+    int rc = check_edits(c, n_edits, edits, sample_rate);
+    if (rc) return rc;
+    for (uint32_t k = 0; k < n_edits; k++)
+        if (edits[k].instance < l->inst0 || edits[k].instance - l->inst0 >= l->n)
+            return fail(DSPI_ERANGE, "edit %u names instance %u, outside lane %u's window [%u, %u)", k, edits[k].instance, lane, l->inst0, l->inst0 + l->n);
+    if (n_edits == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(c->desc.device));
+    // The lane's first edit allocates its staging, and an engine whose skip rows were never set (no set_params, apply,
+    // import, copy or edit yet) remasks every row once: both wait for every lane and the engine stream first.
+    const bool skip_set = eq_skip_set(c->eq_m) && eq_skip_set(c->eq_o);
+    if (!l->bulk_edit.marks || !skip_set) {
+        CU_OK(drain(c));
+        if (!skip_set && (rc = bulk::finish_skip(c, c->stream, nullptr)) != DSPI_OK) return rc;
+    }
+    CU_OK(lane_begin(c, *l));
+    bulk::LaneScope scope{ l->inst0, l->n, l->ring };
+    rc = bulk::edit<typename A::Stores>(c, l->stream, l->bulk, l->bulk_edit, &scope, n_edits, edits, exact_db, sample_rate, nullptr, d_results);
+    CU_OK(cudaEventRecord(l->ev_last, l->stream));
+    return rc;
+}
+
+template <class A>
+int lane_set_preset_mute(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
+{
+    Lane *l = lane_of(c, lane);
+    if (!l) return DSPI_EINVAL;
+    int rc = check_range(c, inst0, n);
+    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    unsigned char *buf = nullptr;
+    CU_OK(l->ring.take((size_t)5 * n * 4, &buf));
+    preset_rows(c, inst0, n, states, sample_rate_hz, (uint32_t *)buf);
+    CU_OK(lane_begin(c, *l));
+    CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, (size_t)c->d.N_pad * 4, buf, (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, l->stream));
+    CU_OK(l->ring.done(l->stream));
+    CU_OK(cudaEventRecord(l->ev_last, l->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+int lane_set_spdif_tx(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
+{
+    Lane *l = lane_of(c, lane);
+    if (!l) return DSPI_EINVAL;
+    if (!tx) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(c, inst0, n);
+    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    unsigned char *buf = nullptr;
+    CU_OK(l->ring.take((size_t)n * 12, &buf));
+    uint64_t *cs = (uint64_t *)buf;                                          // channel status words, then block positions
+    uint32_t *bp = (uint32_t *)(buf + (size_t)n * 8);
+    if (!spdif_tx_unpack(tx, n, bp, cs)) return fail(DSPI_EINVAL, "block_pos must be 0..191");
+    CU_OK(lane_begin(c, *l));
+    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp, (size_t)n * 4, cudaMemcpyHostToDevice, l->stream));
+    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs, (size_t)n * 8, cudaMemcpyHostToDevice, l->stream));
+    CU_OK(l->ring.done(l->stream));
+    CU_OK(cudaEventRecord(l->ev_last, l->stream));
+    return DSPI_OK;
+}
+
+template <class A>
+int lane_reset_instances(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n)
+{
+    Lane *l = lane_of(c, lane);
+    if (!l) return DSPI_EINVAL;
+    int rc = check_range(c, inst0, n);
+    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    CU_OK(lane_begin(c, *l));
+    CU_OK(reset_range(c, inst0, n, l->stream));
+    CU_OK(cudaEventRecord(l->ev_last, l->stream));
     return DSPI_OK;
 }
 
@@ -1236,7 +1369,10 @@ int state_import(ChainHost<A> *c, const void *blob, size_t len)
     CU_OK(cudaMemcpyAsync(on.data(), c->d.env + (size_t)4 * c->d.N_pad, (size_t)c->d.N * 4, cudaMemcpyDeviceToHost, c->stream));
     CU_OK(cudaStreamSynchronize(c->stream));
     c->env_instances = 0;
-    for (uint32_t x : on) c->env_instances += x ? 1u : 0u;
+    for (uint32_t i = 0; i < c->d.N; i++) {
+        c->env_mode[i] = on[i] ? 1 : 0;
+        c->env_instances += on[i] ? 1u : 0u;
+    }
     return DSPI_OK;
 }
 
@@ -1327,6 +1463,7 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
         memcpy(&on, img + (size_t)i * stride + env_off, 4);
         before += cur[i] ? 1u : 0u;
         after += on ? 1u : 0u;
+        c->env_mode[inst0 + i] = on ? 1 : 0;
     }
     uint32_t chunk = 0;
     CU_OK(c->resp.stage(size, n, c->stream, &chunk));
@@ -1391,6 +1528,7 @@ int copy_instances(ChainHost<A> *c, uint32_t n, const uint32_t *src, const uint3
     for (uint32_t k = 0; k < n; k++) {
         before += mode[dst[k] - lo] ? 1u : 0u;
         after += mode[src[k] - lo] ? 1u : 0u;
+        c->env_mode[dst[k]] = mode[src[k] - lo] ? 1 : 0;
     }
     RoleRange rm, ro;
     role_ranges(c, rm, ro);

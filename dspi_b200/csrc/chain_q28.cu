@@ -1076,6 +1076,17 @@ int dspi_chainq_lane_process_subframes_device(dspi_chainq *c, uint32_t lane, uin
 }
 void *dspi_chainq_lane_stream(dspi_chainq *c, uint32_t lane) { return dspi::lane_stream(c, lane); }
 int dspi_chainq_lane_sync(dspi_chainq *c, uint32_t lane) { return dspi::lane_sync(c, lane); }
+int dspi_chainq_lane_edit_bulk_device(dspi_chainq *c, uint32_t lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate,
+                                 int32_t *d_results)
+{
+    return dspi::lane_edit_bulk_device(c, lane, n_edits, edits, exact_db, sample_rate, d_results);
+}
+int dspi_chainq_lane_set_preset_mute(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
+{
+    return dspi::lane_set_preset_mute(c, lane, inst0, n, states, sample_rate_hz);
+}
+int dspi_chainq_lane_set_spdif_tx(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx) { return dspi::lane_set_spdif_tx(c, lane, inst0, n, tx); }
+int dspi_chainq_lane_reset_instances(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n) { return dspi::lane_reset_instances(c, lane, inst0, n); }
 
 
 }  // extern "C"

@@ -93,6 +93,7 @@ struct dspi_eq {
     uint32_t tm_T, tm_ld, tm_rows;
     // kernel choice (float engines): re-derived after every coefficient upload
     bool sig_dirty;
+    bool sig_stale;          // rows re-packed by a lane control call since the last choice (eq_choice_stale)
     void *jit;               // run-time specialised K1 (eq_jit.cu) or nullptr = ahead-of-time kernels
     char kinfo[320];
     dspi::ResponseBuffers resp;   // frequency table and host staging of dspi_eq_response_*
@@ -561,6 +562,51 @@ int eq_set_skip(dspi_eq *e, const uint8_t *d_skip, cudaStream_t s)
     if (rc) return rc;
     CU_OK(cudaStreamSynchronize(s));
     return DSPI_OK;
+}
+
+// ---- lane control calls of the chain engines: one instance window's rows, never synchronising --------------------------
+bool eq_skip_set(const dspi_eq *e) { return e->d_skip && (e->desc.arith == DSPI_ARITH_Q28 || e->d_modes_eff); }
+
+int eq_remask_rows(dspi_eq *e, uint32_t ch0, uint32_t n, const RoleRange &rr, cudaStream_t s)
+{
+    if (n == 0 || !e->d_skip) return DSPI_OK;
+    if (!eq_skip_set(e)) return fail(DSPI_EINVAL, "skip rows were never set on this engine");
+    CU_OK(cudaSetDevice(e->desc.device));
+    for (uint32_t r = 0; r < rr.roles; r++) {
+        const size_t c = (size_t)ch0 + (size_t)r * rr.stride;
+        if (e->desc.arith == DSPI_ARITH_Q28)         // groups of 32 channels; c is a multiple of 32
+            CU_OK(launch_skip_q28((int32_t *)e->d_coef + c / 32 * DSPI_MAX_BANDS * 20 * 32, e->d_skip + c, n, s));
+        else
+            CU_OK(launch_mask_modes(e->d_modes + c, e->d_skip + c, e->d_modes_eff + c, n, s));
+        e->launches++;
+    }
+    e->sig_stale = e->desc.arith != DSPI_ARITH_Q28;
+    return DSPI_OK;
+}
+
+int eq_pack_rows(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s, const RoleRange &rr, uint32_t win0, uint32_t win_n)
+{
+    if (n == 0) return DSPI_OK;
+    CU_OK(cudaSetDevice(e->desc.device));
+    if (e->desc.arith == DSPI_ARITH_Q28)
+        CU_OK(launch_pack_q28((const dspi_biquad_q28 *)e->d_aos, ch0, n, (int32_t *)e->d_coef, s, rr));
+    else
+        CU_OK(launch_pack_f32((const dspi_biquad_f32 *)e->d_aos, ch0, n, (float *)e->d_coef, e->d_modes, e->cpl, s, rr));
+    e->launches++;
+    e->sig_stale = e->desc.arith != DSPI_ARITH_Q28;
+    RoleRange w;
+    w.roles = rr.roles;
+    w.stride = rr.stride;
+    return eq_remask_rows(e, win0, win_n, w, s);
+}
+
+bool eq_choice_stale(const dspi_eq *e) { return e->sig_stale; }
+
+int eq_refresh_choice(dspi_eq *e)
+{
+    e->sig_stale = false;
+    CU_OK(cudaSetDevice(e->desc.device));
+    return refresh_kernel_choice(e);
 }
 
 // the device arrays that make up an engine's coefficient + filter state (checkpointing by the chain engines)

@@ -85,6 +85,19 @@ int eq_unpack_range(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s, const 
 // usb_audio.c:721-728 (bypass_master_eq), :879-884 (muted / disabled outputs).  `d_skip` is [n_channels]
 // device memory owned by the caller; call again after changing it.
 int eq_set_skip(dspi_eq *e, const uint8_t *d_skip, cudaStream_t s);
+// Lane control calls of the chain engines.  Other lanes' K1 / K2 launches may be in flight, so these touch the rows of one
+// instance window only, row ch0 + r * rr.stride + i for r < rr.roles and i < n, and never synchronise:
+//   eq_pack_rows    eq_pack_range's pack (any RoleRange), then the skip remask of the window rows [win0, win0 + win_n) per role
+//   eq_remask_rows  the skip rows of the window into the effective modes (float) or the packed store (Q28); refused until
+//                   eq_set_skip ran once (eq_skip_set), since the first remask covers every row
+// Neither re-selects the K1 kernel: that reads every row's modes, synchronises and may load a module.  They mark the choice
+// stale instead (eq_choice_stale), and the chain engine's next engine-level call re-selects it (eq_refresh_choice) once
+// the lanes' work has finished.  Only speed depends on the choice: every K1 warp checks its own rows' topology.
+bool eq_skip_set(const dspi_eq *e);
+int eq_pack_rows(dspi_eq *e, uint32_t ch0, uint32_t n, cudaStream_t s, const RoleRange &rr, uint32_t win0, uint32_t win_n);
+int eq_remask_rows(dspi_eq *e, uint32_t ch0, uint32_t n, const RoleRange &rr, cudaStream_t s);
+bool eq_choice_stale(const dspi_eq *e);
+int eq_refresh_choice(dspi_eq *e);
 int eq_process_on(dspi_eq *e, void *d_samples, uint32_t T, uint32_t ld, cudaStream_t s);
 int eq_process_range_on(dspi_eq *e, void *d_rows, uint32_t T, uint32_t ld, uint32_t ch0, uint32_t n, cudaStream_t s);
 // staged copy-in / kernel / copy-out pipeline of channels [ch0, ch0 + n_ch) against `remote` rows [n_ch][T] (pinned host
