@@ -1019,13 +1019,6 @@ struct HostRing {
     }
 };
 
-// The scope of a lane control call (chain_host.cuh, Lane): the instance window it may touch and the pinned ring its uploads
-// go through.  Engine-level calls pass none: they touch every row, stage through pageable memory and synchronise.
-struct LaneScope {
-    uint32_t inst0, n;
-    HostRing &ring;
-};
-
 // d_results of a lane edit: grouped edit j of a chunk is edit pos[j] of the call, whose instance is segment seg[j]
 static __global__ void edit_marks_kernel(const int32_t *__restrict__ marks, const uint32_t *__restrict__ pos, const uint32_t *__restrict__ seg,
                                          uint32_t n, int32_t *__restrict__ out)
@@ -1046,11 +1039,14 @@ inline int fail_cuda(cudaError_t e, const char *what)
 // stage.results is 0 (the others are left alone): state into the mirrors, coefficients from the recipes at fs (or at
 // rates[i] when rates is not null), the clamped recipes into the records, mirrors back into the packed stores.  With `inst`
 // (device, [nc]) instance i is first + inst[i]; with `band_mask` (device, [roles][nc]) only the masked bands are computed.
-// Issued on s; an engine-level call's pack synchronises, a lane's (lane != null) packs and remasks its window's rows only.
-template <class S, class Engine>
-int recalculate_filters(Engine *c, cudaStream_t s, Stage &stage, const LaneScope *lane, uint32_t first, uint32_t nc, float fs, const float *rates,
-                        const uint32_t *inst = nullptr, const uint16_t *band_mask = nullptr)
+// Issued on queue q (chain_host.cuh) with its staging; the engine's queue packs synchronously, a lane's packs and remasks its
+// window's rows only.
+template <class S, class Engine, class Queue>
+int recalculate_filters(Engine *c, Queue &q, uint32_t first, uint32_t nc, float fs, const float *rates, const uint32_t *inst = nullptr,
+                        const uint16_t *band_mask = nullptr)
 {
+    const cudaStream_t s = q.stream;
+    const Stage &stage = q.bulk;
     RoleRange rm, ro;
     rm.roles = 2; ro.roles = S::kRoles - 2;
     rm.stride = ro.stride = c->d.N_pad;
@@ -1069,43 +1065,44 @@ int recalculate_filters(Engine *c, cudaStream_t s, Stage &stage, const LaneScope
                                                                                    (size_t)nc * kMaxBands, kMaxBands, stage.results, inst, band_mask);
     if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "recipe record kernel");
     c->launches += 3;
-    if (lane) {
-        rc = eq_pack_rows(c->eq_m, first, nc, s, rm, lane->inst0, lane->n);
-        return rc == DSPI_OK ? eq_pack_rows(c->eq_o, first, nc, s, ro, lane->inst0, lane->n) : rc;
+    if (q.lane) {
+        rc = eq_pack_rows(c->eq_m, first, nc, s, rm, q.inst0, q.n);
+        return rc == DSPI_OK ? eq_pack_rows(c->eq_o, first, nc, s, ro, q.inst0, q.n) : rc;
     }
     rc = eq_pack_range(c->eq_m, first, nc, s, rm);
     if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, first, nc, s, ro);
     return rc;
 }
 
-// The skip rows into the sub-engines' effective modes after the last chunk, on s: every row, synchronising (engine
-// level), or the rows of a lane's window (lane != null; eq_skip_set must hold for both sub-engines).
-template <class Engine>
-int finish_skip(Engine *c, cudaStream_t s, const LaneScope *lane)
+// The skip rows into the sub-engines' effective modes after the last chunk, on queue q: every row, synchronising (the
+// engine's queue), or the rows of a lane's window (eq_skip_set must hold for both sub-engines).
+template <class Engine, class Queue>
+int finish_skip(Engine *c, Queue &q)
 {
-    if (lane) {
+    if (q.lane) {
         RoleRange rm, ro;
         rm.roles = 2; ro.roles = Engine::Arith::kOuts;
         rm.stride = ro.stride = c->d.N_pad;
-        const int rc = eq_remask_rows(c->eq_m, lane->inst0, lane->n, rm, s);
-        return rc == DSPI_OK ? eq_remask_rows(c->eq_o, lane->inst0, lane->n, ro, s) : rc;
+        const int rc = eq_remask_rows(c->eq_m, q.inst0, q.n, rm, q.stream);
+        return rc == DSPI_OK ? eq_remask_rows(c->eq_o, q.inst0, q.n, ro, q.stream) : rc;
     }
-    int rc = eq_set_skip(c->eq_m, c->d.skip_m, s);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, s);
+    int rc = eq_set_skip(c->eq_m, c->d.skip_m, q.stream);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, q.stream);
     return rc;
 }
 
-// The ingest path for an engine (dspi_chain or dspi_chainq) whose arguments are checked.  Everything runs on the engine
-// stream, behind earlier process calls; the last step (eq_set_skip) synchronises it.  Per chunk, stage_packets(i0, nc) puts
+// The ingest path for an engine (dspi_chain or dspi_chainq) whose arguments are checked.  Everything runs on the engine's
+// queue, behind earlier process calls; the last step (eq_set_skip) synchronises it.  Per chunk, stage_packets(i0, nc) puts
 // the packets of instances [i0, i0 + nc) of the call into stage.packets on the engine stream; `codes` (device, [kChunk]) is
 // what goes back to results, stage.results (the ingest kernel's codes) when it is null.
 template <class S, class Engine, class StagePackets>
-int ingest(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_bulk_host *host, int gain_mode, float fs, int32_t *results,
-           const int32_t *codes, StagePackets &&stage_packets)
+int ingest(Engine *c, uint32_t inst0, uint32_t n, const dspi_bulk_host *host, int gain_mode, float fs, int32_t *results, const int32_t *codes,
+           StagePackets &&stage_packets)
 {
+    Stage &stage = c->q.bulk;
     cudaError_t e = stage.ensure(S::kRoles);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
-    cudaStream_t s = c->stream;
+    cudaStream_t s = c->q.stream;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk, first = inst0 + i0;
         int rc = stage_packets(i0, nc);
@@ -1116,22 +1113,23 @@ int ingest(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_bulk_
                                                                                  stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "ingest kernel");
         c->launches++;
-        if ((rc = recalculate_filters<S>(c, s, stage, nullptr, first, nc, fs, nullptr)) != DSPI_OK) return rc;
+        if ((rc = recalculate_filters<S>(c, c->q, first, nc, fs, nullptr)) != DSPI_OK) return rc;
         if ((e = cudaMemcpyAsync(results + i0, codes ? codes : stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
             return fail_cuda(e, "result copy");
     }
-    return finish_skip(c, s, nullptr);
+    return finish_skip(c, c->q);
 }
 
 // dspi_chain(q)_set_rate_device for checked arguments: per chunk the rates go to stage.rates, rate_kernel re-derives the
 // rate-dependent rows of current instances and stages their recipes, and the filters are recalculated at each one's rate.
 // results (host, may be null) gets the marks.  On the engine stream behind earlier work; returns when the engine is updated.
 template <class S, class Engine>
-int set_rate(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const float *rates, int32_t *results)
+int set_rate(Engine *c, uint32_t inst0, uint32_t n, const float *rates, int32_t *results)
 {
+    Stage &stage = c->q.bulk;
     cudaError_t e = stage.ensure(S::kRoles);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
-    cudaStream_t s = c->stream;
+    cudaStream_t s = c->q.stream;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk, first = inst0 + i0;
         if ((e = cudaMemcpyAsync(stage.rates, rates + i0, (size_t)nc * sizeof(float), cudaMemcpyHostToDevice, s)) != cudaSuccess)
@@ -1139,12 +1137,12 @@ int set_rate(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const float *r
         rate_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.rates, stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "rate kernel");
         c->launches++;
-        int rc = recalculate_filters<S>(c, s, stage, nullptr, first, nc, 0.0f, stage.rates);
+        int rc = recalculate_filters<S>(c, c->q, first, nc, 0.0f, stage.rates);
         if (rc != DSPI_OK) return rc;
         if (results && (e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
             return fail_cuda(e, "result copy");
     }
-    return finish_skip(c, s, nullptr);
+    return finish_skip(c, c->q);
 }
 
 // dspi_chain(q)_edit_bulk_device for checked arguments.  Edits of different instances commute, so the list is cut into
@@ -1154,16 +1152,19 @@ int set_rate(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const float *r
 // with their segment table in one copy; edit_kernel applies them, and when an edit of the chunk lies in the eq section the
 // touched bands go through the filter recalculation by instance list and band mask.  eq_set_skip at the end follows the
 // skip rows and synchronises.  results (host, may be null) gets the mark of each edit's instance.
-// Everything is issued on s with the stages given.  A lane edit (lane != null, every instance inside its window) uploads
-// through the lane's pinned ring, remasks its window's rows only and does not synchronise; d_results (device, may be
-// null) gets the marks there.
-template <class S, class Engine>
-int edit(Engine *c, cudaStream_t s, Stage &stage, EditStage &es, const LaneScope *lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db,
-         float fs, int32_t *results, int32_t *d_results = nullptr)
+// Everything is issued on queue q with its staging, every instance inside its window.  A lane edit uploads through the
+// lane's pinned ring, remasks its window's rows only and does not synchronise; results is device memory there.
+template <class S, class Engine, class Queue>
+int edit(Engine *c, Queue &q, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float fs, int32_t *results)
 {
-    const uint32_t base = lane ? lane->inst0 : 0;          // es.seg and es.last are indexed by instance - base
+    const cudaStream_t s = q.stream;
+    Stage &stage = q.bulk;
+    EditStage &es = q.bulk_edit;
+    int32_t *d_results = q.lane ? results : nullptr;
+    if (q.lane) results = nullptr;
+    const uint32_t base = q.inst0;                         // es.seg and es.last are indexed by instance - base
     cudaError_t e = stage.ensure(S::kRoles);
-    if (e == cudaSuccess) e = es.ensure(S::kRoles, lane ? lane->n : c->desc.n_instances);
+    if (e == cudaSuccess) e = es.ensure(S::kRoles, q.n);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
     constexpr uint32_t eq0 = DSPI_WIRE_OFF(eq), eq1 = DSPI_WIRE_OFF(eq) + S::kRoles * kMaxBands * 16;
     std::vector<int32_t> marks;                            // per segment of the call (never more than the edits)
@@ -1209,7 +1210,7 @@ int edit(Engine *c, cudaStream_t s, Stage &stage, EditStage &es, const LaneScope
         // d_results, each grouped edit's position in the call and its segment)
         const size_t bytes = (size_t)E * sizeof(dspi_bulk_edit) + (size_t)(2 * nseg + 1) * sizeof(uint32_t) + (d_results ? (size_t)2 * E * sizeof(uint32_t) : 0);
         unsigned char *img = es.h_in.data();
-        if (lane && (e = lane->ring.take(bytes, &img)) != cudaSuccess) return fail_cuda(e, "edit staging");
+        if (q.lane && (e = q.ring.take(bytes, &img)) != cudaSuccess) return fail_cuda(e, "edit staging");
         dspi_bulk_edit *ed_h = reinterpret_cast<dspi_bulk_edit *>(img);
         uint32_t *off_h = reinterpret_cast<uint32_t *>(img + (size_t)E * sizeof(dspi_bulk_edit));
         uint32_t *pos_h = off_h + 2 * nseg + 1;
@@ -1228,7 +1229,7 @@ int edit(Engine *c, cudaStream_t s, Stage &stage, EditStage &es, const LaneScope
         for (uint32_t g = 0; g < nseg; g++) es.seg[es.inst[g] - base] = 0;
         memcpy(off_h + nseg + 1, es.inst.data(), (size_t)nseg * sizeof(uint32_t));
         if ((e = cudaMemcpyAsync(es.d_in, img, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return fail_cuda(e, "edit copy");
-        if (lane && (e = lane->ring.done(s)) != cudaSuccess) return fail_cuda(e, "edit staging");
+        if (q.lane && (e = q.ring.done(s)) != cudaSuccess) return fail_cuda(e, "edit staging");
         const dspi_bulk_edit *d_edits = reinterpret_cast<const dspi_bulk_edit *>(es.d_in);
         const uint32_t *d_off = reinterpret_cast<const uint32_t *>(es.d_in + (size_t)E * sizeof(dspi_bulk_edit)), *d_inst = d_off + nseg + 1;
         edit_kernel<S><<<(nseg + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, nseg, d_edits, d_off, d_inst, exact_db ? kGainExact : kGainTaylor,
@@ -1242,7 +1243,7 @@ int edit(Engine *c, cudaStream_t s, Stage &stage, EditStage &es, const LaneScope
             c->launches++;
         }
         if (bands) {
-            const int rc = recalculate_filters<S>(c, s, stage, lane, 0, nseg, fs, nullptr, d_inst, es.band_mask);
+            const int rc = recalculate_filters<S>(c, q, 0, nseg, fs, nullptr, d_inst, es.band_mask);
             if (rc != DSPI_OK) return rc;
         }
         if (results) {
@@ -1251,7 +1252,7 @@ int edit(Engine *c, cudaStream_t s, Stage &stage, EditStage &es, const LaneScope
                 return fail_cuda(e, "mark copy");
         }
     }
-    const int rc = finish_skip(c, s, lane);
+    const int rc = finish_skip(c, q);
     if (rc != DSPI_OK) return rc;
     for (uint32_t k = 0; results && k < n_edits; k++) results[k] = marks[seg_of[k]];
     return DSPI_OK;
@@ -1259,11 +1260,11 @@ int edit(Engine *c, cudaStream_t s, Stage &stage, EditStage &es, const LaneScope
 
 // dspi_chain(q)_apply_bulk_device for checked arguments
 template <class S, class Engine>
-int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host, int exact_db,
-          float fs, int32_t *results)
+int apply(Engine *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host, int exact_db, float fs,
+          int32_t *results)
 {
-    return ingest<S>(c, stage, inst0, n, host, exact_db ? kGainExact : kGainTaylor, fs, results, nullptr, [&](uint32_t i0, uint32_t nc) -> int {
-        const cudaError_t e = cudaMemcpyAsync(stage.packets, packets + i0, (size_t)nc * kPacketBytes, cudaMemcpyHostToDevice, c->stream);
+    return ingest<S>(c, inst0, n, host, exact_db ? kGainExact : kGainTaylor, fs, results, nullptr, [&](uint32_t i0, uint32_t nc) -> int {
+        const cudaError_t e = cudaMemcpyAsync(c->q.bulk.packets, packets + i0, (size_t)nc * kPacketBytes, cudaMemcpyHostToDevice, c->q.stream);
         return e == cudaSuccess ? DSPI_OK : fail_cuda(e, "packet copy");
     });
 }
@@ -1271,19 +1272,19 @@ int apply(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_wire_b
 // dspi_chain(q)_apply_preset_device for checked arguments: images -> packets by preset_decode_kernel, then the ingest path
 // with the flash conversion; the preset result codes go back
 template <class S, class Engine>
-int apply_preset(Engine *c, Stage &stage, PresetStage &ps, uint32_t inst0, uint32_t n, const void *images, size_t stride,
-                 const dspi_preset_load *load, const dspi_bulk_host *host, float fs, int32_t *results)
+int apply_preset(Engine *c, PresetStage &ps, uint32_t inst0, uint32_t n, const void *images, size_t stride, const dspi_preset_load *load,
+                 const dspi_bulk_host *host, float fs, int32_t *results)
 {
     constexpr size_t kSlot = sizeof(SlotOf<S>);
     cudaError_t e = ps.ensure(kSlot);
     if (e != cudaSuccess) return fail_cuda(e, "preset staging buffers");
-    return ingest<S>(c, stage, inst0, n, host, kGainFlash, fs, results, ps.results, [&](uint32_t i0, uint32_t nc) -> int {
-        cudaStream_t s = c->stream;
+    return ingest<S>(c, inst0, n, host, kGainFlash, fs, results, ps.results, [&](uint32_t i0, uint32_t nc) -> int {
+        cudaStream_t s = c->q.stream;
         cudaError_t e = cudaMemcpy2DAsync(ps.images, kSlot, static_cast<const unsigned char *>(images) + (size_t)i0 * stride, stride, kSlot, nc,
                                           cudaMemcpyHostToDevice, s);
         if (e == cudaSuccess) e = cudaMemcpyAsync(ps.load, load + i0, (size_t)nc * sizeof(dspi_preset_load), cudaMemcpyHostToDevice, s);
         if (e != cudaSuccess) return fail_cuda(e, "image copy");
-        preset_decode_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(ps.images, ps.load, nc, stage.packets, ps.results);
+        preset_decode_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(ps.images, ps.load, nc, c->q.bulk.packets, ps.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "preset decode kernel");
         c->launches++;
         return DSPI_OK;
@@ -1293,30 +1294,32 @@ int apply_preset(Engine *c, Stage &stage, PresetStage &ps, uint32_t inst0, uint3
 // The clamped recipes dspi_chain(q)_set_eq_params_device hands back ([n][roles][12], host memory) -> the records, on the
 // engine stream; returns when they are there.
 template <class S, class Engine>
-int record_recipes(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, const dspi_eq_param *recipes)
+int record_recipes(Engine *c, uint32_t inst0, uint32_t n, const dspi_eq_param *recipes)
 {
+    Stage &stage = c->q.bulk;
     cudaError_t e = stage.ensure(S::kRoles);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
     constexpr uint32_t per = S::kRoles * kMaxBands;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;
-        e = cudaMemcpyAsync(stage.recipes, recipes + (size_t)i0 * per, (size_t)nc * per * sizeof(dspi_eq_param), cudaMemcpyHostToDevice, c->stream);
+        e = cudaMemcpyAsync(stage.recipes, recipes + (size_t)i0 * per, (size_t)nc * per * sizeof(dspi_eq_param), cudaMemcpyHostToDevice, c->q.stream);
         if (e != cudaSuccess) return fail_cuda(e, "recipe copy");
-        record_recipes_kernel<<<(nc * per + 255) / 256, 256, 0, c->stream>>>(c->rec, inst0 + i0, nc, S::kRoles, stage.recipes, kMaxBands, per, nullptr);
+        record_recipes_kernel<<<(nc * per + 255) / 256, 256, 0, c->q.stream>>>(c->rec, inst0 + i0, nc, S::kRoles, stage.recipes, kMaxBands, per, nullptr);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "recipe record kernel");
         c->launches++;
     }
-    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return fail_cuda(e, "recipe record");
+    if ((e = cudaStreamSynchronize(c->q.stream)) != cudaSuccess) return fail_cuda(e, "recipe record");
     return DSPI_OK;
 }
 
 // dspi_chain(q)_collect_bulk_device for checked arguments: on the engine stream, behind everything issued before; reads only.
 template <class S, class Engine>
-int collect(Engine *c, Stage &stage, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
+int collect(Engine *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
 {
+    Stage &stage = c->q.bulk;
     cudaError_t e = stage.ensure(S::kRoles);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
-    cudaStream_t s = c->stream;
+    cudaStream_t s = c->q.stream;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;
         bulk_collect_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->rec, inst0 + i0, nc, stage.packets, stage.host, stage.results);
@@ -1339,7 +1342,7 @@ int collect_preset(Engine *c, PresetStage &ps, uint32_t inst0, uint32_t n, const
     constexpr size_t kSlot = sizeof(SlotOf<S>);
     cudaError_t e = ps.ensure(kSlot);
     if (e != cudaSuccess) return fail_cuda(e, "preset staging buffers");
-    cudaStream_t s = c->stream;
+    cudaStream_t s = c->q.stream;
     uint8_t *slots = reinterpret_cast<uint8_t *>(ps.load);
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;

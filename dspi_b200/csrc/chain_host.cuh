@@ -73,28 +73,45 @@ struct IndexLists {
     }
 };
 
-// Where a process call is issued: its stage streams and events, its packet schedule, and the stream it starts from and
-// joins back to.  The engine's own calls issue on the engine context (c->stream, c->st, c->sched), a lane's on the lane's.
-struct Issue {
-    cudaStream_t stream;
-    ChainStreams &st;
-    PacketSchedule &sched;
-};
-
-// A lane (dspi_chain_lane_*): an issue queue of its own, bound to the instance window [inst0, inst0 + n).  Its calls start
-// behind the engine stream as it was when they were issued (ev_engine) and end with ev_last, which engine-level calls
-// wait for (join_lanes).  Its control calls stage through a device staging of its own, allocated by its first edit, and
-// a ring of pinned host buffers.
-struct Lane {
-    bool open = false;
+// An issue queue: the stream a call is issued on and where it ends, the stage streams and packet schedule of its process
+// calls, the staging of its control calls, and the instance window [inst0, inst0 + n) its calls may touch.  The engine
+// issues on one over every instance (ChainHost::q).  A lane (dspi_chain_lane_*) is another, over its window: its calls
+// start behind the engine stream as it was when they were issued (ev_engine) and end with ev_last, which engine-level calls
+// wait for (join_lanes).  The device staging is allocated by the queue's first call that needs it.
+struct Queue {
+    bool lane = false;
     uint32_t inst0 = 0, n = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_engine = nullptr, ev_last = nullptr;
+    cudaStream_t stream = nullptr;   // the engine stream callers see, or the lane's; stages run on st.* between ev_begin and ev_done
     ChainStreams st;
-    PacketSchedule sched;
-    bulk::Stage bulk;                // recipes and reject codes of the lane's edits
+    PacketSchedule sched;            // packet lengths of the current call
+    bulk::Stage bulk;                // device staging of the bulk applies, collects and edits
     bulk::EditStage bulk_edit;
     bulk::HostRing ring;             // edits, fade rows and transmitter rows on their way to the device
+    cudaEvent_t ev_engine = nullptr, ev_last = nullptr;   // a lane's
+
+    // `lane` set first
+    cudaError_t create(const SmPartition &p, uint32_t max_frames)
+    {
+        cudaError_t e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+        if (e == cudaSuccess && lane) e = cudaEventCreateWithFlags(&ev_engine, cudaEventDisableTiming);
+        if (e == cudaSuccess && lane) e = cudaEventCreateWithFlags(&ev_last, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = st.create(p);
+        return e == cudaSuccess ? sched.create(max_frames) : e;
+    }
+
+    // waits for the queue's calls; a lane's queue is closed after it (no stream)
+    void destroy()
+    {
+        if (stream) cudaStreamSynchronize(stream);
+        st.destroy();
+        sched.destroy();
+        bulk.destroy();
+        bulk_edit.destroy();
+        ring.destroy();
+        for (cudaEvent_t *ev : { &ev_engine, &ev_last })
+            if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
+        if (stream) { cudaStreamDestroy(stream); stream = nullptr; }
+    }
 };
 
 // One engine: dspi_chain and dspi_chainq are this record for their arithmetic.
@@ -103,9 +120,8 @@ struct ChainHost {
     using Arith = A;
     dspi_chain_desc desc;
     typename A::Dev d;
-    cudaStream_t stream;             // the engine stream callers see; stages run on st.* between ev_begin and ev_done
+    Queue q;                         // the engine's own issue queue, over every instance
     SmPartition part;                // the modulator's SMs and the rest, shared by the engine's and the lanes' stage streams
-    ChainStreams st;
     typename A::Biquad *d_aos;       // [N_pad][roles][12] instance-major mirror of filters[][]
     dspi_eq *eq_m, *eq_o;            // EQ engines over the master rows (2 N_pad channels) and the output rows (kOuts N_pad)
     std::vector<void *> allocs;
@@ -118,21 +134,18 @@ struct ChainHost {
     uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
     std::vector<uint8_t> env_mode;   // [N] each instance's envelope-mode flag (env row 4 != 0), as the calls issued so far leave it
     uint32_t vmm_packets;            // capacity of d.vmm in packets
-    PacketSchedule sched;            // packet lengths of the current call
     ResponseBuffers resp;            // frequency table of *_response_*; host staging of *_response_host and the instance image calls
-    bulk::Stage bulk;                // device staging of *_apply_bulk_device / _collect_bulk_device, allocated by the first call
     bulk::PresetStage preset;        // device staging of *_apply_preset_device / _collect_preset_device, allocated by the first call
-    bulk::EditStage bulk_edit;       // staging of *_edit_bulk_device, allocated by the first call
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
     IndexLists copy_lists;           // device instance lists of *_copy_instances, allocated by the first call
-    Lane lanes[DSPI_CHAIN_MAX_LANES];
+    Queue lanes[DSPI_CHAIN_MAX_LANES];   // open while it has a stream
     uint32_t open_lanes;
 };
 
 // Engine-level calls run after every lane call issued before them: the engine stream waits for each open lane's last
-// call.  Every engine-level entry point passes its handle through here.  After lane control calls re-packed EQ rows,
-// the K1 kernel choice is stale (eq_choice_stale): the first engine-level call waits for that work and re-selects it.
-// With no lane open and no lane control call since the last such call it does nothing.
+// call.  Every engine-level entry point passes its handle through here (chain_abi.inc).  After lane control calls
+// re-packed EQ rows, the K1 kernel choice is stale (eq_choice_stale): the first engine-level call waits for that work and
+// re-selects it.  With no lane open and no lane control call since the last such call it does nothing.
 template <class H>
 H *join_lanes(H *c)
 {
@@ -140,12 +153,12 @@ H *join_lanes(H *c)
     const bool stale = eq_choice_stale(c->eq_m) || eq_choice_stale(c->eq_o);
     if (!c->open_lanes && !stale) return c;
     cudaSetDevice(c->desc.device);
-    for (Lane &l : c->lanes)
-        if (l.open && cudaStreamWaitEvent(c->stream, l.ev_last, 0) != cudaSuccess) {
+    for (Queue &l : c->lanes)
+        if (l.stream && cudaStreamWaitEvent(c->q.stream, l.ev_last, 0) != cudaSuccess) {
             cudaGetLastError();
             cudaStreamSynchronize(l.stream);                                // the same order, from the host
         }
-    if (stale && cudaStreamSynchronize(c->stream) == cudaSuccess) {         // a failed choice leaves the ahead-of-time kernels
+    if (stale && cudaStreamSynchronize(c->q.stream) == cudaSuccess) {       // a failed choice leaves the ahead-of-time kernels
         if (eq_choice_stale(c->eq_m)) eq_refresh_choice(c->eq_m);
         if (eq_choice_stale(c->eq_o)) eq_refresh_choice(c->eq_o);
     }
@@ -158,44 +171,65 @@ H *join_lanes(H *c)
 template <class A>
 cudaError_t drain(ChainHost<A> *c)
 {
-    for (Lane &l : c->lanes)
-        if (l.open) {
+    for (Queue &l : c->lanes)
+        if (l.stream) {
             const cudaError_t e = cudaStreamSynchronize(l.stream);
             if (e != cudaSuccess) return e;
         }
-    return cudaStreamSynchronize(c->stream);
+    return cudaStreamSynchronize(c->q.stream);
 }
 
-void lane_release(Lane &l)
+// the queue of an engine-level call, or of an open lane; NULL with the error set
+template <class A>
+Queue *engine_queue(ChainHost<A> *c)
 {
-    if (l.stream) cudaStreamSynchronize(l.stream);
-    l.st.destroy();
-    l.sched.destroy();
-    l.bulk.destroy();
-    l.bulk_edit.destroy();
-    l.ring.destroy();
-    for (cudaEvent_t *ev : { &l.ev_engine, &l.ev_last })
-        if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
-    if (l.stream) { cudaStreamDestroy(l.stream); l.stream = nullptr; }
-    l.open = false;
+    if (!c) fail(DSPI_EINVAL, "null argument");
+    return c ? &c->q : nullptr;
+}
+
+template <class A>
+Queue *lane_queue(ChainHost<A> *c, uint32_t lane)
+{
+    if (!c) { fail(DSPI_EINVAL, "null argument"); return nullptr; }
+    if (lane >= DSPI_CHAIN_MAX_LANES || !c->lanes[lane].stream) { fail(DSPI_EINVAL, "lane %u is not open", lane); return nullptr; }
+    return &c->lanes[lane];
+}
+
+// Every call on a queue is issued between these two, and they are all that differs between the engine's queue and a
+// lane's.  A lane's call starts behind the engine stream as it is now and ends by recording ev_last; it does not wait for
+// the device.  An engine-level call starts behind every lane (join_lanes, at its entry point) and returns once its work
+// is done, unless it is a process call (`wait` false).  `rc` is what issuing the call returned.
+template <class A>
+cudaError_t begin_call(ChainHost<A> *c, Queue &q)
+{
+    if (!q.lane) return cudaSuccess;
+    const cudaError_t e = cudaEventRecord(q.ev_engine, c->q.stream);
+    return e == cudaSuccess ? cudaStreamWaitEvent(q.stream, q.ev_engine, 0) : e;
+}
+
+inline int end_call(Queue &q, int rc, bool wait = true)
+{
+    CU_OK(q.lane ? cudaEventRecord(q.ev_last, q.stream) : wait && rc == DSPI_OK ? cudaStreamSynchronize(q.stream) : cudaSuccess);
+    return rc;
 }
 
 template <class A, typename T>
 cudaError_t dev_alloc(ChainHost<A> *c, T **p, size_t count, bool zero = true)
 {
-    void *q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
+    void *m = nullptr;
+    cudaError_t e = cudaMalloc(&m, count * sizeof(T));
     if (e != cudaSuccess) return e;
-    c->allocs.push_back(q);
-    *p = (T *)q;
-    return zero ? cudaMemsetAsync(q, 0, count * sizeof(T), c->stream) : cudaSuccess;
+    c->allocs.push_back(m);
+    *p = (T *)m;
+    return zero ? cudaMemsetAsync(m, 0, count * sizeof(T), c->q.stream) : cudaSuccess;
 }
 
-template <class A>
-int check_range(const ChainHost<A> *c, uint32_t inst0, uint32_t n)
+// instances [inst0, inst0 + n) inside the window of q
+int check_range(const Queue &q, uint32_t inst0, uint32_t n)
 {
-    if ((uint64_t)inst0 + n > c->desc.n_instances)
-        return fail(DSPI_ERANGE, "instances [%u, %llu) outside engine of %u", inst0, (unsigned long long)inst0 + n, c->desc.n_instances);
+    if (inst0 < q.inst0 || (uint64_t)inst0 + n > (uint64_t)q.inst0 + q.n)
+        return fail(DSPI_ERANGE, "instances [%u, %llu) outside the %s [%u, %u)", inst0, (unsigned long long)inst0 + n,
+                    q.lane ? "lane's window" : "engine's instances", q.inst0, q.inst0 + q.n);
     return DSPI_OK;
 }
 
@@ -308,13 +342,13 @@ size_t image_plan(ChainHost<A> *c, uint32_t use, image::Plan &pl)
     return pl.bytes;
 }
 
-// the pipeline reset of instances [inst0, inst0 + n) on the engine stream, or on s
+// the pipeline reset of instances [inst0, inst0 + n) on s
 template <class A>
-cudaError_t reset_range(ChainHost<A> *c, uint32_t inst0, uint32_t n, cudaStream_t s = nullptr)
+cudaError_t reset_range(ChainHost<A> *c, uint32_t inst0, uint32_t n, cudaStream_t s)
 {
     image::Plan pl;
     if (!image_plan(c, kReset, pl)) return cudaErrorInvalidValue;
-    image::instance_image_kernel<image::kReset><<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, s ? s : c->stream>>>(pl, inst0, n, nullptr);
+    image::instance_image_kernel<image::kReset><<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, s>>>(pl, inst0, n, nullptr);
     c->launches++;
     return cudaGetLastError();
 }
@@ -323,8 +357,8 @@ cudaError_t reset_range(ChainHost<A> *c, uint32_t inst0, uint32_t n, cudaStream_
 template <class A>
 cudaError_t init_states(ChainHost<A> *c)
 {
-    cudaError_t e = reset_range(c, 0, c->d.N_pad);
-    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
+    cudaError_t e = reset_range(c, 0, c->d.N_pad, c->q.stream);
+    return e == cudaSuccess ? cudaStreamSynchronize(c->q.stream) : e;
 }
 
 // a new engine's transmitters: block position 0, the channel status init_spdif_buffer() stamps (audio_spdif.c:82-88)
@@ -332,9 +366,9 @@ template <class A>
 cudaError_t init_spdif_tx(ChainHost<A> *c)
 {
     const std::vector<uint64_t> cs(c->d.N_pad, kSpdifDefaultCs40);
-    cudaError_t e = cudaMemsetAsync(c->tx.bp, 0, (size_t)c->d.N_pad * 4, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(c->tx.cs40, cs.data(), (size_t)c->d.N_pad * 8, cudaMemcpyHostToDevice, c->stream);
-    return e == cudaSuccess ? cudaStreamSynchronize(c->stream) : e;
+    cudaError_t e = cudaMemsetAsync(c->tx.bp, 0, (size_t)c->d.N_pad * 4, c->q.stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(c->tx.cs40, cs.data(), (size_t)c->d.N_pad * 8, cudaMemcpyHostToDevice, c->q.stream);
+    return e == cudaSuccess ? cudaStreamSynchronize(c->q.stream) : e;
 }
 
 // ---- lifetime ----------------------------------------------------------------------------------------------------------
@@ -343,16 +377,13 @@ int destroy(H *c)
 {
     if (!c) return DSPI_OK;
     cudaSetDevice(c->desc.device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    for (Lane &l : c->lanes) lane_release(l);
+    if (c->q.stream) cudaStreamSynchronize(c->q.stream);
+    for (Queue &l : c->lanes) l.destroy();
     c->open_lanes = 0;
-    c->st.destroy();
+    c->q.destroy();
     c->part.destroy();
-    c->sched.destroy();
     c->resp.destroy();
-    c->bulk.destroy();
     c->preset.destroy();
-    c->bulk_edit.destroy();
     c->copy_lists.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
@@ -361,7 +392,6 @@ int destroy(H *c)
     if (c->d_spdif) cudaFree(c->d_spdif);
     if (c->d_pdmout) cudaFree(c->d_pdmout);
     if (c->d.vmm) cudaFree(c->d.vmm);
-    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
     cudaGetLastError();
     return DSPI_OK;
@@ -404,18 +434,17 @@ int create(H **out, const dspi_chain_desc *desc)
         if (rc == DSPI_OK) rc = dspi_eq_create(&c->eq_o, &ed);
         if (rc != DSPI_OK) { destroy(c); return rc; }
     }
-    cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = c->part.create(desc->device, desc->n_instances);
-    if (e == cudaSuccess) e = c->st.create(c->part);
+    c->q.n = desc->n_instances;
+    cudaError_t e = c->part.create(desc->device, desc->n_instances);
+    if (e == cudaSuccess) e = c->q.create(c->part, d.max_frames);
     if (e != cudaSuccess && c->part.g_pdm) {                                // no streams in the partition: run without one
         cudaGetLastError();
-        c->st.destroy();
+        c->q.destroy();
         c->part.destroy();
-        e = c->st.create(c->part);
+        e = c->q.create(c->part, d.max_frames);
     }
 #define TRY(x) if (e == cudaSuccess) e = (x)
-    TRY(c->sched.create(d.max_frames));
-    d.off = c->sched.d_off;
+    d.off = c->q.sched.d_off;
     TRY(dev_alloc(c, &c->d_aos, Np * A::kRoles * DSPI_MAX_BANDS));
     TRY(dev_alloc(c, &d.preamp, 2 * Np));
     TRY(dev_alloc(c, &d.flags, Np));
@@ -454,7 +483,7 @@ int create(H **out, const dspi_chain_desc *desc)
     TRY(dev_alloc(c, &c->rec.packets, Np));
     TRY(dev_alloc(c, &c->rec.host, Np));
     TRY(dev_alloc(c, &c->rec.mark, Np));
-    TRY(cudaMemsetAsync(c->rec.mark, DSPI_BULK_UNSET, Np, c->stream));
+    TRY(cudaMemsetAsync(c->rec.mark, DSPI_BULK_UNSET, Np, c->q.stream));
     TRY(init_states(c));
     TRY(init_spdif_tx(c));
 #undef TRY
@@ -507,7 +536,7 @@ template <class A>
 int set_params(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Params *params)
 {
     if (!c || !params) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     const auto &d = c->d;
@@ -515,8 +544,8 @@ int set_params(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Pa
     constexpr int O = A::kOuts;
     ParamRows<A> r(n);
     decltype(r.xf) xf_cur(7 * n);
-    CU_OK(cudaMemcpy2DAsync(xf_cur.data(), (size_t)n * 4, d.xf + inst0, Np * 4, (size_t)n * 4, 7, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaMemcpy2DAsync(xf_cur.data(), (size_t)n * 4, d.xf + inst0, Np * 4, (size_t)n * 4, 7, cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     for (uint32_t i = 0; i < n; i++) {
         const typename A::Params &p = params[i];
         A::pack(p, i, n, r);
@@ -553,7 +582,7 @@ int set_params(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Pa
     auto put = [&](auto *dst_base, const auto &src, int rows) -> cudaError_t {
         const size_t elem = sizeof(*dst_base);
         return cudaMemcpy2DAsync((char *)dst_base + (size_t)inst0 * elem, Np * elem, src.data(), (size_t)n * elem, (size_t)n * elem, rows,
-                                 cudaMemcpyHostToDevice, c->stream);
+                                 cudaMemcpyHostToDevice, c->q.stream);
     };
     CU_OK(put(d.preamp, r.preamp, 2));
     CU_OK(put(d.flags, r.flags, 1));
@@ -571,11 +600,11 @@ int set_params(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Pa
     CU_OK(put(d.o_flags, r.oflags, O));
     CU_OK(put(d.o_dly, r.dly, O));
     CU_OK(put(d.skip_m, r.skip_m, 2));
-    CU_OK(bulk::mark_stale(c->rec, inst0, n, c->stream));
+    CU_OK(bulk::mark_stale(c->rec, inst0, n, c->q.stream));
     CU_OK(put(d.skip_o, r.skip_o, O));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    rc = eq_set_skip(c->eq_m, d.skip_m, c->stream);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, d.skip_o, c->stream);
+    CU_OK(cudaStreamSynchronize(c->q.stream));
+    rc = eq_set_skip(c->eq_m, d.skip_m, c->q.stream);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, d.skip_o, c->q.stream);
     return rc;
 }
 
@@ -602,33 +631,34 @@ void preset_rows(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_preset_
 }
 
 // preset-mute envelope of instances [inst0, inst0+n): states == NULL leaves envelope mode (the constant preset_mute_gain of
-// set_params applies again)
+// set_params applies again); on queue q (the engine's or a lane's)
 template <class A>
-int set_preset_mute(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
+int set_preset_mute(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
 {
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    if (!q) return DSPI_EINVAL;
+    int rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    const size_t Np = c->d.N_pad;
-    std::vector<uint32_t> rows((size_t)5 * n);
-    preset_rows(c, inst0, n, states, sample_rate_hz, rows.data());
-    CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, Np * 4, rows.data(), (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    unsigned char *buf = nullptr;
+    CU_OK(q->ring.take((size_t)5 * n * 4, &buf));
+    preset_rows(c, inst0, n, states, sample_rate_hz, (uint32_t *)buf);
+    CU_OK(begin_call(c, *q));
+    CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, (size_t)c->d.N_pad * 4, buf, (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, q->stream));
+    CU_OK(q->ring.done(q->stream));
+    return end_call(*q, DSPI_OK);
 }
 
 template <class A>
 int get_preset_mute(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states)
 {
     if (!c || !states) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     const size_t Np = c->d.N_pad;
     std::vector<uint32_t> rows((size_t)3 * n);
-    CU_OK(cudaMemcpy2DAsync(rows.data(), (size_t)n * 4, c->d.env + inst0, Np * 4, (size_t)n * 4, 3, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaMemcpy2DAsync(rows.data(), (size_t)n * 4, c->d.env + inst0, Np * 4, (size_t)n * 4, 3, cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     for (uint32_t i = 0; i < n; i++) {
         memset(&states[i], 0, sizeof(states[i]));
         states[i].loading = (uint8_t)rows[0 * n + i];
@@ -643,17 +673,17 @@ template <class A>
 int set_dynamics_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_dynamics_config *cfgs, float sample_rate)
 {
     if (!c || !cfgs) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     dspi_dynamics_config *d_cfg = nullptr;
     CU_OK(cudaMalloc((void **)&d_cfg, (size_t)n * sizeof(*cfgs)));
-    cudaError_t e = cudaMemcpyAsync(d_cfg, cfgs, (size_t)n * sizeof(*cfgs), cudaMemcpyHostToDevice, c->stream);
+    cudaError_t e = cudaMemcpyAsync(d_cfg, cfgs, (size_t)n * sizeof(*cfgs), cudaMemcpyHostToDevice, c->q.stream);
     if (e == cudaSuccess) {
-        A::dynamics<<<(n + 127) / 128, 128, 0, c->stream>>>(c->d, c->rec, inst0, n, d_cfg, sample_rate);
+        A::dynamics<<<(n + 127) / 128, 128, 0, c->q.stream>>>(c->d, c->rec, inst0, n, d_cfg, sample_rate);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->q.stream);
     cudaFree(d_cfg);
     if (e != cudaSuccess) return fail(DSPI_ECUDA, "dynamics coefficient generation: %s", cudaGetErrorString(e));
     c->launches++;
@@ -666,28 +696,29 @@ int apply_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_wi
 {
     if (!c || !packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
     if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::apply<typename A::Stores>(c, c->bulk, inst0, n, packets, host, exact_db, sample_rate, results);
+    return bulk::apply<typename A::Stores>(c, inst0, n, packets, host, exact_db, sample_rate, results);
 }
 
 template <class A>
 int set_rate_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results)
 {
     if (!c || !sample_rates) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);                     // before the rates are read: n counts them
+    int rc = check_range(c->q, inst0, n);                     // before the rates are read: n counts them
     if (rc) return rc;
     for (uint32_t i = 0; i < n; i++)
         if (!(sample_rates[i] > 0.0f) || sample_rates[i] > 3.4e38f) return fail(DSPI_EINVAL, "sample_rates[%u] must be positive and finite", i);
     if (n == 0) return DSPI_OK;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::set_rate<typename A::Stores>(c, c->bulk, inst0, n, sample_rates, results);
+    return bulk::set_rate<typename A::Stores>(c, inst0, n, sample_rates, results);
 }
 
-// the argument checks of *_edit_bulk_device (c not NULL)
+// the argument checks of *_edit_bulk_device on queue q: every edit well formed and naming an instance of the engine,
+// then every instance inside q's window
 template <class A>
-int check_edits(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *edits, float sample_rate)
+int check_edits(ChainHost<A> *c, const Queue &q, uint32_t n_edits, const dspi_bulk_edit *edits, float sample_rate)
 {
     if (!edits) return fail(DSPI_EINVAL, "null argument");
     if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
@@ -705,27 +736,39 @@ int check_edits(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *edits, 
             if (lo < p[1] && hi > p[0]) return fail(DSPI_EINVAL, "edit %u: bytes [%u, %u) touch a control-plane section", k, lo, hi);
         if (e.instance >= c->desc.n_instances) return fail(DSPI_ERANGE, "edit %u names instance %u, outside engine of %u", k, e.instance, c->desc.n_instances);
     }
+    for (uint32_t k = 0; k < n_edits; k++)
+        if (edits[k].instance < q.inst0 || edits[k].instance - q.inst0 >= q.n)
+            return fail(DSPI_ERANGE, "edit %u names instance %u, outside the lane's window [%u, %u)", k, edits[k].instance, q.inst0, q.inst0 + q.n);
     return DSPI_OK;
 }
 
+// results: host memory for the engine's queue, device memory for a lane's (may be NULL)
 template <class A>
-int edit_bulk_device(ChainHost<A> *c, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results)
+int edit_bulk_device(ChainHost<A> *c, Queue *q, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results)
 {
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    const int rc = check_edits(c, n_edits, edits, sample_rate);
+    if (!q) return DSPI_EINVAL;
+    int rc = check_edits(c, *q, n_edits, edits, sample_rate);
     if (rc || n_edits == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::edit<typename A::Stores>(c, c->stream, c->bulk, c->bulk_edit, nullptr, n_edits, edits, exact_db, sample_rate, results);
+    // A lane's first edit allocates its staging, and an engine whose skip rows were never set (no set_params, apply,
+    // import, copy or edit yet) remasks every row once: both wait for every lane and the engine stream first.
+    const bool skip_set = eq_skip_set(c->eq_m) && eq_skip_set(c->eq_o);
+    if (q->lane && (!q->bulk_edit.marks || !skip_set)) {
+        CU_OK(drain(c));
+        if (!skip_set && (rc = bulk::finish_skip(c, c->q)) != DSPI_OK) return rc;
+    }
+    CU_OK(begin_call(c, *q));
+    return end_call(*q, bulk::edit<typename A::Stores>(c, *q, n_edits, edits, exact_db, sample_rate, results));
 }
 
 template <class A>
 int collect_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
 {
     if (!c || !packets) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::collect<typename A::Stores>(c, c->bulk, inst0, n, packets, host, results);
+    return bulk::collect<typename A::Stores>(c, inst0, n, packets, host, results);
 }
 
 template <class A>
@@ -736,10 +779,10 @@ int apply_preset_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void 
     if (!c || !images || !load || !host || !results) return fail(DSPI_EINVAL, "null argument");
     if (image_stride < kSlot) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, kSlot);
     if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::apply_preset<typename A::Stores>(c, c->bulk, c->preset, inst0, n, images, image_stride, load, host, sample_rate, results);
+    return bulk::apply_preset<typename A::Stores>(c, c->preset, inst0, n, images, image_stride, load, host, sample_rate, results);
 }
 
 template <class A>
@@ -749,7 +792,7 @@ int collect_preset_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const uin
     constexpr size_t kSlot = sizeof(bulk::SlotOf<typename A::Stores>);
     if (!c || !slot_indices || !images) return fail(DSPI_EINVAL, "null argument");
     if (image_stride < kSlot) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, kSlot);
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     return bulk::collect_preset<typename A::Stores>(c, c->preset, inst0, n, slot_indices, images, image_stride, results);
@@ -759,22 +802,22 @@ template <class A>
 int upload_biquads(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Biquad *biquads)
 {
     if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     using B = typename A::Biquad;
     const size_t row = (size_t)A::kRoles * DSPI_MAX_BANDS;
-    CU_OK(cudaMemcpyAsync(c->d_aos + inst0 * row, biquads, n * row * sizeof(B), cudaMemcpyHostToDevice, c->stream));
+    CU_OK(cudaMemcpyAsync(c->d_aos + inst0 * row, biquads, n * row * sizeof(B), cudaMemcpyHostToDevice, c->q.stream));
     const uint32_t Np = c->d.N_pad, items = n * A::kRoles * DSPI_MAX_BANDS;
-    A::scatter<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (B *)eq_aos_mirror(c->eq_m), (B *)eq_aos_mirror(c->eq_o), 1);
+    A::scatter<<<(items + 255) / 256, 256, 0, c->q.stream>>>(c->d_aos, inst0, n, Np, (B *)eq_aos_mirror(c->eq_m), (B *)eq_aos_mirror(c->eq_o), 1);
     CU_OK(cudaGetLastError());
     c->launches++;
     for (int role = 0; role < A::kRoles; role++) {
-        rc = role < 2 ? eq_pack_range(c->eq_m, role * Np + inst0, n, c->stream) : eq_pack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
+        rc = role < 2 ? eq_pack_range(c->eq_m, role * Np + inst0, n, c->q.stream) : eq_pack_range(c->eq_o, (role - 2) * Np + inst0, n, c->q.stream);
         if (rc) return rc;
     }
-    CU_OK(bulk::mark_stale(c->rec, inst0, n, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(bulk::mark_stale(c->rec, inst0, n, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     return DSPI_OK;
 }
 
@@ -782,12 +825,12 @@ template <class A>
 int set_eq_params_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_eq_param *recipes, float sample_rate)
 {
     if (!c || !recipes) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     // the sub-engines generate and pack on their own streams: everything issued on the engine stream so far (an
     // asynchronous process_device in particular) must have finished reading the coefficient stores first
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     const uint32_t Np = c->d.N_pad;
     std::vector<dspi_eq_param> tmp((size_t)n * DSPI_MAX_BANDS);
     for (int role = 0; role < A::kRoles; role++) {                  // filter_recipes[role][band] of every instance -> one engine range per role
@@ -799,28 +842,28 @@ int set_eq_params_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_eq_pa
         for (uint32_t i = 0; i < n; i++)                            // the clamps, written back like the reference does
             memcpy(&recipes[((size_t)i * A::kRoles + role) * DSPI_MAX_BANDS], &tmp[(size_t)i * DSPI_MAX_BANDS], DSPI_MAX_BANDS * sizeof(dspi_eq_param));
     }
-    return bulk::record_recipes<typename A::Stores>(c, c->bulk, inst0, n, recipes);
+    return bulk::record_recipes<typename A::Stores>(c, inst0, n, recipes);
 }
 
 template <class A>
 int download_biquads(ChainHost<A> *c, uint32_t inst0, uint32_t n, typename A::Biquad *biquads)
 {
     if (!c || !biquads) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     using B = typename A::Biquad;
     const uint32_t Np = c->d.N_pad, items = n * A::kRoles * DSPI_MAX_BANDS;
     for (int role = 0; role < A::kRoles; role++) {
-        rc = role < 2 ? eq_unpack_range(c->eq_m, role * Np + inst0, n, c->stream) : eq_unpack_range(c->eq_o, (role - 2) * Np + inst0, n, c->stream);
+        rc = role < 2 ? eq_unpack_range(c->eq_m, role * Np + inst0, n, c->q.stream) : eq_unpack_range(c->eq_o, (role - 2) * Np + inst0, n, c->q.stream);
         if (rc) return rc;
     }
-    A::scatter<<<(items + 255) / 256, 256, 0, c->stream>>>(c->d_aos, inst0, n, Np, (B *)eq_aos_mirror(c->eq_m), (B *)eq_aos_mirror(c->eq_o), 0);
+    A::scatter<<<(items + 255) / 256, 256, 0, c->q.stream>>>(c->d_aos, inst0, n, Np, (B *)eq_aos_mirror(c->eq_m), (B *)eq_aos_mirror(c->eq_o), 0);
     CU_OK(cudaGetLastError());
     c->launches++;
     const size_t row = (size_t)A::kRoles * DSPI_MAX_BANDS;
-    CU_OK(cudaMemcpyAsync(biquads, c->d_aos + inst0 * row, n * row * sizeof(B), cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaMemcpyAsync(biquads, c->d_aos + inst0 * row, n * row * sizeof(B), cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     return DSPI_OK;
 }
 
@@ -864,10 +907,10 @@ int eq_stage(ChainHost<A> *c, dspi_eq *eq, uint32_t roles, void *rows, uint32_t 
 }
 
 // One call over instances [inst0, inst0 + n) and the schedule x.sched has checked, with the kernel set K, issued on the
-// context x: its offsets go to the device first, on x.stream, where the call also ends.  The caller's buffers hold rows for
+// queue x: its offsets go to the device first, on x.stream, where the call also ends.  The caller's buffers hold rows for
 // the n instances.  d_spdif: words, or subframes when `subframes` is set (either may be NULL).
 template <class A, class K>
-int run_stages(ChainHost<A> *c, const Issue &x, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames,
+int run_stages(ChainHost<A> *c, Queue &x, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames,
                void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
 {
     PacketSchedule &ps = x.sched;
@@ -958,49 +1001,34 @@ int run_stages(ChainHost<A> *c, const Issue &x, uint32_t inst0, uint32_t n, cons
     return DSPI_OK;
 }
 
-// Instances [inst0, inst0 + n) of a call: inst0 on a 64-instance boundary, so that the pre and post stages' 16-instance
-// warps and every vector access of the SoA arrays stay aligned.  Checked after the arguments check_packets covers.
-template <class A>
-int check_window(const ChainHost<A> *c, uint32_t inst0, uint32_t n)
+// Instances [inst0, inst0 + n) of a call on queue q: inst0 on a 64-instance boundary, so that the pre and post stages'
+// 16-instance warps and every vector access of the SoA arrays stay aligned.  Checked after the arguments check_packets covers.
+int check_window(const Queue &q, uint32_t inst0, uint32_t n)
 {
     if (inst0 % 64u) return fail(DSPI_EINVAL, "first instance %u is not a multiple of 64", inst0);
-    return check_range(c, inst0, n);
+    return check_range(q, inst0, n);
 }
 
 // the window of a whole-engine call (a NULL handle is refused by the checks that follow)
 template <class A>
 uint32_t all_instances(const ChainHost<A> *c) { return c ? c->desc.n_instances : 0; }
 
-// the checks of a call over instances [inst0, inst0 + n) with the schedule ps
+// instances [inst0, inst0 + n) on queue q, every buffer laid out for the n instances (the whole engine: 0, n_instances)
 template <class A>
-int check_call(ChainHost<A> *c, PacketSchedule &ps, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
-               const uint16_t *packet_frames, const void *d_spdif, bool subframes)
-{
-    int rc = check_packets(c, ps, d_pcm, bit_depth, n_packets, packet_frames);
-    if (rc) return rc;
-    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
-    return check_window(c, inst0, n);
-}
-
-template <class A>
-int issue_call(ChainHost<A> *c, const Issue &x, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames,
-               void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
-{
-    return A::with_stages(c->desc, [&](auto k) {
-        return run_stages<A, decltype(k)>(c, x, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
-    });
-}
-
-// instances [inst0, inst0 + n), every buffer laid out for the n instances (the whole engine: 0, n_instances)
-template <class A>
-int process_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
+int process_device(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
                    const uint16_t *packet_frames, void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
 {
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_call(c, c->sched, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, subframes);
-    if (rc || n == 0) return rc;
+    if (!q) return DSPI_EINVAL;
+    int rc = check_packets(c, q->sched, d_pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
+    if (subframes && ((uintptr_t)d_spdif & 15)) return fail(DSPI_EINVAL, "subframes must be 16-byte aligned");
+    if ((rc = check_window(*q, inst0, n)) || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return issue_call(c, Issue{ c->stream, c->st, c->sched }, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
+    CU_OK(begin_call(c, *q));
+    rc = A::with_stages(c->desc, [&](auto k) {
+        return run_stages<A, decltype(k)>(c, *q, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
+    });
+    return end_call(*q, rc, false);
 }
 
 // host memory in and out, staged through the engine's device buffers
@@ -1009,26 +1037,26 @@ int process_host(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *pcm, u
                  const uint16_t *packet_frames, void *spdif_out, bool subframes, uint32_t *pdm_out, typename A::Status *status)
 {
     if (!c) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_packets(c, c->sched, pcm, bit_depth, n_packets, packet_frames);
+    int rc = check_packets(c, c->q.sched, pcm, bit_depth, n_packets, packet_frames);
     if (rc) return rc;
-    if ((rc = check_window(c, inst0, n)) || n == 0) return rc;
+    if ((rc = check_window(c->q, inst0, n)) || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    const size_t N = n, F = c->sched.frames, pairs = (A::kOuts - 1) / 2;   // the sub output has no S/PDIF pair
+    const size_t N = n, F = c->q.sched.frames, pairs = (A::kOuts - 1) / 2;   // the sub output has no S/PDIF pair
     const size_t in_bytes = N * F * (bit_depth == 24 ? 6 : 4), sp_bytes = N * pairs * F * (subframes ? 16 : 8), pd_bytes = N * F * 8 * 4;
     if (in_bytes > c->pcm_bytes) { if (c->d_pcm) cudaFree(c->d_pcm); c->d_pcm = nullptr; c->pcm_bytes = 0; CU_OK(cudaMalloc(&c->d_pcm, in_bytes)); c->pcm_bytes = in_bytes; }
     if (spdif_out && sp_bytes > c->spdif_bytes) { if (c->d_spdif) cudaFree(c->d_spdif); c->d_spdif = nullptr; c->spdif_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_spdif, sp_bytes)); c->spdif_bytes = sp_bytes; }
     if (pdm_out && pd_bytes > c->pdmout_bytes) { if (c->d_pdmout) cudaFree(c->d_pdmout); c->d_pdmout = nullptr; c->pdmout_bytes = 0; CU_OK(cudaMalloc((void **)&c->d_pdmout, pd_bytes)); c->pdmout_bytes = pd_bytes; }
     // the modulator writes the rows of instances with a sub only; the others go back to the caller as zeros, on every call
     // (an earlier call's bits would be there otherwise: a sub switched off since, or a longer call's [N][F][8] layout)
-    if (pdm_out) CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->stream));
-    CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = process_device(c, inst0, n, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
+    if (pdm_out) CU_OK(cudaMemsetAsync(c->d_pdmout, 0, pd_bytes, c->q.stream));
+    CU_OK(cudaMemcpyAsync(c->d_pcm, pcm, in_bytes, cudaMemcpyHostToDevice, c->q.stream));
+    rc = process_device(c, &c->q, inst0, n, c->d_pcm, bit_depth, n_packets, packet_frames, spdif_out ? c->d_spdif : nullptr, subframes,
                         pdm_out ? c->d_pdmout : nullptr, status ? c->d_status : nullptr);
     if (rc) return rc;
-    if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(typename A::Status), cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    if (spdif_out) CU_OK(cudaMemcpyAsync(spdif_out, c->d_spdif, sp_bytes, cudaMemcpyDeviceToHost, c->q.stream));
+    if (pdm_out) CU_OK(cudaMemcpyAsync(pdm_out, c->d_pdmout, pd_bytes, cudaMemcpyDeviceToHost, c->q.stream));
+    if (status) CU_OK(cudaMemcpyAsync(status, c->d_status, N * sizeof(typename A::Status), cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     return DSPI_OK;
 }
 
@@ -1042,226 +1070,103 @@ int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32
     const std::vector<uint16_t> table(n_packets, (uint16_t)fpp);
     const uint32_t n = c->desc.n_instances;
     return host ? process_host(c, 0, n, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status)
-                : process_device(c, 0, n, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status);
+                : process_device(c, &c->q, 0, n, pcm, bit_depth, n_packets, table.data(), spdif, false, pdm, status);
 }
 
 // ---- lanes: issue queues of one engine over disjoint instance windows, whose calls run concurrently -------------------
+// A lane takes process calls and the control calls a running clock group needs (edits, fades, transmitter restamps and
+// resets): set_preset_mute, set_spdif_tx, reset_instances, edit_bulk_device and process_device on its queue.
 template <class A>
 int lane_open(ChainHost<A> *c, uint32_t inst0, uint32_t n, uint32_t *lane)
 {
     if (!c || !lane) return fail(DSPI_EINVAL, "null argument");
     if (inst0 % 64u) return fail(DSPI_EINVAL, "first instance %u is not a multiple of 64", inst0);
     if (n == 0) return fail(DSPI_EINVAL, "a lane's window holds at least one instance");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc) return rc;
-    for (const Lane &l : c->lanes)
-        if (l.open && inst0 < l.inst0 + l.n && l.inst0 < inst0 + n)
+    for (const Queue &l : c->lanes)
+        if (l.stream && inst0 < l.inst0 + l.n && l.inst0 < inst0 + n)
             return fail(DSPI_EINVAL, "window [%u, %u) overlaps the open lane window [%u, %u)", inst0, inst0 + n, l.inst0, l.inst0 + l.n);
     uint32_t id = 0;
-    while (id < DSPI_CHAIN_MAX_LANES && c->lanes[id].open) id++;
+    while (id < DSPI_CHAIN_MAX_LANES && c->lanes[id].stream) id++;
     if (id == DSPI_CHAIN_MAX_LANES) return fail(DSPI_ERANGE, "%d lanes are open already", DSPI_CHAIN_MAX_LANES);
     CU_OK(cudaSetDevice(c->desc.device));
-    Lane &l = c->lanes[id];
-    cudaError_t e = cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&l.ev_engine, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&l.ev_last, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = l.st.create(c->part);
-    if (e == cudaSuccess) e = l.sched.create(c->desc.max_frames);
+    Queue &l = c->lanes[id];
+    l.lane = true;
+    l.inst0 = inst0;
+    l.n = n;
+    const cudaError_t e = l.create(c->part, c->desc.max_frames);
     if (e != cudaSuccess) {
-        lane_release(l);
+        l.destroy();
         cudaGetLastError();
         return fail(e == cudaErrorMemoryAllocation ? DSPI_ENOMEM : DSPI_ECUDA, "lane setup: %s", cudaGetErrorString(e));
     }
-    l.open = true;
-    l.inst0 = inst0;
-    l.n = n;
     c->open_lanes++;
     *lane = id;
     return DSPI_OK;
 }
 
-// the open lane `lane` of c, or NULL with the error set
-template <class A>
-Lane *lane_of(ChainHost<A> *c, uint32_t lane)
-{
-    if (!c) { fail(DSPI_EINVAL, "null argument"); return nullptr; }
-    if (lane >= DSPI_CHAIN_MAX_LANES || !c->lanes[lane].open) { fail(DSPI_EINVAL, "lane %u is not open", lane); return nullptr; }
-    return &c->lanes[lane];
-}
-
-// instances [inst0, inst0 + n) inside lane l's window, and where its calls start
-int check_lane_window(const Lane *l, uint32_t lane, uint32_t inst0, uint32_t n)
-{
-    if (inst0 < l->inst0 || (uint64_t)inst0 + n > (uint64_t)l->inst0 + l->n)
-        return fail(DSPI_ERANGE, "instances [%u, %llu) outside lane %u's window [%u, %u)", inst0, (unsigned long long)inst0 + n, lane, l->inst0,
-                    l->inst0 + l->n);
-    return DSPI_OK;
-}
-
-template <class A>
-cudaError_t lane_begin(ChainHost<A> *c, Lane &l)
-{
-    cudaError_t e = cudaEventRecord(l.ev_engine, c->stream);
-    return e == cudaSuccess ? cudaStreamWaitEvent(l.stream, l.ev_engine, 0) : e;
-}
-
 template <class A>
 int lane_close(ChainHost<A> *c, uint32_t lane)
 {
-    Lane *l = lane_of(c, lane);
+    Queue *l = lane_queue(c, lane);
     if (!l) return DSPI_EINVAL;
     CU_OK(cudaSetDevice(c->desc.device));
-    lane_release(*l);                                                       // waits for the lane's calls
+    l->destroy();                                                           // waits for the lane's calls
     c->open_lanes--;
     return DSPI_OK;
-}
-
-// process_device on a lane: the range call's checks, then a window check; issued behind the engine stream as it is now
-template <class A>
-int lane_process(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
-                 const uint16_t *packet_frames, void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
-{
-    Lane *l = lane_of(c, lane);
-    if (!l) return DSPI_EINVAL;
-    int rc = check_call(c, l->sched, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, subframes);
-    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(lane_begin(c, *l));
-    rc = issue_call(c, Issue{ l->stream, l->st, l->sched }, inst0, n, d_pcm, bit_depth, packet_frames, d_spdif, subframes, d_pdm, d_status);
-    CU_OK(cudaEventRecord(l->ev_last, l->stream));
-    return rc;
 }
 
 template <class A>
 void *lane_stream(ChainHost<A> *c, uint32_t lane)
 {
-    return c && lane < DSPI_CHAIN_MAX_LANES && c->lanes[lane].open ? (void *)c->lanes[lane].stream : nullptr;
+    return c && lane < DSPI_CHAIN_MAX_LANES ? (void *)c->lanes[lane].stream : nullptr;
 }
 
 template <class A>
 int lane_sync(ChainHost<A> *c, uint32_t lane)
 {
-    Lane *l = lane_of(c, lane);
+    Queue *l = lane_queue(c, lane);
     if (!l) return DSPI_EINVAL;
     CU_OK(cudaSetDevice(c->desc.device));
     CU_OK(cudaStreamSynchronize(l->stream));
     return DSPI_OK;
 }
 
-// ---- lane control calls: the engine-level control calls a running clock group needs, issued on its lane ---------------
-// Each takes the engine-level call's checks, then requires every instance it names inside the lane's window.  It is issued
-// like a lane process call (behind the engine stream as it is now, ending with ev_last) and does not wait for the device.
-
+// ---- S/PDIF transmitters -----------------------------------------------------------------------------------------------
+// on queue q (the engine's or a lane's)
 template <class A>
-int lane_edit_bulk_device(ChainHost<A> *c, uint32_t lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate,
-                          int32_t *d_results)
+int set_spdif_tx(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
 {
-    Lane *l = lane_of(c, lane);
-    if (!l) return DSPI_EINVAL;
-    int rc = check_edits(c, n_edits, edits, sample_rate);
-    if (rc) return rc;
-    for (uint32_t k = 0; k < n_edits; k++)
-        if (edits[k].instance < l->inst0 || edits[k].instance - l->inst0 >= l->n)
-            return fail(DSPI_ERANGE, "edit %u names instance %u, outside lane %u's window [%u, %u)", k, edits[k].instance, lane, l->inst0, l->inst0 + l->n);
-    if (n_edits == 0) return DSPI_OK;
-    CU_OK(cudaSetDevice(c->desc.device));
-    // The lane's first edit allocates its staging, and an engine whose skip rows were never set (no set_params, apply,
-    // import, copy or edit yet) remasks every row once: both wait for every lane and the engine stream first.
-    const bool skip_set = eq_skip_set(c->eq_m) && eq_skip_set(c->eq_o);
-    if (!l->bulk_edit.marks || !skip_set) {
-        CU_OK(drain(c));
-        if (!skip_set && (rc = bulk::finish_skip(c, c->stream, nullptr)) != DSPI_OK) return rc;
-    }
-    CU_OK(lane_begin(c, *l));
-    bulk::LaneScope scope{ l->inst0, l->n, l->ring };
-    rc = bulk::edit<typename A::Stores>(c, l->stream, l->bulk, l->bulk_edit, &scope, n_edits, edits, exact_db, sample_rate, nullptr, d_results);
-    CU_OK(cudaEventRecord(l->ev_last, l->stream));
-    return rc;
-}
-
-template <class A>
-int lane_set_preset_mute(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
-{
-    Lane *l = lane_of(c, lane);
-    if (!l) return DSPI_EINVAL;
-    int rc = check_range(c, inst0, n);
-    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    unsigned char *buf = nullptr;
-    CU_OK(l->ring.take((size_t)5 * n * 4, &buf));
-    preset_rows(c, inst0, n, states, sample_rate_hz, (uint32_t *)buf);
-    CU_OK(lane_begin(c, *l));
-    CU_OK(cudaMemcpy2DAsync(c->d.env + inst0, (size_t)c->d.N_pad * 4, buf, (size_t)n * 4, (size_t)n * 4, 5, cudaMemcpyHostToDevice, l->stream));
-    CU_OK(l->ring.done(l->stream));
-    CU_OK(cudaEventRecord(l->ev_last, l->stream));
-    return DSPI_OK;
-}
-
-template <class A>
-int lane_set_spdif_tx(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
-{
-    Lane *l = lane_of(c, lane);
-    if (!l) return DSPI_EINVAL;
+    if (!q) return DSPI_EINVAL;
     if (!tx) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
-    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
+    int rc = check_range(*q, inst0, n);
+    if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     unsigned char *buf = nullptr;
-    CU_OK(l->ring.take((size_t)n * 12, &buf));
+    CU_OK(q->ring.take((size_t)n * 12, &buf));
     uint64_t *cs = (uint64_t *)buf;                                          // channel status words, then block positions
     uint32_t *bp = (uint32_t *)(buf + (size_t)n * 8);
     if (!spdif_tx_unpack(tx, n, bp, cs)) return fail(DSPI_EINVAL, "block_pos must be 0..191");
-    CU_OK(lane_begin(c, *l));
-    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp, (size_t)n * 4, cudaMemcpyHostToDevice, l->stream));
-    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs, (size_t)n * 8, cudaMemcpyHostToDevice, l->stream));
-    CU_OK(l->ring.done(l->stream));
-    CU_OK(cudaEventRecord(l->ev_last, l->stream));
-    return DSPI_OK;
-}
-
-template <class A>
-int lane_reset_instances(ChainHost<A> *c, uint32_t lane, uint32_t inst0, uint32_t n)
-{
-    Lane *l = lane_of(c, lane);
-    if (!l) return DSPI_EINVAL;
-    int rc = check_range(c, inst0, n);
-    if (rc || (rc = check_lane_window(l, lane, inst0, n)) || n == 0) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(lane_begin(c, *l));
-    CU_OK(reset_range(c, inst0, n, l->stream));
-    CU_OK(cudaEventRecord(l->ev_last, l->stream));
-    return DSPI_OK;
-}
-
-// ---- S/PDIF transmitters -----------------------------------------------------------------------------------------------
-template <class A>
-int set_spdif_tx(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx)
-{
-    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
-    if (rc || n == 0) return rc;
-    std::vector<uint32_t> bp(n);
-    std::vector<uint64_t> cs(n);
-    if (!spdif_tx_unpack(tx, n, bp.data(), cs.data())) return fail(DSPI_EINVAL, "block_pos must be 0..191");
-    CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));   // behind earlier calls
-    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    CU_OK(begin_call(c, *q));
+    CU_OK(cudaMemcpyAsync(c->tx.bp + inst0, bp, (size_t)n * 4, cudaMemcpyHostToDevice, q->stream));   // behind earlier calls
+    CU_OK(cudaMemcpyAsync(c->tx.cs40 + inst0, cs, (size_t)n * 8, cudaMemcpyHostToDevice, q->stream));
+    CU_OK(q->ring.done(q->stream));
+    return end_call(*q, DSPI_OK);
 }
 
 template <class A>
 int get_spdif_tx(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
 {
     if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     std::vector<uint32_t> bp(n);
     std::vector<uint64_t> cs(n);
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaMemcpyAsync(bp.data(), c->tx.bp + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaMemcpyAsync(cs.data(), c->tx.cs40 + inst0, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaMemcpyAsync(bp.data(), c->tx.bp + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaMemcpyAsync(cs.data(), c->tx.cs40 + inst0, (size_t)n * 8, cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     spdif_tx_pack(bp.data(), cs.data(), n, tx);
     return DSPI_OK;
 }
@@ -1322,10 +1227,10 @@ int state_export(ChainHost<A> *c, void *blob, size_t cap)
     memcpy(blob, &h, hdr);
     char *p = (char *)blob + hdr;
     for (auto &s : v) {
-        CU_OK(cudaMemcpyAsync(p, s.first, s.second, cudaMemcpyDeviceToHost, c->stream));
+        CU_OK(cudaMemcpyAsync(p, s.first, s.second, cudaMemcpyDeviceToHost, c->q.stream));
         p += s.second;
     }
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     return DSPI_OK;
 }
 
@@ -1354,20 +1259,20 @@ int state_import(ChainHost<A> *c, const void *blob, size_t len)
     CU_OK(cudaSetDevice(c->desc.device));
     const char *p = (const char *)blob + hdr;
     for (auto &s : v) {
-        CU_OK(cudaMemcpyAsync(s.first, p, s.second, cudaMemcpyHostToDevice, c->stream));
+        CU_OK(cudaMemcpyAsync(s.first, p, s.second, cudaMemcpyHostToDevice, c->q.stream));
         p += s.second;
     }
-    CU_OK(cudaStreamSynchronize(c->stream));
-    int rc = eq_state_load(c->eq_m, p, (int)h.cpl_m, c->stream);
+    CU_OK(cudaStreamSynchronize(c->q.stream));
+    int rc = eq_state_load(c->eq_m, p, (int)h.cpl_m, c->q.stream);
     p += eq_state_bytes(c->eq_m, (int)h.cpl_m);
-    if (rc == DSPI_OK) rc = eq_state_load(c->eq_o, p, (int)h.cpl_o, c->stream);
+    if (rc == DSPI_OK) rc = eq_state_load(c->eq_o, p, (int)h.cpl_o, c->q.stream);
     if (rc) return rc;
-    rc = eq_state_imported(c->eq_m, c->stream);
-    if (rc == DSPI_OK) rc = eq_state_imported(c->eq_o, c->stream);
+    rc = eq_state_imported(c->eq_m, c->q.stream);
+    if (rc == DSPI_OK) rc = eq_state_imported(c->eq_o, c->q.stream);
     if (rc) return rc;
     std::vector<uint32_t> on(c->d.N);
-    CU_OK(cudaMemcpyAsync(on.data(), c->d.env + (size_t)4 * c->d.N_pad, (size_t)c->d.N * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaMemcpyAsync(on.data(), c->d.env + (size_t)4 * c->d.N_pad, (size_t)c->d.N * 4, cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     c->env_instances = 0;
     for (uint32_t i = 0; i < c->d.N; i++) {
         c->env_mode[i] = on[i] ? 1 : 0;
@@ -1393,7 +1298,7 @@ int check_images(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *images
     *size = image_plan(c, kInImage, *plan);
     if (*size == 0) return fail(DSPI_EINVAL, "instance image plan exceeds its tables");
     if (stride < *size) return fail(DSPI_EINVAL, "image_stride %zu below the image size %zu", stride, *size);
-    return check_range(c, inst0, n);
+    return check_range(c->q, inst0, n);
 }
 
 // the EQ sub-engines' ranges of instances [inst0, inst0 + n): every role of the master / output engine in one launch
@@ -1413,21 +1318,21 @@ int export_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, void *images, 
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     uint32_t chunk = 0;
-    CU_OK(c->resp.stage(size, n, c->stream, &chunk));
+    CU_OK(c->resp.stage(size, n, c->q.stream, &chunk));
     RoleRange rm, ro;
     role_ranges(c, rm, ro);
-    rc = eq_unpack_range(c->eq_m, inst0, n, c->stream, rm);               // running EQ state into the mirrors, as download_biquads
-    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, inst0, n, c->stream, ro);
+    rc = eq_unpack_range(c->eq_m, inst0, n, c->q.stream, rm);               // running EQ state into the mirrors, as download_biquads
+    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, inst0, n, c->q.stream, ro);
     if (rc) return rc;
     unsigned char *stage = (unsigned char *)c->resp.d_stage;
     for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
         const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
-        image::instance_image_kernel<image::kExport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, inst0 + i0, nc, stage);
+        image::instance_image_kernel<image::kExport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->q.stream>>>(pl, inst0 + i0, nc, stage);
         CU_OK(cudaGetLastError());
         c->launches++;
-        CU_OK(cudaMemcpy2DAsync((char *)images + (size_t)i0 * stride, stride, stage, size, size, nc, cudaMemcpyDeviceToHost, c->stream));
+        CU_OK(cudaMemcpy2DAsync((char *)images + (size_t)i0 * stride, stride, stage, size, size, nc, cudaMemcpyDeviceToHost, c->q.stream));
     }
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     return DSPI_OK;
 }
 
@@ -1455,8 +1360,8 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
         if (pl.f[k].p == (char *)c->d.env) env_off = pl.f[k].off + 4 * 4;
     const size_t Np = c->d.N_pad;
     std::vector<uint32_t> cur((size_t)n);
-    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     uint32_t before = 0, after = 0;
     for (uint32_t i = 0; i < n; i++) {
         uint32_t on;
@@ -1466,12 +1371,12 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
         c->env_mode[inst0 + i] = on ? 1 : 0;
     }
     uint32_t chunk = 0;
-    CU_OK(c->resp.stage(size, n, c->stream, &chunk));
+    CU_OK(c->resp.stage(size, n, c->q.stream, &chunk));
     unsigned char *stage = (unsigned char *)c->resp.d_stage;
     for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
         const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
-        CU_OK(cudaMemcpy2DAsync(stage, size, img + (size_t)i0 * stride, stride, size, nc, cudaMemcpyHostToDevice, c->stream));
-        image::instance_image_kernel<image::kImport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, inst0 + i0, nc, stage);
+        CU_OK(cudaMemcpy2DAsync(stage, size, img + (size_t)i0 * stride, stride, size, nc, cudaMemcpyHostToDevice, c->q.stream));
+        image::instance_image_kernel<image::kImport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->q.stream>>>(pl, inst0 + i0, nc, stage);
         CU_OK(cudaGetLastError());
         c->launches++;
     }
@@ -1480,10 +1385,10 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
     // upload_biquads and set_params do
     RoleRange rm, ro;
     role_ranges(c, rm, ro);
-    rc = eq_pack_range(c->eq_m, inst0, n, c->stream, rm);
-    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, inst0, n, c->stream, ro);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->stream);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->stream);
+    rc = eq_pack_range(c->eq_m, inst0, n, c->q.stream, rm);
+    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, inst0, n, c->q.stream, ro);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->q.stream);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->q.stream);
     return rc;
 }
 
@@ -1519,11 +1424,11 @@ int copy_instances(ChainHost<A> *c, uint32_t n, const uint32_t *src, const uint3
     std::vector<uint32_t> lists((size_t)2 * n);
     memcpy(lists.data(), src, (size_t)n * 4);
     memcpy(lists.data() + n, dst, (size_t)n * 4);
-    CU_OK(cudaMemcpyAsync(c->copy_lists.d, lists.data(), (size_t)2 * n * 4, cudaMemcpyHostToDevice, c->stream));
+    CU_OK(cudaMemcpyAsync(c->copy_lists.d, lists.data(), (size_t)2 * n * 4, cudaMemcpyHostToDevice, c->q.stream));
     // envelope-mode instances: the modes (env row 4) of sources and destinations, behind earlier work
     std::vector<uint32_t> mode((size_t)hi - lo + 1);
-    CU_OK(cudaMemcpyAsync(mode.data(), c->d.env + (size_t)4 * c->d.N_pad + lo, mode.size() * 4, cudaMemcpyDeviceToHost, c->stream));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaMemcpyAsync(mode.data(), c->d.env + (size_t)4 * c->d.N_pad + lo, mode.size() * 4, cudaMemcpyDeviceToHost, c->q.stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     uint32_t before = 0, after = 0;
     for (uint32_t k = 0; k < n; k++) {
         before += mode[dst[k] - lo] ? 1u : 0u;
@@ -1533,32 +1438,33 @@ int copy_instances(ChainHost<A> *c, uint32_t n, const uint32_t *src, const uint3
     RoleRange rm, ro;
     role_ranges(c, rm, ro);
     rm.inst = ro.inst = d_src;
-    int rc = eq_unpack_range(c->eq_m, 0, n, c->stream, rm);               // running EQ state into the mirrors, as export
-    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, 0, n, c->stream, ro);
+    int rc = eq_unpack_range(c->eq_m, 0, n, c->q.stream, rm);               // running EQ state into the mirrors, as export
+    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, 0, n, c->q.stream, ro);
     if (rc) return rc;
-    image::instance_copy_kernel<<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, c->stream>>>(pl, n, d_src, d_dst);
+    image::instance_copy_kernel<<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, c->q.stream>>>(pl, n, d_src, d_dst);
     CU_OK(cudaGetLastError());
     c->launches++;
     c->env_instances = c->env_instances - before + after;
     // the destinations' mirror rows -> packed stores, then the skip masks, as import
     rm.inst = ro.inst = d_dst;
-    rc = eq_pack_range(c->eq_m, 0, n, c->stream, rm);
-    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, 0, n, c->stream, ro);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->stream);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->stream);
+    rc = eq_pack_range(c->eq_m, 0, n, c->q.stream, rm);
+    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, 0, n, c->q.stream, ro);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->q.stream);
+    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->q.stream);
     return rc;
 }
 
+// on queue q (the engine's or a lane's)
 template <class A>
-int reset_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n)
+int reset_instances(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n)
 {
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c, inst0, n);
+    if (!q) return DSPI_EINVAL;
+    int rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(reset_range(c, inst0, n));
-    CU_OK(cudaStreamSynchronize(c->stream));
-    return DSPI_OK;
+    CU_OK(begin_call(c, *q));
+    CU_OK(reset_range(c, inst0, n, q->stream));
+    return end_call(*q, DSPI_OK);
 }
 
 // ---- queries -----------------------------------------------------------------------------------------------------------
@@ -1571,15 +1477,15 @@ int response(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *freqs, ui
     int rc = response_check_args(freqs, n_freqs, fs, out, &why);
     if (rc) return fail(rc, "%s", why);
     if (!c) return fail(DSPI_EINVAL, "null argument");
-    rc = check_range(c, inst0, n);
+    rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(c->resp.upload(freqs, n_freqs, c->stream, &c->launches));
+    CU_OK(c->resp.upload(freqs, n_freqs, c->q.stream, &c->launches));
     using B = typename A::Biquad;
     const B *m_aos = (const B *)eq_aos_mirror(c->eq_m), *o_aos = (const B *)eq_aos_mirror(c->eq_o);
     auto launch = [&](uint32_t i0, uint32_t m, void *dst) -> cudaError_t {
         const dim3 grid((n_freqs + 127) / 128, m < 65535u ? m : 65535u);
-        A::response<<<grid, 128, 0, c->stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
+        A::response<<<grid, 128, 0, c->q.stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
         c->launches++;
         return cudaGetLastError();
     };
@@ -1589,12 +1495,12 @@ int response(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *freqs, ui
     }
     const size_t row_bytes = (size_t)A::kOuts * 2 * n_freqs * 2 * sizeof(float);
     uint32_t rows = 0;
-    CU_OK(c->resp.stage(row_bytes, n, c->stream, &rows));
+    CU_OK(c->resp.stage(row_bytes, n, c->q.stream, &rows));
     for (uint32_t i = 0; i < n; i += rows) {
         const uint32_t m = n - i < rows ? n - i : rows;
         CU_OK(launch(inst0 + i, m, c->resp.d_stage));
-        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->stream));
-        CU_OK(cudaStreamSynchronize(c->stream));
+        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->q.stream));
+        CU_OK(cudaStreamSynchronize(c->q.stream));
     }
     return DSPI_OK;
 }
@@ -1604,12 +1510,12 @@ int sync(ChainHost<A> *c)
 {
     if (!c) return fail(DSPI_EINVAL, "null argument");
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(cudaStreamSynchronize(c->stream));
+    CU_OK(cudaStreamSynchronize(c->q.stream));
     return DSPI_OK;
 }
 
 template <class A>
-void *stream(ChainHost<A> *c) { return c ? (void *)c->stream : nullptr; }
+void *stream(ChainHost<A> *c) { return c ? (void *)c->q.stream : nullptr; }
 
 // SMs reserved for the modulator / left to every other stage (0, 0: no partition, see chain_streams.cuh)
 template <class A>

@@ -904,189 +904,9 @@ struct Q28 : ParamStores {
 
 struct dspi_chainq : dspi::ChainHost<dspi::Q28> {};
 
-extern "C" {
-
-int dspi_chainq_destroy(dspi_chainq *c) { return dspi::destroy(c); }
-int dspi_chainq_create(dspi_chainq **out, const dspi_chain_desc *desc) { return dspi::create(out, desc); }
-int dspi_chainq_reset_state(dspi_chainq *c) { return dspi::reset_state(dspi::join_lanes(c)); }
-
-int dspi_chainq_set_params(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_chain_params_q28 *params) { return dspi::set_params(dspi::join_lanes(c), inst0, n, params); }
-
-int dspi_chainq_set_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
-{
-    return dspi::set_preset_mute(dspi::join_lanes(c), inst0, n, states, sample_rate_hz);
-}
-
-int dspi_chainq_get_preset_mute(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states) { return dspi::get_preset_mute(dspi::join_lanes(c), inst0, n, states); }
-
-int dspi_chainq_set_dynamics_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_dynamics_config *cfgs, float sample_rate)
-{
-    return dspi::set_dynamics_device(dspi::join_lanes(c), inst0, n, cfgs, sample_rate);
-}
-
-int dspi_chainq_apply_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
-                                  int exact_db, float sample_rate, int32_t *results)
-{
-    return dspi::apply_bulk_device(dspi::join_lanes(c), inst0, n, packets, host, exact_db, sample_rate, results);
-}
-
-int dspi_chainq_set_rate_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results)
-{
-    return dspi::set_rate_device(dspi::join_lanes(c), inst0, n, sample_rates, results);
-}
-
-int dspi_chainq_edit_bulk_device(dspi_chainq *c, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate, int32_t *results)
-{
-    return dspi::edit_bulk_device(dspi::join_lanes(c), n_edits, edits, exact_db, sample_rate, results);
-}
-
-int dspi_chainq_collect_bulk_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
-{
-    return dspi::collect_bulk_device(dspi::join_lanes(c), inst0, n, packets, host, results);
-}
-
-int dspi_chainq_apply_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride, const dspi_preset_load *load,
-                                    const dspi_bulk_host *host, float sample_rate, int32_t *results)
-{
-    return dspi::apply_preset_device(dspi::join_lanes(c), inst0, n, images, image_stride, load, host, sample_rate, results);
-}
-
-int dspi_chainq_collect_preset_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
-                                      int32_t *results)
-{
-    return dspi::collect_preset_device(dspi::join_lanes(c), inst0, n, slot_indices, images, image_stride, results);
-}
-
-int dspi_chainq_upload_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_biquad_q28 *biquads) { return dspi::upload_biquads(dspi::join_lanes(c), inst0, n, biquads); }
-int dspi_chainq_download_biquads(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_biquad_q28 *biquads) { return dspi::download_biquads(dspi::join_lanes(c), inst0, n, biquads); }
-
-int dspi_chainq_set_eq_params_device(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_eq_param *recipes, float sample_rate)
-{
-    return dspi::set_eq_params_device(dspi::join_lanes(c), inst0, n, recipes, sample_rate);
-}
-
-int dspi_chainq_process_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *d_spdif,
-                               uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return dspi::process_uniform(dspi::join_lanes(c), d_pcm, bit_depth, n_packets, fpp, d_spdif, d_pdm, d_status, false);
-}
-
-int dspi_chainq_process_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif_out,
-                             uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    return dspi::process_uniform(dspi::join_lanes(c), pcm, bit_depth, n_packets, fpp, spdif_out, pdm_out, status, true);
-}
-
-int dspi_chainq_process_packets_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                       int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return dspi::process_device(dspi::join_lanes(c), 0, dspi::all_instances(c), d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
-}
-
-int dspi_chainq_process_packets_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                     int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    return dspi::process_host(dspi::join_lanes(c), 0, dspi::all_instances(c), pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
-}
-
-int dspi_chainq_process_subframes_device(dspi_chainq *c, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                         dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return dspi::process_device(dspi::join_lanes(c), 0, dspi::all_instances(c), d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
-}
-
-int dspi_chainq_process_subframes_host(dspi_chainq *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, const uint16_t *packet_frames,
-                                       dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    return dspi::process_host(dspi::join_lanes(c), 0, dspi::all_instances(c), pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
-}
-
-int dspi_chainq_process_packets_range_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
-                                    const uint16_t *packet_frames, int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return dspi::process_device(dspi::join_lanes(c), inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
-}
-
-int dspi_chainq_process_packets_range_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
-                                  const uint16_t *packet_frames, int32_t *spdif_out, uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    return dspi::process_host(dspi::join_lanes(c), inst0, n, pcm, bit_depth, n_packets, packet_frames, spdif_out, false, pdm_out, status);
-}
-
-int dspi_chainq_process_subframes_range_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
-                                      const uint16_t *packet_frames, dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return dspi::process_device(dspi::join_lanes(c), inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
-}
-
-int dspi_chainq_process_subframes_range_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
-                                    const uint16_t *packet_frames, dspi_spdif_subframe *subframes, uint32_t *pdm_out, dspi_status_q28 *status)
-{
-    return dspi::process_host(dspi::join_lanes(c), inst0, n, pcm, bit_depth, n_packets, packet_frames, subframes, true, pdm_out, status);
-}
-
-int dspi_chainq_set_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx) { return dspi::set_spdif_tx(dspi::join_lanes(c), inst0, n, tx); }
-int dspi_chainq_get_spdif_tx(dspi_chainq *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx) { return dspi::get_spdif_tx(dspi::join_lanes(c), inst0, n, tx); }
-
-size_t dspi_chainq_state_size(dspi_chainq *c) { return dspi::state_size(c); }
-int dspi_chainq_state_export(dspi_chainq *c, void *blob, size_t cap) { return dspi::state_export(dspi::join_lanes(c), blob, cap); }
-int dspi_chainq_state_import(dspi_chainq *c, const void *blob, size_t len) { return dspi::state_import(dspi::join_lanes(c), blob, len); }
-
-size_t dspi_chainq_instance_image_size(dspi_chainq *c) { return dspi::instance_image_size(c); }
-int dspi_chainq_export_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, void *images, size_t image_stride)
-{
-    return dspi::export_instances(dspi::join_lanes(c), inst0, n, images, image_stride);
-}
-int dspi_chainq_import_instances(dspi_chainq *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride)
-{
-    return dspi::import_instances(dspi::join_lanes(c), inst0, n, images, image_stride);
-}
-int dspi_chainq_reset_instances(dspi_chainq *c, uint32_t inst0, uint32_t n) { return dspi::reset_instances(dspi::join_lanes(c), inst0, n); }
-int dspi_chainq_copy_instances(dspi_chainq *c, uint32_t n, const uint32_t *src, const uint32_t *dst)
-{
-    return dspi::copy_instances(dspi::join_lanes(c), n, src, dst);
-}
-
-int dspi_chainq_response_host(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *out)
-{
-    return dspi::response(dspi::join_lanes(c), inst0, n, freqs_hz, n_freqs, sample_rate, out, true);
-}
-
-int dspi_chainq_response_device(dspi_chainq *c, uint32_t inst0, uint32_t n, const float *freqs_hz, uint32_t n_freqs, float sample_rate, float *d_out)
-{
-    return dspi::response(dspi::join_lanes(c), inst0, n, freqs_hz, n_freqs, sample_rate, d_out, false);
-}
-
-int dspi_chainq_sync(dspi_chainq *c) { return dspi::sync(dspi::join_lanes(c)); }
-void *dspi_chainq_stream(dspi_chainq *c) { return dspi::stream(c); }
-int dspi_chainq_sm_partition(dspi_chainq *c, uint32_t *pdm_sms, uint32_t *rest_sms) { return dspi::sm_partition(c, pdm_sms, rest_sms); }
-uint64_t dspi_chainq_launch_count(dspi_chainq *c) { return dspi::launch_count(c); }
-
-int dspi_chainq_lane_open(dspi_chainq *c, uint32_t inst0, uint32_t n, uint32_t *lane) { return dspi::lane_open(c, inst0, n, lane); }
-int dspi_chainq_lane_close(dspi_chainq *c, uint32_t lane) { return dspi::lane_close(c, lane); }
-int dspi_chainq_lane_process_packets_device(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
-                                        const uint16_t *packet_frames, int32_t *d_spdif, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return dspi::lane_process(c, lane, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_spdif, false, d_pdm, d_status);
-}
-int dspi_chainq_lane_process_subframes_device(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, uint32_t n_packets,
-                                          const uint16_t *packet_frames, dspi_spdif_subframe *d_subframes, uint32_t *d_pdm, dspi_status_q28 *d_status)
-{
-    return dspi::lane_process(c, lane, inst0, n, d_pcm, bit_depth, n_packets, packet_frames, d_subframes, true, d_pdm, d_status);
-}
-void *dspi_chainq_lane_stream(dspi_chainq *c, uint32_t lane) { return dspi::lane_stream(c, lane); }
-int dspi_chainq_lane_sync(dspi_chainq *c, uint32_t lane) { return dspi::lane_sync(c, lane); }
-int dspi_chainq_lane_edit_bulk_device(dspi_chainq *c, uint32_t lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db, float sample_rate,
-                                 int32_t *d_results)
-{
-    return dspi::lane_edit_bulk_device(c, lane, n_edits, edits, exact_db, sample_rate, d_results);
-}
-int dspi_chainq_lane_set_preset_mute(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz)
-{
-    return dspi::lane_set_preset_mute(c, lane, inst0, n, states, sample_rate_hz);
-}
-int dspi_chainq_lane_set_spdif_tx(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx) { return dspi::lane_set_spdif_tx(c, lane, inst0, n, tx); }
-int dspi_chainq_lane_reset_instances(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n) { return dspi::lane_reset_instances(c, lane, inst0, n); }
-
-
-}  // extern "C"
+#define CHAIN dspi_chainq
+#define CHAIN_FN(name) dspi_chainq_##name
+#define CHAIN_PARAMS dspi_chain_params_q28
+#define CHAIN_BIQUAD dspi_biquad_q28
+#define CHAIN_STATUS dspi_status_q28
+#include "chain_abi.inc"

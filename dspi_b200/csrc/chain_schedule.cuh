@@ -38,7 +38,7 @@ struct PacketSchedule {
     OffChunk *chunk = nullptr;                 // parameter block under construction
     uint32_t n_packets = 0, frames = 0, longest = 0;
 
-    cudaError_t create(uint32_t max_frames)
+    __noinline__ cudaError_t create(uint32_t max_frames)     // out of line: the library has always exported it
     {
         cap = max_frames;
         off.assign((size_t)cap + 1, 0u);

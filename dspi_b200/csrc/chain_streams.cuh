@@ -170,8 +170,9 @@ struct ChainStreams {
     cudaStream_t s_front = nullptr, s_out = nullptr, s_pdm = nullptr;
     cudaEvent_t ev_begin = nullptr, ev_done = nullptr, ev_aux = nullptr, ev_front[kMaxSlices] = {}, ev_out[kMaxSlices] = {};
 
-    // the three stage streams in the partition's contexts (or priority streams without one), and the events
-    cudaError_t create(const SmPartition &p)
+    // the three stage streams in the partition's contexts (or priority streams without one), and the events.  This and
+    // destroy() stay out of line: the library has always exported them.
+    __noinline__ cudaError_t create(const SmPartition &p)
     {
         cudaError_t e = p.stream(p.g_pdm, &s_pdm, p.prio_hi);
         if (e == cudaSuccess) e = p.stream(p.g_rest, &s_front, p.prio_mid);
@@ -186,7 +187,7 @@ struct ChainStreams {
         return e;
     }
 
-    void destroy()
+    __noinline__ void destroy()
     {
         for (cudaStream_t *s : { &s_front, &s_out, &s_pdm })
             if (*s) { cudaStreamSynchronize(*s); cudaStreamDestroy(*s); *s = nullptr; }
