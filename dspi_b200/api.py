@@ -64,6 +64,8 @@ SYMBOLS = [
     "dspi_chainq_lane_stream", "dspi_chainq_lane_sync",
     "dspi_chain_lane_edit_bulk_device", "dspi_chain_lane_set_preset_mute", "dspi_chain_lane_set_spdif_tx", "dspi_chain_lane_reset_instances",
     "dspi_chainq_lane_edit_bulk_device", "dspi_chainq_lane_set_preset_mute", "dspi_chainq_lane_set_spdif_tx", "dspi_chainq_lane_reset_instances",
+    "dspi_chain_lane_apply_bulk_device", "dspi_chain_lane_apply_preset_device", "dspi_chain_lane_set_rate_device",
+    "dspi_chainq_lane_apply_bulk_device", "dspi_chainq_lane_apply_preset_device", "dspi_chainq_lane_set_rate_device",
 ]
 
 
@@ -180,6 +182,9 @@ def lib():
             getattr(h, pre + "_lane_set_preset_mute").argtypes = [vp, u32, u32, u32, vp, u32]
             getattr(h, pre + "_lane_set_spdif_tx").argtypes = [vp, u32, u32, u32, vp]
             getattr(h, pre + "_lane_reset_instances").argtypes = [vp, u32, u32, u32]
+            getattr(h, pre + "_lane_apply_bulk_device").argtypes = [vp, u32, u32, u32, vp, vp, C.c_int, C.c_float, vp]
+            getattr(h, pre + "_lane_apply_preset_device").argtypes = [vp, u32, u32, u32, vp, C.c_size_t, vp, vp, C.c_float, vp]
+            getattr(h, pre + "_lane_set_rate_device").argtypes = [vp, u32, u32, u32, vp, vp]
         for pre in ("dspi_eq", "dspi_chain", "dspi_chainq"):
             getattr(h, pre + "_response_host").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
             getattr(h, pre + "_response_device").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
@@ -637,15 +642,20 @@ class _ChainEngine:
         """WIRE_BULK [n] -> instances [inst0, inst0+n) reconfigured on the GPU as ``bulk_params_apply`` and the firmware's main
         loop would; ``host`` BULK_HOST [n] (default: volume 0 dB, not muted).  Returns the firmware's result codes, int32 [n]:
         0 applied, -1 .. -4 rejected (that instance is left exactly as it was)."""
-        w = np.ascontiguousarray(packets, L.WIRE_BULK).reshape(-1)
-        hv = np.zeros(w.shape[0], L.BULK_HOST) if host is None else np.ascontiguousarray(host, L.BULK_HOST).reshape(-1)
-        if hv.shape[0] != w.shape[0]:
-            raise ValueError("packets and host give different instance counts")
+        w, hv = self._bulk_args(packets, host)
         res = np.zeros(w.shape[0], np.int32)
         _check(self._fn("apply_bulk_device")(self._h, int(inst0), int(w.shape[0]), w.ctypes.data_as(C.c_void_p),
                                              hv.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
                                              res.ctypes.data_as(C.c_void_p)))
         return res
+
+    @staticmethod
+    def _bulk_args(packets, host):
+        w = np.ascontiguousarray(packets, L.WIRE_BULK).reshape(-1)
+        hv = np.zeros(w.shape[0], L.BULK_HOST) if host is None else np.ascontiguousarray(host, L.BULK_HOST).reshape(-1)
+        if hv.shape[0] != w.shape[0]:
+            raise ValueError("packets and host give different instance counts")
+        return w, hv
 
     def set_rate_device(self, rates, inst0=0):
         """The USB host switched instances [inst0, inst0+n) to ``rates`` (float [n], one rate per instance, or a scalar for
@@ -683,6 +693,16 @@ class _ChainEngine:
         [inst0, inst0+n) reconfigured on the GPU as ``preset_load`` and the firmware's main loop would.  ``slots``,
         ``master_volume_mode`` and ``dir_master_volume_db`` are scalars or [n]; ``host`` BULK_HOST [n] (default: volume 0 dB,
         not muted).  Returns int32 [n]: 0 loaded, 3 (PRESET_ERR_CRC) rejected (that instance is left exactly as it was)."""
+        img, ld, hv = self._preset_args(images, slots, master_volume_mode, dir_master_volume_db, host)
+        n = img.shape[0]
+        res = np.zeros(n, np.int32)
+        _check(self._fn("apply_preset_device")(self._h, int(inst0), n, img.ctypes.data_as(C.c_void_p), C.c_size_t(img.shape[1]),
+                                               ld.ctypes.data_as(C.c_void_p), hv.ctypes.data_as(C.c_void_p), C.c_float(fs),
+                                               res.ctypes.data_as(C.c_void_p)))
+        return res
+
+    @staticmethod
+    def _preset_args(images, slots, master_volume_mode, dir_master_volume_db, host):
         img = np.ascontiguousarray(images, np.uint8)
         if img.ndim != 2:
             raise ValueError("images must be [n, stride] bytes")
@@ -692,11 +712,7 @@ class _ChainEngine:
         hv = np.zeros(n, L.BULK_HOST) if host is None else np.ascontiguousarray(host, L.BULK_HOST).reshape(-1)
         if hv.shape[0] != n:
             raise ValueError("images and host give different instance counts")
-        res = np.zeros(n, np.int32)
-        _check(self._fn("apply_preset_device")(self._h, int(inst0), n, img.ctypes.data_as(C.c_void_p), C.c_size_t(img.shape[1]),
-                                               ld.ctypes.data_as(C.c_void_p), hv.ctypes.data_as(C.c_void_p), C.c_float(fs),
-                                               res.ctypes.data_as(C.c_void_p)))
-        return res
+        return img, ld, hv
 
     def collect_preset_device(self, slots, inst0=0, n=None):
         """The state part of ``preset_save`` for instances [inst0, inst0+n) (default: as many as ``slots`` gives, or to the
@@ -846,6 +862,31 @@ class _ChainEngine:
     def lane_reset_instances(self, lane, inst0, n):
         """``reset_instances`` issued on a lane ([inst0, inst0+n) inside its window), asynchronous on ``lane_stream(lane)``."""
         _check(self._fn("lane_reset_instances")(self._h, int(lane), int(inst0), int(n)))
+
+    def lane_apply_bulk_device(self, lane, packets, fs, inst0, host=None, exact_db=False, results_ptr=0):
+        """``apply_bulk_device`` issued on a lane ([inst0, inst0+n) inside its window), asynchronous on ``lane_stream(lane)``:
+        returns without waiting.  ``results_ptr`` (device memory, int32 [n], required) receives the firmware's result codes
+        there."""
+        w, hv = self._bulk_args(packets, host)
+        _check(self._fn("lane_apply_bulk_device")(self._h, int(lane), int(inst0), int(w.shape[0]), w.ctypes.data_as(C.c_void_p),
+                                                  hv.ctypes.data_as(C.c_void_p), int(bool(exact_db)), C.c_float(fs),
+                                                  C.c_void_p(int(results_ptr)) if results_ptr else None))
+
+    def lane_apply_preset_device(self, lane, images, fs, inst0, slots=0, master_volume_mode=0, dir_master_volume_db=0.0, host=None,
+                                 results_ptr=0):
+        """``apply_preset_device`` issued on a lane ([inst0, inst0+n) inside its window), asynchronous on ``lane_stream(lane)``:
+        returns without waiting.  ``results_ptr`` (device memory, int32 [n], required) receives the preset result codes there."""
+        img, ld, hv = self._preset_args(images, slots, master_volume_mode, dir_master_volume_db, host)
+        _check(self._fn("lane_apply_preset_device")(self._h, int(lane), int(inst0), int(img.shape[0]), img.ctypes.data_as(C.c_void_p),
+                                                    C.c_size_t(img.shape[1]), ld.ctypes.data_as(C.c_void_p), hv.ctypes.data_as(C.c_void_p),
+                                                    C.c_float(fs), C.c_void_p(int(results_ptr)) if results_ptr else None))
+
+    def lane_set_rate_device(self, lane, rates, inst0, results_ptr=0):
+        """``set_rate_device`` issued on a lane ([inst0, inst0+n) inside its window), asynchronous on ``lane_stream(lane)``:
+        returns without waiting.  ``results_ptr`` (device memory, int32 [n], or 0) receives the ``layouts.BULK_*`` marks there."""
+        r = np.ascontiguousarray(np.asarray(rates, np.float32).reshape(-1))
+        _check(self._fn("lane_set_rate_device")(self._h, int(lane), int(inst0), int(r.size), r.ctypes.data_as(C.c_void_p),
+                                                C.c_void_p(int(results_ptr)) if results_ptr else None))
 
 
 class ChainEngine(_ChainEngine):

@@ -902,7 +902,9 @@ preset_collect_kernel(Record rec, uint32_t inst0, uint32_t n, const uint8_t *__r
 }
 #undef DSPI_SLOT_OFF
 
-// engine-owned staging of one chunk: packets, host volumes, recipes, sample rates (rate switch) and result codes on the device
+// a queue's staging of one chunk: packets, host volumes, recipes, sample rates (rate switch) and result codes on the device.
+// A lane's apply uploads a chunk's packets and host records in one copy: the host records follow the chunk's packets
+// (lane_host), in room kept after the packets.
 struct Stage {
     dspi_wire_bulk_params *packets = nullptr;
     dspi_bulk_host *host = nullptr;
@@ -912,7 +914,7 @@ struct Stage {
     cudaError_t ensure(int roles)
     {
         if (results) return cudaSuccess;
-        cudaError_t e = cudaMalloc((void **)&packets, (size_t)kChunk * kPacketBytes);
+        cudaError_t e = cudaMalloc((void **)&packets, (size_t)kChunk * (kPacketBytes + sizeof(dspi_bulk_host)));
         if (e == cudaSuccess) e = cudaMalloc((void **)&host, (size_t)kChunk * sizeof(dspi_bulk_host));
         if (e == cudaSuccess) e = cudaMalloc((void **)&recipes, (size_t)kChunk * roles * kMaxBands * sizeof(dspi_eq_param));
         if (e == cudaSuccess) e = cudaMalloc((void **)&rates, (size_t)kChunk * sizeof(float));
@@ -925,17 +927,19 @@ struct Stage {
         cudaFree(packets); cudaFree(host); cudaFree(recipes); cudaFree(rates); cudaFree(results);
         packets = nullptr; host = nullptr; recipes = nullptr; rates = nullptr; results = nullptr;
     }
+    dspi_bulk_host *lane_host(uint32_t nc) const { return reinterpret_cast<dspi_bulk_host *>(packets + nc); }
 };
 
-// engine-owned staging of the preset calls, next to Stage
+// a queue's staging of the preset calls, next to Stage.  A lane's preset apply uploads a chunk's images (packed at the slot
+// size), load rows and host records in one copy into `images`, which keeps room for the two after the images.
 struct PresetStage {
-    unsigned char *images = nullptr;                       // [kChunk][slot size], packed
+    unsigned char *images = nullptr;                       // [kChunk][slot size], packed; then room for [kChunk] load and host rows
     dspi_preset_load *load = nullptr;                      // [kChunk]; a collect call keeps its slot indices here, one byte each
     int32_t *results = nullptr;                            // [kChunk] preset result codes, or the marks of a collect
     cudaError_t ensure(size_t slot_bytes)
     {
         if (results) return cudaSuccess;
-        cudaError_t e = cudaMalloc((void **)&images, (size_t)kChunk * slot_bytes);
+        cudaError_t e = cudaMalloc((void **)&images, (size_t)kChunk * (slot_bytes + sizeof(dspi_preset_load) + sizeof(dspi_bulk_host)));
         if (e == cudaSuccess) e = cudaMalloc((void **)&load, (size_t)kChunk * sizeof(dspi_preset_load));
         if (e == cudaSuccess) e = cudaMalloc((void **)&results, (size_t)kChunk * sizeof(int32_t));
         if (e != cudaSuccess) destroy();
@@ -1019,6 +1023,19 @@ struct HostRing {
     }
 };
 
+// A lane's upload of `bytes` to device memory `dst` on q's stream: fill(buf) packs them into a buffer taken from q's ring,
+// which one copy sends; the buffer's event is recorded behind it.
+template <class Queue, class Fill>
+cudaError_t lane_upload(Queue &q, void *dst, size_t bytes, Fill &&fill)
+{
+    unsigned char *buf = nullptr;
+    cudaError_t e = q.ring.take(bytes, &buf);
+    if (e != cudaSuccess) return e;
+    fill(buf);
+    e = cudaMemcpyAsync(dst, buf, bytes, cudaMemcpyHostToDevice, q.stream);
+    return e == cudaSuccess ? q.ring.done(q.stream) : e;
+}
+
 // d_results of a lane edit: grouped edit j of a chunk is edit pos[j] of the call, whose instance is segment seg[j]
 static __global__ void edit_marks_kernel(const int32_t *__restrict__ marks, const uint32_t *__restrict__ pos, const uint32_t *__restrict__ seg,
                                          uint32_t n, int32_t *__restrict__ out)
@@ -1091,58 +1108,66 @@ int finish_skip(Engine *c, Queue &q)
     return rc;
 }
 
-// The ingest path for an engine (dspi_chain or dspi_chainq) whose arguments are checked.  Everything runs on the engine's
-// queue, behind earlier process calls; the last step (eq_set_skip) synchronises it.  Per chunk, stage_packets(i0, nc) puts
-// the packets of instances [i0, i0 + nc) of the call into stage.packets on the engine stream; `codes` (device, [kChunk]) is
-// what goes back to results, stage.results (the ingest kernel's codes) when it is null.
-template <class S, class Engine, class StagePackets>
-int ingest(Engine *c, uint32_t inst0, uint32_t n, const dspi_bulk_host *host, int gain_mode, float fs, int32_t *results, const int32_t *codes,
-           StagePackets &&stage_packets)
+// The ingest path for an engine (dspi_chain or dspi_chainq) whose arguments are checked, issued on queue q with its staging,
+// behind earlier calls on it.  Per chunk, stage_inputs(i0, nc, &d_host) puts the packets of instances [i0, i0 + nc) of the
+// call into stage.packets on q's stream; on a lane it uploads their host records with them and points d_host at them,
+// otherwise ingest copies them to stage.host.  `codes` (device, [kChunk]) is what goes back to results, stage.results (the
+// ingest kernel's codes) when it is null: host memory for the engine's queue, whose last step (eq_set_skip) synchronises
+// it, device memory for a lane's, copied on the lane stream.
+template <class S, class Engine, class Queue, class StageInputs>
+int ingest(Engine *c, Queue &q, uint32_t inst0, uint32_t n, const dspi_bulk_host *host, int gain_mode, float fs, int32_t *results,
+           const int32_t *codes, StageInputs &&stage_inputs)
 {
-    Stage &stage = c->q.bulk;
+    Stage &stage = q.bulk;
     cudaError_t e = stage.ensure(S::kRoles);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
-    cudaStream_t s = c->q.stream;
+    cudaStream_t s = q.stream;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk, first = inst0 + i0;
-        int rc = stage_packets(i0, nc);
+        const dspi_bulk_host *d_host = stage.host;
+        int rc = stage_inputs(i0, nc, &d_host);
         if (rc != DSPI_OK) return rc;
-        if ((e = cudaMemcpyAsync(stage.host, host + i0, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyHostToDevice, s)) != cudaSuccess)
+        if (!q.lane && (e = cudaMemcpyAsync(stage.host, host + i0, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyHostToDevice, s)) != cudaSuccess)
             return fail_cuda(e, "packet copy");
-        bulk_ingest_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.packets, stage.host, gain_mode, fs,
+        bulk_ingest_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.packets, d_host, gain_mode, fs,
                                                                                  stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "ingest kernel");
         c->launches++;
-        if ((rc = recalculate_filters<S>(c, c->q, first, nc, fs, nullptr)) != DSPI_OK) return rc;
-        if ((e = cudaMemcpyAsync(results + i0, codes ? codes : stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
+        if ((rc = recalculate_filters<S>(c, q, first, nc, fs, nullptr)) != DSPI_OK) return rc;
+        if ((e = cudaMemcpyAsync(results + i0, codes ? codes : stage.results, (size_t)nc * sizeof(int32_t),
+                                 q.lane ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s)) != cudaSuccess)
             return fail_cuda(e, "result copy");
     }
-    return finish_skip(c, c->q);
+    return finish_skip(c, q);
 }
 
 // dspi_chain(q)_set_rate_device for checked arguments: per chunk the rates go to stage.rates, rate_kernel re-derives the
 // rate-dependent rows of current instances and stages their recipes, and the filters are recalculated at each one's rate.
-// results (host, may be null) gets the marks.  On the engine stream behind earlier work; returns when the engine is updated.
-template <class S, class Engine>
-int set_rate(Engine *c, uint32_t inst0, uint32_t n, const float *rates, int32_t *results)
+// results (may be null) gets the marks.  On queue q behind earlier work: the engine's returns when the engine is updated
+// and results is host memory; a lane's uploads the rates through its ring and results is device memory.
+template <class S, class Engine, class Queue>
+int set_rate(Engine *c, Queue &q, uint32_t inst0, uint32_t n, const float *rates, int32_t *results)
 {
-    Stage &stage = c->q.bulk;
+    Stage &stage = q.bulk;
     cudaError_t e = stage.ensure(S::kRoles);
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
-    cudaStream_t s = c->q.stream;
+    cudaStream_t s = q.stream;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk, first = inst0 + i0;
-        if ((e = cudaMemcpyAsync(stage.rates, rates + i0, (size_t)nc * sizeof(float), cudaMemcpyHostToDevice, s)) != cudaSuccess)
-            return fail_cuda(e, "rate copy");
+        const size_t bytes = (size_t)nc * sizeof(float);
+        e = q.lane ? lane_upload(q, stage.rates, bytes, [&](unsigned char *b) { memcpy(b, rates + i0, bytes); })
+                   : cudaMemcpyAsync(stage.rates, rates + i0, bytes, cudaMemcpyHostToDevice, s);
+        if (e != cudaSuccess) return fail_cuda(e, "rate copy");
         rate_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->d, c->rec, first, nc, stage.rates, stage.recipes, stage.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "rate kernel");
         c->launches++;
-        int rc = recalculate_filters<S>(c, c->q, first, nc, 0.0f, stage.rates);
+        int rc = recalculate_filters<S>(c, q, first, nc, 0.0f, stage.rates);
         if (rc != DSPI_OK) return rc;
-        if (results && (e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s)) != cudaSuccess)
+        if (results && (e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t),
+                                            q.lane ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s)) != cudaSuccess)
             return fail_cuda(e, "result copy");
     }
-    return finish_skip(c, c->q);
+    return finish_skip(c, q);
 }
 
 // dspi_chain(q)_edit_bulk_device for checked arguments.  Edits of different instances commute, so the list is cut into
@@ -1258,33 +1283,58 @@ int edit(Engine *c, Queue &q, uint32_t n_edits, const dspi_bulk_edit *edits, int
     return DSPI_OK;
 }
 
-// dspi_chain(q)_apply_bulk_device for checked arguments
-template <class S, class Engine>
-int apply(Engine *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host, int exact_db, float fs,
-          int32_t *results)
+// dspi_chain(q)_apply_bulk_device for checked arguments, on queue q
+template <class S, class Engine, class Queue>
+int apply(Engine *c, Queue &q, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host, int exact_db,
+          float fs, int32_t *results)
 {
-    return ingest<S>(c, inst0, n, host, exact_db ? kGainExact : kGainTaylor, fs, results, nullptr, [&](uint32_t i0, uint32_t nc) -> int {
-        const cudaError_t e = cudaMemcpyAsync(c->q.bulk.packets, packets + i0, (size_t)nc * kPacketBytes, cudaMemcpyHostToDevice, c->q.stream);
+    return ingest<S>(c, q, inst0, n, host, exact_db ? kGainExact : kGainTaylor, fs, results, nullptr,
+                     [&](uint32_t i0, uint32_t nc, const dspi_bulk_host **d_host) -> int {
+        const size_t pb = (size_t)nc * kPacketBytes, hb = (size_t)nc * sizeof(dspi_bulk_host);
+        cudaError_t e;
+        if (q.lane) {
+            *d_host = q.bulk.lane_host(nc);
+            e = lane_upload(q, q.bulk.packets, pb + hb, [&](unsigned char *b) {
+                memcpy(b, packets + i0, pb);
+                memcpy(b + pb, host + i0, hb);
+            });
+        } else {
+            e = cudaMemcpyAsync(q.bulk.packets, packets + i0, pb, cudaMemcpyHostToDevice, q.stream);
+        }
         return e == cudaSuccess ? DSPI_OK : fail_cuda(e, "packet copy");
     });
 }
 
-// dspi_chain(q)_apply_preset_device for checked arguments: images -> packets by preset_decode_kernel, then the ingest path
-// with the flash conversion; the preset result codes go back
-template <class S, class Engine>
-int apply_preset(Engine *c, PresetStage &ps, uint32_t inst0, uint32_t n, const void *images, size_t stride, const dspi_preset_load *load,
+// dspi_chain(q)_apply_preset_device for checked arguments, on queue q with its preset staging: images -> packets by
+// preset_decode_kernel, then the ingest path with the flash conversion; the preset result codes go back
+template <class S, class Engine, class Queue>
+int apply_preset(Engine *c, Queue &q, uint32_t inst0, uint32_t n, const void *images, size_t stride, const dspi_preset_load *load,
                  const dspi_bulk_host *host, float fs, int32_t *results)
 {
     constexpr size_t kSlot = sizeof(SlotOf<S>);
+    PresetStage &ps = q.preset;
     cudaError_t e = ps.ensure(kSlot);
     if (e != cudaSuccess) return fail_cuda(e, "preset staging buffers");
-    return ingest<S>(c, inst0, n, host, kGainFlash, fs, results, ps.results, [&](uint32_t i0, uint32_t nc) -> int {
-        cudaStream_t s = c->q.stream;
-        cudaError_t e = cudaMemcpy2DAsync(ps.images, kSlot, static_cast<const unsigned char *>(images) + (size_t)i0 * stride, stride, kSlot, nc,
-                                          cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ps.load, load + i0, (size_t)nc * sizeof(dspi_preset_load), cudaMemcpyHostToDevice, s);
+    return ingest<S>(c, q, inst0, n, host, kGainFlash, fs, results, ps.results, [&](uint32_t i0, uint32_t nc, const dspi_bulk_host **d_host) -> int {
+        cudaStream_t s = q.stream;
+        const unsigned char *src = static_cast<const unsigned char *>(images) + (size_t)i0 * stride;
+        const dspi_preset_load *d_load = ps.load;
+        cudaError_t e;
+        if (q.lane) {
+            const size_t ib = (size_t)nc * kSlot, lb = (size_t)nc * sizeof(dspi_preset_load), hb = (size_t)nc * sizeof(dspi_bulk_host);
+            d_load = reinterpret_cast<const dspi_preset_load *>(ps.images + ib);
+            *d_host = reinterpret_cast<const dspi_bulk_host *>(ps.images + ib + lb);
+            e = lane_upload(q, ps.images, ib + lb + hb, [&](unsigned char *b) {
+                for (uint32_t i = 0; i < nc; i++) memcpy(b + (size_t)i * kSlot, src + (size_t)i * stride, kSlot);
+                memcpy(b + ib, load + i0, lb);
+                memcpy(b + ib + lb, host + i0, hb);
+            });
+        } else {
+            e = cudaMemcpy2DAsync(ps.images, kSlot, src, stride, kSlot, nc, cudaMemcpyHostToDevice, s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(ps.load, load + i0, (size_t)nc * sizeof(dspi_preset_load), cudaMemcpyHostToDevice, s);
+        }
         if (e != cudaSuccess) return fail_cuda(e, "image copy");
-        preset_decode_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(ps.images, ps.load, nc, c->q.bulk.packets, ps.results);
+        preset_decode_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(ps.images, d_load, nc, q.bulk.packets, ps.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "preset decode kernel");
         c->launches++;
         return DSPI_OK;

@@ -84,9 +84,10 @@ struct Queue {
     cudaStream_t stream = nullptr;   // the engine stream callers see, or the lane's; stages run on st.* between ev_begin and ev_done
     ChainStreams st;
     PacketSchedule sched;            // packet lengths of the current call
-    bulk::Stage bulk;                // device staging of the bulk applies, collects and edits
+    bulk::Stage bulk;                // device staging of the bulk applies, rate switches, collects and edits
     bulk::EditStage bulk_edit;
-    bulk::HostRing ring;             // edits, fade rows and transmitter rows on their way to the device
+    bulk::PresetStage preset;        // device staging of the preset applies and collects
+    bulk::HostRing ring;             // a lane's edits, packets, images, rates, fade rows and transmitter rows on their way to the device
     cudaEvent_t ev_engine = nullptr, ev_last = nullptr;   // a lane's
 
     // `lane` set first
@@ -107,6 +108,7 @@ struct Queue {
         sched.destroy();
         bulk.destroy();
         bulk_edit.destroy();
+        preset.destroy();
         ring.destroy();
         for (cudaEvent_t *ev : { &ev_engine, &ev_last })
             if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
@@ -135,7 +137,6 @@ struct ChainHost {
     std::vector<uint8_t> env_mode;   // [N] each instance's envelope-mode flag (env row 4 != 0), as the calls issued so far leave it
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     ResponseBuffers resp;            // frequency table of *_response_*; host staging of *_response_host and the instance image calls
-    bulk::PresetStage preset;        // device staging of *_apply_preset_device / _collect_preset_device, allocated by the first call
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
     IndexLists copy_lists;           // device instance lists of *_copy_instances, allocated by the first call
     Queue lanes[DSPI_CHAIN_MAX_LANES];   // open while it has a stream
@@ -383,7 +384,6 @@ int destroy(H *c)
     c->q.destroy();
     c->part.destroy();
     c->resp.destroy();
-    c->preset.destroy();
     c->copy_lists.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
@@ -690,29 +690,50 @@ int set_dynamics_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_
     return DSPI_OK;
 }
 
+// Before a lane call that configures instances: a lane's first call that needs a staging it lacks (`staged` false)
+// allocates it, and an engine whose skip rows were never set (no set_params, apply, import, copy or edit yet) remasks every
+// row once; both first wait for every lane and the engine stream.  Nothing for the engine's queue.
 template <class A>
-int apply_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
-                      int exact_db, float sample_rate, int32_t *results)
+int lane_prepare(ChainHost<A> *c, const Queue &q, bool staged)
 {
-    if (!c || !packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
-    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    int rc = check_range(c->q, inst0, n);
-    if (rc || n == 0) return rc;
-    CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::apply<typename A::Stores>(c, inst0, n, packets, host, exact_db, sample_rate, results);
+    if (!q.lane) return DSPI_OK;
+    const bool skip_set = eq_skip_set(c->eq_m) && eq_skip_set(c->eq_o);
+    if (staged && skip_set) return DSPI_OK;
+    CU_OK(drain(c));
+    return skip_set ? DSPI_OK : bulk::finish_skip(c, c->q);
 }
 
+// results: host memory for the engine's queue, device memory for a lane's
 template <class A>
-int set_rate_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results)
+int apply_bulk_device(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets, const dspi_bulk_host *host,
+                      int exact_db, float sample_rate, int32_t *results)
 {
-    if (!c || !sample_rates) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c->q, inst0, n);                     // before the rates are read: n counts them
+    if (!q) return DSPI_EINVAL;
+    if (!packets || !host || !results) return fail(DSPI_EINVAL, "null argument");
+    if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
+    int rc = check_range(*q, inst0, n);
+    if (rc || n == 0) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    if ((rc = lane_prepare(c, *q, q->bulk.results != nullptr)) != DSPI_OK) return rc;
+    CU_OK(begin_call(c, *q));
+    return end_call(*q, bulk::apply<typename A::Stores>(c, *q, inst0, n, packets, host, exact_db, sample_rate, results));
+}
+
+// results (may be NULL): host memory for the engine's queue, device memory for a lane's
+template <class A>
+int set_rate_device(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const float *sample_rates, int32_t *results)
+{
+    if (!q) return DSPI_EINVAL;
+    if (!sample_rates) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(*q, inst0, n);                       // before the rates are read: n counts them
     if (rc) return rc;
     for (uint32_t i = 0; i < n; i++)
         if (!(sample_rates[i] > 0.0f) || sample_rates[i] > 3.4e38f) return fail(DSPI_EINVAL, "sample_rates[%u] must be positive and finite", i);
     if (n == 0) return DSPI_OK;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::set_rate<typename A::Stores>(c, inst0, n, sample_rates, results);
+    if ((rc = lane_prepare(c, *q, q->bulk.results != nullptr)) != DSPI_OK) return rc;
+    CU_OK(begin_call(c, *q));
+    return end_call(*q, bulk::set_rate<typename A::Stores>(c, *q, inst0, n, sample_rates, results));
 }
 
 // the argument checks of *_edit_bulk_device on queue q: every edit well formed and naming an instance of the engine,
@@ -750,13 +771,7 @@ int edit_bulk_device(ChainHost<A> *c, Queue *q, uint32_t n_edits, const dspi_bul
     int rc = check_edits(c, *q, n_edits, edits, sample_rate);
     if (rc || n_edits == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    // A lane's first edit allocates its staging, and an engine whose skip rows were never set (no set_params, apply,
-    // import, copy or edit yet) remasks every row once: both wait for every lane and the engine stream first.
-    const bool skip_set = eq_skip_set(c->eq_m) && eq_skip_set(c->eq_o);
-    if (q->lane && (!q->bulk_edit.marks || !skip_set)) {
-        CU_OK(drain(c));
-        if (!skip_set && (rc = bulk::finish_skip(c, c->q)) != DSPI_OK) return rc;
-    }
+    if ((rc = lane_prepare(c, *q, q->bulk_edit.marks != nullptr)) != DSPI_OK) return rc;
     CU_OK(begin_call(c, *q));
     return end_call(*q, bulk::edit<typename A::Stores>(c, *q, n_edits, edits, exact_db, sample_rate, results));
 }
@@ -771,18 +786,22 @@ int collect_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_wire_b
     return bulk::collect<typename A::Stores>(c, inst0, n, packets, host, results);
 }
 
+// results: host memory for the engine's queue, device memory for a lane's
 template <class A>
-int apply_preset_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *images, size_t image_stride, const dspi_preset_load *load,
-                        const dspi_bulk_host *host, float sample_rate, int32_t *results)
+int apply_preset_device(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const void *images, size_t image_stride,
+                        const dspi_preset_load *load, const dspi_bulk_host *host, float sample_rate, int32_t *results)
 {
     constexpr size_t kSlot = sizeof(bulk::SlotOf<typename A::Stores>);
-    if (!c || !images || !load || !host || !results) return fail(DSPI_EINVAL, "null argument");
+    if (!q) return DSPI_EINVAL;
+    if (!images || !load || !host || !results) return fail(DSPI_EINVAL, "null argument");
     if (image_stride < kSlot) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, kSlot);
     if (!(sample_rate > 0.0f) || sample_rate > 3.4e38f) return fail(DSPI_EINVAL, "sample_rate must be positive and finite");
-    int rc = check_range(c->q, inst0, n);
+    int rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::apply_preset<typename A::Stores>(c, c->preset, inst0, n, images, image_stride, load, host, sample_rate, results);
+    if ((rc = lane_prepare(c, *q, q->bulk.results && q->preset.results)) != DSPI_OK) return rc;
+    CU_OK(begin_call(c, *q));
+    return end_call(*q, bulk::apply_preset<typename A::Stores>(c, *q, inst0, n, images, image_stride, load, host, sample_rate, results));
 }
 
 template <class A>
@@ -795,7 +814,7 @@ int collect_preset_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const uin
     int rc = check_range(c->q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::collect_preset<typename A::Stores>(c, c->preset, inst0, n, slot_indices, images, image_stride, results);
+    return bulk::collect_preset<typename A::Stores>(c, c->q.preset, inst0, n, slot_indices, images, image_stride, results);
 }
 
 template <class A>
@@ -1074,8 +1093,9 @@ int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32
 }
 
 // ---- lanes: issue queues of one engine over disjoint instance windows, whose calls run concurrently -------------------
-// A lane takes process calls and the control calls a running clock group needs (edits, fades, transmitter restamps and
-// resets): set_preset_mute, set_spdif_tx, reset_instances, edit_bulk_device and process_device on its queue.
+// A lane takes process calls and the control calls a running clock group needs (edits, fades, transmitter restamps,
+// resets, applies, preset applies and rate switches): set_preset_mute, set_spdif_tx, reset_instances, edit_bulk_device,
+// apply_bulk_device, apply_preset_device, set_rate_device and process_device on its queue.
 template <class A>
 int lane_open(ChainHost<A> *c, uint32_t inst0, uint32_t n, uint32_t *lane)
 {

@@ -964,34 +964,43 @@ void *dspi_chainq_lane_stream(dspi_chainq *c, uint32_t lane);
 int   dspi_chainq_lane_sync  (dspi_chainq *c, uint32_t lane);
 
 /* Lane control calls: the control calls a running clock group needs (a Console edit, a preset-change fade, a transmitter
- * restamp, a device restart), issued on the group's lane so that they neither wait for nor hold up the other groups.
+ * restamp, a device restart, a device connecting, a preset recall, a session rate change), issued on the group's lane so
+ * that they neither wait for nor hold up the other groups.
  *   Semantics.  Each call means exactly what its engine-level counterpart means over the same instances:
  *   _lane_edit_bulk_device is _edit_bulk_device, _lane_set_preset_mute is _set_preset_mute, _lane_set_spdif_tx is
- *   _set_spdif_tx and _lane_reset_instances is _reset_instances, with the same argument checks.  Outputs, state, meters,
- *   envelope, transmitter, configuration record, host record and marks are byte for byte what the same sequence gives on
- *   the engine stream: every lane's calls in issue order, with the control calls issued as engine-level calls.
+ *   _set_spdif_tx, _lane_reset_instances is _reset_instances, _lane_apply_bulk_device is _apply_bulk_device,
+ *   _lane_apply_preset_device is _apply_preset_device and _lane_set_rate_device is _set_rate_device, with the same argument
+ *   checks, result codes, state rules, gain modes and libm policy; a rejected packet or image changes nothing.  Outputs,
+ *   biquads, state, meters, envelope, transmitter, configuration record, host record and marks are byte for byte what the
+ *   same sequence gives on the engine stream: every lane's calls in issue order, with the control calls issued as
+ *   engine-level calls.
  *   Window.  Every instance a call names lies inside the lane's window: each edits[k].instance, or [inst0, inst0 + n) for
  *   the others (inst0 has no alignment rule beyond that).  Otherwise the call fails with DSPI_ERANGE.
  *   Ordering.  A lane control call is ordered against its lane's calls in issue order, and against engine-level calls as
  *   lane process calls are; never against another lane.
- *   No host wait.  The call returns without waiting for the device.  edits, states and tx are read during the call and
- *   may be reused as soon as it returns.  Exceptions, each a growth of a buffer: a lane's first edit allocates its
- *   staging, and an engine whose skip rows were never set (no set_params, apply, import, copy or edit yet) remasks every
- *   row once; both first wait for every lane and the engine stream.  Uploads go through a ring of 8 pinned host buffers
- *   per lane: a call waits when the buffer it takes is still read by a copy 8 uploads back, and a buffer that has to grow
- *   for a larger upload than it carried before is a pinned allocation, which may wait for the device.  A fade arm can
- *   make the lane's next process call grow the envelope table (see Threads above).
- *   Results.  d_results (device memory, [n_edits], may be NULL) receives the mark of each edit's instance at the call's
- *   point in the lane stream, visible on _lane_stream.
- *   K1 kernel choice.  Lane edits re-pack EQ rows but leave the K1 kernel that float engines selected for the topology
- *   of their rows, since other lanes may be running it; the next engine-level call waits for the lanes and selects it
- *   again.  Only speed depends on the choice.
+ *   No host wait.  The call returns without waiting for the device.  edits, states, tx, packets, host, images (at any
+ *   stride >= the slot size), load and sample_rates are read during the call and may be reused as soon as it returns.
+ *   Exceptions, each a growth of a buffer: a lane's first edit, first apply or rate switch, and first preset apply
+ *   allocate its staging, and an engine whose skip rows were never set (no set_params, apply, import, copy or edit yet)
+ *   remasks every row once; these first wait for every lane and the engine stream.  Uploads go through a ring of 8 pinned
+ *   host buffers per lane: a call waits when the buffer it takes is still read by a copy 8 uploads back (an apply or
+ *   preset apply takes one per 1024 instances), and a buffer that has to grow for a larger upload than it carried before
+ *   is a pinned allocation, which may wait for the device.  A fade arm can make the lane's next process call grow the
+ *   envelope table (see Threads above).
+ *   Results.  d_results is device memory, written on the lane stream at the call's point and visible on _lane_stream:
+ *   [n_edits] marks of each edit's instance (may be NULL); [n] firmware codes of a bulk apply and DSPI_PRESET_* codes of a
+ *   preset apply (required, as results is for the engine-level calls); [n] DSPI_BULK_* marks of a rate switch (may be
+ *   NULL).
+ *   K1 kernel choice.  Lane edits, applies, preset applies and rate switches re-pack EQ rows but leave the K1 kernel that
+ *   float engines selected for the topology of their rows, since other lanes may be running it; the next engine-level
+ *   call waits for the lanes and selects it again.  Only speed depends on the choice.
  *   Errors (nothing is written on any error): every refusal of the engine-level call, and an unknown or closed lane, with
  *   DSPI_EINVAL; a window violation with DSPI_ERANGE.
  *   No lane control call made.  Every other call issues exactly the work it issues without them.
- * Left as barriers: _apply_bulk_device and _apply_preset_device stage whole packets and slot images through the engine's
- * 1024-instance staging; _set_rate_device, since a device that changes rate moves to another group's window with
- * _copy_instances, which is engine-level anyway; and every getter, since each returns data to the host. */
+ * Left as barriers: every getter (_collect_bulk_device, _collect_preset_device, _response_*, _export_instances, _get_*),
+ * since each returns data to the host, and the other writes (_set_params, _upload_biquads, _set_eq_params_device,
+ * _set_dynamics_device, _copy_instances, _import_instances), since the wire-packet routes above cover what a Console or a
+ * preset sends and a device that changes rate moves to another group's window with _copy_instances. */
 int dspi_chain_lane_edit_bulk_device  (dspi_chain *c, uint32_t lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db,
                                        float sample_rate, int32_t *d_results);
 int dspi_chain_lane_set_preset_mute   (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_preset_mute *states,
@@ -1004,6 +1013,18 @@ int dspi_chainq_lane_set_preset_mute  (dspi_chainq *c, uint32_t lane, uint32_t i
                                        uint32_t sample_rate_hz);
 int dspi_chainq_lane_set_spdif_tx     (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_spdif_tx *tx);
 int dspi_chainq_lane_reset_instances  (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n);
+int dspi_chain_lane_apply_bulk_device   (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets,
+                                        const dspi_bulk_host *host, int exact_db, float sample_rate, int32_t *d_results);
+int dspi_chain_lane_apply_preset_device (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *images, size_t image_stride,
+                                        const dspi_preset_load *load, const dspi_bulk_host *host, float sample_rate, int32_t *d_results);
+int dspi_chain_lane_set_rate_device     (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const float *sample_rates,
+                                        int32_t *d_results);
+int dspi_chainq_lane_apply_bulk_device  (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_wire_bulk_params *packets,
+                                        const dspi_bulk_host *host, int exact_db, float sample_rate, int32_t *d_results);
+int dspi_chainq_lane_apply_preset_device(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *images, size_t image_stride,
+                                        const dspi_preset_load *load, const dspi_bulk_host *host, float sample_rate, int32_t *d_results);
+int dspi_chainq_lane_set_rate_device    (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const float *sample_rates,
+                                        int32_t *d_results);
 
 /* ---- frequency response of EQ channels and chain instances ------------------------------------ */
 /* The complex transfer function H(e^{j omega}) of the linear, time-invariant part of the path the NEXT process call applies,
