@@ -66,6 +66,10 @@ SYMBOLS = [
     "dspi_chainq_lane_edit_bulk_device", "dspi_chainq_lane_set_preset_mute", "dspi_chainq_lane_set_spdif_tx", "dspi_chainq_lane_reset_instances",
     "dspi_chain_lane_apply_bulk_device", "dspi_chain_lane_apply_preset_device", "dspi_chain_lane_set_rate_device",
     "dspi_chainq_lane_apply_bulk_device", "dspi_chainq_lane_apply_preset_device", "dspi_chainq_lane_set_rate_device",
+    "dspi_chain_lane_collect_bulk_device", "dspi_chain_lane_collect_preset_device", "dspi_chain_lane_export_instances",
+    "dspi_chain_lane_response_device", "dspi_chain_lane_get_preset_mute", "dspi_chain_lane_get_spdif_tx",
+    "dspi_chainq_lane_collect_bulk_device", "dspi_chainq_lane_collect_preset_device", "dspi_chainq_lane_export_instances",
+    "dspi_chainq_lane_response_device", "dspi_chainq_lane_get_preset_mute", "dspi_chainq_lane_get_spdif_tx",
 ]
 
 
@@ -185,6 +189,12 @@ def lib():
             getattr(h, pre + "_lane_apply_bulk_device").argtypes = [vp, u32, u32, u32, vp, vp, C.c_int, C.c_float, vp]
             getattr(h, pre + "_lane_apply_preset_device").argtypes = [vp, u32, u32, u32, vp, C.c_size_t, vp, vp, C.c_float, vp]
             getattr(h, pre + "_lane_set_rate_device").argtypes = [vp, u32, u32, u32, vp, vp]
+            getattr(h, pre + "_lane_collect_bulk_device").argtypes = [vp, u32, u32, u32, vp, vp, vp]
+            getattr(h, pre + "_lane_collect_preset_device").argtypes = [vp, u32, u32, u32, vp, vp, C.c_size_t, vp]
+            getattr(h, pre + "_lane_export_instances").argtypes = [vp, u32, u32, u32, vp, C.c_size_t]
+            getattr(h, pre + "_lane_response_device").argtypes = [vp, u32, u32, u32, vp, u32, C.c_float, vp]
+            getattr(h, pre + "_lane_get_preset_mute").argtypes = [vp, u32, u32, u32, vp]
+            getattr(h, pre + "_lane_get_spdif_tx").argtypes = [vp, u32, u32, u32, vp]
         for pre in ("dspi_eq", "dspi_chain", "dspi_chainq"):
             getattr(h, pre + "_response_host").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
             getattr(h, pre + "_response_device").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
@@ -887,6 +897,51 @@ class _ChainEngine:
         r = np.ascontiguousarray(np.asarray(rates, np.float32).reshape(-1))
         _check(self._fn("lane_set_rate_device")(self._h, int(lane), int(inst0), int(r.size), r.ctypes.data_as(C.c_void_p),
                                                 C.c_void_p(int(results_ptr)) if results_ptr else None))
+
+    # Lane reads: each writes what its engine-level counterpart returns into device memory on ``lane_stream(lane)`` and
+    # returns without waiting; [inst0, inst0+n) lies inside the lane's window.
+
+    def lane_collect_bulk_device(self, lane, inst0, n, packets_ptr, host_ptr=0, results_ptr=0):
+        """``collect_bulk_device`` issued on a lane: WIRE_BULK [n] at ``packets_ptr``, BULK_HOST [n] at ``host_ptr`` and int32
+        [n] marks at ``results_ptr`` (both optional)."""
+        _check(self._fn("lane_collect_bulk_device")(self._h, int(lane), int(inst0), int(n), C.c_void_p(int(packets_ptr)) if packets_ptr else None,
+                                                    C.c_void_p(int(host_ptr)) if host_ptr else None,
+                                                    C.c_void_p(int(results_ptr)) if results_ptr else None))
+
+    def lane_collect_preset_device(self, lane, slots, inst0, images_ptr, stride, n=None, results_ptr=0):
+        """``collect_preset_device`` issued on a lane: uint8 [n, stride] slot images at ``images_ptr`` (stride >= the slot
+        size; the tail of each row is left alone) and int32 [n] marks at ``results_ptr`` (optional).  ``slots`` is a scalar or
+        [n]; it is read during the call."""
+        sl = np.asarray(slots, np.uint8).reshape(-1)
+        n = sl.size if n is None else int(n)
+        sl = np.ascontiguousarray(np.broadcast_to(sl, (max(n, 0),)) if sl.size == 1 else sl)
+        if sl.size != max(n, 0):
+            raise ValueError("slots and n give different instance counts")
+        _check(self._fn("lane_collect_preset_device")(self._h, int(lane), int(inst0), n, sl.ctypes.data_as(C.c_void_p),
+                                                      C.c_void_p(int(images_ptr)) if images_ptr else None, C.c_size_t(int(stride)),
+                                                      C.c_void_p(int(results_ptr)) if results_ptr else None))
+
+    def lane_export_instances(self, lane, inst0, n, images_ptr, stride=None):
+        """``export_instances`` issued on a lane: uint8 [n, stride] instance images at ``images_ptr`` (stride >=
+        ``instance_image_size()``, its default; the tail of each row is left alone)."""
+        stride = self.instance_image_size() if stride is None else int(stride)
+        _check(self._fn("lane_export_instances")(self._h, int(lane), int(inst0), int(n), C.c_void_p(int(images_ptr)) if images_ptr else None,
+                                                 C.c_size_t(stride)))
+
+    def lane_response_device(self, lane, freqs, fs, inst0, n, out_ptr):
+        """``response(freqs, fs, inst0, n, out_ptr)`` issued on a lane: complex64 [n, outputs, 2 inputs, n_freqs] at
+        ``out_ptr``.  ``freqs`` is read during the call."""
+        f = np.ascontiguousarray(freqs, np.float32).reshape(-1)
+        _check(self._fn("lane_response_device")(self._h, int(lane), int(inst0), int(n), f.ctypes.data_as(C.c_void_p), f.size, C.c_float(fs),
+                                                C.c_void_p(int(out_ptr)) if out_ptr else None))
+
+    def lane_get_preset_mute(self, lane, inst0, n, states_ptr):
+        """``get_preset_mute`` issued on a lane: PRESET_MUTE [n] at ``states_ptr``."""
+        _check(self._fn("lane_get_preset_mute")(self._h, int(lane), int(inst0), int(n), C.c_void_p(int(states_ptr)) if states_ptr else None))
+
+    def lane_get_spdif_tx(self, lane, inst0, n, tx_ptr):
+        """``get_spdif_tx`` issued on a lane: SPDIF_TX [n] at ``tx_ptr``."""
+        _check(self._fn("lane_get_spdif_tx")(self._h, int(lane), int(inst0), int(n), C.c_void_p(int(tx_ptr)) if tx_ptr else None))
 
 
 class ChainEngine(_ChainEngine):

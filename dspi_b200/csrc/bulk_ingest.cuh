@@ -620,7 +620,8 @@ __device__ inline void record_dynamics(const Record &rec, uint32_t inst, const d
     rec.host[inst].host_mute = cfg.host_mute;
 }
 
-// REQ_GET_ALL_PARAMS: record -> the packet bulk_params_collect() returns (:66-78 header, :123 pin count), one warp per instance
+// REQ_GET_ALL_PARAMS: record -> the packet bulk_params_collect() returns (:66-78 header, :123 pin count), one warp per instance.
+// host and results may be null (a lane collect writes the caller's device memory, where both are optional).
 template <class S>
 __global__ void __launch_bounds__(kWarps * 32)
 bulk_collect_kernel(Record rec, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *__restrict__ packets, dspi_bulk_host *__restrict__ host,
@@ -658,9 +659,9 @@ bulk_collect_kernel(Record rec, uint32_t inst0, uint32_t n, dspi_wire_bulk_param
     if (lane == 0) {
         bulk_store_1d(packets + i, pkt_s[warp], kPacketBytes);
         tma_store_commit();
-        results[i] = mark;
+        if (results) results[i] = mark;
         tma_store_wait_all<0>();
-    } else if (lane == 1) {
+    } else if (lane == 1 && host) {
         host[i] = mark == DSPI_BULK_UNSET ? dspi_bulk_host{0, 0, 0} : rec.host[inst];
     }
 }
@@ -1362,49 +1363,70 @@ int record_recipes(Engine *c, uint32_t inst0, uint32_t n, const dspi_eq_param *r
     return DSPI_OK;
 }
 
-// dspi_chain(q)_collect_bulk_device for checked arguments: on the engine stream, behind everything issued before; reads only.
-template <class S, class Engine>
-int collect(Engine *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
+// Whether a collect into `packets` goes through q's staging.  bulk_collect_kernel stores whole packets with bulk copies,
+// which need a 16-byte aligned destination, while a dspi_wire_bulk_params pointer may hold any address (the record is
+// packed).  The engine's queue always stages (the caller's memory is on the host); a lane writes the caller's device
+// memory directly when the packets are 16-byte aligned, and otherwise stages and copies device to device.
+template <class Queue>
+bool collect_staged(const Queue &q, const void *packets)
 {
-    Stage &stage = c->q.bulk;
-    cudaError_t e = stage.ensure(S::kRoles);
+    return !q.lane || ((uintptr_t)packets & 15u) != 0;
+}
+
+// dspi_chain(q)_collect_bulk_device for checked arguments, on queue q behind everything issued before it; reads only.
+// Staged (collect_staged): each chunk goes to q's staging, then to the caller's host memory (the engine's queue: the call's
+// end synchronises) or device memory (a lane's).  Otherwise the kernel writes the caller's device memory directly.
+template <class S, class Engine, class Queue>
+int collect(Engine *c, Queue &q, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
+{
+    Stage &stage = q.bulk;
+    const bool staged = collect_staged(q, packets);
+    cudaError_t e = staged ? stage.ensure(S::kRoles) : cudaSuccess;
     if (e != cudaSuccess) return fail_cuda(e, "staging buffers");
-    cudaStream_t s = c->q.stream;
+    cudaStream_t s = q.stream;
+    const cudaMemcpyKind back = q.lane ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;
-        bulk_collect_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->rec, inst0 + i0, nc, stage.packets, stage.host, stage.results);
+        dspi_wire_bulk_params *to_p = staged ? stage.packets : packets + i0;
+        dspi_bulk_host *to_h = staged ? stage.host : host ? host + i0 : nullptr;
+        int32_t *to_r = staged ? stage.results : results ? results + i0 : nullptr;
+        bulk_collect_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->rec, inst0 + i0, nc, to_p, to_h, to_r);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "collect kernel");
         c->launches++;
-        e = cudaMemcpyAsync(packets + i0, stage.packets, (size_t)nc * kPacketBytes, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && host) e = cudaMemcpyAsync(host + i0, stage.host, (size_t)nc * sizeof(dspi_bulk_host), cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && results) e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+        if (!staged) continue;
+        e = cudaMemcpyAsync(packets + i0, stage.packets, (size_t)nc * kPacketBytes, back, s);
+        if (e == cudaSuccess && host) e = cudaMemcpyAsync(host + i0, stage.host, (size_t)nc * sizeof(dspi_bulk_host), back, s);
+        if (e == cudaSuccess && results) e = cudaMemcpyAsync(results + i0, stage.results, (size_t)nc * sizeof(int32_t), back, s);
         if (e != cudaSuccess) return fail_cuda(e, "packet copy");
     }
-    if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return fail_cuda(e, "collect");
     return DSPI_OK;
 }
 
-// dspi_chain(q)_collect_preset_device for checked arguments: on the engine stream, behind everything issued before; reads only
-template <class S, class Engine>
-int collect_preset(Engine *c, PresetStage &ps, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t stride,
-                   int32_t *results)
+// dspi_chain(q)_collect_preset_device for checked arguments, on queue q with its preset staging, behind everything issued
+// before it; reads only.  The slot indices go up with a copy (the engine's queue) or through the lane's ring; images and
+// results come back to host memory (the engine's queue; the call's end synchronises) or to device memory (a lane's).
+template <class S, class Engine, class Queue>
+int collect_preset(Engine *c, Queue &q, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t stride, int32_t *results)
 {
     constexpr size_t kSlot = sizeof(SlotOf<S>);
+    PresetStage &ps = q.preset;
     cudaError_t e = ps.ensure(kSlot);
     if (e != cudaSuccess) return fail_cuda(e, "preset staging buffers");
-    cudaStream_t s = c->q.stream;
+    cudaStream_t s = q.stream;
+    const cudaMemcpyKind back = q.lane ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     uint8_t *slots = reinterpret_cast<uint8_t *>(ps.load);
     for (uint32_t i0 = 0; i0 < n; i0 += kChunk) {
         const uint32_t nc = n - i0 < kChunk ? n - i0 : kChunk;
-        if ((e = cudaMemcpyAsync(slots, slot_indices + i0, nc, cudaMemcpyHostToDevice, s)) != cudaSuccess) return fail_cuda(e, "slot index copy");
+        e = q.lane ? lane_upload(q, slots, nc, [&](unsigned char *b) { memcpy(b, slot_indices + i0, nc); })
+                   : cudaMemcpyAsync(slots, slot_indices + i0, nc, cudaMemcpyHostToDevice, s);
+        if (e != cudaSuccess) return fail_cuda(e, "slot index copy");
         preset_collect_kernel<S><<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(c->rec, inst0 + i0, nc, slots, ps.images, ps.results);
         if ((e = cudaGetLastError()) != cudaSuccess) return fail_cuda(e, "preset collect kernel");
         c->launches++;
-        e = cudaMemcpy2DAsync(static_cast<unsigned char *>(images) + (size_t)i0 * stride, stride, ps.images, kSlot, kSlot, nc, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && results) e = cudaMemcpyAsync(results + i0, ps.results, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+        e = cudaMemcpy2DAsync(static_cast<unsigned char *>(images) + (size_t)i0 * stride, stride, ps.images, kSlot, kSlot, nc, back, s);
+        if (e == cudaSuccess && results) e = cudaMemcpyAsync(results + i0, ps.results, (size_t)nc * sizeof(int32_t), back, s);
         if (e != cudaSuccess) return fail_cuda(e, "image copy");
     }
-    if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return fail_cuda(e, "preset collect");
     return DSPI_OK;
 }
 

@@ -1,6 +1,7 @@
 // chain_host.cuh — the host half of the float and Q28 chain engines (chain_f32.cu, chain_q28.cu): engine record,
 // lifetime, argument checks, parameter uploads, the stage pipeline over packet slices, host staging, S/PDIF transmitter
-// state, checkpoints and the frequency response.  Host code only; each engine file includes it after its kernels.
+// state, checkpoints and the frequency response.  Host code, and the two record kernels of the lane getters; each engine
+// file includes it after its kernels.
 //
 // Everything here is a template over the engine's arithmetic traits A, which supply what differs between the two
 // engines: the types (A::Dev the device record, A::Biquad, A::Status, A::Params, A::Stores the device-side parameter
@@ -87,7 +88,8 @@ struct Queue {
     bulk::Stage bulk;                // device staging of the bulk applies, rate switches, collects and edits
     bulk::EditStage bulk_edit;
     bulk::PresetStage preset;        // device staging of the preset applies and collects
-    bulk::HostRing ring;             // a lane's edits, packets, images, rates, fade rows and transmitter rows on their way to the device
+    bulk::HostRing ring;             // a lane's edits, packets, images, rates, slot indices, fade rows and transmitter rows on their way to the device
+    ResponseBuffers resp;            // frequency table of the response calls; image staging of export (and, the engine's, of import and _response_host)
     cudaEvent_t ev_engine = nullptr, ev_last = nullptr;   // a lane's
 
     // `lane` set first
@@ -110,6 +112,7 @@ struct Queue {
         bulk_edit.destroy();
         preset.destroy();
         ring.destroy();
+        resp.destroy();
         for (cudaEvent_t *ev : { &ev_engine, &ev_last })
             if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
         if (stream) { cudaStreamDestroy(stream); stream = nullptr; }
@@ -136,7 +139,6 @@ struct ChainHost {
     uint32_t env_instances;          // instances in envelope mode (0: the envelope kernel and its table are not needed)
     std::vector<uint8_t> env_mode;   // [N] each instance's envelope-mode flag (env row 4 != 0), as the calls issued so far leave it
     uint32_t vmm_packets;            // capacity of d.vmm in packets
-    ResponseBuffers resp;            // frequency table of *_response_*; host staging of *_response_host and the instance image calls
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
     IndexLists copy_lists;           // device instance lists of *_copy_instances, allocated by the first call
     Queue lanes[DSPI_CHAIN_MAX_LANES];   // open while it has a stream
@@ -383,7 +385,6 @@ int destroy(H *c)
     c->open_lanes = 0;
     c->q.destroy();
     c->part.destroy();
-    c->resp.destroy();
     c->copy_lists.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
@@ -648,14 +649,49 @@ int set_preset_mute(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const
     return end_call(*q, DSPI_OK);
 }
 
-template <class A>
-int get_preset_mute(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_preset_mute *states)
+// dspi_preset_mute records of env rows 0-2 of n instances (row r of instance i at env[r * Np + i]), as get_preset_mute
+// packs them on the host: loading in the low byte of the first word, the reserved bytes zero
+__global__ void __launch_bounds__(128) preset_mute_records_kernel(const uint32_t *__restrict__ env, size_t Np, uint32_t n,
+                                                                  dspi_preset_mute *__restrict__ out)
 {
-    if (!c || !states) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c->q, inst0, n);
+    static_assert(sizeof(dspi_preset_mute) == 12, "dspi_preset_mute");
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t *w = reinterpret_cast<uint32_t *>(out + i);
+    w[0] = env[i] & 0xFFu;
+    w[1] = env[Np + i];
+    w[2] = env[2 * Np + i];
+}
+
+// dspi_spdif_tx records of n transmitters, as spdif_tx_pack makes them; bytewise, since the records are 1-byte aligned
+__global__ void __launch_bounds__(128) spdif_tx_records_kernel(const uint32_t *__restrict__ bp, const uint64_t *__restrict__ cs40, uint32_t n,
+                                                               dspi_spdif_tx *__restrict__ out)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t cs = cs40[i];
+    uint8_t *o = reinterpret_cast<uint8_t *>(out + i);
+    for (int b = 0; b < 5; b++) o[b] = (uint8_t)(cs >> (8 * b));
+    o[5] = (uint8_t)bp[i];
+    o[6] = o[7] = 0;
+}
+
+// on queue q: the engine's returns the records in host memory; a lane's writes them to device memory on its stream
+template <class A>
+int get_preset_mute(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, dspi_preset_mute *states)
+{
+    if (!q) return DSPI_EINVAL;
+    if (!states) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
     const size_t Np = c->d.N_pad;
+    if (q->lane) {
+        CU_OK(begin_call(c, *q));
+        preset_mute_records_kernel<<<(n + 127) / 128, 128, 0, q->stream>>>(c->d.env + inst0, Np, n, states);
+        c->launches++;
+        return end_call(*q, cudaGetLastError() == cudaSuccess ? DSPI_OK : fail(DSPI_ECUDA, "preset-mute record kernel"));
+    }
     std::vector<uint32_t> rows((size_t)3 * n);
     CU_OK(cudaMemcpy2DAsync(rows.data(), (size_t)n * 4, c->d.env + inst0, Np * 4, (size_t)n * 4, 3, cudaMemcpyDeviceToHost, c->q.stream));
     CU_OK(cudaStreamSynchronize(c->q.stream));
@@ -701,6 +737,16 @@ int lane_prepare(ChainHost<A> *c, const Queue &q, bool staged)
     if (staged && skip_set) return DSPI_OK;
     CU_OK(drain(c));
     return skip_set ? DSPI_OK : bulk::finish_skip(c, c->q);
+}
+
+// Before a lane read that needs a staging or frequency table it lacks (`staged` false): wait for every lane and the
+// engine stream, as lane_prepare does before an allocation.  Nothing for the engine's queue.
+template <class A>
+int lane_grow(ChainHost<A> *c, const Queue &q, bool staged)
+{
+    if (!q.lane || staged) return DSPI_OK;
+    CU_OK(drain(c));
+    return DSPI_OK;
 }
 
 // results: host memory for the engine's queue, device memory for a lane's
@@ -776,14 +822,19 @@ int edit_bulk_device(ChainHost<A> *c, Queue *q, uint32_t n_edits, const dspi_bul
     return end_call(*q, bulk::edit<typename A::Stores>(c, *q, n_edits, edits, exact_db, sample_rate, results));
 }
 
+// host, results (may be NULL): host memory for the engine's queue, device memory for a lane's, as packets
 template <class A>
-int collect_bulk_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host, int32_t *results)
+int collect_bulk_device(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *packets, dspi_bulk_host *host,
+                        int32_t *results)
 {
-    if (!c || !packets) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c->q, inst0, n);
+    if (!q) return DSPI_EINVAL;
+    if (!packets) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::collect<typename A::Stores>(c, inst0, n, packets, host, results);
+    if ((rc = lane_grow(c, *q, !bulk::collect_staged(*q, packets) || q->bulk.results != nullptr)) != DSPI_OK) return rc;
+    CU_OK(begin_call(c, *q));
+    return end_call(*q, bulk::collect<typename A::Stores>(c, *q, inst0, n, packets, host, results));
 }
 
 // results: host memory for the engine's queue, device memory for a lane's
@@ -804,17 +855,21 @@ int apply_preset_device(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, c
     return end_call(*q, bulk::apply_preset<typename A::Stores>(c, *q, inst0, n, images, image_stride, load, host, sample_rate, results));
 }
 
+// images, results (may be NULL): host memory for the engine's queue, device memory for a lane's
 template <class A>
-int collect_preset_device(ChainHost<A> *c, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
+int collect_preset_device(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const uint8_t *slot_indices, void *images, size_t image_stride,
                           int32_t *results)
 {
     constexpr size_t kSlot = sizeof(bulk::SlotOf<typename A::Stores>);
-    if (!c || !slot_indices || !images) return fail(DSPI_EINVAL, "null argument");
+    if (!q) return DSPI_EINVAL;
+    if (!slot_indices || !images) return fail(DSPI_EINVAL, "null argument");
     if (image_stride < kSlot) return fail(DSPI_EINVAL, "image_stride %zu below the slot size %zu", image_stride, kSlot);
-    int rc = check_range(c->q, inst0, n);
+    int rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    return bulk::collect_preset<typename A::Stores>(c, c->q.preset, inst0, n, slot_indices, images, image_stride, results);
+    if ((rc = lane_grow(c, *q, q->preset.results != nullptr)) != DSPI_OK) return rc;
+    CU_OK(begin_call(c, *q));
+    return end_call(*q, bulk::collect_preset<typename A::Stores>(c, *q, inst0, n, slot_indices, images, image_stride, results));
 }
 
 template <class A>
@@ -1095,7 +1150,8 @@ int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32
 // ---- lanes: issue queues of one engine over disjoint instance windows, whose calls run concurrently -------------------
 // A lane takes process calls and the control calls a running clock group needs (edits, fades, transmitter restamps,
 // resets, applies, preset applies and rate switches): set_preset_mute, set_spdif_tx, reset_instances, edit_bulk_device,
-// apply_bulk_device, apply_preset_device, set_rate_device and process_device on its queue.
+// apply_bulk_device, apply_preset_device, set_rate_device and process_device on its queue; and the reads it needs
+// (collect_bulk_device, collect_preset_device, export_instances, response, get_preset_mute, get_spdif_tx), into device memory.
 template <class A>
 int lane_open(ChainHost<A> *c, uint32_t inst0, uint32_t n, uint32_t *lane)
 {
@@ -1175,12 +1231,21 @@ int set_spdif_tx(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const ds
     return end_call(*q, DSPI_OK);
 }
 
+// on queue q: the engine's returns the records in host memory; a lane's writes them to device memory on its stream
 template <class A>
-int get_spdif_tx(ChainHost<A> *c, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
+int get_spdif_tx(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, dspi_spdif_tx *tx)
 {
-    if (!c || !tx) return fail(DSPI_EINVAL, "null argument");
-    int rc = check_range(c->q, inst0, n);
+    if (!q) return DSPI_EINVAL;
+    if (!tx) return fail(DSPI_EINVAL, "null argument");
+    int rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
+    if (q->lane) {
+        CU_OK(cudaSetDevice(c->desc.device));
+        CU_OK(begin_call(c, *q));
+        spdif_tx_records_kernel<<<(n + 127) / 128, 128, 0, q->stream>>>(c->tx.bp + inst0, c->tx.cs40 + inst0, n, tx);
+        c->launches++;
+        return end_call(*q, cudaGetLastError() == cudaSuccess ? DSPI_OK : fail(DSPI_ECUDA, "transmitter record kernel"));
+    }
     std::vector<uint32_t> bp(n);
     std::vector<uint64_t> cs(n);
     CU_OK(cudaSetDevice(c->desc.device));
@@ -1312,13 +1377,14 @@ size_t instance_image_size(ChainHost<A> *c)
 
 // arguments of the image calls; *plan filled, *size the image size
 template <class A>
-int check_images(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *images, size_t stride, image::Plan *plan, size_t *size)
+int check_images(ChainHost<A> *c, const Queue *q, uint32_t inst0, uint32_t n, const void *images, size_t stride, image::Plan *plan, size_t *size)
 {
-    if (!c || !images) return fail(DSPI_EINVAL, "null argument");
+    if (!q) return DSPI_EINVAL;
+    if (!images) return fail(DSPI_EINVAL, "null argument");
     *size = image_plan(c, kInImage, *plan);
     if (*size == 0) return fail(DSPI_EINVAL, "instance image plan exceeds its tables");
     if (stride < *size) return fail(DSPI_EINVAL, "image_stride %zu below the image size %zu", stride, *size);
-    return check_range(c->q, inst0, n);
+    return check_range(*q, inst0, n);
 }
 
 // the EQ sub-engines' ranges of instances [inst0, inst0 + n): every role of the master / output engine in one launch
@@ -1329,31 +1395,39 @@ void role_ranges(ChainHost<A> *c, RoleRange &rm, RoleRange &ro)
     rm.stride = ro.stride = c->d.N_pad;
 }
 
+// On queue q with its staging: images is host memory for the engine's queue, device memory for a lane's.  A lane's staging
+// holds chunks of its whole window (at most 32 MiB, kept until the lane closes), so that only its first export allocates
+// it: a later growth would free device memory, which waits for the device.
 template <class A>
-int export_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, void *images, size_t stride)
+int export_instances(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, void *images, size_t stride)
 {
     image::Plan pl;
     size_t size = 0;
-    int rc = check_images(c, inst0, n, images, stride, &pl, &size);
+    int rc = check_images(c, q, inst0, n, images, stride, &pl, &size);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
+    if ((rc = lane_grow(c, *q, q->resp.d_stage != nullptr)) != DSPI_OK) return rc;
     uint32_t chunk = 0;
-    CU_OK(c->resp.stage(size, n, c->q.stream, &chunk));
-    RoleRange rm, ro;
-    role_ranges(c, rm, ro);
-    rc = eq_unpack_range(c->eq_m, inst0, n, c->q.stream, rm);               // running EQ state into the mirrors, as download_biquads
-    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, inst0, n, c->q.stream, ro);
-    if (rc) return rc;
-    unsigned char *stage = (unsigned char *)c->resp.d_stage;
-    for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
-        const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
-        image::instance_image_kernel<image::kExport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->q.stream>>>(pl, inst0 + i0, nc, stage);
-        CU_OK(cudaGetLastError());
-        c->launches++;
-        CU_OK(cudaMemcpy2DAsync((char *)images + (size_t)i0 * stride, stride, stage, size, size, nc, cudaMemcpyDeviceToHost, c->q.stream));
-    }
-    CU_OK(cudaStreamSynchronize(c->q.stream));
-    return DSPI_OK;
+    CU_OK(q->resp.stage(size, q->lane ? q->n : n, q->stream, &chunk));
+    CU_OK(begin_call(c, *q));
+    auto issue = [&]() -> int {
+        RoleRange rm, ro;
+        role_ranges(c, rm, ro);
+        int rc = eq_unpack_range(c->eq_m, inst0, n, q->stream, rm);         // running EQ state into the mirrors, as download_biquads
+        if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, inst0, n, q->stream, ro);
+        if (rc) return rc;
+        unsigned char *stage = (unsigned char *)q->resp.d_stage;
+        for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
+            const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
+            image::instance_image_kernel<image::kExport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, q->stream>>>(pl, inst0 + i0, nc, stage);
+            CU_OK(cudaGetLastError());
+            c->launches++;
+            CU_OK(cudaMemcpy2DAsync((char *)images + (size_t)i0 * stride, stride, stage, size, size, nc,
+                                    q->lane ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, q->stream));
+        }
+        return DSPI_OK;
+    };
+    return end_call(*q, issue());
 }
 
 template <class A>
@@ -1361,7 +1435,7 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
 {
     image::Plan pl;
     size_t size = 0;
-    int rc = check_images(c, inst0, n, images, stride, &pl, &size);
+    int rc = check_images(c, engine_queue(c), inst0, n, images, stride, &pl, &size);
     if (rc || n == 0) return rc;
     const char *img = (const char *)images;
     for (uint32_t i = 0; i < n; i++) {                                       // every header before anything is written
@@ -1391,8 +1465,8 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
         c->env_mode[inst0 + i] = on ? 1 : 0;
     }
     uint32_t chunk = 0;
-    CU_OK(c->resp.stage(size, n, c->q.stream, &chunk));
-    unsigned char *stage = (unsigned char *)c->resp.d_stage;
+    CU_OK(c->q.resp.stage(size, n, c->q.stream, &chunk));
+    unsigned char *stage = (unsigned char *)c->q.resp.d_stage;
     for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
         const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
         CU_OK(cudaMemcpy2DAsync(stage, size, img + (size_t)i0 * stride, stride, size, nc, cudaMemcpyHostToDevice, c->q.stream));
@@ -1488,41 +1562,49 @@ int reset_instances(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n)
 }
 
 // ---- queries -----------------------------------------------------------------------------------------------------------
-// Frequency response of instances [inst0, inst0 + n) on the engine stream; out: device [n][kOuts][2][n_freqs] float2, or
-// host memory filled chunk by chunk through the staging buffer
+// Frequency response of instances [inst0, inst0 + n) on queue q (the engine's, or an open lane's: a NULL q, which the
+// lane entry point refuses before anything else, is a NULL engine here, reported after the arguments as it always was);
+// out: device [n][kOuts][2][n_freqs] float2, or (the engine's queue only) host memory filled chunk by chunk through the
+// staging buffer
 template <class A>
-int response(ChainHost<A> *c, uint32_t inst0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
+int response(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const float *freqs, uint32_t n_freqs, float fs, float *out, bool host)
 {
     const char *why = "";
     int rc = response_check_args(freqs, n_freqs, fs, out, &why);
     if (rc) return fail(rc, "%s", why);
-    if (!c) return fail(DSPI_EINVAL, "null argument");
-    rc = check_range(c->q, inst0, n);
+    if (!q) return fail(DSPI_EINVAL, "null argument");
+    if (q->lane && ((uintptr_t)out & 7u)) return fail(DSPI_EINVAL, "d_out must be 8-byte aligned (the kernel stores {re, im} pairs)");
+    rc = check_range(*q, inst0, n);
     if (rc || n == 0) return rc;
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(c->resp.upload(freqs, n_freqs, c->q.stream, &c->launches));
+    if ((rc = lane_grow(c, *q, q->resp.d_freq != nullptr)) != DSPI_OK) return rc;
+    CU_OK(begin_call(c, *q));
     using B = typename A::Biquad;
     const B *m_aos = (const B *)eq_aos_mirror(c->eq_m), *o_aos = (const B *)eq_aos_mirror(c->eq_o);
     auto launch = [&](uint32_t i0, uint32_t m, void *dst) -> cudaError_t {
         const dim3 grid((n_freqs + 127) / 128, m < 65535u ? m : 65535u);
-        A::response<<<grid, 128, 0, c->q.stream>>>(c->d, m_aos, o_aos, i0, m, c->resp.d_freq, n_freqs, fs, (float2 *)dst);
+        A::response<<<grid, 128, 0, q->stream>>>(c->d, m_aos, o_aos, i0, m, q->resp.d_freq, n_freqs, fs, (float2 *)dst);
         c->launches++;
         return cudaGetLastError();
     };
-    if (!host) {
-        CU_OK(launch(inst0, n, out));
+    auto issue = [&]() -> int {
+        CU_OK(q->resp.upload(freqs, n_freqs, q->stream, &c->launches));
+        if (!host) {
+            CU_OK(launch(inst0, n, out));
+            return DSPI_OK;
+        }
+        const size_t row_bytes = (size_t)A::kOuts * 2 * n_freqs * 2 * sizeof(float);
+        uint32_t rows = 0;
+        CU_OK(q->resp.stage(row_bytes, n, q->stream, &rows));
+        for (uint32_t i = 0; i < n; i += rows) {
+            const uint32_t m = n - i < rows ? n - i : rows;
+            CU_OK(launch(inst0 + i, m, q->resp.d_stage));
+            CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, q->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, q->stream));
+            CU_OK(cudaStreamSynchronize(q->stream));
+        }
         return DSPI_OK;
-    }
-    const size_t row_bytes = (size_t)A::kOuts * 2 * n_freqs * 2 * sizeof(float);
-    uint32_t rows = 0;
-    CU_OK(c->resp.stage(row_bytes, n, c->q.stream, &rows));
-    for (uint32_t i = 0; i < n; i += rows) {
-        const uint32_t m = n - i < rows ? n - i : rows;
-        CU_OK(launch(inst0 + i, m, c->resp.d_stage));
-        CU_OK(cudaMemcpyAsync((char *)out + (size_t)i * row_bytes, c->resp.d_stage, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, c->q.stream));
-        CU_OK(cudaStreamSynchronize(c->q.stream));
-    }
-    return DSPI_OK;
+    };
+    return end_call(*q, issue(), host);
 }
 
 template <class A>

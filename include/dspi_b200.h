@@ -997,10 +997,11 @@ int   dspi_chainq_lane_sync  (dspi_chainq *c, uint32_t lane);
  *   Errors (nothing is written on any error): every refusal of the engine-level call, and an unknown or closed lane, with
  *   DSPI_EINVAL; a window violation with DSPI_ERANGE.
  *   No lane control call made.  Every other call issues exactly the work it issues without them.
- * Left as barriers: every getter (_collect_bulk_device, _collect_preset_device, _response_*, _export_instances, _get_*),
- * since each returns data to the host, and the other writes (_set_params, _upload_biquads, _set_eq_params_device,
- * _set_dynamics_device, _copy_instances, _import_instances), since the wire-packet routes above cover what a Console or a
- * preset sends and a device that changes rate moves to another group's window with _copy_instances. */
+ * Left as barriers: _download_biquads (an instance image carries the biquads with their state), the state blob
+ * (_state_export / _state_import), and the writes _set_params, _upload_biquads, _set_eq_params_device, _set_dynamics_device,
+ * _copy_instances and _import_instances, since the wire-packet routes above cover what a Console or a preset sends and a
+ * device that changes rate moves to another group's window with _copy_instances.  The reads a running group needs have
+ * lane forms (the lane read calls below). */
 int dspi_chain_lane_edit_bulk_device  (dspi_chain *c, uint32_t lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db,
                                        float sample_rate, int32_t *d_results);
 int dspi_chain_lane_set_preset_mute   (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_preset_mute *states,
@@ -1025,6 +1026,56 @@ int dspi_chainq_lane_apply_preset_device(dspi_chainq *c, uint32_t lane, uint32_t
                                         const dspi_preset_load *load, const dspi_bulk_host *host, float sample_rate, int32_t *d_results);
 int dspi_chainq_lane_set_rate_device    (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const float *sample_rates,
                                         int32_t *d_results);
+
+/* Lane read calls: the reads a running clock group needs (a Console connecting reads REQ_GET_ALL_PARAMS, a preset save, a
+ * Console's EQ curve, a checkpoint or a move of a device to another engine, a poll of a fade or a transmitter), issued on
+ * the group's lane so that they neither wait for nor hold up the other groups.
+ *   Semantics.  Each call returns byte for byte what its engine-level counterpart returns over the same instances at the
+ *   same point of the call sequence, after every call issued earlier on the lane and every engine-level call issued before
+ *   it: _lane_collect_bulk_device is _collect_bulk_device (packets, host records, DSPI_BULK_* marks),
+ *   _lane_collect_preset_device is _collect_preset_device (slot images; the stride tail is left as it was),
+ *   _lane_export_instances is _export_instances (instance images with their header; the stride tail is left as it was),
+ *   _lane_response_device is _response_device ({re, im} arrays), _lane_get_preset_mute is _get_preset_mute and
+ *   _lane_get_spdif_tx is _get_spdif_tx (records with their reserved bytes zero).
+ *   Read-only.  A later call on any lane or on the engine gives the bytes it would have given without the read.
+ *   Window.  [inst0, inst0 + n) lies inside the lane's window (inst0 has no alignment rule beyond that); otherwise the call
+ *   fails with DSPI_ERANGE.  n == 0 does nothing.
+ *   Ordering and no host wait.  Ordered as the lane control calls are: behind its lane's calls and the engine-level calls
+ *   issued before it, never against another lane.  The call returns without waiting for the device.
+ *   Outputs.  d_packets, d_host, d_results, d_images, d_out, d_states and d_tx are device memory, written on the lane
+ *   stream and visible on _lane_stream.  d_host and d_results may be NULL, as on the engine-level calls; every other
+ *   output is required.  d_packets may hold any address: packets at a 16-byte aligned address are written in place,
+ *   others go through the lane's staging and a device-to-device copy.  d_out must be 8-byte aligned ({re, im} float
+ *   pairs are stored as such).  slot_indices and freqs_hz are host memory, read during the call: they may be reused as
+ *   soon as it returns.
+ *   Exceptions, each a growth of a buffer: a lane's first preset collect, first export, first response and first collect
+ *   into packets that are not 16-byte aligned allocate its preset staging, image staging, frequency table (256 KiB) and
+ *   bulk staging (unless an apply, rate switch or edit did); these first wait for every lane and the engine stream.  The
+ *   image staging holds chunks of the whole window, so that no later export grows it: one instance image per instance of
+ *   the window, at most 32 MiB (DSPI_HOST_CHUNK_MB), kept until the lane closes even if the lane only ever exports one
+ *   instance.  Slot indices go through the lane's ring of pinned host buffers (see the lane control calls).
+ *   Errors (nothing is written on any error): every refusal of the engine-level call, a NULL required output, a d_out
+ *   that is not 8-byte aligned, and an unknown or closed lane, with DSPI_EINVAL; a window violation with DSPI_ERANGE.
+ *   No lane read call made.  Every other call issues exactly the work it issues without them; the engine-level getters
+ *   stay barriers. */
+int dspi_chain_lane_collect_bulk_device   (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *d_packets,
+                                          dspi_bulk_host *d_host, int32_t *d_results);
+int dspi_chain_lane_collect_preset_device (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const uint8_t *slot_indices,
+                                          void *d_images, size_t image_stride, int32_t *d_results);
+int dspi_chain_lane_export_instances      (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, void *d_images, size_t image_stride);
+int dspi_chain_lane_response_device       (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const float *freqs_hz,
+                                          uint32_t n_freqs, float sample_rate, float *d_out);
+int dspi_chain_lane_get_preset_mute       (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_preset_mute *d_states);
+int dspi_chain_lane_get_spdif_tx          (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_spdif_tx *d_tx);
+int dspi_chainq_lane_collect_bulk_device  (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_wire_bulk_params *d_packets,
+                                          dspi_bulk_host *d_host, int32_t *d_results);
+int dspi_chainq_lane_collect_preset_device(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const uint8_t *slot_indices,
+                                          void *d_images, size_t image_stride, int32_t *d_results);
+int dspi_chainq_lane_export_instances     (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, void *d_images, size_t image_stride);
+int dspi_chainq_lane_response_device      (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const float *freqs_hz,
+                                          uint32_t n_freqs, float sample_rate, float *d_out);
+int dspi_chainq_lane_get_preset_mute      (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_preset_mute *d_states);
+int dspi_chainq_lane_get_spdif_tx         (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_spdif_tx *d_tx);
 
 /* ---- frequency response of EQ channels and chain instances ------------------------------------ */
 /* The complex transfer function H(e^{j omega}) of the linear, time-invariant part of the path the NEXT process call applies,
