@@ -70,6 +70,7 @@ SYMBOLS = [
     "dspi_chain_lane_response_device", "dspi_chain_lane_get_preset_mute", "dspi_chain_lane_get_spdif_tx",
     "dspi_chainq_lane_collect_bulk_device", "dspi_chainq_lane_collect_preset_device", "dspi_chainq_lane_export_instances",
     "dspi_chainq_lane_response_device", "dspi_chainq_lane_get_preset_mute", "dspi_chainq_lane_get_spdif_tx",
+    "dspi_chain_lane_import_instances", "dspi_chain_lane_copy_instances", "dspi_chainq_lane_import_instances", "dspi_chainq_lane_copy_instances",
 ]
 
 
@@ -195,6 +196,8 @@ def lib():
             getattr(h, pre + "_lane_response_device").argtypes = [vp, u32, u32, u32, vp, u32, C.c_float, vp]
             getattr(h, pre + "_lane_get_preset_mute").argtypes = [vp, u32, u32, u32, vp]
             getattr(h, pre + "_lane_get_spdif_tx").argtypes = [vp, u32, u32, u32, vp]
+            getattr(h, pre + "_lane_import_instances").argtypes = [vp, u32, u32, u32, vp, C.c_size_t]
+            getattr(h, pre + "_lane_copy_instances").argtypes = [vp, u32, u32, u32, vp, vp]
         for pre in ("dspi_eq", "dspi_chain", "dspi_chainq"):
             getattr(h, pre + "_response_host").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
             getattr(h, pre + "_response_device").argtypes = [vp, u32, u32, vp, u32, C.c_float, vp]
@@ -528,14 +531,18 @@ class _ChainEngine:
         """Instance ``src[k]`` -> instance ``dst[k]`` on the GPU, as ``export_instances(src[k], 1)`` then
         ``import_instances(..., dst[k])`` would, with no image leaving the device.  ``src`` may repeat; ``dst`` must be
         distinct and share no index with ``src``.  Ordered behind earlier work; returns when the engine is updated."""
+        s, d = self._copy_lists(src, dst)
+        _check(self._fn("copy_instances")(self._h, int(s.size), s.ctypes.data_as(C.c_void_p), d.ctypes.data_as(C.c_void_p)))
+
+    @staticmethod
+    def _copy_lists(src, dst):
         s = np.ascontiguousarray(np.asarray(src, np.int64).reshape(-1))
         d = np.ascontiguousarray(np.asarray(dst, np.int64).reshape(-1))
         if s.shape != d.shape:
             raise ValueError("src and dst give different copy counts")
         if s.size and (min(s.min(), d.min()) < 0 or max(s.max(), d.max()) > 0xFFFFFFFF):
             raise ValueError("instance indices must be 0 .. 2**32 - 1")
-        s, d = s.astype(np.uint32), d.astype(np.uint32)
-        _check(self._fn("copy_instances")(self._h, int(s.size), s.ctypes.data_as(C.c_void_p), d.ctypes.data_as(C.c_void_p)))
+        return s.astype(np.uint32), d.astype(np.uint32)
 
     def reset_instances(self, inst0=0, n=None):
         """``reset_state`` for instances [inst0, inst0+n) only (default: to the end); parameters are kept."""
@@ -942,6 +949,25 @@ class _ChainEngine:
     def lane_get_spdif_tx(self, lane, inst0, n, tx_ptr):
         """``get_spdif_tx`` issued on a lane: SPDIF_TX [n] at ``tx_ptr``."""
         _check(self._fn("lane_get_spdif_tx")(self._h, int(lane), int(inst0), int(n), C.c_void_p(int(tx_ptr)) if tx_ptr else None))
+
+    # Lane moves: a device moving into a lane's window, asynchronous on the lane streams; each returns without waiting.
+
+    def lane_import_instances(self, lane, images, inst0):
+        """``import_instances(images, inst0)`` issued on a lane ([inst0, inst0+n) inside its window): uint8 [n, stride]
+        images in host memory, read during the call."""
+        img = np.ascontiguousarray(images, np.uint8)
+        if img.ndim != 2:
+            raise ValueError("images must be [n, stride] bytes")
+        _check(self._fn("lane_import_instances")(self._h, int(lane), int(inst0), int(img.shape[0]), img.ctypes.data_as(C.c_void_p),
+                                                 C.c_size_t(img.shape[1])))
+
+    def lane_copy_instances(self, src_lane, dst_lane, src, dst):
+        """``copy_instances(src, dst)`` issued on lanes: every ``src[k]`` inside ``src_lane``'s window, every ``dst[k]``
+        inside ``dst_lane``'s (the same lane repacks one group).  Ordered after the calls issued earlier on either lane;
+        later calls on either lane run after it."""
+        s, d = self._copy_lists(src, dst)
+        _check(self._fn("lane_copy_instances")(self._h, int(src_lane), int(dst_lane), int(s.size), s.ctypes.data_as(C.c_void_p),
+                                               d.ctypes.data_as(C.c_void_p)))
 
 
 class ChainEngine(_ChainEngine):

@@ -54,7 +54,8 @@ int fail(int code, const char *fmt, ...)
         if (err__ != cudaSuccess) return fail(DSPI_ECUDA, "%s -> %s (%s:%d)", #expr, cudaGetErrorString(err__), __FILE__, __LINE__); \
     } while (0)
 
-// device copy of the instance lists of *_copy_instances (sources, then destinations); grows to the largest call
+// device copy of the instance lists of *_copy_instances (sources, then destinations); the engine's grows to the largest
+// call, a lane's holds its whole window from its first copy as destination
 struct IndexLists {
     uint32_t *d = nullptr;
     uint32_t cap = 0;                // pairs
@@ -89,7 +90,8 @@ struct Queue {
     bulk::EditStage bulk_edit;
     bulk::PresetStage preset;        // device staging of the preset applies and collects
     bulk::HostRing ring;             // a lane's edits, packets, images, rates, slot indices, fade rows and transmitter rows on their way to the device
-    ResponseBuffers resp;            // frequency table of the response calls; image staging of export (and, the engine's, of import and _response_host)
+    ResponseBuffers resp;            // frequency table of the response calls; image staging of export and import (and, the engine's, of _response_host)
+    IndexLists copy_lists;           // device instance lists of the copies issued on this queue (the destination's, for a lane)
     cudaEvent_t ev_engine = nullptr, ev_last = nullptr;   // a lane's
 
     // `lane` set first
@@ -113,6 +115,7 @@ struct Queue {
         preset.destroy();
         ring.destroy();
         resp.destroy();
+        copy_lists.destroy();
         for (cudaEvent_t *ev : { &ev_engine, &ev_last })
             if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
         if (stream) { cudaStreamDestroy(stream); stream = nullptr; }
@@ -140,7 +143,6 @@ struct ChainHost {
     std::vector<uint8_t> env_mode;   // [N] each instance's envelope-mode flag (env row 4 != 0), as the calls issued so far leave it
     uint32_t vmm_packets;            // capacity of d.vmm in packets
     bulk::Record rec;                // wire-visible configuration of every instance (*_collect_bulk_device); not part of the state blob
-    IndexLists copy_lists;           // device instance lists of *_copy_instances, allocated by the first call
     Queue lanes[DSPI_CHAIN_MAX_LANES];   // open while it has a stream
     uint32_t open_lanes;
 };
@@ -385,7 +387,6 @@ int destroy(H *c)
     c->open_lanes = 0;
     c->q.destroy();
     c->part.destroy();
-    c->copy_lists.destroy();
     if (c->eq_m) dspi_eq_destroy(c->eq_m);
     if (c->eq_o) dspi_eq_destroy(c->eq_o);
     for (void *p : c->allocs) cudaFree(p);
@@ -611,7 +612,7 @@ int set_params(ChainHost<A> *c, uint32_t inst0, uint32_t n, const typename A::Pa
 
 // The envelope rows [5][n] of instances [inst0, inst0+n) that states (or NULL: leave envelope mode) give; env_instances and
 // the mode mirror follow.  Every writer of env row 4 is a call issued from the host (create, _set_preset_mute,
-// _copy_instances, _import_instances, _state_import and the lane fade calls), so the mirror is exact at issue time.
+// _copy_instances, _import_instances, _state_import and their lane forms), so the mirror is exact at issue time.
 template <class A>
 void preset_rows(ChainHost<A> *c, uint32_t inst0, uint32_t n, const dspi_preset_mute *states, uint32_t sample_rate_hz, uint32_t *rows)
 {
@@ -1150,8 +1151,10 @@ int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32
 // ---- lanes: issue queues of one engine over disjoint instance windows, whose calls run concurrently -------------------
 // A lane takes process calls and the control calls a running clock group needs (edits, fades, transmitter restamps,
 // resets, applies, preset applies and rate switches): set_preset_mute, set_spdif_tx, reset_instances, edit_bulk_device,
-// apply_bulk_device, apply_preset_device, set_rate_device and process_device on its queue; and the reads it needs
-// (collect_bulk_device, collect_preset_device, export_instances, response, get_preset_mute, get_spdif_tx), into device memory.
+// apply_bulk_device, apply_preset_device, set_rate_device and process_device on its queue; the reads it needs
+// (collect_bulk_device, collect_preset_device, export_instances, response, get_preset_mute, get_spdif_tx), into device
+// memory; and the moves of devices into its window (import_instances, and copy_instances on the destination's queue,
+// ordered against the source lane too).
 template <class A>
 int lane_open(ChainHost<A> *c, uint32_t inst0, uint32_t n, uint32_t *lane)
 {
@@ -1430,12 +1433,30 @@ int export_instances(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, void
     return end_call(*q, issue());
 }
 
+// Mirror rows -> packed stores of the instances ch0 .. of rm / ro (ranges or lists over the roles), then the skip masks: on
+// the engine's queue every row, synchronising, as upload_biquads and set_params do; on a lane's the rows of its window only.
 template <class A>
-int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *images, size_t stride)
+int pack_instances(ChainHost<A> *c, Queue &q, uint32_t ch0, uint32_t n, const RoleRange &rm, const RoleRange &ro)
+{
+    if (q.lane) {
+        const int rc = eq_pack_rows(c->eq_m, ch0, n, q.stream, rm, q.inst0, q.n);
+        return rc == DSPI_OK ? eq_pack_rows(c->eq_o, ch0, n, q.stream, ro, q.inst0, q.n) : rc;
+    }
+    int rc = eq_pack_range(c->eq_m, ch0, n, q.stream, rm);
+    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, ch0, n, q.stream, ro);
+    return rc == DSPI_OK ? bulk::finish_skip(c, q) : rc;
+}
+
+// On queue q; images is host memory on both, so that every header is checked before anything is written and the envelope
+// modes the images carry (env row 4) keep env_mode exact.  The engine's queue reads the range's modes before the call from
+// the device and returns when the engine is updated.  A lane's takes them from env_mode, sends each chunk of images at the
+// image size from a buffer of its ring into its image staging (which export shares) with one copy, and does not wait.
+template <class A>
+int import_instances(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const void *images, size_t stride)
 {
     image::Plan pl;
     size_t size = 0;
-    int rc = check_images(c, engine_queue(c), inst0, n, images, stride, &pl, &size);
+    int rc = check_images(c, q, inst0, n, images, stride, &pl, &size);
     if (rc || n == 0) return rc;
     const char *img = (const char *)images;
     for (uint32_t i = 0; i < n; i++) {                                       // every header before anything is written
@@ -1448,56 +1469,75 @@ int import_instances(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *im
                         (unsigned long long)h.bytes);
     }
     CU_OK(cudaSetDevice(c->desc.device));
+    if ((rc = lane_prepare(c, *q, q->resp.d_stage != nullptr)) != DSPI_OK) return rc;
     // envelope-mode instances: the range's modes before (behind earlier work) and in the images (env row 4)
     uint32_t env_off = 0;
     for (uint32_t k = 0; k < pl.n_fields; k++)
         if (pl.f[k].p == (char *)c->d.env) env_off = pl.f[k].off + 4 * 4;
     const size_t Np = c->d.N_pad;
-    std::vector<uint32_t> cur((size_t)n);
-    CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->q.stream));
-    CU_OK(cudaStreamSynchronize(c->q.stream));
+    std::vector<uint32_t> cur(q->lane ? 0 : (size_t)n);
+    if (!q->lane) {
+        CU_OK(cudaMemcpyAsync(cur.data(), c->d.env + 4 * Np + inst0, (size_t)n * 4, cudaMemcpyDeviceToHost, q->stream));
+        CU_OK(cudaStreamSynchronize(q->stream));
+    }
     uint32_t before = 0, after = 0;
     for (uint32_t i = 0; i < n; i++) {
         uint32_t on;
         memcpy(&on, img + (size_t)i * stride + env_off, 4);
-        before += cur[i] ? 1u : 0u;
+        before += (q->lane ? c->env_mode[inst0 + i] : cur[i]) ? 1u : 0u;
         after += on ? 1u : 0u;
         c->env_mode[inst0 + i] = on ? 1 : 0;
     }
     uint32_t chunk = 0;
-    CU_OK(c->q.resp.stage(size, n, c->q.stream, &chunk));
-    unsigned char *stage = (unsigned char *)c->q.resp.d_stage;
-    for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
-        const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
-        CU_OK(cudaMemcpy2DAsync(stage, size, img + (size_t)i0 * stride, stride, size, nc, cudaMemcpyHostToDevice, c->q.stream));
-        image::instance_image_kernel<image::kImport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, c->q.stream>>>(pl, inst0 + i0, nc, stage);
-        CU_OK(cudaGetLastError());
-        c->launches++;
-    }
-    c->env_instances = c->env_instances - before + after;
-    // mirrors -> packed stores of the range only (topology words, skip remask, K1 kernel choice), then the skip masks, as
-    // upload_biquads and set_params do
-    RoleRange rm, ro;
-    role_ranges(c, rm, ro);
-    rc = eq_pack_range(c->eq_m, inst0, n, c->q.stream, rm);
-    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, inst0, n, c->q.stream, ro);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->q.stream);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->q.stream);
-    return rc;
+    CU_OK(q->resp.stage(size, q->lane ? q->n : n, q->stream, &chunk));
+    CU_OK(begin_call(c, *q));
+    auto issue = [&]() -> int {
+        unsigned char *stage = (unsigned char *)q->resp.d_stage;
+        for (uint32_t i0 = 0; i0 < n; i0 += chunk) {
+            const uint32_t nc = n - i0 < chunk ? n - i0 : chunk;
+            const char *src = img + (size_t)i0 * stride;
+            if (q->lane)
+                CU_OK(bulk::lane_upload(*q, stage, (size_t)nc * size, [&](unsigned char *b) {
+                    for (uint32_t i = 0; i < nc; i++) memcpy(b + (size_t)i * size, src + (size_t)i * stride, size);
+                }));
+            else
+                CU_OK(cudaMemcpy2DAsync(stage, size, src, stride, size, nc, cudaMemcpyHostToDevice, q->stream));
+            image::instance_image_kernel<image::kImport><<<dim3((nc + 31) / 32, pl.n_tasks), 256, 0, q->stream>>>(pl, inst0 + i0, nc, stage);
+            CU_OK(cudaGetLastError());
+            c->launches++;
+        }
+        c->env_instances = c->env_instances - before + after;
+        // mirrors -> packed stores of the range only (topology words, skip remask, K1 kernel choice), then the skip masks
+        RoleRange rm, ro;
+        role_ranges(c, rm, ro);
+        return pack_instances(c, *q, inst0, n, rm, ro);
+    };
+    return end_call(*q, issue(), false);                                     // the engine's queue synchronised in pack_instances
 }
 
 // Instance src[k] becomes what export_instances(src[k], 1) then import_instances(dst[k], 1) would make of dst[k], with
 // the data moving engine to engine: running EQ state of the sources into the mirrors, every array of the image plan
-// (mirror rows included) from source to destination, then the destinations' mirror rows into the packed stores.
+// (mirror rows included) from source to destination, then the destinations' mirror rows into the packed stores.  Issued on
+// the destination's queue dst_q with its lists.  The engine's (src_q == dst_q) reads the modes of the instances named from
+// the device and returns when the engine is updated.  On lanes every src[k] lies in src_q's window and every dst[k] in
+// dst_q's; the copy runs after the source lane's calls issued before it and the source lane's later calls run after it,
+// the envelope counts come from env_mode, and the call does not wait.
 template <class A>
-int copy_instances(ChainHost<A> *c, uint32_t n, const uint32_t *src, const uint32_t *dst)
+int copy_instances(ChainHost<A> *c, Queue *src_q, Queue *dst_q, uint32_t n, const uint32_t *src, const uint32_t *dst)
 {
-    if (!c || !src || !dst) return fail(DSPI_EINVAL, "null argument");
+    if (!src_q || !dst_q) return DSPI_EINVAL;
+    if (!src || !dst) return fail(DSPI_EINVAL, "null argument");
     const uint32_t N = c->desc.n_instances;
     uint32_t lo = N, hi = 0;                                                // span of every index named, for the envelope count
     for (uint32_t k = 0; k < n; k++) {
         if (src[k] >= N || dst[k] >= N)
             return fail(DSPI_ERANGE, "copy %u names instance %u, outside engine of %u", k, src[k] >= N ? src[k] : dst[k], N);
+        const bool src_out = src[k] - src_q->inst0 >= src_q->n;              // never for the engine's queue
+        if (src_out || dst[k] - dst_q->inst0 >= dst_q->n) {
+            const Queue &w = src_out ? *src_q : *dst_q;
+            return fail(DSPI_ERANGE, "copy %u names instance %u, outside its lane's window [%u, %u)", k, src_out ? src[k] : dst[k], w.inst0,
+                        w.inst0 + w.n);
+        }
         lo = std::min(lo, std::min(src[k], dst[k]));
         hi = std::max(hi, std::max(src[k], dst[k]));
     }
@@ -1513,38 +1553,59 @@ int copy_instances(ChainHost<A> *c, uint32_t n, const uint32_t *src, const uint3
     image::Plan pl;
     if (!image_plan(c, kInImage, pl)) return fail(DSPI_EINVAL, "instance image plan exceeds its tables");
     CU_OK(cudaSetDevice(c->desc.device));
-    CU_OK(c->copy_lists.ensure(n));
-    const uint32_t *d_src = c->copy_lists.d, *d_dst = c->copy_lists.d + n;
-    std::vector<uint32_t> lists((size_t)2 * n);
-    memcpy(lists.data(), src, (size_t)n * 4);
-    memcpy(lists.data() + n, dst, (size_t)n * 4);
-    CU_OK(cudaMemcpyAsync(c->copy_lists.d, lists.data(), (size_t)2 * n * 4, cudaMemcpyHostToDevice, c->q.stream));
-    // envelope-mode instances: the modes (env row 4) of sources and destinations, behind earlier work
-    std::vector<uint32_t> mode((size_t)hi - lo + 1);
-    CU_OK(cudaMemcpyAsync(mode.data(), c->d.env + (size_t)4 * c->d.N_pad + lo, mode.size() * 4, cudaMemcpyDeviceToHost, c->q.stream));
-    CU_OK(cudaStreamSynchronize(c->q.stream));
-    uint32_t before = 0, after = 0;
-    for (uint32_t k = 0; k < n; k++) {
-        before += mode[dst[k] - lo] ? 1u : 0u;
-        after += mode[src[k] - lo] ? 1u : 0u;
-        c->env_mode[dst[k]] = mode[src[k] - lo] ? 1 : 0;
-    }
-    RoleRange rm, ro;
-    role_ranges(c, rm, ro);
-    rm.inst = ro.inst = d_src;
-    int rc = eq_unpack_range(c->eq_m, 0, n, c->q.stream, rm);               // running EQ state into the mirrors, as export
-    if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, 0, n, c->q.stream, ro);
+    Queue &q = *dst_q;
+    int rc = lane_prepare(c, q, q.copy_lists.d != nullptr);
     if (rc) return rc;
-    image::instance_copy_kernel<<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, c->q.stream>>>(pl, n, d_src, d_dst);
-    CU_OK(cudaGetLastError());
-    c->launches++;
-    c->env_instances = c->env_instances - before + after;
-    // the destinations' mirror rows -> packed stores, then the skip masks, as import
-    rm.inst = ro.inst = d_dst;
-    rc = eq_pack_range(c->eq_m, 0, n, c->q.stream, rm);
-    if (rc == DSPI_OK) rc = eq_pack_range(c->eq_o, 0, n, c->q.stream, ro);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_m, c->d.skip_m, c->q.stream);
-    if (rc == DSPI_OK) rc = eq_set_skip(c->eq_o, c->d.skip_o, c->q.stream);
+    CU_OK(q.copy_lists.ensure(q.lane ? q.n : n));                           // a lane's: n <= its window (dst distinct)
+    const uint32_t *d_src = q.copy_lists.d, *d_dst = q.copy_lists.d + n;
+    // envelope-mode instances: the modes (env row 4) of sources and destinations, behind earlier work
+    uint32_t before = 0, after = 0;
+    if (q.lane) {
+        CU_OK(begin_call(c, q));
+        if (src_q != dst_q) CU_OK(cudaStreamWaitEvent(q.stream, src_q->ev_last, 0));
+        CU_OK(bulk::lane_upload(q, q.copy_lists.d, (size_t)2 * n * 4, [&](unsigned char *b) {
+            memcpy(b, src, (size_t)n * 4);
+            memcpy(b + (size_t)n * 4, dst, (size_t)n * 4);
+        }));
+        for (uint32_t k = 0; k < n; k++) {
+            before += c->env_mode[dst[k]];
+            after += c->env_mode[src[k]];
+            c->env_mode[dst[k]] = c->env_mode[src[k]];
+        }
+    } else {
+        std::vector<uint32_t> lists((size_t)2 * n);
+        memcpy(lists.data(), src, (size_t)n * 4);
+        memcpy(lists.data() + n, dst, (size_t)n * 4);
+        CU_OK(cudaMemcpyAsync(q.copy_lists.d, lists.data(), (size_t)2 * n * 4, cudaMemcpyHostToDevice, q.stream));
+        std::vector<uint32_t> mode((size_t)hi - lo + 1);
+        CU_OK(cudaMemcpyAsync(mode.data(), c->d.env + (size_t)4 * c->d.N_pad + lo, mode.size() * 4, cudaMemcpyDeviceToHost, q.stream));
+        CU_OK(cudaStreamSynchronize(q.stream));
+        for (uint32_t k = 0; k < n; k++) {
+            before += mode[dst[k] - lo] ? 1u : 0u;
+            after += mode[src[k] - lo] ? 1u : 0u;
+            c->env_mode[dst[k]] = mode[src[k] - lo] ? 1 : 0;
+        }
+    }
+    auto issue = [&]() -> int {
+        RoleRange rm, ro;
+        role_ranges(c, rm, ro);
+        rm.inst = ro.inst = d_src;
+        int rc = eq_unpack_range(c->eq_m, 0, n, q.stream, rm);               // running EQ state into the mirrors, as export
+        if (rc == DSPI_OK) rc = eq_unpack_range(c->eq_o, 0, n, q.stream, ro);
+        if (rc) return rc;
+        image::instance_copy_kernel<<<dim3((n + 31) / 32, pl.n_tasks), 256, 0, q.stream>>>(pl, n, d_src, d_dst);
+        CU_OK(cudaGetLastError());
+        c->launches++;
+        c->env_instances = c->env_instances - before + after;
+        // the destinations' mirror rows -> packed stores, then the skip masks, as import
+        rm.inst = ro.inst = d_dst;
+        return pack_instances(c, q, 0, n, rm, ro);
+    };
+    rc = end_call(q, issue(), false);                                       // the engine's queue synchronised in pack_instances
+    if (src_q != dst_q) {                                                   // the source lane's next call, and join_lanes, wait for the copy
+        CU_OK(cudaStreamWaitEvent(src_q->stream, q.ev_last, 0));
+        CU_OK(cudaEventRecord(src_q->ev_last, src_q->stream));
+    }
     return rc;
 }
 

@@ -998,10 +998,10 @@ int   dspi_chainq_lane_sync  (dspi_chainq *c, uint32_t lane);
  *   DSPI_EINVAL; a window violation with DSPI_ERANGE.
  *   No lane control call made.  Every other call issues exactly the work it issues without them.
  * Left as barriers: _download_biquads (an instance image carries the biquads with their state), the state blob
- * (_state_export / _state_import), and the writes _set_params, _upload_biquads, _set_eq_params_device, _set_dynamics_device,
- * _copy_instances and _import_instances, since the wire-packet routes above cover what a Console or a preset sends and a
- * device that changes rate moves to another group's window with _copy_instances.  The reads a running group needs have
- * lane forms (the lane read calls below). */
+ * (_state_export / _state_import), and the writes _set_params, _upload_biquads, _set_eq_params_device and
+ * _set_dynamics_device, since the wire-packet routes above cover what a Console or a preset sends.  The reads a running
+ * group needs have lane forms (the lane read calls below), and so do the moves of a device into a group's window (the
+ * lane move calls below). */
 int dspi_chain_lane_edit_bulk_device  (dspi_chain *c, uint32_t lane, uint32_t n_edits, const dspi_bulk_edit *edits, int exact_db,
                                        float sample_rate, int32_t *d_results);
 int dspi_chain_lane_set_preset_mute   (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const dspi_preset_mute *states,
@@ -1076,6 +1076,46 @@ int dspi_chainq_lane_response_device      (dspi_chainq *c, uint32_t lane, uint32
                                           uint32_t n_freqs, float sample_rate, float *d_out);
 int dspi_chainq_lane_get_preset_mute      (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_preset_mute *d_states);
 int dspi_chainq_lane_get_spdif_tx         (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, dspi_spdif_tx *d_tx);
+
+/* Lane move calls: the writes a device needs when it moves (a rate change moves it into another clock group's window, a
+ * move to another engine or GPU imports its image there, a checkpoint is restored into a running group), issued on the
+ * groups' lanes so that they neither wait for nor hold up the other groups.
+ *   Semantics.  _lane_import_instances is _import_instances over [inst0, inst0 + n); _lane_copy_instances is
+ *   _copy_instances(n, src, dst), with the same argument checks and the same all-or-nothing header check: src may repeat,
+ *   dst is distinct and shares no index with src.  Outputs, biquads, running state, meters, envelope, transmitter,
+ *   configuration record and marks are byte for byte what the same sequence gives with these calls issued as engine-level
+ *   calls.
+ *   Window.  Import: [inst0, inst0 + n) lies inside the lane's window.  Copy: every src[k] lies inside src_lane's window and
+ *   every dst[k] inside dst_lane's; src_lane == dst_lane repacks within one group.  Otherwise the call fails with
+ *   DSPI_ERANGE.  n == 0 does nothing.
+ *   Ordering.  An import is ordered as the lane control calls are.  A copy is ordered against both of its lanes: it runs
+ *   after every call issued earlier on either lane and after the engine-level calls issued before it, and every later call
+ *   on either lane runs after it; it is never ordered against a third lane.  So the source lane may free the old slot right
+ *   after the copy (with _lane_reset_instances, say) and the destination still gets the bytes from before the reset.
+ *   Images.  images is host memory (an image from _export_instances, or from _lane_export_instances copied to the host),
+ *   read during the call: it may be reused as soon as the call returns.  Any image_stride >= dspi_chain_instance_image_size
+ *   is accepted.  Host memory lets the call check every header before anything is written, and keep its count of
+ *   envelope-mode instances from the images without reading the device.
+ *   No host wait.  Both calls return without waiting for the device.  src and dst are read during the call.  Exceptions,
+ *   each a growth of a buffer that first waits for every lane and the engine stream: a lane's first import allocates its
+ *   image staging (the one its exports use, sized for its whole window, at most 32 MiB, DSPI_HOST_CHUNK_MB), unless an
+ *   export did; a lane's first copy as destination allocates its instance lists, sized for its window so that no later
+ *   copy grows them; and an engine whose skip rows were never set remasks every row once.  Images and lists go through the
+ *   lane's ring of 8 pinned host buffers (see the lane control calls; a copy's lists through the destination's): one
+ *   buffer carries one staging chunk of images, at most 32 MiB (DSPI_HOST_CHUNK_MB) or one image if that is larger, or
+ *   the 8 n bytes of a copy's lists.
+ *   K1 kernel choice.  As for the lane control calls: both re-pack EQ rows and leave the choice to the next engine-level
+ *   call.
+ *   Errors (nothing is written on any error): every refusal of the engine-level call (NULL images or lists, a stride below
+ *   the image size, a bad magic or version, an image of another arith, band count or size, a duplicate dst, an index
+ *   both a source and a destination), and an unknown or closed lane, with DSPI_EINVAL; a window violation with
+ *   DSPI_ERANGE.
+ *   No lane move made.  Every other call issues exactly the work it issues without them; _import_instances and
+ *   _copy_instances keep their copies, synchronisations and launches. */
+int dspi_chain_lane_import_instances (dspi_chain  *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *images, size_t image_stride);
+int dspi_chain_lane_copy_instances   (dspi_chain  *c, uint32_t src_lane, uint32_t dst_lane, uint32_t n, const uint32_t *src, const uint32_t *dst);
+int dspi_chainq_lane_import_instances(dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *images, size_t image_stride);
+int dspi_chainq_lane_copy_instances  (dspi_chainq *c, uint32_t src_lane, uint32_t dst_lane, uint32_t n, const uint32_t *src, const uint32_t *dst);
 
 /* ---- frequency response of EQ channels and chain instances ------------------------------------ */
 /* The complex transfer function H(e^{j omega}) of the linear, time-invariant part of the path the NEXT process call applies,
