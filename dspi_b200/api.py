@@ -71,6 +71,8 @@ SYMBOLS = [
     "dspi_chainq_lane_collect_bulk_device", "dspi_chainq_lane_collect_preset_device", "dspi_chainq_lane_export_instances",
     "dspi_chainq_lane_response_device", "dspi_chainq_lane_get_preset_mute", "dspi_chainq_lane_get_spdif_tx",
     "dspi_chain_lane_import_instances", "dspi_chain_lane_copy_instances", "dspi_chainq_lane_import_instances", "dspi_chainq_lane_copy_instances",
+    "dspi_chain_lane_process_packets_host", "dspi_chain_lane_process_subframes_host",
+    "dspi_chainq_lane_process_packets_host", "dspi_chainq_lane_process_subframes_host",
 ]
 
 
@@ -177,7 +179,8 @@ def lib():
             for form in ("packets", "subframes"):
                 for where in ("host", "device"):
                     getattr(h, "%s_process_%s_range_%s" % (pre, form, where)).argtypes = [vp, u32, u32, vp, u32, u32, vp, vp, vp, vp]
-                getattr(h, "%s_lane_process_%s_device" % (pre, form)).argtypes = [vp, u32, u32, u32, vp, u32, u32, vp, vp, vp, vp]
+                for where in ("device", "host"):
+                    getattr(h, "%s_lane_process_%s_%s" % (pre, form, where)).argtypes = [vp, u32, u32, u32, vp, u32, u32, vp, vp, vp, vp]
             getattr(h, pre + "_lane_open").argtypes = [vp, u32, u32, vp]
             getattr(h, pre + "_lane_close").argtypes = [vp, u32]
             getattr(h, pre + "_lane_stream").argtypes = [vp, u32]
@@ -264,6 +267,17 @@ class PinnedBuffer:
             self.array = None
             lib().dspi_host_free(self.ptr)
             self.ptr = None
+
+
+def _pinned(buf):
+    """(address, bytes, rows) of a PinnedBuffer or a torch tensor (its memory is checked by the library, not here)"""
+    if isinstance(buf, PinnedBuffer):
+        return buf.ptr, buf.nbytes, buf.shape[0]
+    if hasattr(buf, "data_ptr") and hasattr(buf, "is_contiguous"):
+        if not buf.is_contiguous():
+            raise ValueError("a host buffer must be contiguous")
+        return buf.data_ptr(), buf.numel() * buf.element_size(), buf.shape[0]
+    raise TypeError("a host buffer must be a PinnedBuffer or a pinned torch tensor")
 
 
 class EqEngine:
@@ -846,6 +860,30 @@ class _ChainEngine:
     def lane_process_subframes_device(self, lane, inst0, n, pcm_ptr, bit_depth, packet_frames, subframes_ptr=0, pdm_ptr=0, status_ptr=0):
         """``process_subframes_range_device`` issued on a lane (the range inside its window), asynchronous on ``lane_stream(lane)``."""
         self._lane_process("subframes", lane, inst0, n, pcm_ptr, bit_depth, packet_frames, subframes_ptr, pdm_ptr, status_ptr)
+
+    def lane_process_packets_host(self, lane, inst0, pcm, bit_depth, packet_frames, spdif=None, pdm=None, status=None, subframes=False):
+        """``process_packets_range_host`` (``subframes``: ``process_subframes_range_host``) issued on a lane, over
+        [inst0, inst0 + n) inside its window, n = rows of ``pcm``.  Every buffer is page-locked host memory: a ``PinnedBuffer``
+        or a pinned torch tensor (pageable memory is refused).  ``pcm`` uint8 [n, F * bytes_per_frame]; ``spdif`` [n, pairs, F,
+        2] int32 words or [n, pairs, F, 2, 2] uint32 subframes, ``pdm`` [n, F, 8] uint32 and ``status`` [n] status records,
+        each optional.  Returns without waiting: ``pcm`` is read and the outputs are written on ``lane_stream(lane)``, so
+        reuse ``pcm`` and read the outputs only after an event recorded there (or ``lane_sync``)."""
+        t, F = _packet_table(packet_frames)
+        p, nbytes, n = _pinned(pcm)
+        if nbytes != n * F * (6 if bit_depth == 24 else 4):
+            raise ValueError("pcm must hold n rows of F frames")
+        need = [n * self._PAIRS * F * (16 if subframes else 8), n * F * 32, n * self._STATUS.itemsize]
+        outs = []
+        for buf, want, what in zip((spdif, pdm, status), need, ("spdif", "pdm", "status")):
+            if buf is None:
+                outs.append(None)
+                continue
+            ptr, size, _ = _pinned(buf)
+            if size < want:
+                raise ValueError("%s holds %d bytes, the call writes %d" % (what, size, want))
+            outs.append(C.c_void_p(ptr))
+        form = "subframes" if subframes else "packets"
+        _check(self._fn("lane_process_%s_host" % form)(self._h, int(lane), int(inst0), n, C.c_void_p(p), bit_depth, t.size, t.ctypes.data, *outs))
 
     def lane_stream(self, lane):
         """The stream where the lane's outputs become visible (None for a lane that is not open)."""

@@ -75,6 +75,63 @@ struct IndexLists {
     }
 };
 
+// A lane's device staging of its host process calls (process_lane_host) and the two copy streams that move each packet
+// slice in and out while the stage streams run.  Every buffer holds the whole window at max_frames, so that no later call
+// grows it; each is allocated by the first call that needs it: PCM, status, streams and events by the first host call,
+// PDM by the first one with PDM out, S/PDIF by the first one with words (8 bytes per pair frame) or subframes (16; a
+// later subframe call after words replaces the words buffer once).  Freed when the lane closes.
+struct HostStage {
+    void *d_pcm = nullptr;                   // [n][max_frames] frames of up to 6 bytes
+    void *d_status = nullptr;                // [n] status records
+    uint32_t *d_pdm = nullptr;               // [n][max_frames][8]
+    void *d_spdif = nullptr;                 // [n][pairs][max_frames] pair frames of spdif_frame bytes
+    size_t spdif_frame = 0;
+    cudaStream_t s_in = nullptr, s_back = nullptr;   // host to device (PCM), device to host (S/PDIF, PDM)
+    cudaEvent_t ev_back = nullptr, ev_in[ChainStreams::kMaxSlices] = {}, ev_pdm[ChainStreams::kMaxSlices] = {};
+
+    bool has(size_t sf, bool pdm) const { return s_in && (!pdm || d_pdm) && sf <= spdif_frame; }
+
+    // a window of n instances of pairs S/PDIF pairs and status records of status_bytes; after has() was false, every
+    // lane and the engine stream drained
+    cudaError_t ensure(size_t n, size_t max_frames, size_t pairs, size_t status_bytes, size_t sf, bool pdm)
+    {
+        cudaError_t e = cudaSuccess;
+        if (!s_in) {
+            e = cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking);
+            if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s_back, cudaStreamNonBlocking);
+            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_back, cudaEventDisableTiming);
+            for (int i = 0; i < ChainStreams::kMaxSlices && e == cudaSuccess; i++) {
+                e = cudaEventCreateWithFlags(&ev_in[i], cudaEventDisableTiming);
+                if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_pdm[i], cudaEventDisableTiming);
+            }
+            if (e == cudaSuccess) e = cudaMalloc(&d_pcm, n * max_frames * 6);
+            if (e == cudaSuccess) e = cudaMalloc(&d_status, n * status_bytes);
+            if (e != cudaSuccess) { destroy(); return e; }
+        }
+        if (pdm && !d_pdm) e = cudaMalloc((void **)&d_pdm, n * max_frames * 8 * 4);
+        if (e == cudaSuccess && sf > spdif_frame) {
+            cudaFree(d_spdif);
+            d_spdif = nullptr; spdif_frame = 0;
+            e = cudaMalloc(&d_spdif, n * pairs * max_frames * sf);
+            if (e == cudaSuccess) spdif_frame = sf;
+        }
+        return e;
+    }
+
+    void destroy()
+    {
+        for (cudaStream_t *s : { &s_in, &s_back })
+            if (*s) { cudaStreamSynchronize(*s); cudaStreamDestroy(*s); *s = nullptr; }
+        for (void **p : { &d_pcm, &d_status, (void **)&d_pdm, &d_spdif }) { cudaFree(*p); *p = nullptr; }
+        spdif_frame = 0;
+        if (ev_back) { cudaEventDestroy(ev_back); ev_back = nullptr; }
+        for (int i = 0; i < ChainStreams::kMaxSlices; i++) {
+            if (ev_in[i]) { cudaEventDestroy(ev_in[i]); ev_in[i] = nullptr; }
+            if (ev_pdm[i]) { cudaEventDestroy(ev_pdm[i]); ev_pdm[i] = nullptr; }
+        }
+    }
+};
+
 // An issue queue: the stream a call is issued on and where it ends, the stage streams and packet schedule of its process
 // calls, the staging of its control calls, and the instance window [inst0, inst0 + n) its calls may touch.  The engine
 // issues on one over every instance (ChainHost::q).  A lane (dspi_chain_lane_*) is another, over its window: its calls
@@ -92,6 +149,7 @@ struct Queue {
     bulk::HostRing ring;             // a lane's edits, packets, images, rates, slot indices, fade rows and transmitter rows on their way to the device
     ResponseBuffers resp;            // frequency table of the response calls; image staging of export and import (and, the engine's, of _response_host)
     IndexLists copy_lists;           // device instance lists of the copies issued on this queue (the destination's, for a lane)
+    HostStage host;                  // a lane's staging and copy streams of its host process calls
     cudaEvent_t ev_engine = nullptr, ev_last = nullptr;   // a lane's
 
     // `lane` set first
@@ -116,6 +174,7 @@ struct Queue {
         ring.destroy();
         resp.destroy();
         copy_lists.destroy();
+        host.destroy();
         for (cudaEvent_t *ev : { &ev_engine, &ev_last })
             if (*ev) { cudaEventDestroy(*ev); *ev = nullptr; }
         if (stream) { cudaStreamDestroy(stream); stream = nullptr; }
@@ -981,12 +1040,33 @@ int eq_stage(ChainHost<A> *c, dspi_eq *eq, uint32_t roles, void *rows, uint32_t 
     return DSPI_OK;
 }
 
+// The host buffers of a lane host call (process_lane_host), whose packet slices run_stages copies through the lane's
+// staging hs on its copy streams: each slice's PCM in before its front stage, its S/PDIF rows out after its output stage
+// and its PDM rows out after its modulator.  spdif / pdm NULL: that output is not copied.
+struct HostCopies {
+    HostStage *hs;
+    const void *pcm;
+    void *spdif;
+    uint32_t *pdm;
+    size_t pcm_frame, spdif_frame;   // bytes of one frame of a PCM row, of an S/PDIF row
+    size_t spdif_rows;               // n * pairs
+};
+
+// frames [fb, fe) of `rows` rows of F frames of `frame` bytes, between two buffers of that layout
+inline cudaError_t copy_frames(void *dst, const void *src, size_t rows, size_t F, size_t frame, uint32_t fb, uint32_t fe, cudaMemcpyKind kind,
+                               cudaStream_t s)
+{
+    const size_t pitch = F * frame, off = (size_t)fb * frame;
+    return cudaMemcpy2DAsync((char *)dst + off, pitch, (const char *)src + off, pitch, (size_t)(fe - fb) * frame, rows, kind, s);
+}
+
 // One call over instances [inst0, inst0 + n) and the schedule x.sched has checked, with the kernel set K, issued on the
 // queue x: its offsets go to the device first, on x.stream, where the call also ends.  The caller's buffers hold rows for
-// the n instances.  d_spdif: words, or subframes when `subframes` is set (either may be NULL).
+// the n instances.  d_spdif: words, or subframes when `subframes` is set (either may be NULL).  With hc, the device
+// buffers are the lane's staging and the slices are copied from and to the host as they go (HostCopies).
 template <class A, class K>
 int run_stages(ChainHost<A> *c, Queue &x, uint32_t inst0, uint32_t n, const void *d_pcm, uint32_t bit_depth, const uint16_t *packet_frames,
-               void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status)
+               void *d_spdif, bool subframes, uint32_t *d_pdm, typename A::Status *d_status, const HostCopies *hc = nullptr)
 {
     PacketSchedule &ps = x.sched;
     const uint32_t n_packets = ps.n_packets, F = ps.frames;
@@ -1026,10 +1106,25 @@ int run_stages(ChainHost<A> *c, Queue &x, uint32_t inst0, uint32_t n, const void
     const uint32_t n_warps16 = ((n + 31) & ~31u) / 16;                       // pre / post: 16 instances per warp
     CU_OK(cudaEventRecord(st.ev_begin, x.stream));
     CU_OK(cudaStreamWaitEvent(st.s_front, st.ev_begin, 0));
+    HostStage *hs = hc ? hc->hs : nullptr;
+    if (hs) {
+        // the copy-in stream starts behind this call's beginning (earlier calls have read the PCM staging); the modulator
+        // rows of instances without a sub go back as zeros, so the PDM staging is cleared before the first modulator
+        CU_OK(cudaStreamWaitEvent(hs->s_in, st.ev_begin, 0));
+        if (hc->pdm) {
+            CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_begin, 0));
+            CU_OK(cudaMemsetAsync(d_pdm, 0, (size_t)n * F * 8 * 4, st.s_pdm));
+        }
+    }
     for (uint32_t sl = 0; sl < n_slices; sl++) {
         const uint32_t p0 = slice_bounds[sl], p1 = slice_bounds[sl + 1];
         const uint32_t fb = ps.off[p0], fe = ps.off[p1];
         int rc;
+        if (hs) {                                                            // this slice's PCM frames, in before its front stage
+            CU_OK(copy_frames((void *)d_pcm, hc->pcm, n, F, hc->pcm_frame, fb, fe, cudaMemcpyHostToDevice, hs->s_in));
+            CU_OK(cudaEventRecord(hs->ev_in[sl], hs->s_in));
+            CU_OK(cudaStreamWaitEvent(st.s_front, hs->ev_in[sl], 0));
+        }
         // ---- front: unpack + loudness -> master EQ -> leveller + crossfeed
         K::pre<<<(n_warps16 + 1) / 2, 64, 0, st.s_front>>>(d, inst0, n, (const uint8_t *)d_pcm, bit_depth, fb, fe, F);
         CU_OK(cudaGetLastError());
@@ -1049,11 +1144,24 @@ int run_stages(ChainHost<A> *c, Queue &x, uint32_t inst0, uint32_t n, const void
             K::template outpost<false><<<out_grid, 256, 0, st.s_out>>>(d, inst0, n, p0, p1 - p0, F, (int32_t *)d_spdif, c->tx);
         CU_OK(cudaGetLastError());
         CU_OK(cudaEventRecord(st.ev_out[sl], st.s_out));
+        if (hs && hc->spdif) {                                               // this slice's S/PDIF frames, out after its output stage
+            CU_OK(cudaStreamWaitEvent(hs->s_back, st.ev_out[sl], 0));
+            CU_OK(copy_frames(hc->spdif, d_spdif, hc->spdif_rows, F, hc->spdif_frame, fb, fe, cudaMemcpyDeviceToHost, hs->s_back));
+        }
         // ---- modulator
         CU_OK(cudaStreamWaitEvent(st.s_pdm, st.ev_out[sl], 0));
         K::pdm<<<(n + 127) / 128, 128, 0, st.s_pdm>>>(d, inst0, n, fb, fe, F, d_pdm);
         CU_OK(cudaGetLastError());
         c->launches += 5;
+        if (hs && hc->pdm) {                                                 // and its PDM frames, out after its modulator
+            CU_OK(cudaEventRecord(hs->ev_pdm[sl], st.s_pdm));
+            CU_OK(cudaStreamWaitEvent(hs->s_back, hs->ev_pdm[sl], 0));
+            CU_OK(copy_frames(hc->pdm, d_pdm, n, F, 8 * 4, fb, fe, cudaMemcpyDeviceToHost, hs->s_back));
+        }
+    }
+    if (hs) {                                                                // the call ends after its last copy out
+        CU_OK(cudaEventRecord(hs->ev_back, hs->s_back));
+        CU_OK(cudaStreamWaitEvent(x.stream, hs->ev_back, 0));
     }
     K::ring<<<stream_grid((uint64_t)n * A::kOuts), 256, 0, st.s_out>>>(d, inst0, n, F, n_packets, c->tx.bp);   // after the last outpost launch (stream order)
     CU_OK(cudaGetLastError());
@@ -1135,6 +1243,49 @@ int process_host(ChainHost<A> *c, uint32_t inst0, uint32_t n, const void *pcm, u
     return DSPI_OK;
 }
 
+// a lane host call's buffer: NULL, or page-locked host memory (a copy from pageable memory would make the call wait)
+inline bool page_locked(const void *p)
+{
+    if (!p) return true;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return a.type == cudaMemoryTypeHost;
+}
+
+// process_host's layouts, checks and results on lane q, without waiting: every buffer page-locked, staged through the
+// lane's own device buffers, each packet slice copied in and out on the lane's copy streams as the stages reach it
+// (run_stages), the status after the call.  pcm is read and the outputs written on the lane's timeline.
+template <class A>
+int process_lane_host(ChainHost<A> *c, Queue *q, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth, uint32_t n_packets,
+                      const uint16_t *packet_frames, void *spdif_out, bool subframes, uint32_t *pdm_out, typename A::Status *status)
+{
+    if (!q) return DSPI_EINVAL;
+    int rc = check_packets(c, q->sched, pcm, bit_depth, n_packets, packet_frames);
+    if (rc) return rc;
+    if ((rc = check_window(*q, inst0, n))) return rc;
+    CU_OK(cudaSetDevice(c->desc.device));
+    const void *bufs[4] = { pcm, spdif_out, pdm_out, status };
+    static const char *const names[4] = { "pcm", "the S/PDIF output", "pdm_out", "status" };
+    for (int k = 0; k < 4; k++)
+        if (!page_locked(bufs[k])) return fail(DSPI_EINVAL, "%s is not page-locked host memory", names[k]);
+    if (n == 0) return DSPI_OK;
+    constexpr size_t pairs = (A::kOuts - 1) / 2;                            // the sub output has no S/PDIF pair
+    const size_t sf = spdif_out ? (subframes ? 16 : 8) : 0;
+    HostStage &hs = q->host;
+    if ((rc = lane_grow(c, *q, hs.has(sf, pdm_out != nullptr))) != DSPI_OK) return rc;
+    CU_OK(hs.ensure(q->n, c->desc.max_frames, pairs, sizeof(typename A::Status), sf, pdm_out != nullptr));
+    CU_OK(begin_call(c, *q));
+    const HostCopies hc = { &hs, pcm, spdif_out, pdm_out, (size_t)(bit_depth == 24 ? 6 : 4), sf, (size_t)n * pairs };
+    typename A::Status *d_status = status ? (typename A::Status *)hs.d_status : nullptr;
+    rc = A::with_stages(c->desc, [&](auto k) {
+        return run_stages<A, decltype(k)>(c, *q, inst0, n, hs.d_pcm, bit_depth, packet_frames, spdif_out ? hs.d_spdif : nullptr, subframes,
+                                          pdm_out ? hs.d_pdm : nullptr, d_status, &hc);
+    });
+    if (rc == DSPI_OK && status && cudaMemcpyAsync(status, d_status, (size_t)n * sizeof(*d_status), cudaMemcpyDeviceToHost, q->stream) != cudaSuccess)
+        rc = fail(DSPI_ECUDA, "status copy: %s", cudaGetErrorString(cudaGetLastError()));
+    return end_call(*q, rc, false);
+}
+
 // the uniform schedule: n_packets packets of fpp frames, from device (host == false) or host memory
 template <class A>
 int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32_t n_packets, uint32_t fpp, int32_t *spdif, uint32_t *pdm,
@@ -1151,7 +1302,7 @@ int process_uniform(ChainHost<A> *c, const void *pcm, uint32_t bit_depth, uint32
 // ---- lanes: issue queues of one engine over disjoint instance windows, whose calls run concurrently -------------------
 // A lane takes process calls and the control calls a running clock group needs (edits, fades, transmitter restamps,
 // resets, applies, preset applies and rate switches): set_preset_mute, set_spdif_tx, reset_instances, edit_bulk_device,
-// apply_bulk_device, apply_preset_device, set_rate_device and process_device on its queue; the reads it needs
+// apply_bulk_device, apply_preset_device, set_rate_device, process_device and process_lane_host on its queue; the reads it needs
 // (collect_bulk_device, collect_preset_device, export_instances, response, get_preset_mute, get_spdif_tx), into device
 // memory; and the moves of devices into its window (import_instances, and copy_instances on the destination's queue,
 // ordered against the source lane too).

@@ -922,7 +922,8 @@ int dspi_chainq_process_subframes_range_device(dspi_chainq *c, uint32_t inst0, u
  *   lane's id may be handed out again.
  *   Calls.  _lane_process_packets_device / _lane_process_subframes_device run over any [inst0, inst0 + n) inside the lane's
  *   window (inst0 a multiple of 64, n == 0 does nothing).  Arguments, buffer layout and results are exactly those of
- *   dspi_chain(q)_process_packets_range_device / _process_subframes_range_device over that range.
+ *   dspi_chain(q)_process_packets_range_device / _process_subframes_range_device over that range.  Their host-memory forms
+ *   are the lane host calls below.
  *   Ordering.  Calls on one lane run in issue order.  A lane call runs after every engine-level call issued before it, and
  *   every engine-level call runs after every lane call issued before it.  An engine-level call is any call taking the
  *   engine that is not a lane call: process, range process, set / edit / apply / collect, copy / export / import / reset,
@@ -962,6 +963,51 @@ int   dspi_chainq_lane_process_subframes_device(dspi_chainq *c, uint32_t lane, u
                                                 dspi_spdif_subframe *d_subframes, uint32_t *d_pdm_out, dspi_status_q28 *d_status);
 void *dspi_chainq_lane_stream(dspi_chainq *c, uint32_t lane);
 int   dspi_chainq_lane_sync  (dspi_chainq *c, uint32_t lane);
+
+/* Lane host calls: a clock group's packets served from host memory on its lane (PCM from USB or the network, S/PDIF and PDM
+ * back to the transmitters), so that a host-resident farm neither waits for nor holds up the other groups, and the copies
+ * run while the stages do.
+ *   Semantics.  _lane_process_packets_host / _lane_process_subframes_host have exactly the layouts, argument checks and
+ *   results of dspi_chain(q)_process_packets_range_host / _process_subframes_range_host over [inst0, inst0 + n): the range
+ *   lies inside the lane's window and inst0 is a multiple of 64; PDM rows of instances whose sub is off come back as zeros
+ *   on every call.  Outputs, state, meters, envelope, transmitter and configuration record are byte for byte those of the
+ *   same sequence with these calls issued as the engine-level range host calls.
+ *   Memory.  pcm, spdif_out / subframes, pdm_out and status are page-locked host memory (dspi_host_alloc, cudaHostAlloc,
+ *   cudaHostRegister, a pinned torch tensor); every output may be NULL.  Each non-NULL buffer is checked at its first byte
+ *   and a pageable one is refused with DSPI_EINVAL before anything is issued: a lane call never waits, and a copy from
+ *   pageable memory would.  The caller keeps the whole extent of every buffer page-locked until the call has completed.
+ *   Ordering and lifetime.  Ordered as the lane process calls are: behind its lane's calls in issue order and against
+ *   engine-level calls, never against another lane.  The call returns without waiting for the device.  packet_frames is
+ *   read during the call.  pcm is read, and the outputs written, on the lane's timeline: pcm may be rewritten, and the
+ *   outputs read, only once the lane has reached the end of the call, which an event recorded on _lane_stream after the
+ *   call (or _lane_sync) shows.  This differs from the lane control calls, which read their inputs during the call.
+ *   Pipelining.  The call runs over the packet slices of the stage pipeline.  Each slice's PCM frames are copied in on a
+ *   copy stream of the lane just before its front stage, its S/PDIF frames leave after its output stage and its PDM frames
+ *   after its modulator, on a second copy stream; the status leaves after the call.  So the copies overlap the stages
+ *   and one another, and the device time hides under the link time.  Consecutive calls of one lane do not overlap.
+ *   Staging.  Each lane has its own device staging, sized for its whole window at max_frames so that no later call grows
+ *   it, and two copy streams.  The lane's first host call allocates the PCM (6 bytes per instance-frame) and status
+ *   staging and the streams, its first call with PDM out the PDM staging (32 bytes per instance-frame), its first call with
+ *   words the S/PDIF staging at 8 bytes per pair frame (32 per float, 16 per Q28 instance-frame) and its first call with
+ *   subframes at 16 (64 / 32), replacing a words staging; each of these first waits for every lane and the engine stream.
+ *   _lane_close frees them.  A 1024-instance float window at 6144 frames takes about 0.44 GB for words + PDM, 0.64 GB for
+ *   subframes + PDM.
+ *   Errors (nothing is issued on any error): every refusal of the range host calls, a pageable buffer and an unknown or
+ *   closed lane with DSPI_EINVAL; a range outside the lane's window with DSPI_ERANGE.
+ *   No lane host call made.  Every other call issues exactly the work it issues without them; the engine-level host calls
+ *   stay barriers that return when their outputs are in host memory. */
+int dspi_chain_lane_process_packets_host    (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth,
+                                             uint32_t n_packets, const uint16_t *packet_frames, int32_t *spdif_out, uint32_t *pdm_out,
+                                             dspi_status *status);
+int dspi_chain_lane_process_subframes_host  (dspi_chain *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth,
+                                             uint32_t n_packets, const uint16_t *packet_frames, dspi_spdif_subframe *subframes,
+                                             uint32_t *pdm_out, dspi_status *status);
+int dspi_chainq_lane_process_packets_host   (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth,
+                                             uint32_t n_packets, const uint16_t *packet_frames, int32_t *spdif_out, uint32_t *pdm_out,
+                                             dspi_status_q28 *status);
+int dspi_chainq_lane_process_subframes_host (dspi_chainq *c, uint32_t lane, uint32_t inst0, uint32_t n, const void *pcm, uint32_t bit_depth,
+                                             uint32_t n_packets, const uint16_t *packet_frames, dspi_spdif_subframe *subframes,
+                                             uint32_t *pdm_out, dspi_status_q28 *status);
 
 /* Lane control calls: the control calls a running clock group needs (a Console edit, a preset-change fade, a transmitter
  * restamp, a device restart, a device connecting, a preset recall, a session rate change), issued on the group's lane so
